@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- EM iterations/sec of the B200 DFM hot path (BASELINE.json metric).
+"""bench.py -- EM iterations/sec of the H100 DFM hot path (BASELINE.json metric).
 
 Unit of work: one EM iteration (Kalman filter + RTS smoother E-step, M-step) on one C2-shaped panel
 (N=200, r=8, T=500, FP64).  A "step" = EM_ITERS iterations over this rank's shard of independent
@@ -10,11 +10,14 @@ followed by the path's single collective: one NCCL all-gather of the per-replica
   e2e    : same through the C ABI with pinned HOST buffers (H2D of panel + initial parameters and
            D2H of factors + parameters inside the timed region)
   roofline: dominant kernel's algorithmic bytes (2*T*N*8 per panel-iteration, SURVEY.md 8d) / its
-           CUDA-event duration, against MEASURED_PEAKS.json
+           CUDA-event duration, against MEASURED_PEAKS.json (else the H100 SXM data-sheet HBM3 rate)
   cpu_baseline / --impl reference: the oracle's C port of the same EM (OpenMP over panels) on the
            host cores -- the reference itself is Julia and has no Kalman/EM code (SURVEY.md 0).
 
-python bench.py --gpus N --steps K --warmup W [--impl reference]
+python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float64, at most
+64 MB in all).  The inputs are generated from a fixed seed, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -50,7 +53,7 @@ class ClockSampler:
 
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.dev), f"--query-gpu={q}", "--format=csv,noheader,nounits",
                                           "-lms", "100"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -64,15 +67,16 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"], "gpu": None, "power_limit_w": None}
         time.sleep(0.15)
         self.proc.terminate()
         sm = [float(r[0]) for r in self.rows if len(r) >= 7 and r[0].replace(".", "").isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) >= 7 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for j, n in enumerate(names) if any(len(r) >= 7 and r[3 + j].lower().startswith("active") for r in self.rows)]
+        pl = [float(r[7]) for r in self.rows if len(r) >= 9 and r[7].replace(".", "").isdigit()]
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
-                "samples": len(sm)}
+                "samples": len(sm), "gpu": next((r[8] for r in self.rows if len(r) >= 9), None), "power_limit_w": max(pl) if pl else None}
 
 
 def host_cores():
@@ -180,9 +184,41 @@ def run_reference(args):
                       "e2e": {"value": v, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(path, per_item, whole=None):
+    """Write the outputs of the last timed step as <path>/<name>.npy in float64.  `per_item` arrays share axis 0 (panel or
+    replication); if everything exceeds DUMP_BYTES, a fixed seeded sample of that axis is written instead, with its
+    indices in sample_index.npy.  `whole` arrays are written as they are."""
+    os.makedirs(path, exist_ok=True)
+    per_item = {k: np.asarray(v, dtype=np.float64) for k, v in per_item.items()}
+    whole = {k: np.asarray(v, dtype=np.float64) for k, v in (whole or {}).items()}
+    fixed = sum(a.nbytes for a in whole.values())
+    n = next(iter(per_item.values())).shape[0] if per_item else 0
+    row = sum(a.nbytes for a in per_item.values()) // max(n, 1)
+    if n and fixed + n * row > DUMP_BYTES:
+        keep = max(1, (DUMP_BYTES - fixed) // (row + 8))
+        idx = np.sort(np.random.default_rng(0).choice(n, keep, replace=False))
+        per_item = {k: a[idx] for k, a in per_item.items()}
+        per_item["sample_index"] = idx.astype(np.float64)
+    for k, a in {**per_item, **whole}.items():
+        np.save(os.path.join(path, k + ".npy"), a)
+
+
+def _cm(t, n, rows, cols):
+    """n column-major (rows x cols) blocks of a flat device tensor -> host array (n, rows, cols)."""
+    return t.cpu().numpy().reshape(n, cols, rows).transpose(0, 2, 1)
+
+
+def _l2_mb(dev):
+    import torch
+    return getattr(torch.cuda.get_device_properties(dev), "L2_cache_size", 0) / 2 ** 20
+
+
 def _peak():
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
     if os.path.exists(peaks_path):
         try:
             pk = json.load(open(peaks_path)); peak = float(pk.get("hbm_gbs", peak)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
@@ -276,6 +312,9 @@ def run_c4(args):
     ms = _timed(torch, dist, world, dev, step_device, K_)
     launches = lib.launches - l0
     clk = clocks.stop()
+    if args.dump_outputs:
+        per_var = lambda t, n: t.cpu().numpy().reshape(n, r, H, r).transpose(0, 3, 2, 1)      # -> [., variable, horizon, shock]
+        dump_outputs(args.dump_outputs, dict(irf=per_var(dirf, B)), dict(bands=per_var(dband, len(qs))))
     value = world * B * K_ / (ms * 1e-3)
     nfail = int(torch.isnan(dirf.view(B, -1)).any(1).sum().item())
 
@@ -300,8 +339,8 @@ def run_c4(args):
     roof = {"bound": "hbm", "kernel": als_k, "achieved": alg / (d_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
             "frac": alg / (d_ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src,
             "kernel_share_of_step": d_ms / tot, "dominant_kernel_of_step": dom, "avg_launch_ms": d_ms / d_cnt, "algorithmic_bytes_per_launch": alg,
-            "note": "2*T*N*8 bytes per ALS sweep and panel (SURVEY 8d); the 296 resident panels (73 MB) are re-read from L2, so the "
-                    "kernel is latency / issue bound, not HBM bound",
+            "note": "2*T*N*8 bytes per ALS sweep and panel (SURVEY 8d); the resident panels (two per SM) are re-read every step, "
+                    "mostly from L2, so the kernel is latency / issue bound, not HBM bound",
             "kernel_ms": {n: round(v_[0], 3) for n, v_ in sorted(prof.items(), key=lambda kv: -kv[1][0])}}
     cpu = None
     if rank == 0 and world == 1 and not args.no_cpu:
@@ -326,7 +365,8 @@ def run_c4(args):
                           "config": {"workload": f"C4: {world * B} bootstrap replications of the Stock-Watson panel (T={Tw}, N={ns} estimation "
                                                  f"series, r={r}, VAR({p}), 5.7 % missing): resample -> ALS -> VAR -> IRF(H={H}) -> bands",
                                      "replications_per_gpu": B, "als_sweeps_per_step": sweeps[0], "failed_replications": nfail,
-                                     "l2": "panels are regenerated every step; 296 resident panels = 73 MB < L2 (stated, not flushed)"},
+                                     "l2": f"panels are regenerated every step; {Tw * ns * 8 / 1e6:.2f} MB per panel, two resident panels per SM, "
+                                           f"L2 {_l2_mb(dev):.0f} MB (stated, not flushed)"},
                           "e2e": {"value": world * B * Ke / (ms_e * 1e-3), "unit": "bootstrap replications/s", "h2d_bytes_per_step": h2d,
                                   "d2h_bytes_per_step": d2h, "ms_per_step": ms_e / Ke},
                           "gpu_launches": int(launches), "clocks": clk, "roofline": roof, "cpu_baseline": cpu,
@@ -377,6 +417,10 @@ def run_single_panel(args):
     launches = lib.launches - l0
     clk = clocks.stop()
     iters = int(dit.item())
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {}, dict(F=_cm(dout["F"], 1, T, r)[0], Lam=_cm(dout["Lam"], 1, N, r)[0], R=dout["R"].cpu(),
+                                                 A=_cm(dout["A"], 1, r, k)[0], Q=_cm(dout["Q"], 1, r, r)[0], loglik=dout["loglik"][:iters].cpu(),
+                                                 iters=dit.cpu(), status=dst.cpu()))
     value = world * iters * K_ / (ms * 1e-3)
     hX = dX.cpu().pin_memory()
     hin = {n: t.cpu().pin_memory() for n, t in dict(Lam=dL0, R=dR0, A=dA0, Q=dQ0).items()}
@@ -445,6 +489,8 @@ def main():
     ap.add_argument("--em-iters", type=int, default=50, help="EM iterations per step (SURVEY 8d: fixed 50)")
     ap.add_argument("--path", type=int, default=0)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float64, <= 64 MB in all)")
     ap.add_argument("--config", default="c5", choices=["c5", "c4", "c3", "c2-single"],
                     help="c5 (default, the headline metric): Monte-Carlo shard of C2-shaped panels; c4: bootstrap IRF bands of the "
                          "hom_fac_1 model; c3: one large panel N=2000 r=20 T=2000; c2-single: one C2 panel, EM to convergence")
@@ -532,6 +578,10 @@ def main():
     ms_dev, ms_wall = timed(step_device, K_)
     launches = lib.launches - l0
     clk = clocks.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dict(F=_cm(dout["F"], B, T_, R_), Lam=_cm(dout["Lam"], B, NS, R_), R=dout["R"].view(B, NS).cpu(),
+                                             A=_cm(dout["A"], B, R_, k), Q=_cm(dout["Q"], B, R_, R_), loglik=dout["loglik"].view(B, iters).cpu(),
+                                             iters=dit.cpu(), status=dst.cpu()))
     ms = max(ms_dev, 0.0)
     # library work is on its own stream: the step ends with lib.sync(), so torch-stream events bracket
     # host-synchronised steps; use the larger of event / wall clock (they agree to < 1%)
@@ -569,25 +619,14 @@ def main():
     prof = lib.profile_report(); lib.profile(False)
     tot = sum(v[0] for v in prof.values()) or 1.0
     dom = max(prof, key=lambda n: prof[n][0]) if prof else None
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
-    if os.path.exists(peaks_path):
-        try:
-            pk = json.load(open(peaks_path)); peak = float(pk.get("hbm_gbs", peak)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
+    peak, peak_src = _peak()
     roof = None
     if dom:
         d_ms, d_cnt = prof[dom]
         units_per_launch = B * iters / d_cnt                       # panel-iterations one launch of the dominant kernel processes
         alg_bytes = 2.0 * T_ * NS * 8 * units_per_launch           # SURVEY 8d: 2*T*N*8 bytes per panel-iteration
         ach = alg_bytes / (d_ms / d_cnt * 1e-3) / 1e9
-        traffic = None; traffic_src = None
-        tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tp) and "fused2" in dom:
-            tj = json.load(open(tp)); traffic = tj["dram_bytes_per_panel_iteration"] * units_per_launch; traffic_src = tj["source"]
-        roof = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
-                "traffic_source": traffic_src,
+        roof = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None,
                 "peak_source": peak_src, "kernel_share_of_step": d_ms / tot, "avg_launch_ms": d_ms / d_cnt,
                 "algorithmic_bytes_per_launch": alg_bytes,
                 "kernel_ms": {n: round(v[0], 3) for n, v in sorted(prof.items(), key=lambda kv: -kv[1][0])}}
@@ -655,7 +694,7 @@ def main():
                 "config": {"workload": f"C5 shard of C2-shaped Monte-Carlo panels: {B} panels/GPU, N={NS} r={R_} T={T_} p={P_}, "
                                        f"{iters} EM iterations (Kalman filter + RTS smoother + M-step) per step, then one all-gather",
                            "panels_per_gpu": B, "em_iters_per_step": iters, "parallelism": f"replications x{world}",
-                           "l2": f"inputs {B * T_ * NS * 8 / 1e6:.0f} MB/GPU > 126 MB L2 (no flush needed)",
+                           "l2": f"inputs {B * T_ * NS * 8 / 1e6:.0f} MB/GPU, L2 {_l2_mb(dev):.0f} MB (no flush needed when larger)",
                            "path": args.path, "all_status_ok": status_ok},
                 "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "ms_per_step": ms_e2e / Ke},
                 "gpu_launches": int(launches), "clocks": clk, "roofline": roof, "cpu_baseline": cpu,

@@ -1,8 +1,8 @@
-"""dynamic_factor_models_b200 -- B200-native hot path of QuantEcon/dynamic_factor_models.
+"""dynamic_factor_models_b200 -- H100-native hot path of QuantEcon/dynamic_factor_models.
 
-Host-side mirror (Python, because Julia is not available in this image; the Julia shim that a
+Host-side mirror (Python; the Julia shim that a
 maintainer would add is julia/DFMB200.jl, see INTEGRATION.md) of the reference's `dfm_functions`
-surface over the C ABI in include/dfm_b200.h.  All arithmetic runs in hand-written sm_100a CUDA
+surface over the C ABI in include/dfm_b200.h.  All arithmetic runs in hand-written sm_90a CUDA
 kernels inside lib/libdfm_b200.so; there is no CPU fallback: importing works without a GPU, but
 creating a handle raises if the library or a CUDA device is missing.
 """

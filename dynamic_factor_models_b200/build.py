@@ -1,4 +1,4 @@
-"""Build libdfm_b200.so (CUDA, sm_100a) in-tree with nvcc.  No CPU fallback is ever built here."""
+"""Build libdfm_b200.so (CUDA, sm_90a: H100) in-tree with nvcc.  No CPU fallback is ever built here."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdfm_b200.so")
 SOURCES = ["dfm_api.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

@@ -50,6 +50,7 @@ struct ProfRec { const char* name;
 
 struct dfm_handle {
   int device;
+  int nsm;                     // streaming multiprocessors of the device: sizes grids and the per-panel CTA plans
   cudaStream_t stream;
   cudaStream_t copy_stream;    // second stream: the H2D copies of the streaming host path run here, under the EM kernel
   cudaStream_t d2h_stream;     // third stream: results of finished panels go back while the kernel is still running
@@ -193,14 +194,13 @@ static int launch_fused(dfm_handle* h, const FusedArgs& fa, int B, int T, int N,
 #ifndef DFM_EMU
   if (!dry) {
     DFM_SET_SMEM(k_em_fused<RT>, smem);
-    int dev = 0, nsm = 148, occ = 1;
-    cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+    int occ = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_em_fused<RT>, 128, smem);
     if (occ < 1) occ = 1;
-    grid = std::min(B, nsm * occ);
-  } else grid = std::min(B, 148 * 8);
+    grid = std::min(B, h->nsm * occ);
+  } else grid = std::min(B, h->nsm * 8);
 #endif
-  double* scr = arena->get<double>((size_t)(dry ? std::min(B, 148 * 8) : std::min(B, 148 * 8)) * T * FUSED_SCR(RT));
+  double* scr = arena->get<double>((size_t)std::min(B, h->nsm * 8) * T * FUSED_SCR(RT));
   if (dry) return DFM_OK;
   FusedArgs a2 = fa; a2.scratch = scr;
   L(k_em_fused<RT>, grid, 1, 128, smem, a2);
@@ -214,12 +214,12 @@ struct EmbPlan {
   double *Bpart, *qpart, *Spart, *sxxpart, *Cpart; int* counters;
   size_t smE, smM;
 };
-static EmbPlan emb_plan(int T, int N, int r, int batch) {
+static EmbPlan emb_plan(int T, int N, int r, int batch, int nsm) {
   EmbPlan e{};
   e.on = r <= 32 && !getenv("DFM_NO_EMB");
   if (!e.on) return e;
   e.ncb = (r + 7) / 8;
-  const int target = 2 * 148;
+  const int target = 2 * nsm;
   e.ntE = (T + EMB_TILE - 1) / EMB_TILE;
   int want = (target + e.ntE * batch - 1) / (e.ntE * batch);
   int ns = std::max((N + EMB_MAXSPLIT - 1) / EMB_MAXSPLIT, std::min(want, (N + 31) / 32));
@@ -260,10 +260,10 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
   int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mi = o->max_iter;
   int np = r * (r + 1) / 2;
   int* dsrc = dnt + (size_t)batch * T;
-  int ntFS = (batch <= 296) ? 512 : 256;           // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
+  int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;           // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
   if (getenv("DFM_FS_THREADS")) ntFS = atoi(getenv("DFM_FS_THREADS"));      // (tuning knob: 256 or 512)
   int ncl = 1;                                     // CTAs per panel (thread-block cluster) of the filter / smoother
-  if (dxch && !getenv("DFM_NO_CLUSTER")) { if (batch * 8 <= 148) ncl = 8; else if (batch * 4 <= 148) ncl = 4; else if (batch * 2 <= 148) ncl = 2; }
+  if (dxch && !getenv("DFM_NO_CLUSTER")) { if (batch * 8 <= h->nsm) ncl = 8; else if (batch * 4 <= h->nsm) ncl = 4; else if (batch * 2 <= h->nsm) ncl = 2; }
   if (getenv("DFM_CLUSTER")) ncl = std::max(1, std::min(8, atoi(getenv("DFM_CLUSTER"))));
   L(k_em_state_init, batch, 1, 1, 0, st);
   L(k_em_scan, N, batch, 64, 0, x, dL, T, N, r, st);
@@ -341,16 +341,15 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
 template <int RT>
 static int launch_fused2(dfm_handle* h, const FusedArgs& fa, int B, int T, int N, Arena* arena, bool dry) {
   size_t smem = fused2_smem_doubles<RT>(T, N) * 8;
-  int grid = std::min(B, 148 * 8);
-  double* scr = arena->get<double>((size_t)std::min(B, 148 * 8) * T * FUSED_SCR(RT));
+  int grid = std::min(B, h->nsm * 8);
+  double* scr = arena->get<double>((size_t)std::min(B, h->nsm * 8) * T * FUSED_SCR(RT));
   if (dry) return DFM_OK;
 #ifndef DFM_EMU
   DFM_SET_SMEM(k_em_fused2<RT>, smem);
-  int dev = 0, nsm = 148, occ = 1;
-  cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  int occ = 1;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_em_fused2<RT>, 256, smem);
   if (occ < 1) occ = 1;
-  grid = std::min(B, nsm * occ);
+  grid = std::min(B, h->nsm * occ);
 #endif
   FusedArgs a2 = fa; a2.scratch = scr;
   CUtensorMap tm; int rc_ = make_panel_tmap(h, fa.X, T, (long long)B * N, &tm); if (rc_) return rc_;
@@ -361,14 +360,13 @@ static int launch_fused2(dfm_handle* h, const FusedArgs& fa, int B, int T, int N
 template <int RT>
 static int launch_als_fused2(dfm_handle* h, const AlsFusedArgs& fa, int B, int T, int N) {
   size_t smem = als_fused2_smem_doubles<RT>(T, N) * 8;
-  int grid = std::min(B, 148 * 8);
+  int grid = std::min(B, h->nsm * 8);
 #ifndef DFM_EMU
   DFM_SET_SMEM(k_als_fused2<RT>, smem);
-  int dev = 0, nsm = 148, occ = 1;
-  cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  int occ = 1;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_als_fused2<RT>, 256, smem);
   if (occ < 1) occ = 1;
-  grid = std::min(B, nsm * occ);
+  grid = std::min(B, h->nsm * occ);
 #endif
   CUtensorMap tm; int rc_ = make_panel_tmap(h, fa.Xs, T, (long long)B * N, &tm); if (rc_) return rc_;
   L(k_als_fused2<RT>, grid, 1, 256, smem, fa, tm);
@@ -377,14 +375,13 @@ static int launch_als_fused2(dfm_handle* h, const AlsFusedArgs& fa, int B, int T
 template <int RT>
 static int launch_als_masked(dfm_handle* h, const AlsMaskedArgs& fa, int B, int T, int N) {
   size_t smem = als_masked_smem_doubles<RT>(T, N) * 8;
-  int grid = std::min(B, 148 * 2);
+  int grid = std::min(B, h->nsm * 2);
 #ifndef DFM_EMU
   DFM_SET_SMEM(k_als_masked<RT>, smem);
-  int dev = 0, nsm = 148, occ = 1;
-  cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  int occ = 1;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_als_masked<RT>, 256, smem);
   if (occ < 1) occ = 1;
-  grid = std::min(B, nsm * occ);
+  grid = std::min(B, h->nsm * occ);
 #endif
   L(k_als_masked<RT>, grid, 1, 256, smem, fa);
   return DFM_OK;
@@ -400,21 +397,20 @@ static bool als_fused2_shape_ok(int T, int N, int r) {
 }
 
 // resident CTAs (= panels processed concurrently) of the TMA fused EM kernel
-template <int RT> static int fused2_capacity_t(int T, int N) {
+template <int RT> static int fused2_capacity_t(int nsm, int T, int N) {
 #ifdef DFM_EMU
-  (void)T; (void)N; return 4;
+  (void)nsm; (void)T; (void)N; return 4;
 #else
   size_t smem = fused2_smem_doubles<RT>(T, N) * 8;
   DFM_SET_SMEM(k_em_fused2<RT>, smem);
-  int dev = 0, nsm = 148, occ = 1;
-  cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  int occ = 1;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_em_fused2<RT>, 256, smem);
   return nsm * (occ < 1 ? 1 : occ);
 #endif
 }
-static int fused2_capacity(int r, int T, int N) {
+static int fused2_capacity(int nsm, int r, int T, int N) {
   switch (r) {
-#define DFM_CASEC(RT) case RT: return fused2_capacity_t<RT>(T, N);
+#define DFM_CASEC(RT) case RT: return fused2_capacity_t<RT>(nsm, T, N);
     DFM_CASEC(1) DFM_CASEC(2) DFM_CASEC(3) DFM_CASEC(4) DFM_CASEC(5) DFM_CASEC(6) DFM_CASEC(7) DFM_CASEC(8)
 #undef DFM_CASEC
   }
@@ -477,10 +473,12 @@ int dfm_create_on_stream(int device, void* cuda_stream, dfm_handle** out) {
   dfm_handle* h = new (std::nothrow) dfm_handle();
   if (!h) return DFM_ERR_CUDA;
   h->device = device; h->ws = nullptr; h->ws_bytes = 0; h->launches = 0; h->err[0] = 0;
+  h->nsm = 132;                // H100 SXM; the CUDA build reads the device's count below (the emulation build has no device)
   h->profile = 0; h->prof = new std::vector<ProfRec>();
   h->stream = nullptr; h->own_stream = false;
   h->copy_stream = nullptr; h->pinned_one = nullptr; h->d2h_stream = nullptr; h->done_host = nullptr; h->done_dev = nullptr; h->done_cap = 0;
 #ifndef DFM_EMU
+  if (cudaDeviceGetAttribute(&h->nsm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || h->nsm <= 0) { handle_teardown(h); return DFM_ERR_CUDA; }
   if (cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { h->copy_stream = nullptr; handle_teardown(h); return DFM_ERR_CUDA; }
   if (cudaStreamCreateWithFlags(&h->d2h_stream, cudaStreamNonBlocking) != cudaSuccess) { h->d2h_stream = nullptr; handle_teardown(h); return DFM_ERR_CUDA; }
   if (cudaHostAlloc((void**)&h->pinned_one, sizeof(int), cudaHostAllocDefault) != cudaSuccess) { h->pinned_one = nullptr; handle_teardown(h); return DFM_ERR_CUDA; }
@@ -614,8 +612,8 @@ static int run_pca(dfm_handle* h, const double* dXs, int T, int N, int r, int ba
     int m = std::min(nmax, pca_block(r));
     const size_t sm2 = subspace2_smem_doubles(nmax, m) * 8;
     if (sm2 <= 110 * 1024 && m <= 48 && !getenv("DFM_OLD_SUBSPACE")) {       // iterate in shared memory, products on the tensor path
-      // (one CTA per SM, to keep the resident panels' Gram matrices inside L2, measured slower than two: 15.1 vs 11.5 ms
-      //  for the C5 shard; DFM_SUB2_ONE=1 pads the shared-memory request for that experiment)
+      // (one CTA per SM, to keep the resident panels' Gram matrices inside L2, was slower than two on the C5 shard;
+      //  DFM_SUB2_ONE=1 pads the shared-memory request for that experiment)
       size_t sm2r = getenv("DFM_SUB2_ONE") ? std::max(sm2, (size_t)116 * 1024) : sm2;
       DFM_SET_SMEM(k_subspace_eig2, sm2r);
       L(k_subspace_eig2, batch, 1, 256, sm2r, G, V, nbal, T, nmax, r, m, 500, 1e-13, (int*)nullptr);
@@ -883,7 +881,7 @@ int dfm_em_init_from_factors(dfm_handle* h, const double* Xs, const double* F, i
   if (smV > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "r*p too large");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int np = r * (r + 1) / 2;
-  EmbPlan embi = emb_plan(T, N, r, batch);
+  EmbPlan embi = emb_plan(T, N, r, batch, h->nsm);
   for (int pass = 0; pass < 2; ++pass) {
     Arena a(pass ? h->ws : nullptr);
     double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
@@ -943,10 +941,10 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
     return fail(h, DFM_ERR_ARG, "dfm_em_kalman: bad shape/options");
   // staging tile of the frozen-run phases of the filter / smoother: few panels -> large tiles (one CTA per SM anyway);
   // many panels -> the largest tile that still lets two CTAs share an SM, if any does
-  int stgT = (batch <= 148) ? 256 : 16;
+  int stgT = (batch <= h->nsm) ? 256 : 16;
   {
     const size_t lim2 = 112 * 1024;
-    if (batch <= 148) { while (stgT > 8 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
+    if (batch <= h->nsm) { while (stgT > 8 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
     else if (em_fs_smem_doubles(r, p, 4) * 8 <= lim2) { while (stgT > 4 && em_fs_smem_doubles(r, p, stgT) * 8 > lim2) stgT /= 2; }
     else { while (stgT > 4 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
   }
@@ -962,7 +960,7 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
   if (o->path == 3 && !fused2_ok) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: TMA fused path needs p = 1, r <= 8, even T and a panel that fits shared memory");
   bool fused = (fused_ok || fused2_ok) && o->path != 1;
   const bool use2 = fused2_ok && (o->path == 0 || o->path == 3);
-  EmbPlan emb = emb_plan(T, N, r, batch);
+  EmbPlan emb = emb_plan(T, N, r, batch, h->nsm);
   for (int pass = 0; pass < 2; ++pass) {
     Arena a(pass ? h->ws : nullptr);
     double* dXb = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
@@ -1007,7 +1005,7 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
     // before the data is on the device.  The copy stream uploads the batch in chunks of panels (X and the initial
     // parameters), each chunk followed by a 4-byte copy that sets its "landed" flag; a CTA spins on the flag of the
     // panel it is about to start (ld.acquire.sys) -- the copy engine is in order, so the flag implies the data.  The
-    // upload (PCIe, ~55 GB/s) runs under the kernel (HBM-bound, slower than the link), P0 and the log-likelihood
+    // upload (PCIe) runs under the kernel (HBM-bound, slower than the link), P0 and the log-likelihood
     // pre-fill are done inside the kernel (no other kernel can become resident next to it), and the balance check
     // is deferred: a panel with NaNs ends with status 3, which triggers the scan + general-path fallback below.
     // (Not under a CUDA injection profiler or CUDA_LAUNCH_BLOCKING=1: launches are synchronous there, so a kernel that waits for copies
@@ -1019,9 +1017,9 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
     const bool profiler = getenv("CUDA_INJECTION64_PATH") || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") || (clb && clb[0] == '1') ||
                           (cdmc && atoi(cdmc) == 1);
     if (mem == DFM_MEM_HOST && fused && use2 && !getenv("DFM_NO_PIPELINE") && !profiler) {
-      const int cap = fused2_capacity(r, T, N);
+      const int cap = fused2_capacity(h->nsm, r, T, N);
       if (batch > cap) {
-        int chunk = 32;                                              // ~25 MB of C2-shaped panels: the first CTAs start after ~0.5 ms
+        int chunk = 32;                                              // ~25 MB of C2-shaped panels: the first CTAs start early
         while ((batch + chunk - 1) / chunk > kMaxReadyChunks) chunk *= 2;
         const int nch = (batch + chunk - 1) / chunk;
         cudaStream_t cs = h->copy_stream;
@@ -1182,8 +1180,8 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
       if (getenv("DFM_FUSED_PHASES")) {            // diagnostics: per-phase clock64 totals printed to stderr
         static long long* dph_dev[64] = {nullptr};                    // one diagnostics buffer per device
         long long*& dph = dph_dev[h->device & 63];
-        if (!dph) cudaMalloc((void**)&dph, 148 * 8 * DFM_PH * sizeof(long long));
-        cudaMemsetAsync(dph, 0, 148 * 8 * DFM_PH * sizeof(long long), h->stream);
+        if (!dph) cudaMalloc((void**)&dph, (size_t)h->nsm * 8 * DFM_PH * sizeof(long long));
+        cudaMemsetAsync(dph, 0, (size_t)h->nsm * 8 * DFM_PH * sizeof(long long), h->stream);
         fa.phase_cycles = dph;
       }
 #endif
@@ -1203,11 +1201,11 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
       if (rc) return rc;
 #ifndef DFM_EMU
       if (fa.phase_cycles) {
-        std::vector<long long> hp(148 * 8 * DFM_PH);
+        std::vector<long long> hp((size_t)h->nsm * 8 * DFM_PH);
         cudaStreamSynchronize(h->stream);
         cudaMemcpy(hp.data(), fa.phase_cycles, hp.size() * sizeof(long long), cudaMemcpyDeviceToHost);
         double tot[DFM_PH] = {0}; int nb = 0;
-        for (int g = 0; g < 148 * 8; ++g) { double s_ = 0; for (int k_ = 0; k_ < 12; ++k_) s_ += hp[(size_t)g * DFM_PH + k_]; if (s_ > 0) { ++nb; for (int k_ = 0; k_ < DFM_PH; ++k_) tot[k_] += hp[(size_t)g * DFM_PH + k_]; } }
+        for (int g = 0; g < h->nsm * 8; ++g) { double s_ = 0; for (int k_ = 0; k_ < 12; ++k_) s_ += hp[(size_t)g * DFM_PH + k_]; if (s_ > 0) { ++nb; for (int k_ = 0; k_ < DFM_PH; ++k_) tot[k_] += hp[(size_t)g * DFM_PH + k_]; } }
         const char* nm[12] = {"loop/params", "P0 prep", "P1 E-contract", "P2 cov chain", "P3 fwd means", "P4 loglik", "P5 bwd means", "P7 sums", "P8 M-contract", "P9 solves", "iter close", "outputs"};
         // tick k measures the phase that ENDS at tick k: tick0 ends loop/param load, tick1 ends P0, ...
         double all = 0; for (int k_ = 0; k_ < 12; ++k_) all += tot[k_];

@@ -1,6 +1,6 @@
 // dfm_common.cuh -- launch/sync abstraction + block-cooperative small dense FP64 helpers.
 //
-// Product build: nvcc -gencode arch=compute_100a,code=sm_100a (real CUDA).
+// Product build: nvcc -gencode arch=compute_90a,code=sm_90a (real CUDA, H100).
 // DFM_EMU build (tests/emu only, never shipped or loaded by the package): the SAME kernel
 // source compiled by g++ with one "thread" per block, so index/algebra logic can be checked in
 // the GPU-less build container.  It is a test harness for the kernel source, not a fallback:
@@ -298,8 +298,7 @@ __device__ inline void bc_chol(double* A, int ld, int n, double* dinv, int* info
 // side and is overwritten by its solution.  One thread per row, no barriers inside: consecutive threads touch consecutive
 // addresses (conflict-free), the entries of L and 1 / L_aa (dinv) are warp-uniform broadcasts.  For n <= 32 the row lives
 // in REGISTERS for the whole substitution (fully unrolled over a compile-time bound with uniform guards): re-reading the
-// freshly stored components from shared memory put a store -> load round trip on every step of the serial chain
-// (measured at n = 32: 16 K cycles per solve, one warp busy).
+// freshly stored components from shared memory put a store -> load round trip on every step of the serial chain.
 #ifndef DFM_EMU
 template <int NMAX, bool TRANS>
 __device__ __noinline__ void bt_trsm_reg(const double* L, int ldl, int n, const double* dinv, double* XT, int ldx, int m) {
@@ -359,7 +358,6 @@ __device__ inline void bt_trsm_lower(const double* L, int ldl, int n, const doub
   DFM_SYNC();
 }
 __device__ inline void bt_trsm_lowerT(const double* L, int ldl, int n, const double* dinv, double* XT, int ldx, int m) {     // L' y = x
-  // (the register variant of the transposed solve measured slower than this loop at n = 32: 21 K vs 16 K cycles)
   for (int j = DFM_TID; j < m; j += DFM_NT)
     for (int a = n - 1; a >= 0; --a) {
       double s0 = XT[j + ldx * a], s1 = 0.0, s2 = 0.0, s3 = 0.0;

@@ -9,8 +9,8 @@
 //   SSR         (:366)      sum_{obs} (x - lam'f)^2 = sum_t (q_t - f_t'b_t),  q_t = sum_{i obs} x_it^2   (A_t f_t = b_t)
 //   stop        (:367-368)  |dSSR| < tol T N
 // With ~6 % missing cells the masked Gram matrices cost one rank-one DOWNDATE per missing cell instead of one update
-// per observed cell.  The panel itself (T x N doubles, C1: 247 KB) is re-read from L2 by every step: a bootstrap batch
-// keeps 296 panels = 73 MB in flight, inside the 126 MB L2.
+// per observed cell.  The panel itself (T x N doubles, C1: 247 KB) is re-read by every step: a bootstrap batch
+// keeps two panels per SM in flight (H100: 264 panels = 65 MB, somewhat more than the 50 MB L2).
 // The r x r systems are solved in registers (packed Cholesky, fully unrolled for the template R).
 #pragma once
 #include "dfm_kernels_fused.cuh"
@@ -111,7 +111,7 @@ __global__ void DFM_ALSM_BOUNDS k_als_masked(AlsMaskedArgs a) {
 #pragma unroll
         for (int q = 0; q < R; ++q) c[q] = 0.0;
         int cnt = 0;
-        // the panel comes from L2 (~700 cycles per load): eight loads in flight per thread, then the arithmetic -- the
+        // the panel comes from L2 (long latency per load): eight loads in flight per thread, then the arithmetic -- the
         // branchy one-load-per-iteration loop waited a full round trip for every cell
         for (int t0 = 0; t0 < T; t0 += 8) {
           double vv[8];

@@ -257,7 +257,7 @@ __device__ __forceinline__ void cl_sync(int) {}
 // on warps 0..7.  A warp advances its 8 chunk recursions together: the step  Z <- Phi Z + U  with Z = [k x 8 chunks] is
 // ceil(k/8) x ceil(k/4) DMMA.8x8x4 with the Phi fragments in registers and Z as the B operand from a [k][12] shared tile
 // (conflict-free); the u_t of later steps are pulled into L1 four steps ahead (prefetch.global.L1).  A step costs one
-// dependent DMMA chain (~ceil(k/4) x 26 cycles) instead of ~100 instructions per chunk, and the chains are 4x shorter
+// dependent DMMA chain (~ceil(k/4) DMMA latencies) instead of ~100 instructions per chunk, and the chains are 4x shorter
 // (64 chunks).  ws: >= 256 k doubles of shared workspace.
 #define EM_SC_NW 8
 #define EM_SC_ZS 12

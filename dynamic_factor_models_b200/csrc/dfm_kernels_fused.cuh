@@ -4,7 +4,7 @@
 //
 //  * panel reads: exactly two streaming passes per EM iteration (E-step contraction
 //    b_t = Lam' R^-1 x_t and M-step contraction S_xf = X' E[f]), straight from HBM into FP64
-//    tensor-core fragments: mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4) -- tcgen05 has no FP64 kind and
+//    tensor-core fragments: mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4) -- wgmma has no FP64 kind and
 //    the 1e-5 parity bar needs FP64 (DESIGN.md);
 //  * Lam, 1/R and the T x r state buffer Z (b_t -> f_t|t -> f_t|T in place) live in shared memory;
 //  * the covariance recursion of a balanced panel is data independent and time invariant: warp 0
@@ -70,7 +70,7 @@ __device__ __forceinline__ double w_max(double v) {
 // ---- warp-0 small dense ops on row-major R x R matrices in shared memory ------------------------
 // NOT inlined on the GPU: the chain calls them ~100 times per EM iteration; inlined + unrolled they
 // made one chain step ~40 KB of straight-line code executed by a single warp, i.e. instruction-cache
-// misses all the way (measured: 48K cycles per step in the kernel vs 15K in isolation).
+// misses all the way.
 #ifdef DFM_EMU
 #define DFM_HELPER inline
 #else
@@ -130,7 +130,7 @@ DFM_HELPER double w_inv(double* Ai, const double* A, double* tmp, int* bad) {
   if (R == 8) {
     // register version: lane owns elements (i, j0) and (i, j0+1), i = lane/4, j0 = 2 (lane%4); per
     // pivot four double shuffles (pivot, its row for my columns, its column for my row) -- no shared
-    // memory round trips, ~8x faster than the generic version below (tools/bench_chain.cu)
+    // memory round trips, faster than the generic version below (tools/bench_chain.cu)
     const int lane = threadIdx.x & 31, i = lane >> 2, q = lane & 3, j0 = 2 * q;
     double x0 = A[i * 8 + j0], x1 = A[i * 8 + j0 + 1];
     double pp = 1.0;

@@ -5,8 +5,7 @@
 //    r x r sized, overlapped with the passes and with the mean recursions);
 //  * both passes stream the column-major panel through ONE 2-D tensor-map copy per stage (cp.async.bulk.tensor.2d,
 //    SASS UTMALDG; box = F2_TC periods x 8 series) into an F2_S-stage shared-memory ring guarded by full/empty
-//    mbarriers.  Measured at this occupancy (tools/bench_stream.cu, tools/bench_tma2d.cu): LDG-to-fragment patterns
-//    2.5-3.5 TB/s, TMA ring 6.3-6.8 TB/s;
+//    mbarriers (tools/bench_stream.cu and tools/bench_tma2d.cu compare the load schemes at this occupancy);
 //  * E pass: each consumer warp keeps the 8x8 accumulators of its row blocks in registers across all series blocks;
 //    M pass: S_xf partial tiles per consumer warp + deterministic cross-warp reduction per series block;
 //  * the ring is idle between the passes and doubles as storage for the explicit covariance steps and the level
@@ -27,8 +26,8 @@ struct CUtensorMap { char opaque[128]; };
 namespace dfm {
 
 #ifndef F2_SBS
-#define F2_SBS 1        // 8-series blocks per stage (= per tensor-map copy): a copy costs ~400 cycles + bytes / 27 per CTA whatever
-#endif                  // its size (tools/bench_tma2d.cu), so wider stages raise the rate a single CTA can stream at
+#define F2_SBS 1        // 8-series blocks per stage (= per tensor-map copy): a copy has a fixed cost whatever its size
+#endif                  // (tools/bench_tma2d.cu), so wider stages raise the rate a single CTA can stream at
 #ifndef F2_S
 #define F2_S (4 / F2_SBS)   // ring stages (the ring keeps its size: F2_S * F2_SBS * 8 * F2_TS doubles)
 #endif
@@ -77,7 +76,7 @@ struct F2Ring {
 // [T, B*N] view of the batch (column runs of 800 B; the box is 4 periods wider than the chunk so that the
 // dense row pitch in shared memory is == 4 mod 16, i.e. conflict-free; rows/periods beyond the tensor are
 // zero-filled, rows of the next panel are masked by the consumers).  Eight 1-D bulk copies per stage were
-// issue-bound (~115 cycles per request, serialised over the lanes of a warp: tools/bench_stream.cu).
+// issue-bound (requests serialised over the lanes of a warp: tools/bench_stream.cu).
 __device__ __forceinline__ void f2_produce(F2Ring& rg, const CUtensorMap* tmap, int row0, int T, int N, bool c_outer) {
   const int lane = threadIdx.x & 31;
   const int nsb = (N + 8 * F2_SBS - 1) / (8 * F2_SBS), nck = (T + F2_TC - 1) / F2_TC;      // (stages per pass: series-block groups x chunks)

@@ -101,7 +101,7 @@ __global__ void k_gram(const double* __restrict__ Xs, int T, int N, const int* _
 // B fragments per four DMMA.8x8x4), fragments straight from global memory -- a panel (<= 1 MB) is L2 resident and every
 // 32-byte sector a fragment load touches is used completely; the reduction runs over T (mode 0) or over the balanced
 // columns (mode 1).  grid (ceil(nblocks / 8), B), 256 threads, nblocks = nb16 (nb16 + 1) / 2 with nb16 = ceil(nmax / 16).
-// The scalar k_gram (one thread per entry, 2 T loads per entry) took 24.8 ms for the 1250-panel C5 shard.
+// (The scalar k_gram, one thread per entry and 2 T loads per entry, is kept behind DFM_OLD_GRAM.)
 __global__ void k_gram_tc(const double* __restrict__ Xs, int T, int N, const int* __restrict__ bal_idx,
                           const int* __restrict__ nbal, double* __restrict__ G, int nmax) {
 #ifndef DFM_EMU
@@ -393,7 +393,7 @@ __global__ void k_subspace_eig(double* __restrict__ Gall, double* __restrict__ V
 
 // Y (n x m, ld ldv, shared) = G (n x n, ld n, global: L2 resident) * V (n x m, ld ldv, shared) on the tensor path.  One warp per
 // 8-row block of Y: its A fragments (rows of G) are read straight from L2, EIGHT k-steps ahead of the DMMAs (a fragment
-// load from L2 takes ~500 cycles: two in flight, as in the generic tile product, leave the loop latency bound), and each
+// load from L2 has a long latency: two in flight, as in the generic tile product, leave the loop latency bound), and each
 // fragment feeds all ceil(m / 8) <= 6 column tiles, whose B fragments come conflict-free from the shared iterate.
 __device__ __forceinline__ void gv_product(const double* __restrict__ G, int n, const double* V, double* Y, int ldv, int m);
 // general form: Y (rows x m, ld ldy) = A (rows x K, element (i, l) at A[i + lda * l], global) * V (K x m, ld ldv, shared)

@@ -9,8 +9,8 @@ fails loudly when its CUDA library is missing.
 Modules
 -------
 xlsx_min   stdlib-only .xlsx reader (stands in for ExcelReaders.readxlsheet)
-readin     restatement of /root/reference/readin_functions.jl  (panel ingestion)
-dfm_ref    restatement of /root/reference/dfm_functions.ipynb  (PCA / ALS "EM" /
+readin     restatement of the reference's readin_functions.jl  (panel ingestion)
+dfm_ref    restatement of the reference's dfm_functions.ipynb  (PCA / ALS "EM" /
            loadings / factor VAR / IRF / constraints / Bai-Ng / Amengual-Watson)
            -- PINNED against the golden tables stored in Stock_Watson.ipynb
 kalman_em  FP64 Kalman filter + RTS smoother + EM for the state-space DFM.

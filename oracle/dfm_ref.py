@@ -1,4 +1,4 @@
-"""Restatement of /root/reference/dfm_functions.ipynb (non-parametric DFM path).  ORACLE ONLY.
+"""Restatement of the reference's dfm_functions.ipynb (non-parametric DFM path).  ORACLE ONLY.
 
 FP64 numpy/scipy; missing = NaN; arrays are (T, N) with the same orientation as the
 Julia code.  Citations are raw JSON line numbers of dfm_functions.ipynb.  The

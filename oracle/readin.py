@@ -1,9 +1,9 @@
-"""Restatement of /root/reference/readin_functions.jl (panel ingestion).  ORACLE ONLY.
+"""Restatement of the reference's readin_functions.jl (panel ingestion).  ORACLE ONLY.
 
 Missing values are NaN.  Every function cites the reference lines it follows.
-Runs only where /root/reference exists (this container); its OUTPUT for the two
-notebook configurations is committed under tests/golden/ by
-tests/golden/make_golden.py so that nothing on the GPU box needs the xlsx.
+Needs the reference's data/hom_fac_1.xlsx; its OUTPUT for the two notebook
+configurations is committed under tests/golden/ by tests/golden/make_golden.py so
+that the tests do not need the workbook.
 """
 import numpy as np
 from .xlsx_min import read_sheet, excel_serial_to_ymd

@@ -1,5 +1,5 @@
-"""CPU only: the committed bench lines (profiles/r02_c_bench_*.json, written by bench.py on a B200) carry every key of the
-driver's contract -- a guard against silently dropping one when bench.py is edited."""
+"""CPU only: the committed bench lines (profiles/h100_bench_*.json, written by bench.py on an H100) carry every key a
+consumer of the bench line reads -- a guard against silently dropping one when bench.py is edited."""
 import json
 import os
 
@@ -17,9 +17,9 @@ def _load(name):
     return json.load(open(p))
 
 
-@pytest.mark.parametrize("name", ["r02_c_bench_c5.json", "r02_c_bench_c4.json", "r02_c_bench_c3.json", "r02_c_bench_c2-single.json"])
-def test_bench_line_has_contract_keys(name):
-    d = _load(name)
+@pytest.mark.parametrize("config", ["c5", "c4", "c3", "c2-single"])
+def test_bench_line_has_contract_keys(config):
+    d = _load(f"h100_bench_{config}.json")
     for k in BASE:
         assert k in d, k
     assert "workload" in d["config"] and d["dtype"] == "f64" and d["higher_is_better"] is True
@@ -33,7 +33,7 @@ def test_bench_line_has_contract_keys(name):
 
 
 def test_headline_line():
-    d = _load("r02_c_bench_c5.json")
+    d = _load("h100_bench_c5.json")
     assert d["metric"].startswith("EM iters/sec") and d["scaling"] == "weak" and d["n_gpus"] == 1
     cb = d["cpu_baseline"]
     assert cb and set(("value", "unit", "cores", "kind", "sample")) <= set(cb) and cb["kind"] in ("port", "reference")
@@ -42,6 +42,6 @@ def test_headline_line():
 
 
 def test_reference_arm_line():
-    d = _load("r02_c_bench_ref.json")
+    d = _load("h100_bench_ref.json")
     assert d["impl"] == "reference" and d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
     assert d["cpu_baseline"]["value"] == d["value"]

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path through the C ABI vs the
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI vs the
 oracle, on the reference's own panel (hom_fac_1, committed fixture), seeded synthetic panels,
 edge cases, and size-independent properties at BASELINE.json's full sizes."""
 import numpy as np

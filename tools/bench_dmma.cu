@@ -1,8 +1,9 @@
-// bench_dmma.cu -- FP64 tensor-core MMA issue rate on sm_100a by shape (m8n8k4 / m16n8k4 / m16n8k8 / m16n8k16)
+// bench_dmma.cu -- FP64 tensor-core MMA issue rate on sm_90a by shape (m8n8k4 / m16n8k4 / m16n8k8 / m16n8k16)
 // and plain DFMA, with 1..4 warps per SM sub-partition, independent accumulators.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/bench_dmma.bin tools/bench_dmma.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/bench_dmma.bin tools/bench_dmma.cu
 #include <cuda_runtime.h>
 #include <cstdio>
+#include <vector>
 #include <cstdlib>
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); exit(1); } } while (0)
 
@@ -47,17 +48,19 @@ __global__ void k(int iters, double* out, long long* cyc) {
 
 template <int SHAPE, int NACC>
 void run(const char* name, double fma_per_op, int warps) {
-  double* out; long long* cyc; CK(cudaMalloc(&out, 8)); CK(cudaMalloc(&cyc, 148 * 8));
+  int nsm = 0; CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0));
+  double* out; long long* cyc; CK(cudaMalloc(&out, 8)); CK(cudaMalloc(&cyc, nsm * 8));
   const int iters = 2000;
-  k<SHAPE, NACC><<<148, warps * 32>>>(iters, out, cyc); CK(cudaDeviceSynchronize());
-  k<SHAPE, NACC><<<148, warps * 32>>>(iters, out, cyc); CK(cudaDeviceSynchronize());
-  long long h[148]; CK(cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost));
-  double c = 0; for (int i = 0; i < 148; ++i) c += h[i]; c /= 148;
+  k<SHAPE, NACC><<<nsm, warps * 32>>>(iters, out, cyc); CK(cudaDeviceSynchronize());
+  k<SHAPE, NACC><<<nsm, warps * 32>>>(iters, out, cyc); CK(cudaDeviceSynchronize());
+  std::vector<long long> h(nsm); CK(cudaMemcpy(h.data(), cyc, nsm * 8, cudaMemcpyDeviceToHost));
+  double c = 0; for (int i = 0; i < nsm; ++i) c += h[i]; c /= nsm;
   double ops_per_warp = (double)iters * NACC;
   double per_smsp = c / (ops_per_warp * warps / 4.0);          // cycles per op per sub-partition (warps spread over 4 SMSPs)
   double fma_clk_sm = ops_per_warp * warps * fma_per_op / c;
-  printf("%-22s acc=%d warps/SM=%2d : %7.1f cyc/op/warp  %6.1f cyc/op/SMSP  %6.1f FMA/clk/SM  (%.1f TFLOP/s at 1.9 GHz x 148)\n", name, NACC, warps,
-         c / ops_per_warp, per_smsp, fma_clk_sm, fma_clk_sm * 2 * 148 * 1.9e9 / 1e12);
+  int khz = 0; CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0));
+  printf("%-22s acc=%d warps/SM=%2d : %7.1f cyc/op/warp  %6.1f cyc/op/SMSP  %6.1f FMA/clk/SM  (%.1f TFLOP/s at %.2f GHz x %d SMs)\n", name, NACC,
+         warps, c / ops_per_warp, per_smsp, fma_clk_sm, fma_clk_sm * 2 * nsm * khz * 1e3 / 1e12, khz * 1e-6, nsm);
   cudaFree(out); cudaFree(cyc);
 }
 

@@ -2,7 +2,7 @@
 // one 2-D tensor-map TMA per stage (box = bc periods x br series), mbarrier full/empty ring, consumer
 // warps doing a few FP64 DMMAs per stage.  Sweeps box shape, ring depth, producer count, consumer
 // work and CTAs per SM to find what bounds the pass (issue rate, latency x bytes in flight, DRAM).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/bench_tma2d.bin tools/bench_tma2d.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/bench_tma2d.bin tools/bench_tma2d.cu
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -123,7 +123,8 @@ typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, voi
                               const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 int main(int argc, char** argv) {
-  const int B = 1184, T = 500, N = 200;   // 1184 = 8*148: no tail at any of the grids used
+  int nsm = 0; CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0));
+  const int B = 8 * nsm, T = 500, N = 200;   // no tail at any of the grids used
   double* X; double* out;
   size_t n = (size_t)B * N * T;
   CK(cudaMalloc(&X, n * 8)); CK(cudaMalloc(&out, 4096 * 8));
@@ -135,12 +136,12 @@ int main(int argc, char** argv) {
   cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
 
   {  // ---- overlap test
-    long long* lo; CK(cudaMalloc(&lo, 148 * 4 * 8));
-    std::vector<long long> h(148 * 4);
+    long long* lo; CK(cudaMalloc(&lo, nsm * 4 * 8));
+    std::vector<long long> h(nsm * 4);
     CK(cudaFuncSetAttribute(k_lat, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     printf("overlap test: cycles for K copies issued back to back by one thread (avg / min / issue-only), grid CTAs of 32 threads\n");
     struct LC { int bc, br, grid, bulk; };
-    for (LC lc : {LC{100, 8, 1, 0}, LC{100, 8, 148, 0}, LC{16, 50, 1, 0}, LC{16, 50, 148, 0}, LC{100, 8, 1, 1}, LC{100, 8, 148, 1}, LC{250, 8, 148, 0}}) {
+    for (LC lc : {LC{100, 8, 1, 0}, LC{100, 8, nsm, 0}, LC{16, 50, 1, 0}, LC{16, 50, nsm, 0}, LC{100, 8, 1, 1}, LC{100, 8, nsm, 1}, LC{250, 8, nsm, 0}}) {
       CUtensorMap tm;
       cuuint64_t dims[2] = {(cuuint64_t)T, (cuuint64_t)B * N}; cuuint64_t strides[1] = {(cuuint64_t)T * 8};
       cuuint32_t box[2] = {(cuuint32_t)lc.bc, (cuuint32_t)lc.br}, es[2] = {1, 1};
@@ -159,7 +160,7 @@ int main(int argc, char** argv) {
   }
   struct Cfg { int bc, br, S, nprod, ncons, work, grid; };
   std::vector<Cfg> cfgs;
-  for (int grid : {148, 296}) {
+  for (int grid : {nsm, 2 * nsm}) {
     cfgs.push_back({100, 8, 6, 1, 6, 4, grid});     // the shipped configuration
     cfgs.push_back({100, 8, 6, 1, 6, 0, grid});     // no consumer math
     cfgs.push_back({100, 8, 6, 2, 6, 4, grid});     // two producer warps
@@ -175,9 +176,9 @@ int main(int argc, char** argv) {
     cfgs.push_back({250, 8, 4, 1, 6, 8, grid});
     cfgs.push_back({252, 8, 5, 1, 6, 8, grid});
   }
-  cfgs.push_back({100, 8, 6, 1, 6, 4, 74});         // half the SMs, one CTA each: is the cap per CTA or chip-wide?
-  cfgs.push_back({100, 8, 12, 1, 6, 4, 74});
-  cfgs.push_back({100, 16, 6, 1, 6, 8, 74});
+  cfgs.push_back({100, 8, 6, 1, 6, 4, nsm / 2});    // half the SMs, one CTA each: is the cap per CTA or chip-wide?
+  cfgs.push_back({100, 8, 12, 1, 6, 4, nsm / 2});
+  cfgs.push_back({100, 16, 6, 1, 6, 8, nsm / 2});
   printf("%-5s %-4s %-3s %-5s %-5s %-5s %-5s %10s %10s %12s\n", "bc", "br", "S", "nprod", "ncons", "work", "grid", "ms", "GB/s", "cyc/stage");
   for (auto& c : cfgs) {
     CUtensorMap tm;
@@ -188,8 +189,8 @@ int main(int argc, char** argv) {
     if (rc != CUDA_SUCCESS) { printf("encode failed %d for bc=%d br=%d\n", (int)rc, c.bc, c.br); continue; }
     P p{B, T, N, c.bc, c.br, c.S, c.nprod, c.ncons, c.work};
     size_t smem = (size_t)c.S * c.bc * c.br * 8 + 2 * c.S * 8 + 256;
-    // force the intended residency: pad shared memory so that exactly one (grid <= 148) or two CTAs fit per SM
-    size_t pad = (c.grid > 148) ? 100 * 1024 : 120 * 1024;
+    // force the intended residency: pad shared memory so that exactly one (grid <= SM count) or two CTAs fit per SM
+    size_t pad = (c.grid > nsm) ? 100 * 1024 : 120 * 1024;
     if (smem < pad) smem = pad;
     for (int w = 0; w < 2; ++w) k_ring<<<c.grid, 256, smem>>>(tm, p, out);
     CK(cudaDeviceSynchronize());

@@ -1,13 +1,13 @@
 #!/usr/bin/env python
-"""SASS evidence for profiles/: per-kernel counts of the mnemonics that prove the Blackwell-native paths (FP64 tensor MMA,
+"""SASS evidence: per-kernel counts of the mnemonics that show the Hopper-native paths (FP64 tensor MMA,
 TMA tensor copies, mbarriers) and the E- / M-pass consumer loops of k_em_fused2<8>.  usage: sass_evidence.py lib.so > out.txt"""
 import re, subprocess, sys
 lib = sys.argv[1]
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
 funcs = re.split(r"\n\s*Function : ", sass)[1:]
 keys = ["DMMA", "UTMALDG", "SYNCS", "UBLKCP", "LDS", "STS", "LDG", "STG", "SHFL", "BAR", "ATOM", "MUFU", "DFMA", "DMUL", "DADD", "LDL", "STL", "HMMA", "UTC"]
-print("# SASS mnemonic counts per kernel (cuobjdump -sass of the in-tree libdfm_b200.so, sm_100a)")
-print("# FP64 tensor MMA = DMMA (mma.sync.m8n8k4.f64; tcgen05 has no f64 kind); TMA 2-D tensor copies = UTMALDG; mbarrier ops = SYNCS")
+print("# SASS mnemonic counts per kernel (cuobjdump -sass of the in-tree libdfm_b200.so, sm_90a)")
+print("# FP64 tensor MMA = DMMA (mma.sync.m8n8k4.f64; wgmma has no f64 kind); TMA 2-D tensor copies = UTMALDG; mbarrier ops = SYNCS")
 print(f"{'kernel':70s} " + " ".join(f"{k:>7s}" for k in keys) + "   instr")
 em8 = None
 for f in funcs:

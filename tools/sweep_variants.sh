@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B of kernel variants built by tools/build_variant.sh: default bench line (device + e2e) per variant
-cd /root/repo
+cd "$(dirname "$0")/.."
 for lib in build/variants/libdfm_*.so; do
   n=$(basename $lib .so)
   DFM_BENCH_LIB=$lib timeout 200 python bench.py --no-cpu --steps 5 --warmup 3 2>/dev/null | python -c "
