@@ -62,7 +62,7 @@ def default_library_path():
 
 EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stream", "dfm_destroy", "dfm_sync",
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
-           "dfm_profile_kernel_name", "dfm_debug_fs_prof", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
+           "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
@@ -115,7 +115,6 @@ class Library:
         L.dfm_profile_reset.argtypes = [C.c_void_p]
         L.dfm_profile_kernel_name.argtypes = [C.c_void_p, C.c_int]
         L.dfm_profile_kernel_name.restype = C.c_char_p
-        L.dfm_debug_fs_prof.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_double)]
         L.dfm_create.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
         L.dfm_create_on_stream.argtypes = [C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
         L.dfm_destroy.argtypes = [C.c_void_p]
@@ -171,12 +170,6 @@ class Library:
     def profile(self, on=True):
         self.lib.dfm_profile_reset(self.h)
         self.lib.dfm_profile_enable(self.h, int(on))
-
-    def fs_prof(self, on=1):
-        """Arm (on=1) / read the section timers of k_em_filter_smooth; returns the 64 totals accumulated so far."""
-        out = (C.c_double * 64)()
-        self.check(self.lib.dfm_debug_fs_prof(self.h, int(on), out), "dfm_debug_fs_prof")
-        return list(out)
 
     def profile_report(self):
         """{kernel name: (total ms, launches)} since profile(True)."""

@@ -175,13 +175,8 @@ static int make_panel_tmap(dfm_handle* h, const double* X, int T, long long rows
   cuuint64_t dims[2] = {(cuuint64_t)T, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)T * 8};
   cuuint32_t box[2] = {F2_TS, 8 * F2_SBS}, es[2] = {1, 1};
-  CUtensorMapL2promotion l2p = CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
-  if (const char* e_ = getenv("DFM_TMAP_L2")) {           // A/B knob: 0 none, 1 64 B, 2 128 B, 3 256 B (default)
-    const int v_ = atoi(e_);
-    l2p = v_ == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : v_ == 1 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : v_ == 2 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
-  }
   CUresult rc = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, (void*)X, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_NONE, l2p, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (rc != CUDA_SUCCESS) { snprintf(h->err, sizeof(h->err), "cuTensorMapEncodeTiled failed (%d)", (int)rc); return DFM_ERR_CUDA; }
   return DFM_OK;
 #endif
@@ -216,7 +211,7 @@ struct EmbPlan {
 };
 static EmbPlan emb_plan(int T, int N, int r, int batch, int nsm) {
   EmbPlan e{};
-  e.on = r <= 32 && !getenv("DFM_NO_EMB");
+  e.on = r <= 32;
   if (!e.on) return e;
   e.ncb = (r + 7) / 8;
   const int target = 2 * nsm;
@@ -260,10 +255,9 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
   int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mi = o->max_iter;
   int np = r * (r + 1) / 2;
   int* dsrc = dnt + (size_t)batch * T;
-  int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;           // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
-  if (getenv("DFM_FS_THREADS")) ntFS = atoi(getenv("DFM_FS_THREADS"));      // (tuning knob: 256 or 512)
+  const int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;     // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
   int ncl = 1;                                     // CTAs per panel (thread-block cluster) of the filter / smoother
-  if (dxch && !getenv("DFM_NO_CLUSTER")) { if (batch * 8 <= h->nsm) ncl = 8; else if (batch * 4 <= h->nsm) ncl = 4; else if (batch * 2 <= h->nsm) ncl = 2; }
+  if (dxch) { if (batch * 8 <= h->nsm) ncl = 8; else if (batch * 4 <= h->nsm) ncl = 4; else if (batch * 2 <= h->nsm) ncl = 2; }
   if (getenv("DFM_CLUSTER")) ncl = std::max(1, std::min(8, atoi(getenv("DFM_CLUSTER"))));
   L(k_em_state_init, batch, 1, 1, 0, st);
   L(k_em_scan, N, batch, 64, 0, x, dL, T, N, r, st);
@@ -506,27 +500,6 @@ long long dfm_launch_count(const dfm_handle* h) { return h ? h->launches : -1; }
 const char* dfm_last_error(const dfm_handle* h) { return h ? h->err : "null handle"; }
 
 // ---- per-kernel CUDA-event profiling (bench.py's roofline leg; off by default) -----------------
-// diagnostics: per-section clock64 totals of k_em_filter_smooth (block 0); on = 1 arms and clears, out (16 doubles) reads
-int dfm_debug_fs_prof(dfm_handle* h, int on, double* out) {
-#ifndef DFM_EMU
-  if (!h) return DFM_ERR_ARG;
-  CK(cudaStreamSynchronize(h->stream));
-  long long v[48], w[16];
-  if (out) {
-    CK(cudaMemcpyFromSymbol(v, dfm::g_fs_prof, sizeof(v))); for (int i = 0; i < 48; ++i) out[i] = (double)v[i];
-    CK(cudaMemcpyFromSymbol(w, dfm::g_sub_prof, sizeof(w))); for (int i = 0; i < 16; ++i) out[48 + i] = (double)w[i];
-  }
-  memset(v, 0, sizeof(v)); memset(w, 0, sizeof(w));
-  CK(cudaMemcpyToSymbol(dfm::g_fs_prof, v, sizeof(v)));
-  CK(cudaMemcpyToSymbol(dfm::g_fs_prof_on, &on, sizeof(int)));
-  CK(cudaMemcpyToSymbol(dfm::g_sub_prof, w, sizeof(w)));
-  CK(cudaMemcpyToSymbol(dfm::g_sub_prof_on, &on, sizeof(int)));
-#else
-  (void)h; (void)on; (void)out;
-#endif
-  return DFM_OK;
-}
-
 int dfm_profile_enable(dfm_handle* h, int on) {
   if (!h) return DFM_ERR_ARG;
   h->profile = on ? 1 : 0;
@@ -600,28 +573,21 @@ static int run_pca(dfm_handle* h, const double* dXs, int T, int N, int r, int ba
   int nmax = std::min(N, T);
   if (col_n) L(k_balanced_cols, batch, 1, 1, 0, col_n, T, N, bal_idx, nbal);
   else L(k_all_cols, batch, 1, 128, 0, N, bal_idx, nbal);
-  if (getenv("DFM_OLD_GRAM")) {
-    int gx = (int)std::min<long long>(((long long)nmax * nmax + 255) / 256, 4096);
-    L(k_gram, gx, batch, 256, 0, dXs, T, N, bal_idx, nbal, G, nmax);
-  } else {
-    const int nb16 = (nmax + 15) / 16, nblocks = nb16 * (nb16 + 1) / 2;
-    L(k_gram_tc, (nblocks + 7) / 8, batch, 256, 0, dXs, T, N, bal_idx, nbal, G, nmax);
-  }
+  const int nb16 = (nmax + 15) / 16, nblocks = nb16 * (nb16 + 1) / 2;
+  L(k_gram_tc, (nblocks + 7) / 8, batch, 256, 0, dXs, T, N, bal_idx, nbal, G, nmax);
   if (nmax <= 64) L(k_jacobi, batch, 1, 256, (size_t)(2 * nmax * nmax + 2 * (nmax + 3) + 48) * 8, G, V, nbal, T, nmax, 60, (int*)nullptr);
   else {
     int m = std::min(nmax, pca_block(r));
     const size_t sm2 = subspace2_smem_doubles(nmax, m) * 8;
-    if (sm2 <= 110 * 1024 && m <= 48 && !getenv("DFM_OLD_SUBSPACE")) {       // iterate in shared memory, products on the tensor path
-      // (one CTA per SM, to keep the resident panels' Gram matrices inside L2, was slower than two on the C5 shard;
-      //  DFM_SUB2_ONE=1 pads the shared-memory request for that experiment)
-      size_t sm2r = getenv("DFM_SUB2_ONE") ? std::max(sm2, (size_t)116 * 1024) : sm2;
-      DFM_SET_SMEM(k_subspace_eig2, sm2r);
-      L(k_subspace_eig2, batch, 1, 256, sm2r, G, V, nbal, T, nmax, r, m, 500, 1e-13, (int*)nullptr);
+    if (sm2 <= 110 * 1024 && m <= 48) {       // iterate in shared memory, products on the tensor path
+      // (one CTA per SM, to keep the resident panels' Gram matrices inside L2, was slower than two on the C5 shard)
+      DFM_SET_SMEM(k_subspace_eig2, sm2);
+      L(k_subspace_eig2, batch, 1, 256, sm2, G, V, nbal, T, nmax, r, m, 500, 1e-13, (int*)nullptr);
     } else L(k_subspace_eig, batch, 1, 256, (size_t)(3 * m * m + 3 * m + 72) * 8, G, V, Ysub, nbal, T, nmax, r, m, 500, 1e-13, (int*)nullptr);
   }
   {
     const size_t smF = (size_t)(r / 2 + 2 + 48 + N) * 8, smFast = (size_t)(r / 2 + 2 + 48) * 8 + (size_t)em_lds(nmax) * r * 8 + 64;
-    if (N <= T && r <= 48 && smFast <= 100 * 1024 && !getenv("DFM_OLD_PCAFIN"))
+    if (N <= T && r <= 48 && smFast <= 100 * 1024)
       L(k_pca_finish, batch, 1, 256, std::max(smF, smFast), dXs, T, N, bal_idx, nbal, G, V, nmax, r, dF, status, st, 1);
     else L(k_pca_finish, batch, 1, 128, smF, dXs, T, N, bal_idx, nbal, G, V, nmax, r, dF, status, st, 0);
   }
@@ -691,7 +657,7 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
     long long it = 0;
     int h_active = batch;
     // balanced panels without constraints: all sweeps in ONE fused launch (TMA ring + DMMA passes)
-    if (nc == 0 && als_fused2_shape_ok(T, N, r) && o->nt_min <= T && !getenv("DFM_ALS_GENERAL")) {
+    if (nc == 0 && als_fused2_shape_ok(T, N, r) && o->nt_min <= T) {
       std::vector<AlsState> hs(B);
       CK(cudaMemcpyAsync(hs.data(), st, B * sizeof(AlsState), cudaMemcpyDeviceToHost, h->stream));
       CK(cudaStreamSynchronize(h->stream));
@@ -710,7 +676,7 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
     }
     // panels with missing data, no constraints: all sweeps in ONE launch as well (thread-per-series / thread-per-period
     // masked normal equations, no host synchronisation in the sweep loop)
-    if (h_active > 0 && nc == 0 && als_masked_shape_ok(T, N, r) && !getenv("DFM_ALS_GENERAL")) {
+    if (h_active > 0 && nc == 0 && als_masked_shape_ok(T, N, r)) {
       AlsMaskedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.nt_min = o->nt_min;
       fa.tol = o->tol; fa.max_iter = o->max_iter;
       switch (r) {
@@ -1037,7 +1003,7 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
         CKE(cudaStreamWaitEvent(h->stream, ev0, 0));                   // flags are zero before the kernel can read them
         FusedArgs fa{};
         fa.X = dXb; fa.Lam = dL; fa.R = dR; fa.A = dA; fa.Q = dQ; fa.P0 = dP0; fa.Fs = dFs; fa.PsF = dPsF; fa.loglik = dll;
-        fa.iters = dit; fa.status = dstat; fa.B = batch; fa.T = T; fa.N = N; fa.max_iter = mi; fa.tol = o->tol; fa.phase_cycles = nullptr;
+        fa.iters = dit; fa.status = dstat; fa.B = batch; fa.T = T; fa.N = N; fa.max_iter = mi; fa.tol = o->tol;
         fa.ready = dready; fa.ready_chunk = chunk;
         if (h->done_cap < B) {                                        // completion flags the kernel writes straight into host memory
           if (h->done_host) cudaFreeHost(h->done_host);
@@ -1174,17 +1140,6 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
       FusedArgs fa{};
       fa.X = x; fa.Lam = dL; fa.R = dR; fa.A = dA; fa.Q = dQ; fa.P0 = dP0; fa.Fs = dFs; fa.PsF = dPsF; fa.loglik = dll;
       fa.iters = dit; fa.status = dstat; fa.B = batch; fa.T = T; fa.N = N; fa.max_iter = mi; fa.tol = o->tol;
-      fa.phase_cycles = nullptr;
-#ifndef DFM_EMU
-      if (const char* sg = getenv("DFM_FUSED_STAGGER")) fa.stagger = atoi(sg);
-      if (getenv("DFM_FUSED_PHASES")) {            // diagnostics: per-phase clock64 totals printed to stderr
-        static long long* dph_dev[64] = {nullptr};                    // one diagnostics buffer per device
-        long long*& dph = dph_dev[h->device & 63];
-        if (!dph) cudaMalloc((void**)&dph, (size_t)h->nsm * 8 * DFM_PH * sizeof(long long));
-        cudaMemsetAsync(dph, 0, (size_t)h->nsm * 8 * DFM_PH * sizeof(long long), h->stream);
-        fa.phase_cycles = dph;
-      }
-#endif
       Arena a2(h->ws); a2.off = fused_off;             // scratch pointer (first allocation after dflag in this pass)
       if (use2) {
         switch (r) {
@@ -1199,26 +1154,6 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
 #undef DFM_CASE
       }
       if (rc) return rc;
-#ifndef DFM_EMU
-      if (fa.phase_cycles) {
-        std::vector<long long> hp((size_t)h->nsm * 8 * DFM_PH);
-        cudaStreamSynchronize(h->stream);
-        cudaMemcpy(hp.data(), fa.phase_cycles, hp.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-        double tot[DFM_PH] = {0}; int nb = 0;
-        for (int g = 0; g < h->nsm * 8; ++g) { double s_ = 0; for (int k_ = 0; k_ < 12; ++k_) s_ += hp[(size_t)g * DFM_PH + k_]; if (s_ > 0) { ++nb; for (int k_ = 0; k_ < DFM_PH; ++k_) tot[k_] += hp[(size_t)g * DFM_PH + k_]; } }
-        const char* nm[12] = {"loop/params", "P0 prep", "P1 E-contract", "P2 cov chain", "P3 fwd means", "P4 loglik", "P5 bwd means", "P7 sums", "P8 M-contract", "P9 solves", "iter close", "outputs"};
-        // tick k measures the phase that ENDS at tick k: tick0 ends loop/param load, tick1 ends P0, ...
-        double all = 0; for (int k_ = 0; k_ < 12; ++k_) all += tot[k_];
-        fprintf(stderr, "[dfm fused chain] forward loop %.0f cyc/CTA, backward loop %.0f cyc/CTA\n", tot[12] / (nb ? nb : 1), tot[13] / (nb ? nb : 1));
-        fprintf(stderr, "[dfm fused roles] E pass: producer %.0f, consumer w1 %.0f, chain warp (in slots 12+13) | M pass: producer %.0f, consumer w1 %.0f, sums+solves warp %.0f cyc/CTA\n",
-                tot[14] / (nb ? nb : 1), tot[15] / (nb ? nb : 1), tot[17] / (nb ? nb : 1), tot[18] / (nb ? nb : 1), tot[19] / (nb ? nb : 1));
-        fprintf(stderr, "[dfm fused P3/P5 split] P3 prepass %.0f, explicit %.0f, scan fwd: pw+pass1 %.0f, boundary %.0f, pass2 %.0f | scan bwd: %.0f, %.0f, %.0f cyc/CTA\n",
-                tot[20] / (nb ? nb : 1), tot[21] / (nb ? nb : 1), tot[22] / (nb ? nb : 1), tot[23] / (nb ? nb : 1), tot[24] / (nb ? nb : 1), tot[25] / (nb ? nb : 1),
-                tot[26] / (nb ? nb : 1), tot[27] / (nb ? nb : 1));
-        fprintf(stderr, "[dfm fused phases] %d CTAs, mean cycles per CTA: %.0f\n", nb, all / (nb ? nb : 1));
-        for (int k_ = 0; k_ < 12; ++k_) fprintf(stderr, "  %-14s %6.2f%%  %12.0f cyc/CTA\n", nm[k_], 100.0 * tot[k_] / all, tot[k_] / (nb ? nb : 1));
-      }
-#endif
     } else {
       rc = run_em_general(h, x, o, dL, dR, dA, dQ, dP0, dAn, dQn, dW, dlogR, dC, dBt, dqt, dslr, dnt, dCt, dzp, dzf, dPp, dPf, dFs, dPsF, dSff, dll, st, dit,
                           dstat, active, ntC, nblkC, smFS, stgT, out->PF ? 1 : 0, dxch, emb);

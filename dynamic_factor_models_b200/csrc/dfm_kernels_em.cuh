@@ -201,19 +201,6 @@ __global__ void k_em_contract_bal(const double* __restrict__ Xall, const double*
   }
 }
 
-// diagnostics (dfm_debug_fs_prof): clock64 totals of block 0, thread 0, per section
-#ifndef DFM_EMU
-__device__ long long g_fs_prof[48];
-__device__ int g_fs_prof_on;
-#define FS_T0() long long fs_t_ = (g_fs_prof_on && blockIdx.x == 0 && threadIdx.x == 0) ? clock64() : 0
-#define FS_T(k_) do { if (g_fs_prof_on && blockIdx.x == 0 && threadIdx.x == 0) { long long n_ = clock64(); g_fs_prof[k_] += n_ - fs_t_; fs_t_ = n_; } } while (0)
-#define FS_CNT(k_) do { if (g_fs_prof_on && blockIdx.x == 0 && threadIdx.x == 0) g_fs_prof[k_] += 1; } while (0)
-#else
-#define FS_T0() ((void)0)
-#define FS_T(k_) ((void)0)
-#define FS_CNT(k_) ((void)0)
-#endif
-
 // ---- small dense helpers of the filter / smoother steps ------------------------------------------------------------
 // ---- parallel-in-time treatment of FROZEN RUNS (consecutive periods whose covariances are the stored steady state):
 // the mean recursion  z_t = Phi z_{t -+ 1} + u_t  with a constant k x k matrix is a linear scan.  The run is cut into
@@ -268,7 +255,6 @@ __device__ EM_NOINLINE void em_run_scan_tc(double* __restrict__ zg, int k, int t
   constexpr int KBX = 2 * MB, KR = 8 * MB;             // k-chunks and (zero padded) state rows of a warp's tile
   const int NCH = 8 * EM_SC_NW;
   const int Lc = (L + NCH - 1) / NCH;
-  FS_T0();
   // Rp = Phi^Lc (binary powering on the tensor path; the three buffers rotate)
   for (int e = DFM_TID; e < k * k; e += DFM_NT) { int i = e % k, j = e / k; Rp[e] = (i == j) ? 1.0 : 0.0; base[e] = Phi[e]; }
   DFM_SYNC();
@@ -284,7 +270,6 @@ __device__ EM_NOINLINE void em_run_scan_tc(double* __restrict__ zg, int k, int t
       double* sw = base; base = tmp; tmp = sw;
     }
   }
-  FS_T(27);
   double* bnd = ws + (size_t)EM_SC_NW * 2 * KR * EM_SC_ZS;             // [64][k]: e_c, then in_c
   const int lr = DFM_LANE >> 2, lc = DFM_LANE & 3, wl = DFM_WARP;
   const int w = wl * nc + crank;                        // virtual warp of the cluster: 8 chunks each, EM_SC_NW in total
@@ -376,7 +361,6 @@ __device__ EM_NOINLINE void em_run_scan_tc(double* __restrict__ zg, int k, int t
     }
     DFM_SYNC();
     cl_sync(nc);
-    FS_T(27 + pass);
     if (pass == 1) {
       if (nc > 1) { for (int e = DFM_TID; e < NCH * k; e += DFM_NT) bnd[e] = xbnd[e]; DFM_SYNC(); }
       // incoming states on warp 0: in_0 = z_in, in_{c+1} = Phi^Lc in_c + e_c  (row i of Phi^Lc in the registers of lane i,
@@ -402,7 +386,6 @@ __device__ EM_NOINLINE void em_run_scan_tc(double* __restrict__ zg, int k, int t
         }
       }
       DFM_SYNC();
-      FS_T(30);
     }
   }
 }
@@ -426,7 +409,6 @@ __device__ EM_NOINLINE void em_run_scan(double* __restrict__ zg, int k, int t_fi
 #endif
   (void)nc; (void)crank; (void)xbnd;                   // (this variant is not split: the CTAs of a cluster run it redundantly)
   const int Lc = (L + EM_RUN_NCH - 1) / EM_RUN_NCH;
-  FS_T0();
   // Rp = Phi^Lc
   for (int e = DFM_TID; e < k * k; e += DFM_NT) { int i = e % k, j = e / k; Rp[e] = (i == j) ? 1.0 : 0.0; base[e] = Phi[e]; }
   DFM_SYNC();
@@ -434,7 +416,6 @@ __device__ EM_NOINLINE void em_run_scan(double* __restrict__ zg, int k, int t_fi
     if (ex & 1) { bm_gemm(tmp, k, Rp, k, false, base, k, false, k, k, k, 1.0, 0.0); bm_copy(Rp, k, tmp, k, k, k); }
     if (ex > 1) { bm_gemm(tmp, k, base, k, false, base, k, false, k, k, k, 1.0, 0.0); bm_copy(base, k, tmp, k, k, k); }
   }
-  FS_T(27);
   for (int pass = 1; pass <= 2; ++pass) {
     for (int c = DFM_WARP; c < EM_RUN_NCH; c += DFM_NWARP) {
       double* cur = wb + (size_t)c * 3 * k; double* nxt = cur + k; double* bnd = cur + 2 * k;
@@ -540,7 +521,6 @@ __device__ EM_NOINLINE void em_run_scan(double* __restrict__ zg, int k, int t_fi
       }
     }
     DFM_SYNC();
-    FS_T(27 + pass);
     if (pass == 1) {
       // incoming states: in_0 = z_in, in_{c+1} = Phi^Lc in_c + e_c ; bnd[c] holds e_c and is overwritten by in_c
       double* inc = wb;                                  // 2k doubles (chunk 0's idle cur/nxt buffers): current in_c, next in_c
@@ -556,7 +536,6 @@ __device__ EM_NOINLINE void em_run_scan(double* __restrict__ zg, int k, int t_fi
       double* el = wb + (size_t)(EM_RUN_NCH - 1) * 3 * k + 2 * k;
       for (int i = DFM_TID; i < k; i += DFM_NT) el[i] = inc[i];
       DFM_SYNC();
-      FS_T(30);
     }
   }
 }
@@ -650,7 +629,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
   for (int e = DFM_TID; e < rk; e += DFM_NT) S11[e] = 0.0;
   DFM_SYNC();
   double ll = 0.0;
-  FS_T0();
   // ------------------------------------------------------------------ forward: Kalman filter
   int frozen = 0, last_src = 0, run_known = 0;   // (uniform over the block; run_known: the frozen run in progress ends there)
   double ldS = 0.0;                      // thread 0: 2 sum log diag chol(S) of the last explicit step
@@ -690,9 +668,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
       }
       run_known = t1;
       const int Lr = t1 - t;
-#ifdef DFM_EMU
-      if (getenv("DFM_DEBUG_FREEZE")) printf("[run fwd] b=%d t=%d t1=%d\n", b, t, t1);
-#endif
       if (Lr >= EM_RUN_MIN) {
         // ---- parallel frozen run [t, t1):  zf_t = Phi zf_{t-1} + Kb b_t,  Phi = M - Kb C M[0:r,:],  Kb = Pf[:, 0:r]
         bm_gemm(Tm, r, C, r, false, M, k, false, r, k, r, 1.0, 0.0);             // C M[0:r,:]   (Tm, Wm: rebuilt by the next explicit step)
@@ -713,10 +688,8 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
         }
         DFM_SYNC();
         cl_sync(NC);
-        FS_T(22);
         em_run_scan(zfg, k, t, Lr, +1, T1, zf, T2, T3, Psn, wb, stg, stg_doubles, NC, crank, xbnd);   // (T2, T3, Psn are free between explicit steps)
         cl_sync(NC);
-        FS_T(23);
         double llp = 0.0;
         const double ldS_ = *ldS_sh;
         for (int t0 = t, ti = 0; t0 < t1; t0 += TT, ++ti) {                      // zp_t = M zf_{t-1}, likelihood terms
@@ -755,7 +728,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
         for (int e = DFM_TID; e < k; e += DFM_NT) zf[e] = zfg[(size_t)(t1 - 1) * k + e];
         DFM_SYNC();
         t = t1 - 1;
-        FS_T(1);
         continue;
       }
     }
@@ -778,7 +750,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
       }
       for (int e = DFM_TID; e < k; e += DFM_NT) { zpg[(size_t)t * k + e] = zp[e]; zfg[(size_t)t * k + e] = zf[e]; }
       DFM_SYNC();
-      FS_T(2);
       continue;
     }
     frozen = 0;
@@ -808,26 +779,20 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
       for (int e = DFM_TID; e < k; e += DFM_NT) zp[e] = tv[e];
       DFM_SYNC();
     }
-    FS_T(10);
     for (int e = DFM_TID; e < rr; e += DFM_NT) { int i = e % r, j = e / r; L[e] = Pp[i + k * j]; }
     for (int e = DFM_TID; e < rk; e += DFM_NT) { int j = e % k, a = e / k; Tm[e] = Pp[a + k * j]; }       // TmT[j + k a] = Pp[a, j]
     DFM_SYNC();
-    FS_T(16);
     bc_chol(L, r, r, dvL, info);                                                // Pff = L L'
-    FS_T(17);
     bm_gemm(T4, r, C, r, false, L, r, false, r, r, r, 1.0, 0.0);               // C L
     bm_gemm(S, r, L, r, true, T4, r, false, r, r, r, 1.0, 0.0);                // L' C L
     for (int e = DFM_TID; e < r; e += DFM_NT) S[e + r * e] += 1.0;
     DFM_SYNC();
     bm_symmetrize(S, r, r);
-    FS_T(18);
     bc_chol(S, r, r, dvS, info);                                                // S = Ls Ls'
     bt_trsm_lower(L, r, r, dvL, Tm, k, k);                                      // TmT = (L^-1 Pp[0:r,:])'
-    FS_T(19);
     for (int e = DFM_TID; e < rk; e += DFM_NT) Wm[e] = Tm[e];
     DFM_SYNC();
     bt_trsm_lower(S, r, r, dvS, Wm, k, k);                                      // WmT = (Ls^-1 Tm)'
-    FS_T(11);
     // Pf = Pp - Tm'Tm + Wm'Wm  (both products on the same tile -> lane mapping: an element stays with one thread)
     wt_gemm(Wm, 1, k, Wm, 1, k, k, k, r, [&](int i, int j, double v) { Pf[i + k * j] = Pp[i + k * j] + v; });
     wt_gemm(Tm, 1, k, Tm, 1, k, k, k, r, [&](int i, int j, double v) { Pf[i + k * j] -= v; });
@@ -837,7 +802,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
     DFM_SYNC();
     for (int i = DFM_TID; i < k; i += DFM_NT) { double s = zp[i]; for (int a = 0; a < r; ++a) s += Pf[i + k * a] * g[a]; zf[i] = s; }
     DFM_SYNC();
-    FS_T(12);
     if (DFM_TID == 0) {
       ldS = 0.0;
       for (int a = 0; a < r; ++a) ldS -= 2.0 * log(dvS[a]);
@@ -857,11 +821,7 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
       frozen = (dm <= 1e-14 * pm) ? 1 : 0;
     }
     DFM_SYNC();
-    FS_T(13); FS_CNT(8);
   }
-#ifdef DFM_EMU
-  if (getenv("DFM_DEBUG_FREEZE")) { int nf = 0; for (int t = 0; t < T; ++t) nf += (src[t] != t); printf("[freeze] b=%d T=%d k=%d frozen forward steps %d\n", b, T, k, nf); }
-#endif
   // ------------------------------------------------------------------ backward: RTS smoother
   for (int e = DFM_TID; e < kk; e += DFM_NT) Psn[e] = Pf[e];
   for (int e = DFM_TID; e < k; e += DFM_NT) zsn[e] = zf[e];
@@ -893,9 +853,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
       }
       const int tl = info[1] + 1, Lr = t - tl + 1;
       brun_known = tl - 1;
-#ifdef DFM_EMU
-      if (getenv("DFM_DEBUG_FREEZE")) printf("[run bwd] b=%d t=%d tl=%d\n", b, t, tl);
-#endif
       if (Lr >= EM_RUN_MIN) {
         // zs_t = J zs_{t+1} + v_t,  v_t = zf_t - J zp_{t+1}   (J is in T3)
         const int lds = em_lds(k);
@@ -914,10 +871,8 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
         }
         DFM_SYNC();
         cl_sync(NC);
-        FS_T(24);
         em_run_scan(zfg, k, t, Lr, -1, T3, zsn, T1, Pf, T2, wb, stg, stg_doubles, NC, crank, xbnd);   // (T1, Pf, T2 are free here; zfg now holds zs_t)
         cl_sync(NC);
-        FS_T(25);
         // Gram sums of the smoothed means: S00 (k x k), S11 (r x k) as DMMA products over tiles of zs rows staged in shared
         // memory; a warp's output tiles stay in registers over the tiles of the run
         const double cnt = (double)Lr;
@@ -962,7 +917,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
           }
         }
         DFM_SYNC();
-        FS_T(26);
         // zs_tl (k) -> tv for the Sff2 correction; fold the register sums into the shared accumulators
         for (int e = DFM_TID; e < k; e += DFM_NT) tv[e] = zfg[(size_t)tl * k + e];
         if (in_regs && NC > 1) {
@@ -1006,14 +960,12 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
         for (int e = DFM_TID; e < k; e += DFM_NT) zsn[e] = tv[e];
         DFM_SYNC();
         t = tl;
-        FS_T(4);
         continue;
       }
     }
     for (int e = DFM_TID; e < k; e += DFM_NT) { zp[e] = zpg[(size_t)(t + 1) * k + e]; zf[e] = zfg[(size_t)t * k + e]; }
     if (!ps_frozen) for (int e = DFM_TID; e < kk; e += DFM_NT) { T1[e] = Ppg[(size_t)sp * kk + e]; Pf[e] = Pfg[(size_t)sf * kk + e]; }
     DFM_SYNC();
-    FS_T(14);
     if (newJ) {
       // J = Pf M' Pp^-1, row by row:  T3 <- Pf M' (companion structure: columns >= r are a shift of Pf), T2 = chol(Pp) on
       // warp 0 meanwhile, then  L y = x, L' z = y  on the rows of T3 (thread per row)
@@ -1025,21 +977,18 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
       wt_gemm(Pf, 1, k, M, 1, k, k, r, k, [&](int i, int j, double v) { T3[i + k * j] = v; });
       DFM_SYNC();
       bc_chol(T2, k, k, dvL, info);
-      FS_T(20);
       // J = (Pf M') Pp^-1 = (Pf M') U U',  U = L^-T:  U' = L^-1 by forward substitution on the rows of the identity (thread per
       // row, registers), then two tensor-core products -- the back substitution, whose row stays in shared memory, cost
       // 16 K cycles at k = 32
       for (int e = DFM_TID; e < kk; e += DFM_NT) { const int j = e % k, a = e / k; Pp[e] = (j == a) ? 1.0 : 0.0; }
       DFM_SYNC();
       bt_trsm_lower(T2, k, k, dvL, Pp, k, k);                                   // Pp[j + k a] = (L^-1)[a, j]  (= U[j, a])
-      FS_T(21);
       wt_gemm(T3, 1, k, Pp, k, 1, k, k, k, [&](int i, int j, double v) { T2[i + k * j] = v; });      // (Pf M') U
       DFM_SYNC();
       wt_gemm(T2, 1, k, Pp, 1, k, k, k, k, [&](int i, int j, double v) { T3[i + k * j] = v; });      // ... U' = J
       DFM_SYNC();
       jpp = sp; jpf = sf;
     }
-    FS_T(15);
     for (int e = DFM_TID; e < k; e += DFM_NT) dv[e] = zsn[e] - zp[e];
     if (!ps_frozen) for (int e = DFM_TID; e < kk; e += DFM_NT) T1[e] = Psn[e] - T1[e];     // D = Ps(t+1) - Pp(t+1)
     DFM_SYNC();
@@ -1058,7 +1007,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
         ps_frozen = (dm <= 1e-14 * pm) ? 1 : 0;      // from the next period on: Ps = Psn, Tm as they are
       }
     } else DFM_SYNC();
-    FS_T(7);
     for (int e = DFM_TID; e < rk; e += DFM_NT) { int i = e % r, j = e / r; S11[e] += zsn[i] * zs[j] + Tm[e]; }
     for (int e = DFM_TID; e < kk; e += DFM_NT) { int i = e % k, j = e / k; S00[e] += zs[i] * zs[j] + Ps[e]; }
     for (int e = DFM_TID; e < rr; e += DFM_NT) {
@@ -1072,7 +1020,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
     for (int e = DFM_TID; e < kk; e += DFM_NT) Psn[e] = Ps[e];
     for (int e = DFM_TID; e < k; e += DFM_NT) zsn[e] = zs[e];
     DFM_SYNC();
-    FS_T(3); FS_CNT(9);
   }
   // ------------------------------------------------------------------ transition M-step
   // A = S11 S00^-1 (row by row: S00 A[i,:]' = S11[i,:]') ;  Q = (Sff2 - A S11') / (T-1)
@@ -1092,7 +1039,6 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
   bm_symmetrize(T4, r, r);
   for (int e = DFM_TID; e < rk; e += DFM_NT) Anew_[(size_t)b * rk + e] = Wm[e];
   for (int e = DFM_TID; e < rr; e += DFM_NT) { Qnew_[(size_t)b * rr + e] = T4[e]; SffAll_[(size_t)b * rr + e] = SffA[e]; }
-  FS_T(6);
   if (DFM_TID == 0 && crank == 0) {                  // (one CTA of the cluster updates the panel's state: the update is not idempotent)
     int it = st[b].iters;
     loglik_[(size_t)b * max_iter + it] = ll;

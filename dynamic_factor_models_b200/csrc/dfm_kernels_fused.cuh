@@ -28,7 +28,6 @@ namespace dfm {
 #define LI(n_, c_) ((c_) * Np + (n_))
 __host__ __device__ inline int pad4mod16(int x) { return x + ((4 - x % 16) + 16) % 16; }
 
-#define DFM_PH 32   // diagnostic slots per CTA
 struct FusedArgs {
   const double* X;      // [B][N][T] column-major panels
   double* Lam;          // [B][N*r] column-major (in: init, out: final)
@@ -50,14 +49,7 @@ struct FusedArgs {
   int* done;                 // streaming host path: done[b] = 1 (mapped pinned host memory) once panel b's results are in device memory
   double* P0out;             // non-NULL: compute P0 in the kernel (Lyapunov doubling of (A, Q), p0_steps steps, as k_lyapunov)
   int p0_steps;              //           and store it here ([B][r*r]).  With ready or P0out set the kernel also pre-fills its loglik rows.
-  int stagger;               // diagnostics: start delay (cycles) of the second co-resident CTA wave (0 = off)
-  long long* phase_cycles;   // optional [gridDim.x][DFM_PH] per-phase clock64() totals (diagnostics; NULL = off)
 };
-#ifdef DFM_EMU
-#define DFM_TICK(k_) ((void)0)
-#else
-#define DFM_TICK(k_) do { if (a.phase_cycles && threadIdx.x == 0) { long long now_ = clock64(); a.phase_cycles[(size_t)blockIdx.x * DFM_PH + (k_)] += now_ - tick_; tick_ = now_; } } while (0)
-#endif
 #define FUSED_SCR(R_) (5 * (R_) * (R_) + 1)
 
 __device__ __forceinline__ double w_max(double v) {
@@ -210,7 +202,7 @@ __device__ __forceinline__ void w_matpow(double* pw, const double* Cf, int ex0, 
 // in parallel) instead of nch - 1 serial matrix-vector steps.
 template <int R>
 __device__ __forceinline__ void blk_recur(double* Z, int Tp, const double* Cf, double* pw, double* pw2, double* bnd, int t0, int n, int dir, int nthr,
-                                          long long* prof = nullptr, bool pw_ready = false, const double* pl1 = nullptr, const double* pl2 = nullptr,
+                                          bool pw_ready = false, const double* pl1 = nullptr, const double* pl2 = nullptr,
                                           const double* pl3 = nullptr, const double* pl4 = nullptr) {
   if (n <= 0) return;
   // nthr = number of threads taking part (threads 0 .. nthr-1 of the CTA, a multiple of 32); they synchronise
@@ -220,12 +212,6 @@ __device__ __forceinline__ void blk_recur(double* Z, int Tp, const double* Cf, d
 #define BLK_SYNC() asm volatile("bar.sync 2, %0;" ::"r"(nthr) : "memory")
 #else
 #define BLK_SYNC() ((void)0)
-#endif
-#ifndef DFM_EMU
-  long long pt_ = prof ? clock64() : 0;
-#define BLK_PROF(k_) do { if (prof && threadIdx.x == 0) { long long now_ = clock64(); prof[k_] += now_ - pt_; pt_ = now_; } } while (0)
-#else
-#define BLK_PROF(k_) ((void)0)
 #endif
   // ng = number of 8-lane groups of the CTA (blockDim / 8).  chunk length: odd (=> the 4 groups of a
   // warp hit different banks) and at most ng chunks.  bnd: [(3 ng + 1) R + R R] doubles.
@@ -273,7 +259,6 @@ __device__ __forceinline__ void blk_recur(double* Z, int Tp, const double* Cf, d
   }
 #endif
   BLK_SYNC();
-  BLK_PROF(0);
   if (nch > 1) {
     // ---- boundary propagation: bnd[g] = true state entering chunk g (g >= 1)
 #ifdef DFM_EMU
@@ -339,7 +324,6 @@ __device__ __forceinline__ void blk_recur(double* Z, int Tp, const double* Cf, d
     }
 #endif
     BLK_SYNC();
-    BLK_PROF(1);
     // ---- pass 2: add Cf^(s+1) bnd[g]
 #ifdef DFM_EMU
     for (int g = 1; g < nch; ++g) {
@@ -369,9 +353,7 @@ __device__ __forceinline__ void blk_recur(double* Z, int Tp, const double* Cf, d
     }
 #endif
     BLK_SYNC();
-    BLK_PROF(2);
   }
-#undef BLK_PROF
 #undef BLK_SYNC
 }
 
@@ -409,9 +391,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
   double* scr = a.scratch + (size_t)DFM_BX * T * FUSED_SCR(R);
   // per explicit step t: scr[t*SCR + {0:Pf, RR:Phi, 2RR:J, 3RR:W, 4RR:Ps, 5RR: ld}]
   const double eps = 1e-14;
-#ifndef DFM_EMU
-  long long tick_ = clock64();
-#endif
 
   for (int b = DFM_BX; b < a.B; b += DFM_GX) {
     const double* X = a.X + (size_t)b * T * N;
@@ -427,7 +406,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
     int it = 0, status = 0;
     double ll_prev = 0.0;
     for (; it < a.max_iter; ++it) {
-      DFM_TICK(0);
       // ---------------------------------------------------------------- P0: prep
       double slr_p = 0.0;
       for (int i = DFM_TID; i < N; i += DFM_NT) { double rv = Rv[i]; rinv[i] = 1.0 / rv; slr_p += log(rv); if (!(rv > 0.0)) ctl[2] = 1; }
@@ -440,7 +418,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
         C[e] = s;
       }
       DFM_SYNC();
-      DFM_TICK(1);
       // ---------------------------------------------------------------- P1: E-step contraction (panel pass 1)
       double qacc = 0.0;
 #ifdef DFM_EMU
@@ -493,7 +470,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       qacc = block_sum(qacc, red);
       if (DFM_TID == 0) scal[2] = qacc;
       DFM_SYNC();
-      DFM_TICK(2);
       // ---------------------------------------------------------------- P2: covariance chain (warp 0, data independent)
       if (DFM_WARP == 0) {
         int* bad = &ctl[2];
@@ -592,9 +568,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
           } else --t;
         }
         if (DFM_LANE == 0) { ctl[0] = nE; ctl[1] = tb; ctl[3] = frozen; }
-#ifdef DFM_EMU
-        if (getenv("DFM_DEBUG_CHAIN")) printf("[chain] b=%d it=%d nE=%d frozen=%d tb=%d (T=%d)\n", b, it, nE, frozen, tb, T);
-#endif
         // I - J_inf M  (for the parallel pre-pass of the backward mean recursion)
         if (frozen) {
           w_gemm<R>(IJM, Jinf, false, M, false);
@@ -604,13 +577,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       }
       DFM_SYNC();
       const int nE = ctl[0], frozen = ctl[3];
-#ifndef DFM_EMU
-      if (a.phase_cycles && threadIdx.x == 0) {      // diagnostics: chain lengths
-        a.phase_cycles[(size_t)blockIdx.x * DFM_PH + 12] += nE; a.phase_cycles[(size_t)blockIdx.x * DFM_PH + 13] += (ctl[1] < 0 ? T - 1 : T - 1 - ctl[1]);
-        a.phase_cycles[(size_t)blockIdx.x * DFM_PH + 14] += 1; a.phase_cycles[(size_t)blockIdx.x * DFM_PH + 15] += frozen;
-      }
-#endif
-      DFM_TICK(3);
       // ---------------------------------------------------------------- P3: forward means
       // parallel pre-pass over the frozen range: Z[t] <- Pf_inf b_t
       for (int t = nE + DFM_TID; t < T; t += DFM_NT) {
@@ -643,7 +609,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       DFM_SYNC();
       // frozen steps: z_t = Phi_inf z_{t-1} + u_t, parallel in time over the CTA
       if (frozen) blk_recur<R>(Z, Tp, Phinf, T1, T2, bnd, (nE > 0 ? nE : 1), T - (nE > 0 ? nE : 1), +1, 128);
-      DFM_TICK(4);
       // ---------------------------------------------------------------- P4: log-likelihood (parallel over t)
       double llp = 0.0;
       for (int t = DFM_TID; t < T; t += DFM_NT) {
@@ -667,7 +632,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       }
       llp = block_sum(llp, red);
       const double ll = llp - 0.5 * scal[2];
-      DFM_TICK(5);
       // ---------------------------------------------------------------- P5: backward means
       if (frozen) {
         int lo = nE - 1;
@@ -700,7 +664,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
         }
       }
       DFM_SYNC();
-      DFM_TICK(6);
       // ---------------------------------------------------------------- P7: mean parts of the moment sums
       for (int e = DFM_TID; e < 2 * RR; e += DFM_NT) {
         int which = e / RR, ee = e % RR, i = ee / R, j = ee % R;
@@ -709,7 +672,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
         else { for (int t = 1; t < T; ++t) s += Z[ZI(t, i)] * Z[ZI(t - 1, j)]; S11m[ee] = s; }
       }
       DFM_SYNC();
-      DFM_TICK(7);
       // ---------------------------------------------------------------- P8: M-step contraction (panel pass 2)
 #ifdef DFM_EMU
       for (int n = 0; n < N; ++n) {
@@ -757,7 +719,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       }
 #endif
       DFM_SYNC();
-      DFM_TICK(8);
       // ---------------------------------------------------------------- P9: M-step solves
       if (DFM_WARP == 0) {
         int* bad = &ctl[2];
@@ -802,7 +763,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       }
       DFM_SYNC();
       for (int e = DFM_TID; e < RR; e += DFM_NT) { M[e] = Phi[e]; Q[e] = Pn[e]; }
-      DFM_TICK(9);
       if (DFM_TID == 0) a.loglik[(size_t)b * a.max_iter + it] = ll;
       DFM_SYNC();
       if (ctl[2] || !(ll == ll)) { status = 3; ++it; break; }
@@ -810,7 +770,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
       ll_prev = ll;
       if (conv) { ++it; break; }
     }
-    DFM_TICK(10);
     // ---- outputs
     for (int e = DFM_TID; e < N * R; e += DFM_NT) { int i = e % N, c = e / N; a.Lam[(size_t)b * N * R + e] = Lam[LI(i, c)]; }
     for (int e = DFM_TID; e < N; e += DFM_NT) a.R[(size_t)b * N + e] = Rv[e];
@@ -833,7 +792,6 @@ __global__ void DFM_FUSED_BOUNDS k_em_fused(FusedArgs a) {
     }
     if (DFM_TID == 0) { a.iters[b] = it > a.max_iter ? a.max_iter : it; a.status[b] = status; }
     DFM_SYNC();
-    DFM_TICK(11);
   }
 }
 

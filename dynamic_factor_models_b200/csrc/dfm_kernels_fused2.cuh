@@ -231,24 +231,13 @@ __device__ __forceinline__ void f2_consume_M(F2Ring& rg, int cw, int T, int N, i
 }
 #endif  // !DFM_EMU
 
+// the mean recursions P3-P5 run on warps 0..F2_NCW (named barrier 2) while the chain warp does the backward covariances
+#define F2_PNT_GPU ((F2_NCW + 1) * 32)
 #ifdef DFM_EMU
-#define F2_ROLE_T0() ((void)0)
-#define F2_ROLE_T1(k_) ((void)0)
-#define F2_SUB(k_) ((void)0)
-#define F2_SUBP(k_) nullptr
 #define F2_PSYNC() ((void)0)
 #define F2_PTID 0
 #define F2_PNT 1
-#define F2_PNT_GPU ((F2_NCW + 1) * 32)
 #else
-// diagnostics: time from the start of a pass until this warp role is done (lane 0 of the warp)
-#define F2_ROLE_T0() long long role_t0_ = a.phase_cycles ? clock64() : 0
-#define F2_ROLE_T1(k_) do { if (a.phase_cycles && DFM_LANE == 0) a.phase_cycles[(size_t)blockIdx.x * DFM_PH + (k_)] += clock64() - role_t0_; } while (0)
-// sub-phase split of the tick interval in progress (thread 0): cycles since the last DFM_TICK / F2_SUB
-#define F2_SUB(k_) do { if (a.phase_cycles && threadIdx.x == 0) { long long now_ = clock64(); a.phase_cycles[(size_t)blockIdx.x * DFM_PH + (k_)] += now_ - sub_; sub_ = now_; } } while (0)
-#define F2_SUBP(k_) (a.phase_cycles ? a.phase_cycles + (size_t)blockIdx.x * DFM_PH + (k_) : nullptr)
-// the mean recursions P3-P5 run on warps 0..F2_NCW (named barrier 2) while the chain warp does the backward covariances
-#define F2_PNT_GPU ((F2_NCW + 1) * 32)
 #define F2_PSYNC() asm volatile("bar.sync 2, %0;" ::"n"(F2_PNT_GPU) : "memory")
 #define F2_PTID ((int)threadIdx.x)
 #define F2_PNT F2_PNT_GPU
@@ -303,13 +292,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
   F2Ring rg; rg.ring = ring; rg.full = fullb; rg.empty = emptyb; rg.rs = 0; rg.rph = 0; rg.wrap = false;
 #endif
   const double eps = 1e-14;
-#ifndef DFM_EMU
-  long long tick_ = clock64();
-#endif
 
-#ifndef DFM_EMU
-  if (a.stagger > 0 && blockIdx.x >= gridDim.x / 2) { long long t0_ = clock64(); while (clock64() - t0_ < a.stagger) __nanosleep(500); }
-#endif
   for (int b = DFM_BX; b < a.B; b += DFM_GX) {
     const double* X = a.X + (size_t)b * T * N;
 #ifndef DFM_EMU
@@ -360,7 +343,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
     int it = 0, status = 0;
     double ll_prev = 0.0;
     for (; it < a.max_iter; ++it) {
-      DFM_TICK(0);
       // ---------------------------------------------------------------- P0: prep
       double slr_p = 0.0;
       for (int i = DFM_TID; i < N; i += DFM_NT) { double rv = Rv[i]; rinv[i] = 1.0 / rv; slr_p += log(rv); if (!(rv > 0.0)) ctl[2] = 1; }
@@ -400,7 +382,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         for (int e = DFM_TID; e < RR; e += DFM_NT) { double s = 0.0; for (int sl = 0; sl < nsl; ++sl) s += T1[sl * RR + e]; C[e] = s; }
       }
       DFM_SYNC();
-      DFM_TICK(1);
       // ---- covariance chain (data independent).  Forward part: on the chain warp concurrently with the E pass;
       //      backward part (smoothed covariances + covariance parts of the moment sums): on the chain warp
       //      concurrently with the mean recursions P3-P5, which only need the forward quantities (Pf, Phi, J).
@@ -410,9 +391,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         for (int e = DFM_LANE; e < RR; e += DFM_WSZ) { int i = e / R, j = e % R; Pp[e] = a.P0[(size_t)b * RR + i + R * j]; }
         DFM_WSYNC();
         int nE = T, frozen_at = -1, t = 0;
-#ifndef DFM_EMU
-        long long c0_ = clock64();
-#endif
         while (t < T) {
           double ldp = w_inv<R>(Pi, Pp, tmp, bad);
           for (int e = DFM_LANE; e < RR; e += DFM_WSZ) Wm[e] = Pi[e] + C[e];
@@ -453,9 +431,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         }
         const int frozen = nE < T;
         if (DFM_LANE == 0) { ctl[0] = nE; ctl[3] = frozen; }
-#ifndef DFM_EMU
-        if (a.phase_cycles && DFM_LANE == 0) a.phase_cycles[(size_t)blockIdx.x * DFM_PH + 12] += clock64() - c0_;
-#endif
         // I - J_inf M  (for the parallel pre-pass of the backward mean recursion)
         if (frozen) {
           w_gemm<R>(IJM, Jinf, false, M, false);
@@ -491,9 +466,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       auto chain_bwd = [&]() {
         const int nE = ctl[0], frozen = ctl[3];
         int t;
-#ifndef DFM_EMU
-        long long c1_ = a.phase_cycles ? clock64() : 0;
-#endif
         // backward covariance chain + covariance parts of the moment sums
         for (int e = DFM_LANE; e < RR; e += DFM_WSZ) {
           double v = frozen ? Pfinf[e] : (GSC(T - 1))[e];
@@ -546,12 +518,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
           } else --t;
         }
         if (DFM_LANE == 0) ctl[1] = tb;
-#ifndef DFM_EMU
-        if (a.phase_cycles && DFM_LANE == 0) a.phase_cycles[(size_t)blockIdx.x * DFM_PH + 13] += clock64() - c1_;
-#endif
-#ifdef DFM_EMU
-        if (getenv("DFM_DEBUG_CHAIN")) printf("[chain] b=%d it=%d nE=%d frozen=%d tb=%d (T=%d)\n", b, it, nE, frozen, tb, T);
-#endif
         DFM_WSYNC();
       };
       // ---------------------------------------------------------------- P1: E-step contraction (panel pass 1)
@@ -570,9 +536,8 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         // TMA pass (see f2_produce / f2_consume_E): warp 0 produces, warps 1..6 consume, warp 7 runs the
         // data-independent covariance chain concurrently
         const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
-        F2_ROLE_T0();
-        if (DFM_WARP == 0) { f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true); F2_ROLE_T1(14); }
-        else if (DFM_WARP <= F2_NCW) { qacc += f2_consume_E<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, rinv); if (DFM_WARP == 1) F2_ROLE_T1(15); }
+        if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true);
+        else if (DFM_WARP <= F2_NCW) qacc += f2_consume_E<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, rinv);
         else {
           rg.skip(nitems);                                                   // keep the ring position in step
           chain_fwd();
@@ -584,12 +549,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       chain_bwd();
 #endif
       DFM_SYNC();                                            // E pass and forward chain complete
-      DFM_TICK(2);
       const int nE = ctl[0], frozen = ctl[3];
-      DFM_TICK(3);
-#ifndef DFM_EMU
-      long long sub_ = a.phase_cycles ? clock64() : 0;
-#endif
 #ifndef DFM_EMU
       if (DFM_WARP == F2_NCW + 1) chain_bwd();                 // warp 7: backward covariance chain, concurrently with P3-P5 on warps 0..6
       else
@@ -615,7 +575,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         for (int i = 0; i < R; ++i) Z[ZI(t, i)] = u[i];
       }
       F2_PSYNC();
-      F2_SUB(20);
       if (DFM_WARP == 0) {
         // explicit steps
         for (int t = 0; t < nE; ++t) {
@@ -632,10 +591,8 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         }
       }
       F2_PSYNC();
-      F2_SUB(21);
       // frozen steps: z_t = Phi_inf z_{t-1} + u_t, parallel in time over the CTA
-      if (frozen) blk_recur<R>(Z, Tp, Phinf, Phi, Pi, bnd, (nE > 0 ? nE : 1), T - (nE > 0 ? nE : 1), +1, F2_PNT_GPU, F2_SUBP(22), true, Pp, Pi, Pf, Jm);
-      DFM_TICK(4);
+      if (frozen) blk_recur<R>(Z, Tp, Phinf, Phi, Pi, bnd, (nE > 0 ? nE : 1), T - (nE > 0 ? nE : 1), +1, F2_PNT_GPU, true, Pp, Pi, Pf, Jm);
       // ---------------------------------------------------------------- P4: log-likelihood
       // innovation form: ll_t = -1/2 (N log 2pi + sum log R + ld_t + quad_t),
       //   quad_t = -(zp'C zp + 2 zp'W d + d'W d),  zp = M zf_{t-1}, d = zf_t - zp,  W = Pi + C
@@ -752,7 +709,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         scal[3] = llp;
 #endif
       }
-      DFM_TICK(5);
       // ---------------------------------------------------------------- P5: backward means
       if (frozen) {
         int lo = nE - 1;
@@ -770,7 +726,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       }
       F2_PSYNC();
       // frozen range: z_t = J_inf z_{t+1} + v_t, parallel in time over the CTA
-      if (frozen) blk_recur<R>(Z, Tp, Jinf, Pn, Pi, bnd, T - 2, (T - 2) - (nE - 1) + 1, -1, F2_PNT_GPU, F2_SUBP(25), true, ring + F2_RTAIL(R), ring + F2_RTAIL(R) + RR, ring + F2_RTAIL(R) + 2 * RR, ring + F2_RTAIL(R) + 3 * RR);
+      if (frozen) blk_recur<R>(Z, Tp, Jinf, Pn, Pi, bnd, T - 2, (T - 2) - (nE - 1) + 1, -1, F2_PNT_GPU, true, ring + F2_RTAIL(R), ring + F2_RTAIL(R) + RR, ring + F2_RTAIL(R) + 2 * RR, ring + F2_RTAIL(R) + 3 * RR);
       if (DFM_WARP == 0) {
         const int lo = frozen ? nE - 1 : T;
         // explicit range: zs_t = zf_t + J_t (zs_{t+1} - M zf_t)
@@ -787,8 +743,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       }
       DFM_SYNC();
       const double ll = scal[3];
-      DFM_TICK(6);
-      DFM_TICK(7);
       // ---- moment sums + M-step r x r solves (all inputs are ready before the M pass): on the chain warp,
       //      concurrently with the pass
       auto mstep_small = [&]() {
@@ -863,13 +817,11 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
         const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
-        F2_ROLE_T0();
-        if (DFM_WARP == 0) { f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false); F2_ROLE_T1(17); }
-        else if (DFM_WARP <= F2_NCW) { f2_consume_M<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part); if (DFM_WARP == 1) F2_ROLE_T1(18); }
+        if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false);
+        else if (DFM_WARP <= F2_NCW) f2_consume_M<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part);
         else {
           rg.skip(nitems);
           mstep_small();
-          F2_ROLE_T1(19);
         }
       }
 #endif
@@ -877,7 +829,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       mstep_small();
 #endif
       DFM_SYNC();
-      DFM_TICK(8);
       // ---------------------------------------------------------------- P9: M-step solves
       DFM_SYNC();
       for (int n = DFM_TID; n < N; n += DFM_NT) {
@@ -899,7 +850,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       }
       DFM_SYNC();
       for (int e = DFM_TID; e < RR; e += DFM_NT) { M[e] = Phi[e]; Q[e] = Pn[e]; }
-      DFM_TICK(9);
       if (DFM_TID == 0) a.loglik[(size_t)b * a.max_iter + it] = ll;
       DFM_SYNC();
       if (ctl[2] || !(ll == ll)) { status = 3; ++it; break; }
@@ -907,7 +857,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       ll_prev = ll;
       if (conv) { ++it; break; }
     }
-    DFM_TICK(10);
     // ---- outputs
     for (int e = DFM_TID; e < N * R; e += DFM_NT) { int i = e % N, c = e / N; a.Lam[(size_t)b * N * R + e] = Lam[LI(i, c)]; }
     for (int e = DFM_TID; e < N; e += DFM_NT) a.R[(size_t)b * N + e] = Rv[e];
@@ -936,7 +885,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
 #ifndef DFM_EMU
     if (a.done && threadIdx.x == 0) *(volatile int*)(a.done + b) = 1;
 #endif
-    DFM_TICK(11);
   }
 }
 

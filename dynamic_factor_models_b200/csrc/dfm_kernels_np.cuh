@@ -73,35 +73,11 @@ __global__ void k_all_cols(int N, int* bal_idx, int* nbal) {
 }
 
 // Gram of the balanced block: mode 0 (nbal <= T): G = Xb'Xb (nbal x nbal); mode 1: G = Xb Xb' (T x T).
-// G stored dense with leading dimension n = min(nbal, T).  grid (ceil(nmax^2/NT), B).
-__global__ void k_gram(const double* __restrict__ Xs, int T, int N, const int* __restrict__ bal_idx,
-                       const int* __restrict__ nbal, double* __restrict__ G, int nmax) {
-  int b = DFM_BY;
-  int nb = nbal[b];
-  int mode = (nb <= T) ? 0 : 1;
-  int n = mode ? T : nb;
-  const double* X = Xs + (size_t)b * T * N;
-  const int* idx = bal_idx + (size_t)b * N;
-  double* g = G + (size_t)b * nmax * nmax;
-  for (long long e = (long long)DFM_BX * DFM_NT + DFM_TID; e < (long long)n * n; e += (long long)DFM_GX * DFM_NT) {
-    int a = (int)(e % n), c = (int)(e / n);
-    if (a < c) continue;
-    double s = 0.0;
-    if (mode == 0) {
-      const double* xa = X + (size_t)idx[a] * T; const double* xc = X + (size_t)idx[c] * T;
-      for (int t = 0; t < T; ++t) s += xa[t] * xc[t];
-    } else {
-      for (int j = 0; j < nb; ++j) { const double* col = X + (size_t)idx[j] * T; s += col[a] * col[c]; }
-    }
-    g[a + (size_t)n * c] = s; g[c + (size_t)n * a] = s;
-  }
-}
-
-// Gram matrix on the FP64 tensor path: one WARP per 16 x 16 block of the lower triangle (2 x 2 DMMA tiles: two A and two
+// G stored dense with leading dimension n = min(nbal, T).
+// On the FP64 tensor path: one WARP per 16 x 16 block of the lower triangle (2 x 2 DMMA tiles: two A and two
 // B fragments per four DMMA.8x8x4), fragments straight from global memory -- a panel (<= 1 MB) is L2 resident and every
 // 32-byte sector a fragment load touches is used completely; the reduction runs over T (mode 0) or over the balanced
 // columns (mode 1).  grid (ceil(nblocks / 8), B), 256 threads, nblocks = nb16 (nb16 + 1) / 2 with nb16 = ceil(nmax / 16).
-// (The scalar k_gram, one thread per entry and 2 T loads per entry, is kept behind DFM_OLD_GRAM.)
 __global__ void k_gram_tc(const double* __restrict__ Xs, int T, int N, const int* __restrict__ bal_idx,
                           const int* __restrict__ nbal, double* __restrict__ G, int nmax) {
 #ifndef DFM_EMU
@@ -460,16 +436,6 @@ __device__ __forceinline__ void gv_product(const double* __restrict__ G, int n, 
 __host__ __device__ inline size_t subspace2_smem_doubles(int n, int m) {
   return 2 * (size_t)em_lds(n) * m + 3 * (size_t)m * m + 2 * (m + 2) + 64 + 2 * m + 64;
 }
-// diagnostics (dfm_debug_fs_prof slots 48..63): clock64 section totals of CTA 0 of k_subspace_eig2
-#ifndef DFM_EMU
-__device__ long long g_sub_prof[16];
-__device__ int g_sub_prof_on;
-#define SB_T0() long long sb_t_ = (g_sub_prof_on && blockIdx.x == 0 && threadIdx.x == 0) ? clock64() : 0
-#define SB_T(k_) do { if (g_sub_prof_on && blockIdx.x == 0 && threadIdx.x == 0) { long long n_ = clock64(); g_sub_prof[k_] += n_ - sb_t_; sb_t_ = n_; } } while (0)
-#else
-#define SB_T0() ((void)0)
-#define SB_T(k_) ((void)0)
-#endif
 #ifdef DFM_EMU
 #define SUB2_BOUNDS
 #else
@@ -502,36 +468,25 @@ __global__ void SUB2_BOUNDS k_subspace_eig2(double* __restrict__ Gall, double* _
   DFM_SYNC();
   int it = 0;
   double res = 1.0;
-  SB_T0();
   for (; it < maxit; ++it) {
     // ---- orthonormalise V (CholQR, twice): S = V'V = L L', V <- V L^-T  (row-wise transposed solve)
     for (int pass = 0; pass < 2; ++pass) {
       wt_gemm(V, ldv, 1, V, ldv, 1, m, m, n, [&](int a, int c, double v) { S[a + m * c] = v; });
       DFM_SYNC();
       bm_symmetrize(S, m, m);
-      SB_T(0);
       bc_chol(S, m, m, dinv, info);
-      SB_T(1);
       bt_trsm_lower(S, m, m, dinv, V, ldv, n);
-      SB_T(2);
     }
     // Rayleigh-Ritz + convergence test: first after three cycles (9 products: a well separated factor spectrum has converged
     // by then), afterwards every second cycle -- the Jacobi solve of the projected matrix is the expensive, serial part
     const bool rr = (it >= 2 && ((it - 2) & 1) == 0) || it + 1 >= maxit;
     // ---- Y = G V
     gv_product(G, n, V, Y, ldv, m);
-    SB_T(3);
     if (rr) {
       wt_gemm(V, ldv, 1, Y, ldv, 1, m, m, n, [&](int a, int c, double v) { H[a + m * c] = v; });
       DFM_SYNC();
       bm_symmetrize(H, m, m);
-      SB_T(4);
-#ifndef DFM_EMU
-      { const int nsw = jacobi_core(H, W, m, cs, red, 40); if (g_sub_prof_on && blockIdx.x == 0 && threadIdx.x == 0) g_sub_prof[10] += nsw; }
-#else
       jacobi_core(H, W, m, cs, red, 40);
-#endif
-      SB_T(5);
       if (DFM_TID == 0) {                                 // Ritz values in descending order (selection with used flags in cs: O(m^2))
         for (int i = 0; i < m; ++i) cs[i] = 0.0;
         for (int j = 0; j < m; ++j) {
@@ -560,7 +515,6 @@ __global__ void SUB2_BOUNDS k_subspace_eig2(double* __restrict__ Gall, double* _
         rmax = fmax(rmax, sqrt(s_));
       }
       res = rmax / fabs(theta[0]);
-      SB_T(6);
       if (res <= tol) { ++it; break; }
     }
     // next iterate: V <- normalised G^3 V (Y = G V is there)
@@ -580,11 +534,7 @@ __global__ void SUB2_BOUNDS k_subspace_eig2(double* __restrict__ Gall, double* _
       }
       DFM_SYNC();
     }
-    SB_T(7);
   }
-#ifndef DFM_EMU
-  if (g_sub_prof_on && blockIdx.x == 0 && threadIdx.x == 0) { g_sub_prof[8] += it; g_sub_prof[9] += 1; }
-#endif
   // ---- leave results where k_pca_finish looks for them
   for (int e = DFM_TID; e < n * m; e += DFM_NT) Vg[e] = V[(e % n) + (size_t)ldv * (e / n)];
   DFM_SYNC();

@@ -63,9 +63,6 @@ int dfm_profile_enable(dfm_handle* h, int on);
 int dfm_profile_query(dfm_handle* h, const char* kernel_name /*NULL = all*/, double* ms, long long* count);
 int dfm_profile_reset(dfm_handle* h);
 const char* dfm_profile_kernel_name(dfm_handle* h, int i);
-/* Diagnostics of the general path's filter/smoother kernel: per-section clock64() totals of CTA 0 (64 slots: 48 of the filter/smoother + 16 of k_subspace_eig2; see
- * tools/fs_prof.py).  on = 1 arms and clears the counters, out (64 doubles, may be NULL) receives the totals so far. */
-int dfm_debug_fs_prof(dfm_handle* h, int on, double* out);
 
 /* ---- a2: standardize_data, dfm_functions.ipynb:501-509 ------------------------------- */
 /* Xs = (X - mean)/std per column over non-missing entries, population std. */
