@@ -56,6 +56,18 @@ class EmOut(C.Structure):
                 ("F", C.c_void_p), ("PF", C.c_void_p), ("loglik", C.c_void_p), ("iters", C.c_void_p), ("status", C.c_void_p)]
 
 
+class SsOpts(C.Structure):
+    _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("batch", C.c_int), ("mem", C.c_int)]
+
+
+class SsOut(C.Structure):
+    _fields_ = [("F", C.c_void_p), ("PF", C.c_void_p), ("common", C.c_void_p), ("xhat", C.c_void_p), ("xvar", C.c_void_p),
+                ("loglik", C.c_void_p), ("status", C.c_void_p)]
+
+
+SS_OUTPUTS = ("F", "PF", "common", "xhat", "xvar")
+
+
 def default_library_path():
     return os.path.join(HERE, "lib", "libdfm_b200.so")
 
@@ -63,7 +75,7 @@ def default_library_path():
 EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stream", "dfm_destroy", "dfm_sync",
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
-           "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_init_from_factors",
+           "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_kalman_smooth", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -130,6 +142,7 @@ class Library:
         L.dfm_irf.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_ip,
                               C.c_int, C.c_int, C.c_void_p]
         L.dfm_em_kalman.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(EmOpts), C.POINTER(EmInit), C.POINTER(EmOut)]
+        L.dfm_kalman_smooth.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsOpts), C.POINTER(EmInit), C.POINTER(SsOut)]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p]
         L.dfm_bootstrap_panels.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 8
@@ -192,6 +205,14 @@ class Library:
         ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in init.items()})
         ou = EmOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
         self.check(self.lib.dfm_em_kalman(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_em_kalman")
+
+    def kalman_smooth_raw(self, X, T, N, r, p, H, B, params, out, mem):
+        """Pointer-level dfm_kalman_smooth (ints = device or host addresses).  params: dict Lam, R, A, Q[, P0]; out: dict of
+        F, PF, common, xhat, xvar, loglik, status (missing or 0 = NULL)."""
+        o = SsOpts(T=T, N=N, r=r, p=p, H=H, batch=B, mem=mem)
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
+        ou = SsOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
+        self.check(self.lib.dfm_kalman_smooth(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_kalman_smooth")
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)
@@ -399,4 +420,28 @@ class Library:
         if want_PF:
             pf = oPF.reshape(B, T, r, r)
             res["PF"] = pf if b else pf[0]
+        return res
+
+    def kalman_smooth(self, X, Lam, R, A, Q, p=1, P0=None, H=0, outputs=SS_OUTPUTS):
+        """Smoothed factors, forecasts and imputed values at FIXED parameters (dfm_kalman_smooth).  X (T, N) or (B, T, N)
+        standardized with NaN; parameters as em_kalman.  Returns F (T+H, r), PF (T+H, r, r), common / xhat / xvar (T+H, N)
+        -- those named in `outputs` -- plus loglik and status (per panel for batched input)."""
+        X = np.asarray(X, float); b = X.shape[0] if X.ndim == 3 else None
+        T, N = X.shape[-2:]; r = np.asarray(Lam).shape[-1]; B = b or 1; Tp = T + H
+        o = SsOpts(T=T, N=N, r=r, p=p, H=H, batch=B, mem=MEM_HOST)
+        bufs = dict(X=to_cm(X), Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float), A=to_cm(A), Q=to_cm(Q),
+                    P0=to_cm(P0) if P0 is not None else None)
+        ini = EmInit(Lam=_ptr(bufs["Lam"]), R=_ptr(bufs["R"]), A=_ptr(bufs["A"]), Q=_ptr(bufs["Q"]), P0=_ptr(bufs["P0"]))
+        size = dict(F=Tp * r, PF=Tp * r * r, common=Tp * N, xhat=Tp * N, xvar=Tp * N)
+        outs = {n: np.empty(B * size[n]) for n in outputs}
+        oll = np.empty(B); ost = np.empty(B, dtype=np.int32)
+        ou = SsOut(loglik=_ptr(oll), status=_ptr(ost), **{n: _ptr(a_) for n, a_ in outs.items()})
+        self.check(self.lib.dfm_kalman_smooth(self.h, _ptr(bufs["X"]), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_kalman_smooth")
+        res = dict(loglik=oll if b else float(oll[0]), status=ost if b else int(ost[0]))
+        for n, a_ in outs.items():
+            if n == "PF":
+                pf = a_.reshape(B, Tp, r, r)
+                res[n] = pf if b else pf[0]
+            else:
+                res[n] = from_cm(a_, Tp, r if n == "F" else N, b)
         return res

@@ -194,6 +194,47 @@ def _estimate_parametric(m, method, lib):
     return None
 
 
+def kalman_smooth(X, Lam, R, A, Q, p=1, P0=None, H=0, lib=None, **kw):
+    """Smoothed factors, H-period forecasts and imputed values of a standardized panel at given state-space parameters
+    (dfm_kalman_smooth).  See Library.kalman_smooth."""
+    return (lib or get_library()).kalman_smooth(X, Lam, R, A, Q, p=p, P0=P0, H=H, **kw)
+
+
+def forecast(m, H, lib=None):
+    """Nowcasts, forecasts and imputed values from a model estimated with `estimate(m, Parametric())`.
+
+    Runs the Kalman filter and smoother once at the EM estimates `m.em` over the estimation block (rows
+    initperiod..lastperiod, series with inclcode == 1, standardized as `estimate` standardizes them) and H periods after it.
+    Returns a dict, rows = periods initperiod .. lastperiod + H (1-based, in `periods`), columns = the estimation series
+    (indices into m.data's columns in `series`):
+      factor (T+H, r), factor_var (T+H, r, r)   E[f_t | data] and its covariance (standardized units, as m.factor);
+      xhat (T+H, ns)   E[x_it | data] in data units: the data where observed, the nowcast / forecast / imputed value otherwise;
+      xvar (T+H, ns)   Var[x_it | data] in data units: 0 where observed;
+      common (T+H, ns) the common component lambda_i' E[f_t | data] in data units (xmean + xstd * common, as compute_series);
+      loglik           log-likelihood of the observed cells at m.em's parameters.
+    Series left out of the model (too few observations for the ALS step) have NaN columns."""
+    if m.em is None:
+        raise ValueError("forecast needs a model estimated with Parametric()")
+    if H < 0:
+        raise ValueError("H must be >= 0")
+    lib = lib or get_library()
+    i0, i1 = m.initperiod, m.lastperiod
+    incl = np.flatnonzero(m.inclcode == 1)
+    X = m.data[:, incl][i0 - 1:i1]
+    Xs, xmean, xstd = lib.standardize(X)                               # the standardisation of _estimate_parametric
+    out_model = np.isnan(m.lambda_est[:, 0])
+    Xs = np.where(out_model[None, :], np.nan, Xs)
+    e = m.em
+    r = e["Lam"].shape[1]; p = e["A"].shape[1] // r
+    Lam = np.where(out_model[:, None], np.nan, e["Lam"])
+    o = lib.kalman_smooth(Xs, Lam, e["R"], e["A"], e["Q"], p=p, P0=e["P0"], H=H)
+    if o["status"] != 0:
+        raise RuntimeError(f"forecast: device status {o['status']}")
+    return dict(periods=np.arange(i0, i1 + H + 1), series=incl, factor=o["F"], factor_var=o["PF"],
+                xhat=xmean + xstd * o["xhat"], xvar=xstd ** 2 * o["xvar"], common=xmean + xstd * o["common"],
+                loglik=o["loglik"])
+
+
 def em_init_from_factors(Xs, F, p=1, lib=None):
     return (lib or get_library()).em_init_from_factors(Xs, F, p)
 

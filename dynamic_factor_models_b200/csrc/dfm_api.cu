@@ -6,6 +6,7 @@
 #include "dfm_kernels_np.cuh"
 #include "dfm_kernels_em.cuh"
 #include "dfm_kernels_emb.cuh"
+#include "dfm_kernels_ss.cuh"
 #include "dfm_kernels_fused.cuh"
 #include "dfm_kernels_fused2.cuh"
 #include "dfm_kernels_als_masked.cuh"
@@ -28,6 +29,10 @@ static inline cudaError_t cudaMalloc(void** p, size_t n) { *p = malloc(n ? n : 1
 static inline cudaError_t cudaFree(void* p) { free(p); return 0; }
 static inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { memcpy(d, s, n); return 0; }
 static inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) { memset(d, v, n); return 0; }
+static inline cudaError_t cudaMemcpy2DAsync(void* d, size_t dp, const void* s, size_t sp, size_t w, size_t rows, cudaMemcpyKind, cudaStream_t) {
+  for (size_t j = 0; j < rows; ++j) memcpy((char*)d + j * dp, (const char*)s + j * sp, w);
+  return 0;
+}
 static inline cudaError_t cudaStreamCreate(cudaStream_t* s) { *s = nullptr; return 0; }
 static inline cudaError_t cudaStreamDestroy(cudaStream_t) { return 0; }
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return 0; }
@@ -247,6 +252,59 @@ static int emb_launch_M(dfm_handle* h, const EmbPlan& e, const double* x, const 
   return DFM_OK;
 }
 
+// Staging tile (periods) of the frozen-run phases of k_em_filter_smooth: few panels -> large tiles (one CTA per SM
+// anyway); many panels -> the largest tile that still lets two CTAs share an SM, if any does.
+static int fs_stage_periods(int nsm, int batch, int r, int p) {
+  int stgT = (batch <= nsm) ? 256 : 16;
+  const size_t lim2 = 112 * 1024;
+  if (batch <= nsm) { while (stgT > 8 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
+  else if (em_fs_smem_doubles(r, p, 4) * 8 <= lim2) { while (stgT > 4 && em_fs_smem_doubles(r, p, stgT) * 8 > lim2) stgT /= 2; }
+  else { while (stgT > 4 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
+  return stgT;
+}
+
+// CTAs per panel (thread-block cluster) of the filter / smoother
+static int fs_cluster_size(const dfm_handle* h, int batch, const double* dxch) {
+  int ncl = 1;
+  if (dxch) { if (batch * 8 <= h->nsm) ncl = 8; else if (batch * 4 <= h->nsm) ncl = 4; else if (batch * 2 <= h->nsm) ncl = 2; }
+  if (getenv("DFM_CLUSTER")) ncl = std::max(1, std::min(8, atoi(getenv("DFM_CLUSTER"))));
+  return ncl;
+}
+
+// One launch of k_em_filter_smooth over the batch; a cluster per panel when ncl > 1 (set to 1 if the cluster cannot be placed).
+static int launch_filter_smooth(dfm_handle* h, int& ncl, int batch, int ntFS, size_t smFS, const double* dA, const double* dQ,
+                                const double* dP0, const double* dC, const double* dBt, const double* dqt, const double* dslr, const int* dnt,
+                                const double* dCt, int T, int r, int p, double* dzp, double* dzf, double* dPp, double* dPf, double* dFs,
+                                double* dPsF, double* dSff, double* dAn, double* dQn, double* dll, int mi, double tol, EmState* st, int* dsrc,
+                                int stgT, int want_psf, double* dxch) {
+#ifndef DFM_EMU
+  if (ncl > 1) {
+    // few panels: a thread-block cluster per panel (the CTAs split the parallel phases of the frozen runs)
+    PROF_BEGIN("k_em_filter_smooth");
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(batch * ncl)); cfg.blockDim = dim3((unsigned)ntFS); cfg.dynamicSmemBytes = smFS; cfg.stream = h->stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)ncl; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    cudaError_t ce = cudaLaunchKernelEx(&cfg, k_em_filter_smooth, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf,
+                          dPp, dPf, dFs, dPsF, dSff, dAn, dQn, dll, mi, tol, st, dsrc, stgT, want_psf, dxch);
+    PROF_END(); h->launches++;
+    if (ce != cudaSuccess) {                       // the cluster could not be placed: run the plain one-CTA-per-panel launch instead
+      (void)cudaGetLastError();
+      ncl = 1;
+      L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf,
+        dFs, dPsF, dSff, dAn, dQn, dll, mi, tol, st, dsrc, stgT, want_psf, (double*)nullptr);
+    }
+    return DFM_OK;
+  }
+#else
+  (void)dxch;
+#endif
+  L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf,
+    dFs, dPsF, dSff, dAn, dQn, dll, mi, tol, st, dsrc, stgT, want_psf, (double*)nullptr);
+  return DFM_OK;
+}
+
 // General multi-kernel EM path on device-resident data (any r, p, missing data).
 static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, double* dL, double* dR, double* dA, double* dQ, double* dP0,
                           double* dAn, double* dQn, double* dW, double* dlogR, double* dC, double* dBt, double* dqt, double* dslr, int* dnt,
@@ -256,9 +314,7 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
   int np = r * (r + 1) / 2;
   int* dsrc = dnt + (size_t)batch * T;
   const int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;     // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
-  int ncl = 1;                                     // CTAs per panel (thread-block cluster) of the filter / smoother
-  if (dxch) { if (batch * 8 <= h->nsm) ncl = 8; else if (batch * 4 <= h->nsm) ncl = 4; else if (batch * 2 <= h->nsm) ncl = 2; }
-  if (getenv("DFM_CLUSTER")) ncl = std::max(1, std::min(8, atoi(getenv("DFM_CLUSTER"))));
+  int ncl = fs_cluster_size(h, batch, dxch);
   L(k_em_state_init, batch, 1, 1, 0, st);
   L(k_em_scan, N, batch, 64, 0, x, dL, T, N, r, st);
   L(k_em_prep, batch, 1, 128, 0, dL, dR, N, r, p, dW, dlogR, dC, dA, dAn, dQ, dQn, st, mi, 0, emb.on ? 1 : 0);
@@ -288,29 +344,8 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
         default: emb_launch_E<4>(h, emb, x, dW, dR, dlogR, T, N, r, batch, dBt, dqt, dslr, dnt, st); break;
       }
     }
-#ifndef DFM_EMU
-    if (ncl > 1) {
-      // few panels: a thread-block cluster per panel (the CTAs split the parallel phases of the frozen runs)
-      PROF_BEGIN("k_em_filter_smooth");
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3((unsigned)(batch * ncl)); cfg.blockDim = dim3((unsigned)ntFS); cfg.dynamicSmemBytes = smFS; cfg.stream = h->stream;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)ncl; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      cudaError_t ce = cudaLaunchKernelEx(&cfg, k_em_filter_smooth, (const double*)dA, (const double*)dQ, (const double*)dP0, (const double*)dC,
-                            (const double*)dBt, (const double*)dqt, (const double*)dslr, (const int*)dnt, (const double*)dCt, T, r, p, dzp, dzf,
-                            dPp, dPf, dFs, dPsF, dSff, dAn, dQn, dll, mi, o->tol, st, dsrc, stgT, want_psf, dxch);
-      PROF_END(); h->launches++;
-      if (ce != cudaSuccess) {                       // the cluster could not be placed: run the plain one-CTA-per-panel launch instead
-        (void)cudaGetLastError();
-        ncl = 1;
-        L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf,
-          dFs, dPsF, dSff, dAn, dQn, dll, mi, o->tol, st, dsrc, stgT, want_psf, (double*)nullptr);
-      }
-    } else
-#endif
-    L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf,
-      dFs, dPsF, dSff, dAn, dQn, dll, mi, o->tol, st, dsrc, stgT, want_psf, (double*)nullptr);
+    launch_filter_smooth(h, ncl, batch, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf, dFs, dPsF, dSff,
+                         dAn, dQn, dll, mi, o->tol, st, dsrc, stgT, want_psf, dxch);
     if (any_missing || !emb.on) L(k_em_mstep_series, N, batch, 64, (size_t)(2 * np + r + 8) * 8, x, dFs, dPsF, dSff, T, N, r, dL, dR, st, emb_on);
     if (any_bal && emb.on) {
       switch (emb.ncb) {
@@ -905,15 +940,7 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
   int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mem = o->mem, mi = o->max_iter;
   if (T <= 1 || N <= 0 || r <= 0 || r > 64 || p <= 0 || batch <= 0 || mi <= 0 || o->tol < 0)
     return fail(h, DFM_ERR_ARG, "dfm_em_kalman: bad shape/options");
-  // staging tile of the frozen-run phases of the filter / smoother: few panels -> large tiles (one CTA per SM anyway);
-  // many panels -> the largest tile that still lets two CTAs share an SM, if any does
-  int stgT = (batch <= h->nsm) ? 256 : 16;
-  {
-    const size_t lim2 = 112 * 1024;
-    if (batch <= h->nsm) { while (stgT > 8 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
-    else if (em_fs_smem_doubles(r, p, 4) * 8 <= lim2) { while (stgT > 4 && em_fs_smem_doubles(r, p, stgT) * 8 > lim2) stgT /= 2; }
-    else { while (stgT > 4 && em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) stgT /= 2; }
-  }
+  const int stgT = fs_stage_periods(h->nsm, batch, r, p);
   size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
   if (smFS > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: state dimension r*p too large for the general path");
   CK(cudaSetDevice(h->device));
@@ -1173,6 +1200,119 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
     }
     rc = copy_out(h, out->loglik, dll, B * mi, mem); if (rc) return rc;
     rc = copy_out(h, out->iters, dit, B, mem); if (rc) return rc;
+    rc = copy_out(h, out->status, dstat, B, mem); if (rc) return rc;
+  }
+  return finish(h, mem);
+}
+
+// ------------------------------------------------------------------------------------ a'': smoothing / nowcasting / forecasting
+// One E-step of the general path at fixed parameters on panels padded with H all-missing periods, then k_ss_project.
+// Nothing here writes the parameter buffers: k_em_prep runs only in its opening mode (W, log R, C), k_em_filter_smooth's
+// transition M-step goes to scratch, and no measurement M-step or closing step is launched.
+int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, const dfm_em_init* params, const dfm_ss_out* out) {
+  if (!h || !X || !o || !params || !out || !params->Lam || !params->R || !params->A || !params->Q)
+    return fail(h, DFM_ERR_ARG, "dfm_kalman_smooth: null argument");
+  const int T = o->T, N = o->N, r = o->r, p = o->p, H = o->H, batch = o->batch, mem = o->mem;
+  if (T <= 0 || N <= 0 || r <= 0 || r > 64 || p <= 0 || H < 0 || batch <= 0 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE) ||
+      (long long)T + H < 2)
+    return fail(h, DFM_ERR_ARG, "dfm_kalman_smooth: bad shape/options");
+  const int Tp = T + H;
+  const int stgT = fs_stage_periods(h->nsm, batch, r, p);
+  const size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
+  if (r * p > 48 || smFS > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_kalman_smooth: state dimension r*p too large for the general path");
+  const size_t smP = ss_project_smem_doubles(r) * 8;
+  CK(cudaSetDevice(h->device));
+  const size_t B = batch, TN = (size_t)Tp * N; const int k = r * p, kk = k * k, rr = r * r, rk = r * k, np = r * (r + 1) / 2;
+  const int ntC = tpt_threads(np + r), nblkC = (Tp + ntC - 1) / ntC;
+  const bool dev_out = mem == DFM_MEM_DEVICE;
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    // padded panel: needed unless the input is already on the device with nothing to pad
+    double* dXp = (mem == DFM_MEM_HOST || H > 0) ? a.get<double>(B * TN) : nullptr;
+    double* dL = mem == DFM_MEM_HOST ? a.get<double>(B * N * r) : nullptr;
+    double* dR = mem == DFM_MEM_HOST ? a.get<double>(B * N) : nullptr;
+    double* dA = mem == DFM_MEM_HOST ? a.get<double>(B * rk) : nullptr;
+    double* dQ = mem == DFM_MEM_HOST ? a.get<double>(B * rr) : nullptr;
+    double* dP0 = a.get<double>(B * kk);
+    double* dFs = a.get<double>(B * Tp * r); double* dPsF = a.get<double>(B * Tp * np);
+    double* dll = a.get<double>(B); EmState* st = a.get<EmState>(B);
+    int* dit = a.get<int>(B); int* dstat = a.get<int>(B);
+    double* dAn = a.get<double>(B * rk); double* dQn = a.get<double>(B * rr); double* dW = a.get<double>(B * N * r);
+    double* dlogR = a.get<double>(B * N); double* dC = a.get<double>(B * rr); double* dBt = a.get<double>(B * Tp * r);
+    double* dqt = a.get<double>(B * Tp); double* dslr = a.get<double>(B * Tp);
+    int* dnt = a.get<int>(2 * B * Tp);                      // n_t, then src_t of the frozen-step logic
+    double* dCt = a.get<double>(B * Tp * np); double* dzp = a.get<double>(B * Tp * k); double* dzf = a.get<double>(B * Tp * k);
+    double* dPp = a.get<double>(B * Tp * kk); double* dPf = a.get<double>(B * Tp * kk); double* dSff = a.get<double>(B * rr);
+    double* dxch = a.get<double>(B * (16 + 64 * (size_t)k + 16 * ((size_t)kk + rk)));
+    double* dPFfull = (out->PF && !dev_out) ? a.get<double>(B * Tp * rr) : nullptr;
+    double* dcom = (out->common && !dev_out) ? a.get<double>(B * TN) : nullptr;
+    double* dxh = (out->xhat && !dev_out) ? a.get<double>(B * TN) : nullptr;
+    double* dxv = (out->xvar && !dev_out) ? a.get<double>(B * TN) : nullptr;
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    int rc = DFM_OK;
+    // ---- staging: padded panels and parameters
+    const double* x = X;
+    if (mem == DFM_MEM_HOST) {
+      if (H > 0) {
+        CK(cudaMemcpy2DAsync(dXp, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, B * N, cudaMemcpyHostToDevice, h->stream));
+        long long n = (long long)B * N * H;
+        L(k_ss_pad, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)nullptr, T, Tp, (long long)B * N, dXp);
+      } else CK(cudaMemcpyAsync(dXp, X, B * TN * 8, cudaMemcpyHostToDevice, h->stream));
+      x = dXp;
+    } else if (H > 0) {
+      long long n = (long long)B * TN;
+      L(k_ss_pad, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, X, T, Tp, (long long)B * N, dXp);
+      x = dXp;
+    }
+    const double *pL, *pR, *pA, *pQ;
+    rc = stage_in(h, params->Lam, dL, B * N * r, mem, &pL); if (rc) return rc;
+    rc = stage_in(h, params->R, dR, B * N, mem, &pR); if (rc) return rc;
+    rc = stage_in(h, params->A, dA, B * rk, mem, &pA); if (rc) return rc;
+    rc = stage_in(h, params->Q, dQ, B * rr, mem, &pQ); if (rc) return rc;
+    if (params->P0) CK(cudaMemcpyAsync(dP0, params->P0, B * kk * 8, dev_out ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+    else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, pA, pQ, r, p, dP0, 12);
+    // ---- one E-step (the general path's kernels; k_em_prep in its opening mode only reads Lam, R)
+    L(k_em_state_init, batch, 1, 1, 0, st);
+    L(k_em_scan, N, batch, 64, 0, x, pL, Tp, N, r, st);
+    L(k_em_prep, batch, 1, 128, 0, pL, pR, N, r, p, dW, dlogR, dC, (double*)nullptr, (const double*)nullptr, (double*)nullptr,
+      (const double*)nullptr, st, 1, 0, 0);
+    L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, pL, dW, pR, dlogR, dC, Tp, N, r, dBt, dqt, dslr, dnt, dCt, st);
+    L(k_em_contract_bal, (Tp + 31) / 32, batch, 256, 8 * 32 * 3 * 8, x, dW, pR, dlogR, Tp, N, r, dBt, dqt, dslr, dnt, st);
+    int ncl = fs_cluster_size(h, batch, dxch);
+    const int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;
+    rc = launch_filter_smooth(h, ncl, batch, ntFS, smFS, pA, pQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, Tp, r, p, dzp, dzf, dPp, dPf, dFs, dPsF,
+                              dSff, dAn, dQn, dll, 1, 0.0, st, dnt + B * Tp, stgT, 1, dxch);
+    if (rc) return rc;
+    L(k_em_collect, batch, 1, 1, 0, st, dit, dstat);
+    L(k_ss_nan_failed, batch, 1, 256, 0, (const EmState*)st, Tp, r, dFs, dPsF, dll);
+    // ---- projection onto the series
+    double* ocom = dev_out ? out->common : dcom;
+    double* oxh = dev_out ? out->xhat : dxh;
+    double* oxv = dev_out ? out->xvar : dxv;
+    if (ocom || oxh || oxv) {
+      DFM_SET_SMEM(k_ss_project, smP);
+      const int nst = (N + SS_NS - 1) / SS_NS, ntt = (Tp + SS_TP - 1) / SS_TP;
+      const int per = std::max(1, 65535 / nst);            // panels per launch (grid.y limit)
+      for (int b0 = 0; b0 < batch; b0 += per) {
+        const int nb = std::min(per, batch - b0);
+        L(k_ss_project, ntt, nst * nb, 256, smP, x, (const double*)dFs, (const double*)dPsF, pL, pR, (const EmState*)st, Tp, N, r, b0,
+          ocom, oxh, oxv);
+      }
+    }
+    // ---- results
+    rc = copy_out(h, out->F, dFs, B * Tp * r, mem); if (rc) return rc;
+    if (out->PF) {
+      long long n = (long long)Tp * rr;
+      double* dst = dev_out ? out->PF : dPFfull;
+      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, dPsF, Tp, r, dst);
+      if (!dev_out) { rc = copy_out(h, out->PF, dPFfull, B * Tp * rr, mem); if (rc) return rc; }
+    }
+    if (!dev_out) {
+      rc = copy_out(h, out->common, dcom, B * TN, mem); if (rc) return rc;
+      rc = copy_out(h, out->xhat, dxh, B * TN, mem); if (rc) return rc;
+      rc = copy_out(h, out->xvar, dxv, B * TN, mem); if (rc) return rc;
+    }
+    rc = copy_out(h, out->loglik, dll, B, mem); if (rc) return rc;
     rc = copy_out(h, out->status, dstat, B, mem); if (rc) return rc;
   }
   return finish(h, mem);

@@ -202,6 +202,33 @@ typedef struct {            /* outputs; any pointer may be NULL */
 int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* opts, const dfm_em_init* init,
                   const dfm_em_out* out);
 
+/* ---- a'': smoothing, nowcasting and forecasting with a fitted state-space model --------- */
+/* The model of dfm_em_kalman at GIVEN parameters (no M-step): one Kalman filter + RTS smoother pass over the panel and H
+ * periods after it.  A forecast period is one in which no series is observed, so the same pass gives the smoothed
+ * factors of t <= T (the ragged edge included), the forecasts of t > T, and E[x_it | data] for every missing cell. */
+typedef struct {
+  int T, N, r, p;             /* in-sample panel T x N, STANDARDIZED, NaN = missing (as dfm_em_kalman) */
+  int H;                      /* periods T+1 .. T+H to forecast; 0 = smoothing only */
+  int batch, mem;
+} dfm_ss_opts;
+
+typedef struct {              /* any pointer may be NULL (not computed); per panel back to back; all column-major */
+  double* F;                  /* (T+H) x r        E[f_t | observed x]  (forecasts for t > T) */
+  double* PF;                 /* r x r x (T+H)    Var[f_t | observed x] */
+  double* common;             /* (T+H) x N        lambda_i' E[f_t | x]  (compute_series, dfm_functions.ipynb:552) */
+  double* xhat;               /* (T+H) x N        E[x_it | x]: x_it where observed, common_it otherwise */
+  double* xvar;               /* (T+H) x N        Var[x_it | x]: 0 where observed, lambda_i' PF_t lambda_i + R_i otherwise */
+  double* loglik;             /* [batch]          log-likelihood of the observed cells */
+  int* status;                /* [batch]          0, or DFM_ERR_NOT_PD (a covariance not positive definite or R_i <= 0: that
+                                                   panel's outputs are NaN) */
+} dfm_ss_out;
+
+/* X: T x N standardized panels back to back; params: (Lam, R, A, Q) per panel as dfm_em_kalman's initial parameters,
+ * P0 == NULL => the same stationary prior by Lyapunov doubling.  A series whose Lambda row or R_i is NaN is out of the
+ * model: its columns of common / xhat / xvar are NaN.  Size limits and error codes as dfm_em_kalman's general path
+ * (k = r*p <= 48); H < 0 is DFM_ERR_ARG.  The parameter arrays are only read.  Synchronous for host memory. */
+int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* opts, const dfm_em_init* params, const dfm_ss_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

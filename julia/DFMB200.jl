@@ -194,4 +194,27 @@ function estimate!(m, method = Main.NonParametric(); lam_constr_f = nothing, lam
     return (loglik = ll[1:it[]], iters = it[], Lam = Lam, R = R, A = A, Q = Q)
 end
 
+struct SsOpts; T::Cint; N::Cint; r::Cint; p::Cint; H::Cint; batch::Cint; mem::Cint; end
+struct SsOut; F::Ptr{Cdouble}; PF::Ptr{Cdouble}; common::Ptr{Cdouble}; xhat::Ptr{Cdouble}; xvar::Ptr{Cdouble}
+              loglik::Ptr{Cdouble}; status::Ptr{Cint}; end
+
+"""Smoothed factors, `H`-period forecasts and imputed values of the standardized panel `Xs` (NaN = missing) at the parameters
+`em` returned by `estimate!(m, Parametric())` (dfm_kalman_smooth).  Rows 1..T+H; `xhat`/`xvar`/`common` in standardized units."""
+function kalman_smooth(Xs::Matrix{Float64}, em, H::Integer)
+    h = gethandle()
+    T, N = size(Xs); r = size(em.Lam, 2); p = size(em.A, 2) ÷ r; Tp = T + H
+    F = Matrix{Float64}(undef, Tp, r); PF = Array{Float64}(undef, r, r, Tp)
+    common = Matrix{Float64}(undef, Tp, N); xhat = similar(common); xvar = similar(common)
+    ll = Ref{Cdouble}(NaN); st = Ref{Cint}(0)
+    GC.@preserve Xs em F PF common xhat xvar begin
+        opts = Ref(SsOpts(T, N, r, p, H, 1, MEM_HOST))
+        init = Ref(EmInit(pointer(em.Lam), pointer(em.R), pointer(em.A), pointer(em.Q), C_NULL))
+        out = Ref(SsOut(pointer(F), pointer(PF), pointer(common), pointer(xhat), pointer(xvar),
+                        Base.unsafe_convert(Ptr{Cdouble}, ll), Base.unsafe_convert(Ptr{Cint}, st)))
+        check(ccall((:dfm_kalman_smooth, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ref{SsOpts}, Ref{EmInit}, Ref{SsOut}), h, Xs, opts, init, out),
+              "dfm_kalman_smooth")
+    end
+    return (F = F, PF = PF, common = common, xhat = xhat, xvar = xvar, loglik = ll[], status = st[])
+end
+
 end # module
