@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <new>
 #include <thread>
+#include <type_traits>
 #include <vector>
 #ifndef DFM_EMU
 #include <dlfcn.h>
@@ -187,25 +188,51 @@ static int make_panel_tmap(dfm_handle* h, const double* X, int T, long long rows
 #endif
 }
 
-template <int RT>
-static int launch_fused(dfm_handle* h, const FusedArgs& fa, int B, int T, int N, double** scratch_out, Arena* arena, bool dry) {
-  size_t smem = fused_smem_doubles<RT>(T, N) * 8;
-  int grid = B;
-#ifndef DFM_EMU
-  if (!dry) {
-    DFM_SET_SMEM(k_em_fused<RT>, smem);
-    int occ = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_em_fused<RT>, 128, smem);
-    if (occ < 1) occ = 1;
-    grid = std::min(B, h->nsm * occ);
-  } else grid = std::min(B, h->nsm * 8);
+// f(std::integral_constant<int, V>{}) for the run-time value v = V in [Lo, Hi]: the one place where a run-time size
+// (r for the fused kernels, the column-block count for the contraction kernels) picks a kernel template.  The
+// callers have checked the range; a value outside it takes Hi.
+template <int Lo, int Hi, typename F>
+static auto dispatch(int v, F&& f) {
+  if constexpr (Lo == Hi) return f(std::integral_constant<int, Lo>{});
+  else {
+    if (v == Lo) return f(std::integral_constant<int, Lo>{});
+    return dispatch<Lo + 1, Hi>(v, f);
+  }
+}
+
+// Grid of a persistent kernel that loops over the B panels: as many CTAs as are resident on the device at once.  The
+// fused kernels' scratch has one row per CTA for min(B, nsm * 8) CTAs, which bounds the emulation build's grid too.
+template <typename K>
+static int resident_grid(const dfm_handle* h, K kern, int threads, size_t smem, int B) {
+#ifdef DFM_EMU
+  (void)kern; (void)threads; (void)smem;
+  return std::min(B, h->nsm * 8);
+#else
+  DFM_SET_SMEM(kern, smem);
+  int occ = 1;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
+  if (occ < 1) occ = 1;
+  return std::min(B, h->nsm * occ);
 #endif
-  double* scr = arena->get<double>((size_t)std::min(B, h->nsm * 8) * T * FUSED_SCR(RT));
-  if (dry) return DFM_OK;
-  FusedArgs a2 = fa; a2.scratch = scr;
-  L(k_em_fused<RT>, grid, 1, 128, smem, a2);
-  (void)scratch_out;
-  return DFM_OK;
+}
+
+// One launch of the fused EM kernel over all panels of fa (fa.scratch: min(B, nsm * 8) * T * FUSED_SCR(r) doubles):
+// k_em_fused2 (TMA panel ring, even T) when use2, else k_em_fused.
+static int launch_em_fused(dfm_handle* h, const FusedArgs& fa, int r, bool use2) {
+  return dispatch<1, 8>(r, [&](auto R) -> int {
+    constexpr int RT = decltype(R)::value;
+    if (use2) {
+      const size_t smem = fused2_smem_doubles<RT>(fa.T, fa.N) * 8;
+      const int grid = resident_grid(h, k_em_fused2<RT>, 256, smem, fa.B);
+      CUtensorMap tm; int rc = make_panel_tmap(h, fa.X, fa.T, (long long)fa.B * fa.N, &tm); if (rc) return rc;
+      L(k_em_fused2<RT>, grid, 1, 256, smem, fa, tm);
+    } else {
+      const size_t smem = fused_smem_doubles<RT>(fa.T, fa.N) * 8;
+      const int grid = resident_grid(h, k_em_fused<RT>, 128, smem, fa.B);
+      L(k_em_fused<RT>, grid, 1, 128, smem, fa);
+    }
+    return DFM_OK;
+  });
 }
 
 // Multi-CTA contraction kernels of the general path for balanced panels (dfm_kernels_emb.cuh): split factors and buffers.
@@ -235,21 +262,66 @@ static EmbPlan emb_plan(int T, int N, int r, int batch, int nsm) {
   e.smM = ((size_t)2 * r * r + (size_t)2 * EMB_TILE * (r + 1) + 96) * 8;
   return e;
 }
-template <int NCB>
-static int emb_launch_E(dfm_handle* h, const EmbPlan& e, const double* x, const double* dW, const double* dR, const double* dlogR, int T, int N,
-                        int r, int batch, double* dBt, double* dqt, double* dslr, int* dnt, EmState* st) {
-  DFM_SET_SMEM(k_emb_contract<NCB>, e.smE);
-  L(k_emb_contract<NCB>, e.ntE, e.nsE * batch, 256, e.smE, x, dW, dR, dlogR, T, N, r, e.nsE, e.nper, batch, e.Bpart, e.qpart, e.counters,
-    dBt, dqt, dslr, dnt, st);
-  return DFM_OK;
+static void emb_launch_E(dfm_handle* h, const EmbPlan& e, const double* x, const double* dW, const double* dR, const double* dlogR, int T, int N,
+                         int r, int batch, double* dBt, double* dqt, double* dslr, int* dnt, EmState* st) {
+  dispatch<1, 4>(e.ncb, [&](auto C) {
+    constexpr int NCB = decltype(C)::value;
+    DFM_SET_SMEM(k_emb_contract<NCB>, e.smE);
+    L(k_emb_contract<NCB>, e.ntE, e.nsE * batch, 256, e.smE, x, dW, dR, dlogR, T, N, r, e.nsE, e.nper, batch, e.Bpart, e.qpart, e.counters,
+      dBt, dqt, dslr, dnt, st);
+  });
 }
-template <int NCB>
-static int emb_launch_M(dfm_handle* h, const EmbPlan& e, const double* x, const double* dFs, const double* dSff, int T, int N, int r, int batch,
-                        double* dL, double* dR, double* dW, double* dlogR, EmState* st) {
-  DFM_SET_SMEM(k_emb_mstep<NCB>, e.smM);
-  L(k_emb_mstep<NCB>, e.ntM, e.tsM * batch, 256, e.smM, x, dFs, dSff, T, N, r, e.tsM, e.tper, batch, e.Spart, e.sxxpart,
-    e.counters + (size_t)batch * e.ntE, dL, dR, dW, dlogR, e.Cpart, st);
-  return DFM_OK;
+static void emb_launch_M(dfm_handle* h, const EmbPlan& e, const double* x, const double* dFs, const double* dSff, int T, int N, int r, int batch,
+                         double* dL, double* dR, double* dW, double* dlogR, EmState* st) {
+  dispatch<1, 4>(e.ncb, [&](auto C) {
+    constexpr int NCB = decltype(C)::value;
+    DFM_SET_SMEM(k_emb_mstep<NCB>, e.smM);
+    L(k_emb_mstep<NCB>, e.ntM, e.tsM * batch, 256, e.smM, x, dFs, dSff, T, N, r, e.tsM, e.tper, batch, e.Spart, e.sxxpart,
+      e.counters + (size_t)batch * e.ntE, dL, dR, dW, dlogR, e.Cpart, st);
+  });
+}
+
+// Device scratch of the general EM path for B panels of T periods.  dfm_em_kalman and dfm_kalman_smooth (on the panels
+// padded to T + H periods) allocate it with gen_bufs; the multi-CTA contraction partials only when emb.on.
+struct GenBufs {
+  double *An, *Qn, *W, *logR, *C, *Bt, *qt, *slr;
+  int* nt;                                        // [2][B][T]: n_t, then src_t of the frozen-step logic
+  double *Ct, *zp, *zf, *Pp, *Pf, *Sff;
+  double* xch;                                    // cluster exchange (scalars, boundary states, Gram partials)
+  EmbPlan emb;
+};
+static GenBufs gen_bufs(Arena& a, const EmbPlan& emb, size_t B, int T, int N, int r, int p) {
+  const size_t k = (size_t)r * p, kk = k * k, rr = (size_t)r * r, rk = r * k, np = (size_t)r * (r + 1) / 2;
+  GenBufs g;
+  g.An = a.get<double>(B * rk); g.Qn = a.get<double>(B * rr); g.W = a.get<double>(B * N * r); g.logR = a.get<double>(B * N);
+  g.C = a.get<double>(B * rr); g.Bt = a.get<double>(B * T * r); g.qt = a.get<double>(B * T); g.slr = a.get<double>(B * T);
+  g.nt = a.get<int>(2 * B * T); g.Ct = a.get<double>(B * T * np); g.zp = a.get<double>(B * T * k); g.zf = a.get<double>(B * T * k);
+  g.Pp = a.get<double>(B * T * kk); g.Pf = a.get<double>(B * T * kk); g.Sff = a.get<double>(B * rr);
+  g.xch = a.get<double>(B * (16 + 64 * k + 16 * (kk + rk)));
+  g.emb = emb;
+  if (emb.on) {
+    g.emb.Bpart = a.get<double>((size_t)emb.nsE * B * T * r); g.emb.qpart = a.get<double>((size_t)emb.nsE * B * T);
+    g.emb.Spart = a.get<double>((size_t)emb.tsM * B * N * r); g.emb.sxxpart = a.get<double>((size_t)emb.tsM * B * N);
+    g.emb.Cpart = a.get<double>(B * emb.ntM * rr); g.emb.counters = a.get<int>(B * (size_t)(emb.ntE + emb.ntM));
+  }
+  return g;
+}
+
+// Device buffers of one dfm_em_kalman call that its fused and general paths share: the uploaded panels (host input
+// only), the parameters updated in place, the results, and the fused kernels' scratch.
+struct EmBufs {
+  double *X, *L, *R, *A, *Q, *P0, *Fs, *PsF, *ll, *PF;
+  EmState* st;
+  int *it, *stat, *active, *flag;
+  int* ready;                                     // streaming host path: one "landed" flag per chunk of panels
+  double* scratch;                                // fused kernels: min(B, nsm * 8) * T * FUSED_SCR(r) doubles
+};
+static FusedArgs fused_args(const EmBufs& d, const dfm_em_opts* o, const double* x) {
+  FusedArgs fa{};
+  fa.X = x; fa.Lam = d.L; fa.R = d.R; fa.A = d.A; fa.Q = d.Q; fa.P0 = d.P0; fa.Fs = d.Fs; fa.PsF = d.PsF; fa.loglik = d.ll;
+  fa.iters = d.it; fa.status = d.stat; fa.scratch = d.scratch; fa.B = o->batch; fa.T = o->T; fa.N = o->N; fa.max_iter = o->max_iter;
+  fa.tol = o->tol;
+  return fa;
 }
 
 // Staging tile (periods) of the frozen-run phases of k_em_filter_smooth: few panels -> large tiles (one CTA per SM
@@ -271,12 +343,14 @@ static int fs_cluster_size(const dfm_handle* h, int batch, const double* dxch) {
   return ncl;
 }
 
-// One launch of k_em_filter_smooth over the batch; a cluster per panel when ncl > 1 (set to 1 if the cluster cannot be placed).
-static int launch_filter_smooth(dfm_handle* h, int& ncl, int batch, int ntFS, size_t smFS, const double* dA, const double* dQ,
-                                const double* dP0, const double* dC, const double* dBt, const double* dqt, const double* dslr, const int* dnt,
-                                const double* dCt, int T, int r, int p, double* dzp, double* dzf, double* dPp, double* dPf, double* dFs,
-                                double* dPsF, double* dSff, double* dAn, double* dQn, double* dll, int mi, double tol, EmState* st, int* dsrc,
-                                int stgT, int want_psf, double* dxch) {
+// One launch of k_em_filter_smooth over the batch (T periods in g); a cluster per panel when ncl > 1 (set to 1 if the
+// cluster cannot be placed).  A, Q, mi, tol and want_psf are the caller's: the EM loop's, or one E-step at fixed parameters.
+static int launch_filter_smooth(dfm_handle* h, int& ncl, const GenBufs& g, int batch, int T, int r, int p, const double* dA, const double* dQ,
+                                const double* dP0, double* dFs, double* dPsF, double* dll, EmState* st, int mi, double tol, int want_psf) {
+  const int stgT = fs_stage_periods(h->nsm, batch, r, p);
+  const size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
+  const int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;     // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
+  int* dsrc = g.nt + (size_t)batch * T;
 #ifndef DFM_EMU
   if (ncl > 1) {
     // few panels: a thread-block cluster per panel (the CTAs split the parallel phases of the frozen runs)
@@ -286,47 +360,38 @@ static int launch_filter_smooth(dfm_handle* h, int& ncl, int batch, int ntFS, si
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)ncl; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    cudaError_t ce = cudaLaunchKernelEx(&cfg, k_em_filter_smooth, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf,
-                          dPp, dPf, dFs, dPsF, dSff, dAn, dQn, dll, mi, tol, st, dsrc, stgT, want_psf, dxch);
+    cudaError_t ce = cudaLaunchKernelEx(&cfg, k_em_filter_smooth, dA, dQ, dP0, g.C, g.Bt, g.qt, g.slr, g.nt, g.Ct, T, r, p, g.zp, g.zf,
+                                        g.Pp, g.Pf, dFs, dPsF, g.Sff, g.An, g.Qn, dll, mi, tol, st, dsrc, stgT, want_psf, g.xch);
     PROF_END(); h->launches++;
-    if (ce != cudaSuccess) {                       // the cluster could not be placed: run the plain one-CTA-per-panel launch instead
-      (void)cudaGetLastError();
-      ncl = 1;
-      L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf,
-        dFs, dPsF, dSff, dAn, dQn, dll, mi, tol, st, dsrc, stgT, want_psf, (double*)nullptr);
-    }
-    return DFM_OK;
+    if (ce == cudaSuccess) return DFM_OK;
+    (void)cudaGetLastError();                      // the cluster could not be placed: run the plain one-CTA-per-panel launch instead
+    ncl = 1;
   }
-#else
-  (void)dxch;
 #endif
-  L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf,
-    dFs, dPsF, dSff, dAn, dQn, dll, mi, tol, st, dsrc, stgT, want_psf, (double*)nullptr);
+  L(k_em_filter_smooth, batch, 1, ntFS, smFS, dA, dQ, dP0, g.C, g.Bt, g.qt, g.slr, g.nt, g.Ct, T, r, p, g.zp, g.zf, g.Pp, g.Pf,
+    dFs, dPsF, g.Sff, g.An, g.Qn, dll, mi, tol, st, dsrc, stgT, want_psf, (double*)nullptr);
   return DFM_OK;
 }
 
 // General multi-kernel EM path on device-resident data (any r, p, missing data).
-static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, double* dL, double* dR, double* dA, double* dQ, double* dP0,
-                          double* dAn, double* dQn, double* dW, double* dlogR, double* dC, double* dBt, double* dqt, double* dslr, int* dnt,
-                          double* dCt, double* dzp, double* dzf, double* dPp, double* dPf, double* dFs, double* dPsF, double* dSff, double* dll,
-                          EmState* st, int* dit, int* dstat, int* active, int ntC, int nblkC, size_t smFS, int stgT, int want_psf, double* dxch, const EmbPlan& emb) {
-  int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mi = o->max_iter;
-  int np = r * (r + 1) / 2;
-  int* dsrc = dnt + (size_t)batch * T;
-  const int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;     // few panels: more warps for the parallel frozen runs; many: two CTAs per SM
-  int ncl = fs_cluster_size(h, batch, dxch);
-  L(k_em_state_init, batch, 1, 1, 0, st);
-  L(k_em_scan, N, batch, 64, 0, x, dL, T, N, r, st);
-  L(k_em_prep, batch, 1, 128, 0, dL, dR, N, r, p, dW, dlogR, dC, dA, dAn, dQ, dQn, st, mi, 0, emb.on ? 1 : 0);
+static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, const EmBufs& d, const GenBufs& g, int want_psf) {
+  const int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mi = o->max_iter;
+  const int np = r * (r + 1) / 2;
+  const int ntC = tpt_threads(np + r), nblkC = (T + ntC - 1) / ntC;
+  const EmbPlan& emb = g.emb;
+  int ncl = fs_cluster_size(h, batch, g.xch);
+  L(k_em_state_init, batch, 1, 1, 0, d.st);
+  L(k_em_scan, N, batch, 64, 0, x, d.L, T, N, r, d.st);
+  L(k_em_prep, batch, 1, 128, 0, d.L, d.R, N, r, p, g.W, g.logR, g.C, d.A, g.An, d.Q, g.Qn, d.st, mi, 0, emb.on ? 1 : 0);
   if (emb.on) {
-    L(k_emb_cinit, emb.ntM, batch, 256, 0, dL, dW, N, r, emb.Cpart, st);
-    L(k_emb_close, batch, 1, 256, 0, N, r, p, emb.ntM, emb.Cpart, dC, dA, dAn, dQ, dQn, st, mi, 0);
+    L(k_emb_cinit, emb.ntM, batch, 256, 0, d.L, g.W, N, r, emb.Cpart, d.st);
+    L(k_emb_close, batch, 1, 256, 0, N, r, p, emb.ntM, emb.Cpart, g.C, d.A, g.An, d.Q, g.Qn, d.st, mi, 0);
   }
   // how many panels have missing data?  (decides which contraction kernels are launched at all: one sync, before the loop)
   int n_missing = batch;
   if (emb.on) {
-    L(k_em_count_missing, 1, 1, 128, 48 * 8, st, batch, active);
-    CK(cudaMemcpyAsync(&n_missing, active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    L(k_em_count_missing, 1, 1, 128, 48 * 8, d.st, batch, d.active);
+    CK(cudaMemcpyAsync(&n_missing, d.active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     CK(cudaMemsetAsync(emb.counters, 0, sizeof(int) * (size_t)batch * (emb.ntE + emb.ntM), h->stream));
   }
@@ -334,86 +399,45 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
   const int emb_on = emb.on ? 1 : 0;
   int h_active = batch;
   for (int it = 0; it < mi && h_active > 0; ++it) {
-    if (any_missing) L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, dL, dW, dR, dlogR, dC, T, N, r, dBt, dqt, dslr, dnt, dCt, st);
+    if (any_missing) L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, d.L, g.W, d.R, g.logR, g.C, T, N, r, g.Bt, g.qt, g.slr, g.nt, g.Ct, d.st);
     if (any_bal) {                                                          // (each returns at once for panels of the other kind)
-      if (!emb.on) L(k_em_contract_bal, (T + 31) / 32, batch, 256, 8 * 32 * 3 * 8, x, dW, dR, dlogR, T, N, r, dBt, dqt, dslr, dnt, st);
-      else switch (emb.ncb) {
-        case 1: emb_launch_E<1>(h, emb, x, dW, dR, dlogR, T, N, r, batch, dBt, dqt, dslr, dnt, st); break;
-        case 2: emb_launch_E<2>(h, emb, x, dW, dR, dlogR, T, N, r, batch, dBt, dqt, dslr, dnt, st); break;
-        case 3: emb_launch_E<3>(h, emb, x, dW, dR, dlogR, T, N, r, batch, dBt, dqt, dslr, dnt, st); break;
-        default: emb_launch_E<4>(h, emb, x, dW, dR, dlogR, T, N, r, batch, dBt, dqt, dslr, dnt, st); break;
-      }
+      if (!emb.on) L(k_em_contract_bal, (T + 31) / 32, batch, 256, 8 * 32 * 3 * 8, x, g.W, d.R, g.logR, T, N, r, g.Bt, g.qt, g.slr, g.nt, d.st);
+      else emb_launch_E(h, emb, x, g.W, d.R, g.logR, T, N, r, batch, g.Bt, g.qt, g.slr, g.nt, d.st);
     }
-    launch_filter_smooth(h, ncl, batch, ntFS, smFS, dA, dQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, T, r, p, dzp, dzf, dPp, dPf, dFs, dPsF, dSff,
-                         dAn, dQn, dll, mi, o->tol, st, dsrc, stgT, want_psf, dxch);
-    if (any_missing || !emb.on) L(k_em_mstep_series, N, batch, 64, (size_t)(2 * np + r + 8) * 8, x, dFs, dPsF, dSff, T, N, r, dL, dR, st, emb_on);
+    launch_filter_smooth(h, ncl, g, batch, T, r, p, d.A, d.Q, d.P0, d.Fs, d.PsF, d.ll, d.st, mi, o->tol, want_psf);
+    if (any_missing || !emb.on) L(k_em_mstep_series, N, batch, 64, (size_t)(2 * np + r + 8) * 8, x, d.Fs, d.PsF, g.Sff, T, N, r, d.L, d.R, d.st, emb_on);
     if (any_bal && emb.on) {
-      switch (emb.ncb) {
-        case 1: emb_launch_M<1>(h, emb, x, dFs, dSff, T, N, r, batch, dL, dR, dW, dlogR, st); break;
-        case 2: emb_launch_M<2>(h, emb, x, dFs, dSff, T, N, r, batch, dL, dR, dW, dlogR, st); break;
-        case 3: emb_launch_M<3>(h, emb, x, dFs, dSff, T, N, r, batch, dL, dR, dW, dlogR, st); break;
-        default: emb_launch_M<4>(h, emb, x, dFs, dSff, T, N, r, batch, dL, dR, dW, dlogR, st); break;
-      }
-      L(k_emb_close, batch, 1, 256, 0, N, r, p, emb.ntM, emb.Cpart, dC, dA, dAn, dQ, dQn, st, mi, 1);
+      emb_launch_M(h, emb, x, d.Fs, g.Sff, T, N, r, batch, d.L, d.R, g.W, g.logR, d.st);
+      L(k_emb_close, batch, 1, 256, 0, N, r, p, emb.ntM, emb.Cpart, g.C, d.A, g.An, d.Q, g.Qn, d.st, mi, 1);
     }
-    if (any_missing || !emb.on) L(k_em_prep, batch, 1, 128, 0, dL, dR, N, r, p, dW, dlogR, dC, dA, dAn, dQ, dQn, st, mi, 1, emb_on);
+    if (any_missing || !emb.on) L(k_em_prep, batch, 1, 128, 0, d.L, d.R, N, r, p, g.W, g.logR, g.C, d.A, g.An, d.Q, g.Qn, d.st, mi, 1, emb_on);
     if (o->tol > 0 && ((it & 3) == 3)) {
-      L(k_em_count_active, 1, 1, 128, 48 * 8, st, batch, active);
-      CK(cudaMemcpyAsync(&h_active, active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+      L(k_em_count_active, 1, 1, 128, 48 * 8, d.st, batch, d.active);
+      CK(cudaMemcpyAsync(&h_active, d.active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
       CK(cudaStreamSynchronize(h->stream));
     }
   }
-  L(k_em_collect, batch, 1, 1, 0, st, dit, dstat);
+  L(k_em_collect, batch, 1, 1, 0, d.st, d.it, d.stat);
   return DFM_OK;
 }
 
-template <int RT>
-static int launch_fused2(dfm_handle* h, const FusedArgs& fa, int B, int T, int N, Arena* arena, bool dry) {
-  size_t smem = fused2_smem_doubles<RT>(T, N) * 8;
-  int grid = std::min(B, h->nsm * 8);
-  double* scr = arena->get<double>((size_t)std::min(B, h->nsm * 8) * T * FUSED_SCR(RT));
-  if (dry) return DFM_OK;
-#ifndef DFM_EMU
-  DFM_SET_SMEM(k_em_fused2<RT>, smem);
-  int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_em_fused2<RT>, 256, smem);
-  if (occ < 1) occ = 1;
-  grid = std::min(B, h->nsm * occ);
-#endif
-  FusedArgs a2 = fa; a2.scratch = scr;
-  CUtensorMap tm; int rc_ = make_panel_tmap(h, fa.X, T, (long long)B * N, &tm); if (rc_) return rc_;
-  L(k_em_fused2<RT>, grid, 1, 256, smem, a2, tm);
-  return DFM_OK;
+static int launch_als_fused2(dfm_handle* h, const AlsFusedArgs& fa, int r) {
+  return dispatch<1, 8>(r, [&](auto R) -> int {
+    constexpr int RT = decltype(R)::value;
+    const size_t smem = als_fused2_smem_doubles<RT>(fa.T, fa.N) * 8;
+    const int grid = resident_grid(h, k_als_fused2<RT>, 256, smem, fa.B);
+    CUtensorMap tm; int rc = make_panel_tmap(h, fa.Xs, fa.T, (long long)fa.B * fa.N, &tm); if (rc) return rc;
+    L(k_als_fused2<RT>, grid, 1, 256, smem, fa, tm);
+    return DFM_OK;
+  });
 }
-
-template <int RT>
-static int launch_als_fused2(dfm_handle* h, const AlsFusedArgs& fa, int B, int T, int N) {
-  size_t smem = als_fused2_smem_doubles<RT>(T, N) * 8;
-  int grid = std::min(B, h->nsm * 8);
-#ifndef DFM_EMU
-  DFM_SET_SMEM(k_als_fused2<RT>, smem);
-  int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_als_fused2<RT>, 256, smem);
-  if (occ < 1) occ = 1;
-  grid = std::min(B, h->nsm * occ);
-#endif
-  CUtensorMap tm; int rc_ = make_panel_tmap(h, fa.Xs, T, (long long)B * N, &tm); if (rc_) return rc_;
-  L(k_als_fused2<RT>, grid, 1, 256, smem, fa, tm);
-  return DFM_OK;
-}
-template <int RT>
-static int launch_als_masked(dfm_handle* h, const AlsMaskedArgs& fa, int B, int T, int N) {
-  size_t smem = als_masked_smem_doubles<RT>(T, N) * 8;
-  int grid = std::min(B, h->nsm * 2);
-#ifndef DFM_EMU
-  DFM_SET_SMEM(k_als_masked<RT>, smem);
-  int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_als_masked<RT>, 256, smem);
-  if (occ < 1) occ = 1;
-  grid = std::min(B, h->nsm * occ);
-#endif
-  L(k_als_masked<RT>, grid, 1, 256, smem, fa);
-  return DFM_OK;
+static void launch_als_masked(dfm_handle* h, const AlsMaskedArgs& fa, int r) {
+  dispatch<1, 8>(r, [&](auto R) {
+    constexpr int RT = decltype(R)::value;
+    const size_t smem = als_masked_smem_doubles<RT>(fa.T, fa.N) * 8;
+    const int grid = resident_grid(h, k_als_masked<RT>, 256, smem, fa.B);
+    L(k_als_masked<RT>, grid, 1, 256, smem, fa);
+  });
 }
 static bool als_masked_shape_ok(int T, int N, int r) {
   if (r < 1 || r > 8) return false;
@@ -423,27 +447,6 @@ static bool als_fused2_shape_ok(int T, int N, int r) {
   if (r < 1 || r > 8 || T < 4 || (T & 1)) return false;
   return ((size_t)FZ * pad4mod16(T) + (size_t)r * pad4mod16(N) + (size_t)N + 4 * (size_t)r * r + 2 * r + 48 +
           2 * F2_NCW * 72 + (size_t)F2_S * F2_STG + 32) * 8 <= 113 * 1024;
-}
-
-// resident CTAs (= panels processed concurrently) of the TMA fused EM kernel
-template <int RT> static int fused2_capacity_t(int nsm, int T, int N) {
-#ifdef DFM_EMU
-  (void)nsm; (void)T; (void)N; return 4;
-#else
-  size_t smem = fused2_smem_doubles<RT>(T, N) * 8;
-  DFM_SET_SMEM(k_em_fused2<RT>, smem);
-  int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_em_fused2<RT>, 256, smem);
-  return nsm * (occ < 1 ? 1 : occ);
-#endif
-}
-static int fused2_capacity(int nsm, int r, int T, int N) {
-  switch (r) {
-#define DFM_CASEC(RT) case RT: return fused2_capacity_t<RT>(nsm, T, N);
-    DFM_CASEC(1) DFM_CASEC(2) DFM_CASEC(3) DFM_CASEC(4) DFM_CASEC(5) DFM_CASEC(6) DFM_CASEC(7) DFM_CASEC(8)
-#undef DFM_CASEC
-  }
-  return 1;
 }
 
 static bool fused2_shape_ok(int T, int N, int r, int p) {
@@ -457,6 +460,143 @@ static bool fused_shape_ok(int T, int N, int r, int p) {
   if (p != 1 || r < 1 || r > 8 || T < 3) return false;
   return ((size_t)FZ * pad4mod16(T) + (size_t)r * pad4mod16(N) + 3 * (size_t)N + 31 * (size_t)r * r + 66 * (size_t)r + 128) * 8 <= kMaxSmem;
 }
+
+#ifndef DFM_EMU
+// ---------------------------------------------------------------- streaming host path of dfm_em_kalman
+// Host buffers + TMA fused kernel + more panels than are resident at once: ONE launch of the EM kernel, started
+// before the data is on the device.  The copy stream uploads the batch in chunks of panels (X and the initial
+// parameters), each chunk followed by a 4-byte copy that sets its "landed" flag; a CTA spins on the flag of the
+// panel it is about to start (ld.acquire.sys) -- the copy engine is in order, so the flag implies the data.  The
+// upload (PCIe) runs under the kernel (HBM-bound, slower than the link), P0 and the log-likelihood
+// pre-fill are done inside the kernel (no other kernel can become resident next to it), and the balance check
+// is deferred: a panel with NaNs ends with status 3, which triggers the scan + general-path fallback.
+// (Not under a CUDA injection profiler or CUDA_LAUNCH_BLOCKING=1: launches are synchronous there, so a kernel that waits for copies
+//  enqueued after its launch would never finish.  DFM_NO_PIPELINE=1 forces the upload-then-compute path too.)
+static bool em_streaming_applies(const dfm_handle* h, const dfm_em_opts* o) {
+  const char* clb = getenv("CUDA_LAUNCH_BLOCKING");
+  const char* cdmc = getenv("CUDA_DEVICE_MAX_CONNECTIONS");
+  // ... nor with CUDA_DEVICE_MAX_CONNECTIONS=1 (common in torch.distributed set-ups): all streams then share one hardware
+  // queue, so the uploads could be queued BEHIND the kernel that waits for them.
+  const bool profiler = getenv("CUDA_INJECTION64_PATH") || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") || (clb && clb[0] == '1') ||
+                        (cdmc && atoi(cdmc) == 1);
+  if (getenv("DFM_NO_PIPELINE") || profiler) return false;
+  const int resident = dispatch<1, 8>(o->r, [&](auto R) {
+    constexpr int RT = decltype(R)::value;
+    return resident_grid(h, k_em_fused2<RT>, 256, fused2_smem_doubles<RT>(o->T, o->N) * 8, o->batch);
+  });
+  return resident < o->batch;
+}
+
+// The whole dfm_em_kalman call on the streaming host path.  Returns an error code, or DFM_OK with *fallback = false
+// when the results are in `out`, or DFM_OK with *fallback = true when some panel has missing data: the panels are on
+// the device then (d.X), the parameters have to be staged again, and the general path has to run on the whole batch.
+static int em_streaming(dfm_handle* h, const double* X, const dfm_em_opts* o, const dfm_em_init* init, const dfm_em_out* out,
+                        const EmBufs& d, bool* fallback) {
+  const int T = o->T, N = o->N, r = o->r, batch = o->batch, mi = o->max_iter;
+  const size_t B = batch, TN = (size_t)T * N; const int k = r * o->p, kk = k * k, rr = r * r, rk = r * k;
+  *fallback = false;
+  int chunk = 32;                                              // ~25 MB of C2-shaped panels: the first CTAs start early
+  while ((batch + chunk - 1) / chunk > kMaxReadyChunks) chunk *= 2;
+  const int nch = (batch + chunk - 1) / chunk;
+  cudaStream_t cs = h->copy_stream;
+  cudaEvent_t ev0 = nullptr, ev_k = nullptr;
+  CK(cudaEventCreateWithFlags(&ev0, cudaEventDisableTiming));
+  { cudaError_t e_ = cudaEventCreateWithFlags(&ev_k, cudaEventDisableTiming); if (e_ != cudaSuccess) { cudaEventDestroy(ev0); CK(e_); } }
+#define CKE(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { cudaEventDestroy(ev0); cudaEventDestroy(ev_k); CK(e_); } } while (0)
+  // the workspace is shared with whatever the previous call on this handle left in flight on h->stream (a
+  // DFM_MEM_DEVICE call returns before completion): the copy stream must not touch it before that work is done
+  CKE(cudaEventRecord(ev_k, h->stream));
+  CKE(cudaStreamWaitEvent(cs, ev_k, 0));
+  CKE(cudaStreamWaitEvent(h->d2h_stream, ev_k, 0));
+  CKE(cudaMemsetAsync(d.ready, 0, (size_t)nch * sizeof(int), cs));
+  CKE(cudaEventRecord(ev0, cs));
+  CKE(cudaStreamWaitEvent(h->stream, ev0, 0));                   // flags are zero before the kernel can read them
+  FusedArgs fa = fused_args(d, o, d.X);
+  fa.ready = d.ready; fa.ready_chunk = chunk;
+  if (h->done_cap < B) {                                        // completion flags the kernel writes straight into host memory
+    if (h->done_host) cudaFreeHost(h->done_host);
+    h->done_host = nullptr; h->done_cap = 0;
+    CKE(cudaHostAlloc((void**)&h->done_host, B * sizeof(int), cudaHostAllocMapped));
+    CKE(cudaHostGetDevicePointer((void**)&h->done_dev, h->done_host, 0));
+    h->done_cap = B;
+  }
+#undef CKE
+  memset(h->done_host, 0, B * sizeof(int));
+  fa.done = h->done_dev;
+  fa.P0out = init->P0 ? nullptr : d.P0; fa.p0_steps = 12;        // P0 in the kernel unless the caller gave one (the loglik rows are pre-filled there too)
+  int rc = launch_em_fused(h, fa, r, true);
+  if (rc) { cudaEventDestroy(ev0); cudaEventDestroy(ev_k); return rc; }
+  cudaError_t up = cudaSuccess;                                  // first failure while enqueueing the upload
+  for (int c = 0; c < nch && up == cudaSuccess; ++c) {
+    size_t b0 = (size_t)c * chunk, bc = std::min<size_t>(chunk, B - b0);
+#define DFM_UP(dst, src, n_) do { if (up == cudaSuccess) up = cudaMemcpyAsync((dst), (src), (size_t)(n_) * 8, cudaMemcpyHostToDevice, cs); } while (0)
+    DFM_UP(d.X + b0 * TN, X + b0 * TN, bc * TN); DFM_UP(d.L + b0 * N * r, init->Lam + b0 * N * r, bc * N * r);
+    DFM_UP(d.R + b0 * N, init->R + b0 * N, bc * N); DFM_UP(d.A + b0 * rk, init->A + b0 * rk, bc * rk); DFM_UP(d.Q + b0 * rr, init->Q + b0 * rr, bc * rr);
+    if (init->P0) DFM_UP(d.P0 + b0 * kk, init->P0 + b0 * kk, bc * kk);
+#undef DFM_UP
+    if (up == cudaSuccess) up = cudaMemcpyAsync(d.ready + c, h->pinned_one, sizeof(int), cudaMemcpyHostToDevice, cs);
+  }
+  if (up != cudaSuccess) {
+    // an upload could not be enqueued: the kernel is already running and would wait for its flags for ever ->
+    // raise every flag (the CTAs then run on whatever is in the buffers), drain, report the error
+    cudaMemsetAsync(d.ready, 1, (size_t)nch * sizeof(int), cs);
+    cudaStreamSynchronize(cs); cudaStreamSynchronize(h->stream);
+    cudaEventDestroy(ev0); cudaEventDestroy(ev_k);
+    (void)cudaGetLastError();
+    snprintf(h->err, sizeof(h->err), "dfm_em_kalman: host-to-device upload failed (%s)", cudaGetErrorString(up));
+    return DFM_ERR_CUDA;
+  }
+  // results of finished panels go back on a third stream while the kernel is still running: the host polls the
+  // completion flags and ships whole chunks of 128 panels in order (everything except the unpacked PF, which
+  // needs a kernel of its own after the EM kernel)
+  {
+    const size_t dch = 128;
+    volatile const int* dn = h->done_host;
+    size_t next = 0; bool kernel_done = false;
+    auto ship = [&](size_t b0, size_t b1) {
+      const size_t nb = b1 - b0;
+#define DFM_OUTS(dst, src, per) if (dst) cudaMemcpyAsync((dst) + b0 * (per), (src) + b0 * (per), nb * (per) * sizeof(*(src)), cudaMemcpyDeviceToHost, h->d2h_stream)
+      DFM_OUTS(out->F, d.Fs, (size_t)T * r); DFM_OUTS(out->Lam, d.L, (size_t)N * r); DFM_OUTS(out->R, d.R, (size_t)N); DFM_OUTS(out->A, d.A, (size_t)rk);
+      DFM_OUTS(out->Q, d.Q, (size_t)rr); DFM_OUTS(out->P0, d.P0, (size_t)kk); DFM_OUTS(out->loglik, d.ll, (size_t)mi);
+      DFM_OUTS(out->iters, d.it, (size_t)1); DFM_OUTS(out->status, d.stat, (size_t)1);
+#undef DFM_OUTS
+    };
+    while (next < B) {
+      size_t b1 = std::min<size_t>(B, next + dch);
+      bool all = true;
+      if (!kernel_done) for (size_t bb = next; bb < b1; ++bb) if (!dn[bb]) { all = false; break; }
+      if (all) { ship(next, b1); next = b1; continue; }
+      cudaError_t q = cudaStreamQuery(h->stream);
+      if (q != cudaErrorNotReady) kernel_done = true;            // finished (or failed: reported by the synchronize below)
+      else std::this_thread::yield();
+    }
+  }
+  if (out->PF) {
+    long long n = (long long)T * rr;
+    L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, d.PsF, T, r, d.PF);
+    cudaMemcpyAsync(out->PF, d.PF, B * T * rr * sizeof(double), cudaMemcpyDeviceToHost, h->stream);
+  }
+  std::vector<int> hstat(B);
+  CK(cudaMemcpyAsync(hstat.data(), d.stat, B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  cudaEventRecord(ev_k, h->stream);
+  cudaStreamSynchronize(h->d2h_stream);
+  cudaError_t e1 = cudaStreamSynchronize(cs), e2 = cudaStreamSynchronize(h->stream);
+  cudaEventDestroy(ev0); cudaEventDestroy(ev_k);
+  if (e1 != cudaSuccess || e2 != cudaSuccess) CK(e1 != cudaSuccess ? e1 : e2);
+  bool failed = false;
+  for (size_t bb = 0; bb < B; ++bb) failed = failed || hstat[bb] == 3;
+  if (failed) {                                                // NaN log-likelihood somewhere: missing data or a numerical failure?
+    CK(cudaMemsetAsync(d.flag, 0, sizeof(int), h->stream));
+    L(k_em_scan_fused, N, batch, 64, 0, d.X, d.L, d.R, T, N, r, d.flag);      // (X only matters: Lam/R of failed panels are NaN anyway)
+    int hflag = 0;
+    CK(cudaMemcpyAsync(&hflag, d.flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    *fallback = hflag != 0;
+  }
+  if (!*fallback) CK(cudaGetLastError());
+  return DFM_OK;
+}
+#endif
 
 extern "C" {
 
@@ -700,12 +840,7 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
       for (size_t b = 0; b < B; ++b) if (hs[b].nobs != (long long)T * N || hs[b].status != 0) balanced = false;
       if (balanced) {
         AlsFusedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.tol = o->tol; fa.max_iter = o->max_iter;
-        switch (r) {
-#define DFM_CASEA(RT) case RT: rc = launch_als_fused2<RT>(h, fa, batch, T, N); break;
-          DFM_CASEA(1) DFM_CASEA(2) DFM_CASEA(3) DFM_CASEA(4) DFM_CASEA(5) DFM_CASEA(6) DFM_CASEA(7) DFM_CASEA(8)
-#undef DFM_CASEA
-        }
-        if (rc) return rc;
+        rc = launch_als_fused2(h, fa, r); if (rc) return rc;
         h_active = 0;
       }
     }
@@ -714,12 +849,7 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
     if (h_active > 0 && nc == 0 && als_masked_shape_ok(T, N, r)) {
       AlsMaskedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.nt_min = o->nt_min;
       fa.tol = o->tol; fa.max_iter = o->max_iter;
-      switch (r) {
-#define DFM_CASEA(RT) case RT: rc = launch_als_masked<RT>(h, fa, batch, T, N); break;
-        DFM_CASEA(1) DFM_CASEA(2) DFM_CASEA(3) DFM_CASEA(4) DFM_CASEA(5) DFM_CASEA(6) DFM_CASEA(7) DFM_CASEA(8)
-#undef DFM_CASEA
-      }
-      if (rc) return rc;
+      launch_als_masked(h, fa, r);
       h_active = 0;
     }
     while (it < o->max_iter && h_active > 0) {                                       // :352
@@ -912,12 +1042,7 @@ int dfm_em_init_from_factors(dfm_handle* h, const double* Xs, const double* F, i
       CK(cudaMemsetAsync(dR, 0, B * N * sizeof(double), h->stream));
       L(k_emb_init_flags, N, batch, 64, 0, x, T, N, est, miss);
       L(k_gram_small, batch, 1, 128, 0, f, T, r, dFtF, (const AlsState*)nullptr);
-      switch (embi.ncb) {
-        case 1: emb_launch_M<1>(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est); break;
-        case 2: emb_launch_M<2>(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est); break;
-        case 3: emb_launch_M<3>(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est); break;
-        default: emb_launch_M<4>(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est); break;
-      }
+      emb_launch_M(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est);
       L(k_als_lambda, N, batch, 64, smL, x, f, T, N, r, 0, 2, dL, dR, (const double*)nullptr, 0, (const int*)nullptr,
         (const double*)nullptr, (const double*)nullptr, (const double*)nullptr, (AlsState*)nullptr, (const int*)miss);
     } else
@@ -945,262 +1070,80 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
   if (smFS > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: state dimension r*p too large for the general path");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int k = r * p, kk = k * k, rr = r * r, rk = r * k, np = r * (r + 1) / 2;
-  int ntC = tpt_threads(np + r);
-  int nblkC = (T + ntC - 1) / ntC;
   const bool fused_ok = fused_shape_ok(T, N, r, p);
   if (o->path == 2 && !fused_ok) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs p = 1, r <= 8 and a panel that fits shared memory");
   const bool fused2_ok = fused2_shape_ok(T, N, r, p);
   if (o->path == 3 && !fused2_ok) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: TMA fused path needs p = 1, r <= 8, even T and a panel that fits shared memory");
-  bool fused = (fused_ok || fused2_ok) && o->path != 1;
+  const bool try_fused = (fused_ok || fused2_ok) && o->path != 1;      // the path is only chosen after the NaN scan
   const bool use2 = fused2_ok && (o->path == 0 || o->path == 3);
-  EmbPlan emb = emb_plan(T, N, r, batch, h->nsm);
+  const EmbPlan emb = emb_plan(T, N, r, batch, h->nsm);
   for (int pass = 0; pass < 2; ++pass) {
     Arena a(pass ? h->ws : nullptr);
-    double* dXb = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
-    double* dL = a.get<double>(B * N * r); double* dR = a.get<double>(B * N);
-    double* dA = a.get<double>(B * rk); double* dQ = a.get<double>(B * rr); double* dP0 = a.get<double>(B * kk);
-    double* dFs = a.get<double>(B * T * r); double* dPsF = a.get<double>(B * T * np);
-    double* dll = a.get<double>(B * mi); EmState* st = a.get<EmState>(B);
-    int* dit = a.get<int>(B); int* dstat = a.get<int>(B); int* active = a.get<int>(4);
-    double* dPFfull = out->PF ? a.get<double>(B * T * rr) : nullptr;
-    double *dAn = nullptr, *dQn = nullptr, *dW = nullptr, *dlogR = nullptr, *dC = nullptr, *dBt = nullptr, *dqt = nullptr,
-           *dslr = nullptr, *dCt = nullptr, *dzp = nullptr, *dzf = nullptr, *dPp = nullptr, *dPf = nullptr, *dSff = nullptr;
-    int* dnt = nullptr; double* dxch = nullptr;
-    int* dflag = a.get<int>(4);
-    int* dready = a.get<int>(kMaxReadyChunks);          // streaming host path: one "landed" flag per chunk of panels
-    const size_t fused_off = a.off;                     // the fused kernels' scratch starts here (re-derived at launch time)
-    if ((fused_ok || fused2_ok) && o->path != 1) {      // superset allocation: the path is only chosen after the NaN scan
-      FusedArgs dummy{};
-      switch (r) {
-#define DFM_CASE(RT) case RT: launch_fused<RT>(h, dummy, batch, T, N, nullptr, &a, true); break;
-        DFM_CASE(1) DFM_CASE(2) DFM_CASE(3) DFM_CASE(4) DFM_CASE(5) DFM_CASE(6) DFM_CASE(7) DFM_CASE(8)
-#undef DFM_CASE
-      }
-    }
-    {   // general-path buffers (also the fallback when the scan finds missing data)
-      dAn = a.get<double>(B * rk); dQn = a.get<double>(B * rr); dW = a.get<double>(B * N * r); dlogR = a.get<double>(B * N);
-      dC = a.get<double>(B * rr); dBt = a.get<double>(B * T * r); dqt = a.get<double>(B * T); dslr = a.get<double>(B * T);
-      dnt = a.get<int>(2 * B * T) /* n_t, then src_t of the frozen-step logic */; dCt = a.get<double>(B * T * np); dzp = a.get<double>(B * T * k); dzf = a.get<double>(B * T * k);
-      dPp = a.get<double>(B * T * kk); dPf = a.get<double>(B * T * kk); dSff = a.get<double>(B * rr);
-      dxch = a.get<double>(B * (16 + 64 * (size_t)k + 16 * ((size_t)kk + rk)));      // cluster exchange (scalars, boundary states, Gram partials)
-      if (emb.on) {
-        emb.Bpart = a.get<double>((size_t)emb.nsE * B * T * r); emb.qpart = a.get<double>((size_t)emb.nsE * B * T);
-        emb.Spart = a.get<double>((size_t)emb.tsM * B * N * r); emb.sxxpart = a.get<double>((size_t)emb.tsM * B * N);
-        emb.Cpart = a.get<double>(B * emb.ntM * rr); emb.counters = a.get<int>(B * (size_t)(emb.ntE + emb.ntM));
-      }
-    }
+    EmBufs d;
+    d.X = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
+    d.L = a.get<double>(B * N * r); d.R = a.get<double>(B * N);
+    d.A = a.get<double>(B * rk); d.Q = a.get<double>(B * rr); d.P0 = a.get<double>(B * kk);
+    d.Fs = a.get<double>(B * T * r); d.PsF = a.get<double>(B * T * np);
+    d.ll = a.get<double>(B * mi); d.st = a.get<EmState>(B);
+    d.it = a.get<int>(B); d.stat = a.get<int>(B); d.active = a.get<int>(4);
+    d.PF = out->PF ? a.get<double>(B * T * rr) : nullptr;
+    d.flag = a.get<int>(4);
+    d.ready = a.get<int>(kMaxReadyChunks);
+    d.scratch = try_fused ? a.get<double>((size_t)std::min(batch, h->nsm * 8) * T * FUSED_SCR(r)) : nullptr;
+    const GenBufs g = gen_bufs(a, emb, B, T, N, r, p);        // also the fallback when the scan finds missing data
     if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
     int rc = DFM_OK;
-    bool computed = false;                // set when the pipelined branch already produced device results via the general path
+    bool fused = try_fused;
+    bool uploaded = false;                // the streaming host path found missing data: the panels are on the device already
 #ifndef DFM_EMU
-    // ---------------------------------------------------------------- streaming host path
-    // Host buffers + TMA fused kernel + more panels than are resident at once: ONE launch of the EM kernel, started
-    // before the data is on the device.  The copy stream uploads the batch in chunks of panels (X and the initial
-    // parameters), each chunk followed by a 4-byte copy that sets its "landed" flag; a CTA spins on the flag of the
-    // panel it is about to start (ld.acquire.sys) -- the copy engine is in order, so the flag implies the data.  The
-    // upload (PCIe) runs under the kernel (HBM-bound, slower than the link), P0 and the log-likelihood
-    // pre-fill are done inside the kernel (no other kernel can become resident next to it), and the balance check
-    // is deferred: a panel with NaNs ends with status 3, which triggers the scan + general-path fallback below.
-    // (Not under a CUDA injection profiler or CUDA_LAUNCH_BLOCKING=1: launches are synchronous there, so a kernel that waits for copies
-    //  enqueued after its launch would never finish.  DFM_NO_PIPELINE=1 forces the upload-then-compute path too.)
-    const char* clb = getenv("CUDA_LAUNCH_BLOCKING");
-    const char* cdmc = getenv("CUDA_DEVICE_MAX_CONNECTIONS");
-    // ... nor with CUDA_DEVICE_MAX_CONNECTIONS=1 (common in torch.distributed set-ups): all streams then share one hardware
-    // queue, so the uploads could be queued BEHIND the kernel that waits for them.
-    const bool profiler = getenv("CUDA_INJECTION64_PATH") || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") || (clb && clb[0] == '1') ||
-                          (cdmc && atoi(cdmc) == 1);
-    if (mem == DFM_MEM_HOST && fused && use2 && !getenv("DFM_NO_PIPELINE") && !profiler) {
-      const int cap = fused2_capacity(h->nsm, r, T, N);
-      if (batch > cap) {
-        int chunk = 32;                                              // ~25 MB of C2-shaped panels: the first CTAs start early
-        while ((batch + chunk - 1) / chunk > kMaxReadyChunks) chunk *= 2;
-        const int nch = (batch + chunk - 1) / chunk;
-        cudaStream_t cs = h->copy_stream;
-        cudaEvent_t ev0 = nullptr, ev_k = nullptr;
-        CK(cudaEventCreateWithFlags(&ev0, cudaEventDisableTiming));
-        { cudaError_t e_ = cudaEventCreateWithFlags(&ev_k, cudaEventDisableTiming); if (e_ != cudaSuccess) { cudaEventDestroy(ev0); CK(e_); } }
-#define CKE(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { cudaEventDestroy(ev0); cudaEventDestroy(ev_k); CK(e_); } } while (0)
-        // the workspace is shared with whatever the previous call on this handle left in flight on h->stream (a
-        // DFM_MEM_DEVICE call returns before completion): the copy stream must not touch it before that work is done
-        CKE(cudaEventRecord(ev_k, h->stream));
-        CKE(cudaStreamWaitEvent(cs, ev_k, 0));
-        CKE(cudaStreamWaitEvent(h->d2h_stream, ev_k, 0));
-        CKE(cudaMemsetAsync(dready, 0, (size_t)nch * sizeof(int), cs));
-        CKE(cudaEventRecord(ev0, cs));
-        CKE(cudaStreamWaitEvent(h->stream, ev0, 0));                   // flags are zero before the kernel can read them
-        FusedArgs fa{};
-        fa.X = dXb; fa.Lam = dL; fa.R = dR; fa.A = dA; fa.Q = dQ; fa.P0 = dP0; fa.Fs = dFs; fa.PsF = dPsF; fa.loglik = dll;
-        fa.iters = dit; fa.status = dstat; fa.B = batch; fa.T = T; fa.N = N; fa.max_iter = mi; fa.tol = o->tol;
-        fa.ready = dready; fa.ready_chunk = chunk;
-        if (h->done_cap < B) {                                        // completion flags the kernel writes straight into host memory
-          if (h->done_host) cudaFreeHost(h->done_host);
-          h->done_host = nullptr; h->done_cap = 0;
-          CKE(cudaHostAlloc((void**)&h->done_host, B * sizeof(int), cudaHostAllocMapped));
-          CKE(cudaHostGetDevicePointer((void**)&h->done_dev, h->done_host, 0));
-          h->done_cap = B;
-        }
-#undef CKE
-        memset(h->done_host, 0, B * sizeof(int));
-        fa.done = h->done_dev;
-        fa.P0out = init->P0 ? nullptr : dP0; fa.p0_steps = 12;        // P0 in the kernel unless the caller gave one (the loglik rows are pre-filled there too)
-        {
-          Arena a2(h->ws); a2.off = fused_off;
-          switch (r) {
-#define DFM_CASEP(RT) case RT: rc = launch_fused2<RT>(h, fa, batch, T, N, &a2, false); break;
-            DFM_CASEP(1) DFM_CASEP(2) DFM_CASEP(3) DFM_CASEP(4) DFM_CASEP(5) DFM_CASEP(6) DFM_CASEP(7) DFM_CASEP(8)
-#undef DFM_CASEP
-          }
-        }
-        if (rc) { cudaEventDestroy(ev0); cudaEventDestroy(ev_k); return rc; }
-        cudaError_t up = cudaSuccess;                                  // first failure while enqueueing the upload
-        for (int c = 0; c < nch && up == cudaSuccess; ++c) {
-          size_t b0 = (size_t)c * chunk, bc = std::min<size_t>(chunk, B - b0);
-#define DFM_UP(dst, src, n_) do { if (up == cudaSuccess) up = cudaMemcpyAsync((dst), (src), (size_t)(n_) * 8, cudaMemcpyHostToDevice, cs); } while (0)
-          DFM_UP(dXb + b0 * TN, X + b0 * TN, bc * TN); DFM_UP(dL + b0 * N * r, init->Lam + b0 * N * r, bc * N * r);
-          DFM_UP(dR + b0 * N, init->R + b0 * N, bc * N); DFM_UP(dA + b0 * rk, init->A + b0 * rk, bc * rk); DFM_UP(dQ + b0 * rr, init->Q + b0 * rr, bc * rr);
-          if (init->P0) DFM_UP(dP0 + b0 * kk, init->P0 + b0 * kk, bc * kk);
-#undef DFM_UP
-          if (up == cudaSuccess) up = cudaMemcpyAsync(dready + c, h->pinned_one, sizeof(int), cudaMemcpyHostToDevice, cs);
-        }
-        if (up != cudaSuccess) {
-          // an upload could not be enqueued: the kernel is already running and would wait for its flags for ever ->
-          // raise every flag (the CTAs then run on whatever is in the buffers), drain, report the error
-          cudaMemsetAsync(dready, 1, (size_t)nch * sizeof(int), cs);
-          cudaStreamSynchronize(cs); cudaStreamSynchronize(h->stream);
-          cudaEventDestroy(ev0); cudaEventDestroy(ev_k);
-          (void)cudaGetLastError();
-          snprintf(h->err, sizeof(h->err), "dfm_em_kalman: host-to-device upload failed (%s)", cudaGetErrorString(up));
-          return DFM_ERR_CUDA;
-        }
-        // results of finished panels go back on a third stream while the kernel is still running: the host polls the
-        // completion flags and ships whole chunks of 128 panels in order (everything except the unpacked PF, which
-        // needs a kernel of its own after the EM kernel)
-        {
-          const size_t dch = 128;
-          volatile const int* dn = h->done_host;
-          size_t next = 0; bool kernel_done = false;
-          auto ship = [&](size_t b0, size_t b1) {
-            const size_t nb = b1 - b0;
-#define DFM_OUTS(dst, src, per) if (dst) cudaMemcpyAsync((dst) + b0 * (per), (src) + b0 * (per), nb * (per) * sizeof(*(src)), cudaMemcpyDeviceToHost, h->d2h_stream)
-            DFM_OUTS(out->F, dFs, (size_t)T * r); DFM_OUTS(out->Lam, dL, (size_t)N * r); DFM_OUTS(out->R, dR, (size_t)N); DFM_OUTS(out->A, dA, (size_t)rk);
-            DFM_OUTS(out->Q, dQ, (size_t)rr); DFM_OUTS(out->P0, dP0, (size_t)kk); DFM_OUTS(out->loglik, dll, (size_t)mi);
-            DFM_OUTS(out->iters, dit, (size_t)1); DFM_OUTS(out->status, dstat, (size_t)1);
-#undef DFM_OUTS
-          };
-          while (next < B) {
-            size_t b1 = std::min<size_t>(B, next + dch);
-            bool all = true;
-            if (!kernel_done) for (size_t bb = next; bb < b1; ++bb) if (!dn[bb]) { all = false; break; }
-            if (all) { ship(next, b1); next = b1; continue; }
-            cudaError_t q = cudaStreamQuery(h->stream);
-            if (q != cudaErrorNotReady) kernel_done = true;            // finished (or failed: reported by the synchronize below)
-            else std::this_thread::yield();
-          }
-        }
-        if (out->PF) {
-          long long n = (long long)T * rr;
-          L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, dPsF, T, r, dPFfull);
-          cudaMemcpyAsync(out->PF, dPFfull, B * T * rr * sizeof(double), cudaMemcpyDeviceToHost, h->stream);
-        }
-        std::vector<int> hstat(B);
-        CK(cudaMemcpyAsync(hstat.data(), dstat, B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-        cudaEventRecord(ev_k, h->stream);
-        cudaStreamSynchronize(h->d2h_stream);
-        cudaError_t e1 = cudaStreamSynchronize(cs), e2 = cudaStreamSynchronize(h->stream);
-        cudaEventDestroy(ev0); cudaEventDestroy(ev_k);
-        if (e1 != cudaSuccess || e2 != cudaSuccess) CK(e1 != cudaSuccess ? e1 : e2);
-        bool unbalanced = false, failed = false;
-        for (size_t bb = 0; bb < B; ++bb) failed = failed || hstat[bb] == 3;
-        if (failed) {                                                // NaN log-likelihood somewhere: missing data or a numerical failure?
-          CK(cudaMemsetAsync(dflag, 0, sizeof(int), h->stream));
-          L(k_em_scan_fused, N, batch, 64, 0, dXb, dL, dR, T, N, r, dflag);      // (X only matters: Lam/R of failed panels are NaN anyway)
-          int hflag = 0;
-          CK(cudaMemcpyAsync(&hflag, dflag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-          CK(cudaStreamSynchronize(h->stream));
-          unbalanced = hflag != 0;
-        }
-        if (!unbalanced) { CK(cudaGetLastError()); return DFM_OK; }
-        // a chunk has missing data: everything is on the device already -> general path on the whole batch
-        if (o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
-        fused = false;
-        const double* xg = dXb;
-        // earlier chunks were already updated in place by the fused kernel: restore the initial parameters
-        CK(cudaMemcpyAsync(dL, init->Lam, B * N * r * 8, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(dR, init->R, B * N * 8, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(dA, init->A, B * rk * 8, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(dQ, init->Q, B * rr * 8, cudaMemcpyHostToDevice, h->stream));
-        if (init->P0) CK(cudaMemcpyAsync(dP0, init->P0, B * kk * 8, cudaMemcpyHostToDevice, h->stream));
-        if (!init->P0) L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, dA, dQ, r, p, dP0, 12);
-        { long long n = (long long)B * mi; L(k_fill, (int)std::min<long long>((n + 255) / 256, 1024), 1, 256, 0, dll, n, DFM_NAN); }
-        rc = run_em_general(h, xg, o, dL, dR, dA, dQ, dP0, dAn, dQn, dW, dlogR, dC, dBt, dqt, dslr, dnt, dCt, dzp, dzf, dPp, dPf, dFs, dPsF, dSff, dll, st, dit,
-                            dstat, active, ntC, nblkC, smFS, stgT, out->PF ? 1 : 0, dxch, emb);
-        if (rc) return rc;
-        computed = true;
-      }
+    if (mem == DFM_MEM_HOST && use2 && em_streaming_applies(h, o)) {
+      rc = em_streaming(h, X, o, init, out, d, &uploaded);
+      if (rc || !uploaded) return rc;
+      if (o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
+      fused = false;                      // general path on the whole batch (the fused kernel updated earlier chunks in place)
     }
 #endif
-    if (!computed) {
-    const double* x; rc = stage_in(h, X, dXb, B * TN, mem, &x); if (rc) return rc;
+    const double* x = d.X;
+    if (!uploaded) { rc = stage_in(h, X, d.X, B * TN, mem, &x); if (rc) return rc; }
     cudaMemcpyKind kin = mem == DFM_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    CK(cudaMemcpyAsync(dL, init->Lam, B * N * r * 8, kin, h->stream));
-    CK(cudaMemcpyAsync(dR, init->R, B * N * 8, kin, h->stream));
-    CK(cudaMemcpyAsync(dA, init->A, B * rk * 8, kin, h->stream));
-    CK(cudaMemcpyAsync(dQ, init->Q, B * rr * 8, kin, h->stream));
-    if (init->P0) CK(cudaMemcpyAsync(dP0, init->P0, B * kk * 8, kin, h->stream));
-    else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, dA, dQ, r, p, dP0, 12);
+    CK(cudaMemcpyAsync(d.L, init->Lam, B * N * r * 8, kin, h->stream));
+    CK(cudaMemcpyAsync(d.R, init->R, B * N * 8, kin, h->stream));
+    CK(cudaMemcpyAsync(d.A, init->A, B * rk * 8, kin, h->stream));
+    CK(cudaMemcpyAsync(d.Q, init->Q, B * rr * 8, kin, h->stream));
+    if (init->P0) CK(cudaMemcpyAsync(d.P0, init->P0, B * kk * 8, kin, h->stream));
+    else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, d.A, d.Q, r, p, d.P0, 12);
     {
       long long n = (long long)B * mi;
-      L(k_fill, (int)std::min<long long>((n + 255) / 256, 1024), 1, 256, 0, dll, n, DFM_NAN);
+      L(k_fill, (int)std::min<long long>((n + 255) / 256, 1024), 1, 256, 0, d.ll, n, DFM_NAN);
     }
     if (fused) {                          // balanced panel, all series in the model?
-      CK(cudaMemsetAsync(dflag, 0, sizeof(int), h->stream));
-      L(k_em_scan_fused, N, batch, 64, 0, x, dL, dR, T, N, r, dflag);
+      CK(cudaMemsetAsync(d.flag, 0, sizeof(int), h->stream));
+      L(k_em_scan_fused, N, batch, 64, 0, x, d.L, d.R, T, N, r, d.flag);
       int hflag = 0;
-      CK(cudaMemcpyAsync(&hflag, dflag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+      CK(cudaMemcpyAsync(&hflag, d.flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
       CK(cudaStreamSynchronize(h->stream));
       if (hflag) {
         if (o->path == 2 || o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
         fused = false;
       }
     }
-    if (fused) {
-      FusedArgs fa{};
-      fa.X = x; fa.Lam = dL; fa.R = dR; fa.A = dA; fa.Q = dQ; fa.P0 = dP0; fa.Fs = dFs; fa.PsF = dPsF; fa.loglik = dll;
-      fa.iters = dit; fa.status = dstat; fa.B = batch; fa.T = T; fa.N = N; fa.max_iter = mi; fa.tol = o->tol;
-      Arena a2(h->ws); a2.off = fused_off;             // scratch pointer (first allocation after dflag in this pass)
-      if (use2) {
-        switch (r) {
-#define DFM_CASE2(RT) case RT: rc = launch_fused2<RT>(h, fa, batch, T, N, &a2, false); break;
-          DFM_CASE2(1) DFM_CASE2(2) DFM_CASE2(3) DFM_CASE2(4) DFM_CASE2(5) DFM_CASE2(6) DFM_CASE2(7) DFM_CASE2(8)
-#undef DFM_CASE2
-        }
-      } else
-      switch (r) {
-#define DFM_CASE(RT) case RT: rc = launch_fused<RT>(h, fa, batch, T, N, nullptr, &a2, false); break;
-        DFM_CASE(1) DFM_CASE(2) DFM_CASE(3) DFM_CASE(4) DFM_CASE(5) DFM_CASE(6) DFM_CASE(7) DFM_CASE(8)
-#undef DFM_CASE
-      }
-      if (rc) return rc;
-    } else {
-      rc = run_em_general(h, x, o, dL, dR, dA, dQ, dP0, dAn, dQn, dW, dlogR, dC, dBt, dqt, dslr, dnt, dCt, dzp, dzf, dPp, dPf, dFs, dPsF, dSff, dll, st, dit,
-                          dstat, active, ntC, nblkC, smFS, stgT, out->PF ? 1 : 0, dxch, emb);
-      if (rc) return rc;
-    }
-    }   // !computed
-    rc = copy_out(h, out->Lam, dL, B * N * r, mem); if (rc) return rc;
-    rc = copy_out(h, out->R, dR, B * N, mem); if (rc) return rc;
-    rc = copy_out(h, out->A, dA, B * rk, mem); if (rc) return rc;
-    rc = copy_out(h, out->Q, dQ, B * rr, mem); if (rc) return rc;
-    rc = copy_out(h, out->P0, dP0, B * kk, mem); if (rc) return rc;
-    rc = copy_out(h, out->F, dFs, B * T * r, mem); if (rc) return rc;
+    if (fused) rc = launch_em_fused(h, fused_args(d, o, x), r, use2);
+    else rc = run_em_general(h, x, o, d, g, out->PF ? 1 : 0);
+    if (rc) return rc;
+    rc = copy_out(h, out->Lam, d.L, B * N * r, mem); if (rc) return rc;
+    rc = copy_out(h, out->R, d.R, B * N, mem); if (rc) return rc;
+    rc = copy_out(h, out->A, d.A, B * rk, mem); if (rc) return rc;
+    rc = copy_out(h, out->Q, d.Q, B * rr, mem); if (rc) return rc;
+    rc = copy_out(h, out->P0, d.P0, B * kk, mem); if (rc) return rc;
+    rc = copy_out(h, out->F, d.Fs, B * T * r, mem); if (rc) return rc;
     if (out->PF) {
       long long n = (long long)T * rr;
-      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, dPsF, T, r, dPFfull);
-      rc = copy_out(h, out->PF, dPFfull, B * T * rr, mem); if (rc) return rc;
+      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, d.PsF, T, r, d.PF);
+      rc = copy_out(h, out->PF, d.PF, B * T * rr, mem); if (rc) return rc;
     }
-    rc = copy_out(h, out->loglik, dll, B * mi, mem); if (rc) return rc;
-    rc = copy_out(h, out->iters, dit, B, mem); if (rc) return rc;
-    rc = copy_out(h, out->status, dstat, B, mem); if (rc) return rc;
+    rc = copy_out(h, out->loglik, d.ll, B * mi, mem); if (rc) return rc;
+    rc = copy_out(h, out->iters, d.it, B, mem); if (rc) return rc;
+    rc = copy_out(h, out->status, d.stat, B, mem); if (rc) return rc;
   }
   return finish(h, mem);
 }
@@ -1237,13 +1180,7 @@ int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, cons
     double* dFs = a.get<double>(B * Tp * r); double* dPsF = a.get<double>(B * Tp * np);
     double* dll = a.get<double>(B); EmState* st = a.get<EmState>(B);
     int* dit = a.get<int>(B); int* dstat = a.get<int>(B);
-    double* dAn = a.get<double>(B * rk); double* dQn = a.get<double>(B * rr); double* dW = a.get<double>(B * N * r);
-    double* dlogR = a.get<double>(B * N); double* dC = a.get<double>(B * rr); double* dBt = a.get<double>(B * Tp * r);
-    double* dqt = a.get<double>(B * Tp); double* dslr = a.get<double>(B * Tp);
-    int* dnt = a.get<int>(2 * B * Tp);                      // n_t, then src_t of the frozen-step logic
-    double* dCt = a.get<double>(B * Tp * np); double* dzp = a.get<double>(B * Tp * k); double* dzf = a.get<double>(B * Tp * k);
-    double* dPp = a.get<double>(B * Tp * kk); double* dPf = a.get<double>(B * Tp * kk); double* dSff = a.get<double>(B * rr);
-    double* dxch = a.get<double>(B * (16 + 64 * (size_t)k + 16 * ((size_t)kk + rk)));
+    const GenBufs g = gen_bufs(a, EmbPlan{}, B, Tp, N, r, p);
     double* dPFfull = (out->PF && !dev_out) ? a.get<double>(B * Tp * rr) : nullptr;
     double* dcom = (out->common && !dev_out) ? a.get<double>(B * TN) : nullptr;
     double* dxh = (out->xhat && !dev_out) ? a.get<double>(B * TN) : nullptr;
@@ -1274,14 +1211,12 @@ int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, cons
     // ---- one E-step (the general path's kernels; k_em_prep in its opening mode only reads Lam, R)
     L(k_em_state_init, batch, 1, 1, 0, st);
     L(k_em_scan, N, batch, 64, 0, x, pL, Tp, N, r, st);
-    L(k_em_prep, batch, 1, 128, 0, pL, pR, N, r, p, dW, dlogR, dC, (double*)nullptr, (const double*)nullptr, (double*)nullptr,
+    L(k_em_prep, batch, 1, 128, 0, pL, pR, N, r, p, g.W, g.logR, g.C, (double*)nullptr, (const double*)nullptr, (double*)nullptr,
       (const double*)nullptr, st, 1, 0, 0);
-    L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, pL, dW, pR, dlogR, dC, Tp, N, r, dBt, dqt, dslr, dnt, dCt, st);
-    L(k_em_contract_bal, (Tp + 31) / 32, batch, 256, 8 * 32 * 3 * 8, x, dW, pR, dlogR, Tp, N, r, dBt, dqt, dslr, dnt, st);
-    int ncl = fs_cluster_size(h, batch, dxch);
-    const int ntFS = (batch <= 2 * h->nsm) ? 512 : 256;
-    rc = launch_filter_smooth(h, ncl, batch, ntFS, smFS, pA, pQ, dP0, dC, dBt, dqt, dslr, dnt, dCt, Tp, r, p, dzp, dzf, dPp, dPf, dFs, dPsF,
-                              dSff, dAn, dQn, dll, 1, 0.0, st, dnt + B * Tp, stgT, 1, dxch);
+    L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, pL, g.W, pR, g.logR, g.C, Tp, N, r, g.Bt, g.qt, g.slr, g.nt, g.Ct, st);
+    L(k_em_contract_bal, (Tp + 31) / 32, batch, 256, 8 * 32 * 3 * 8, x, g.W, pR, g.logR, Tp, N, r, g.Bt, g.qt, g.slr, g.nt, st);
+    int ncl = fs_cluster_size(h, batch, g.xch);
+    rc = launch_filter_smooth(h, ncl, g, batch, Tp, r, p, pA, pQ, dP0, dFs, dPsF, dll, st, 1, 0.0, 1);
     if (rc) return rc;
     L(k_em_collect, batch, 1, 1, 0, st, dit, dstat);
     L(k_ss_nan_failed, batch, 1, 256, 0, (const EmState*)st, Tp, r, dFs, dPsF, dll);
