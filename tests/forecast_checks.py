@@ -9,7 +9,7 @@ from oracle.dgp import simulate_panel
 from dynamic_factor_models_b200 import DFMError
 from dynamic_factor_models_b200._lib import MEM_DEVICE, MEM_HOST
 from forecast_oracle import smooth_forecast
-from parity_checks import rmse
+from parity_checks import ll_atol, rmse
 
 
 def _params(X, r, p):
@@ -17,13 +17,13 @@ def _params(X, r, p):
     return K.init_from_factors(X, F0, p)
 
 
-def compare(got, ref, ll_rtol=1e-10):
+def compare(got, ref, ll_rtol=1e-10, ll_atol=0.0):
     assert rmse(got["F"], ref["F"]) < 1e-8, rmse(got["F"], ref["F"])
     np.testing.assert_allclose(got["PF"], ref["PF"], rtol=1e-7, atol=1e-10)
     for n in ("common", "xhat", "xvar"):
         assert (np.isnan(got[n]) == np.isnan(ref[n])).all(), n
         np.testing.assert_allclose(got[n], ref[n], rtol=1e-7, atol=1e-10, err_msg=n)
-    np.testing.assert_allclose(got["loglik"], ref["loglik"], rtol=ll_rtol)
+    np.testing.assert_allclose(got["loglik"], ref["loglik"], rtol=ll_rtol, atol=ll_atol)
 
 
 def check_observed_cells(X, got):
@@ -38,15 +38,18 @@ def check_observed_cells(X, got):
     assert np.isfinite(got["xhat"][unobs]).all() and (got["xvar"][unobs] > 0.0).all()
 
 
-def check_kalman_smooth(lib, N=24, r=3, T=70, p=1, miss=0.0, H=0, rep=9, exclude=()):
+def check_kalman_smooth(lib, N=24, r=3, T=70, p=1, miss=0.0, H=0, rep=9, exclude=(), holes=(), ll_cell_tol=0.0):
+    """holes and ll_cell_tol as in parity_checks.check_em."""
     X, _ = simulate_panel(N, r, T, rep=rep, missing_frac=miss)
+    for t0, t1, i in holes:
+        X[t0:t1, i] = np.nan
     Lam, Rv, A, Q = _params(X, r, p)
     for i in exclude:
         Lam[i] = np.nan
     ref = smooth_forecast(X, Lam, Rv, A, Q, None, p, H)
     got = lib.kalman_smooth(X, Lam, Rv, A, Q, p=p, H=H)
     assert got["status"] == 0
-    compare(got, ref)
+    compare(got, ref, ll_atol=ll_atol(X, ll_cell_tol))
     check_observed_cells(X, got)
     for i in exclude:
         assert np.isnan(got["common"][:, i]).all() and np.isnan(got["xhat"][:, i]).all() and np.isnan(got["xvar"][:, i]).all()
