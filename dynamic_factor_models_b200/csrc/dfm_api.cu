@@ -19,12 +19,38 @@
 #include <vector>
 #ifndef DFM_EMU
 #include <dlfcn.h>
+#else
+#include <map>
+#include <mutex>
 #endif
 
 #ifdef DFM_EMU
 // ---- minimal CUDA-runtime stand-ins for the host-emulation test build -------------------------
 typedef int cudaError_t;
-enum { cudaSuccess = 0 };
+enum { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorInvalidConfiguration = 9 };
+// The launch limits of the H100 that the emulated launches are held to, so that a launch the device would refuse fails
+// here too: it does not run, and the next cudaGetLastError() returns the error (the entry point then returns DFM_ERR_CUDA).
+static thread_local cudaError_t g_emu_last_err = cudaSuccess;
+static std::mutex g_emu_attr_mu;
+static std::map<const void*, size_t> g_emu_smem_attr;        // cudaFuncAttributeMaxDynamicSharedMemorySize per kernel
+static inline void emu_set_error(cudaError_t e) { if (g_emu_last_err == cudaSuccess) g_emu_last_err = e; }
+static inline void emu_set_smem(const void* kern, size_t bytes) {
+  if (bytes > 227 * 1024) { emu_set_error(cudaErrorInvalidValue); return; }   // the attribute's ceiling on sm_90
+  std::lock_guard<std::mutex> lk(g_emu_attr_mu);
+  g_emu_smem_attr[kern] = bytes;
+}
+static inline bool emu_launch_ok(const void* kern, long long gx, long long gy, long long nt, size_t smem) {
+  size_t attr = 0;
+  {
+    std::lock_guard<std::mutex> lk(g_emu_attr_mu);
+    auto it = g_emu_smem_attr.find(kern);
+    if (it != g_emu_smem_attr.end()) attr = it->second;
+  }
+  const bool ok = smem <= std::max<size_t>(48 * 1024, attr) && nt >= 1 && nt <= 1024 && gx >= 1 && gx <= 2147483647LL && gy >= 1 &&
+                  gy <= 65535;
+  if (!ok) emu_set_error(cudaErrorInvalidConfiguration);
+  return ok;
+}
 enum cudaMemcpyKind { cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice };
 static inline cudaError_t cudaMalloc(void** p, size_t n) { *p = malloc(n ? n : 1); return *p ? 0 : 2; }
 static inline cudaError_t cudaFree(void* p) { free(p); return 0; }
@@ -39,9 +65,12 @@ static inline cudaError_t cudaStreamDestroy(cudaStream_t) { return 0; }
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return 0; }
 static inline cudaError_t cudaSetDevice(int) { return 0; }
 static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return 0; }
-static inline cudaError_t cudaGetLastError() { return 0; }
-static inline const char* cudaGetErrorString(cudaError_t) { return "emu"; }
-#define DFM_SET_SMEM(kern, bytes) ((void)0)
+static inline cudaError_t cudaGetLastError() { cudaError_t e = g_emu_last_err; g_emu_last_err = cudaSuccess; return e; }
+static inline const char* cudaGetErrorString(cudaError_t e) {
+  return e == cudaErrorInvalidConfiguration ? "emu: launch past a device limit (grid, block or shared memory)"
+       : e == cudaErrorInvalidValue ? "emu: shared-memory attribute past the device limit" : "emu";
+}
+#define DFM_SET_SMEM(kern, bytes) emu_set_smem((const void*)(kern), (size_t)(bytes))    // (kern: a kernel or a pointer to one)
 #else
 #define DFM_SET_SMEM(kern, bytes) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes))
 #endif
@@ -75,6 +104,9 @@ namespace {
 
 const size_t kMaxSmem = 220 * 1024;
 const int kMaxReadyChunks = 4096;
+// Entry points whose launches put the batch on gridDim.y (at most 65535 blocks) refuse larger batches with
+// DFM_ERR_UNSUPPORTED; callers split such batches.
+const int kMaxGridBatch = 65535;
 
 struct Arena {
   char* base; size_t off;
@@ -106,8 +138,14 @@ int fail(dfm_handle* h, int code, const char* msg) {
   if (h->profile) { cudaEventCreate(&pr__.e0); cudaEventCreate(&pr__.e1); cudaEventRecord(pr__.e0, h->stream); }
 #define PROF_END() if (h->profile) { cudaEventRecord(pr__.e1, h->stream); h->prof->push_back(pr__); }
 #endif
+#ifdef DFM_EMU
+#define L(kern, gx, gy, nt, smem, ...)                                                             \
+  do { if (emu_launch_ok((const void*)(kern), (gx), (gy), (nt), (smem))) DFM_LAUNCH(kern, gx, gy, nt, smem, h->stream, __VA_ARGS__); \
+       h->launches++; } while (0)
+#else
 #define L(kern, gx, gy, nt, smem, ...)                                                             \
   do { PROF_BEGIN(#kern); DFM_LAUNCH(kern, gx, gy, nt, smem, h->stream, __VA_ARGS__); PROF_END(); h->launches++; } while (0)
+#endif
 
 int ensure_ws(dfm_handle* h, size_t bytes) {
   if (bytes <= h->ws_bytes) return DFM_OK;
@@ -205,7 +243,8 @@ static auto dispatch(int v, F&& f) {
 template <typename K>
 static int resident_grid(const dfm_handle* h, K kern, int threads, size_t smem, int B) {
 #ifdef DFM_EMU
-  (void)kern; (void)threads; (void)smem;
+  (void)threads;
+  DFM_SET_SMEM(kern, smem);
   return std::min(B, h->nsm * 8);
 #else
   DFM_SET_SMEM(kern, smem);
@@ -721,6 +760,7 @@ int dfm_shard_range(long long n_rep, int rank, int world, long long* begin, long
 int dfm_standardize(dfm_handle* h, const double* X, int T, int N, int batch, int mem, double* Xs, double* xmean,
                     double* xstd) {
   if (!h || !X || !Xs || T <= 0 || N <= 0 || batch <= 0) return fail(h, DFM_ERR_ARG, "dfm_standardize: bad argument");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_standardize: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N;
   for (int pass = 0; pass < 2; ++pass) {
@@ -772,6 +812,7 @@ static int run_pca(dfm_handle* h, const double* dXs, int T, int N, int r, int ba
 int dfm_pca_score(dfm_handle* h, const double* X, int T, int N, int r, int batch, int mem, double* score) {
   if (!h || !X || !score || T <= 0 || N <= 0 || r <= 0 || batch <= 0 || r > std::min(T, N)) return fail(h, DFM_ERR_ARG, "dfm_pca_score: bad argument");
   if (r > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_pca_score: r > 48");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_pca_score: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int nmax = std::min(N, T);
   for (int pass = 0; pass < 2; ++pass) {
@@ -799,10 +840,16 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
       (o->n_constr > 0 && (!o->constr_index || !o->constr_R || !o->constr_r)) || o->n_constr > 64)
     return fail(h, DFM_ERR_ARG, "dfm_estimate_factor: bad shape/options");
   if (!F_init && r > 48) return fail(h, DFM_ERR_UNSUPPORTED, "PCA init: r > 48 (pass F_init)");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_estimate_factor: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int nmax = std::min(N, T), np = r * (r + 1) / 2, nc = o->n_constr;
   int ntF = tpt_threads(np + r);
   int nblk = (T + ntF - 1) / ntF;
+  // k_als_factor's per-thread packed systems: in shared memory up to r = 40 at the 32-thread floor of tpt_threads, in a
+  // global scratch from the workspace past that (r <= 64)
+  size_t smF = ((size_t)(np + r) * ntF + 48) * 8;
+  const bool sys_global = smF > kMaxSmem;
+  if (sys_global) smF = 48 * 8;
   for (int pass = 0; pass < 2; ++pass) {
     Arena a(pass ? h->ws : nullptr);
     double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
@@ -815,6 +862,7 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
     double* dF = a.get<double>(B * T * r); double* dLam = a.get<double>(B * N * r); double* dR2 = a.get<double>(B * N);
     double* FtF = a.get<double>(B * r * r); double* LtL = a.get<double>(B * r * r); double* ssrp = a.get<double>(B * nblk);
     int* cidx = a.get<int>(nc + 1); double* cR = a.get<double>((size_t)nc * r + 1); double* cr = a.get<double>(nc + 1);
+    double* gsys = sys_global ? a.get<double>(B * nblk * (size_t)(np + r) * ntF) : nullptr;
     if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
     const double* x; int rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
     if (nc > 0) {
@@ -828,7 +876,6 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
                   if (fi != dF) CK(cudaMemcpyAsync(dF, fi, B * T * r * sizeof(double), cudaMemcpyDeviceToDevice, h->stream)); }
     else { rc = run_pca(h, dXs, T, N, r, batch, cn, bal, nbal, G, V, Ysub, dF, nullptr, st); if (rc) return rc; }   // :345-348
     size_t smL = (size_t)(2 * np + 2 * r + 8 + (size_t)r * nc + (size_t)nc * (nc + 1) / 2 + nc) * 8;
-    size_t smF = ((size_t)(np + r) * ntF + 48) * 8;
     long long it = 0;
     int h_active = batch;
     // balanced panels without constraints: all sweeps in ONE fused launch (TMA ring + DMMA passes)
@@ -856,7 +903,7 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
       if (nc > 0) L(k_gram_small, batch, 1, 128, 0, dF, T, r, FtF, st);
       L(k_als_lambda, N, batch, 64, smL, dXs, dF, T, N, r, o->nt_min, 0, dLam, (double*)nullptr, FtF, nc, cidx, cR, cr, ds, st);   // :355-362
       L(k_gram_small, batch, 1, 128, 0, dLam, N, r, LtL, st);
-      L(k_als_factor, nblk, batch, ntF, smF, dXs, dLam, LtL, T, N, r, dF, ssrp, st);                                             // :364-366
+      L(k_als_factor, nblk, batch, ntF, smF, dXs, dLam, LtL, T, N, r, dF, ssrp, st, gsys);                                           // :364-366
       L(k_als_check, batch, 1, 1, 0, st, ssrp, nblk, o->tol, T, N, o->max_iter);                                                // :367-368
       ++it;
       if ((it & 1) == 0 || it >= o->max_iter || it < 2) {
@@ -895,6 +942,7 @@ int dfm_estimate_loading_ex(dfm_handle* h, const double* data, const double* F, 
   if (T <= 1 || ns <= 0 || r <= 0 || r > 64 || batch <= 0 || L_ <= 0 || L_ > 16 || nc < 0 || nc > 64 ||
       (nc > 0 && (!o->constr_index || !o->constr_R || !o->constr_r)))
     return fail(h, DFM_ERR_ARG, "dfm_estimate_loading: bad shape/options");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_estimate_loading: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch; int K = r + 1, np = K * (K + 1) / 2;
   for (int pass = 0; pass < 2; ++pass) {
@@ -981,6 +1029,7 @@ int dfm_irf(dfm_handle* h, const double* M, const double* Q, const double* G, in
   if (!h || !M || !Q || !G || !shock_ids || !irf || k <= 0 || r <= 0 || H <= 0 || n_shock <= 0 || batch <= 0)
     return fail(h, DFM_ERR_ARG, "dfm_irf: bad argument");
   for (int j = 0; j < n_shock; ++j) if (shock_ids[j] < 0 || shock_ids[j] >= r) return fail(h, DFM_ERR_ARG, "dfm_irf: shock id out of range");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_irf: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch;
   for (int pass = 0; pass < 2; ++pass) {
@@ -1010,6 +1059,7 @@ int dfm_em_init_from_factors(dfm_handle* h, const double* Xs, const double* F, i
   if (T - p <= k) return fail(h, DFM_ERR_TOO_FEW_OBS, "dfm_em_init_from_factors: T - p <= r*p");
   size_t smV = ((size_t)k * k + (size_t)k * r + (size_t)r * r + 16) * 8 + (size_t)T + 16;
   if (smV > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "r*p too large");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_init_from_factors: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int np = r * (r + 1) / 2;
   EmbPlan embi = emb_plan(T, N, r, batch, h->nsm);
@@ -1065,6 +1115,7 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
   int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mem = o->mem, mi = o->max_iter;
   if (T <= 1 || N <= 0 || r <= 0 || r > 64 || p <= 0 || batch <= 0 || mi <= 0 || o->tol < 0)
     return fail(h, DFM_ERR_ARG, "dfm_em_kalman: bad shape/options");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: batch > 65535");
   const int stgT = fs_stage_periods(h->nsm, batch, r, p);
   size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
   if (smFS > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: state dimension r*p too large for the general path");
@@ -1159,6 +1210,7 @@ int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, cons
   if (T <= 0 || N <= 0 || r <= 0 || r > 64 || p <= 0 || H < 0 || batch <= 0 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE) ||
       (long long)T + H < 2)
     return fail(h, DFM_ERR_ARG, "dfm_kalman_smooth: bad shape/options");
+  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_kalman_smooth: batch > 65535");
   const int Tp = T + H;
   const int stgT = fs_stage_periods(h->nsm, batch, r, p);
   const size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
@@ -1301,9 +1353,7 @@ int dfm_bootstrap_panels(dfm_handle* h, const dfm_boot_opts* o, const double* F0
     rc = stage_in(h, uar_ser, dse, (size_t)ns, mem, &ba.uar_ser); if (rc) return rc;
     rc = stage_in(h, data, dda, (size_t)Tw * ns, mem, &ba.data); if (rc) return rc;
     ba.X = dX; ba.Tw = Tw; ba.ns = ns; ba.r = r; ba.p = p; ba.L = Lg; ba.nres = nres; ba.burn = o->burn; ba.seed = o->seed; ba.rep0 = o->rep0;
-#ifndef DFM_EMU
     DFM_SET_SMEM(k_bootstrap_panels, smem);
-#endif
     L(k_bootstrap_panels, batch, 1, 256, smem, ba);
     if (hst) { rc = copy_out(h, X, dX, B * ns * Tw, mem); if (rc) return rc; }
   }
@@ -1431,9 +1481,7 @@ int dfm_percentiles(dfm_handle* h, const double* recs, long long n, int d, const
     if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
     const double* r_; int rc = stage_in(h, recs, dr, (size_t)n * d, mem, &r_); if (rc) return rc;
     CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
-#ifndef DFM_EMU
     DFM_SET_SMEM(k_percentiles, smem);
-#endif
     L(k_percentiles, d, 1, 256, smem, r_, (int)n, d, dq, nq, (int)npad, dout);
     if (mem == DFM_MEM_HOST) { rc = copy_out(h, out, dout, (size_t)nq * d, mem); if (rc) return rc; }
     else CK(cudaStreamSynchronize(h->stream));                                               // (dq lives in the shared workspace)

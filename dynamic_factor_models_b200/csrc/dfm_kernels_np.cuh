@@ -775,18 +775,20 @@ __global__ void k_als_lambda(const double* __restrict__ Xs, const double* __rest
 
 // F-step (:364-366): one THREAD per period t; per-thread packed normal equations in shared memory.
 // A_t = Lam'Lam - sum_{i missing at t} lam_i lam_i'  (series with NaN Lam are excluded everywhere).
-// grid (ceil(T/NT), B); shared: (np + r) * NT + 40 doubles.
+// grid (ceil(T/NT), B); shared: (np + r) * NT + 48 doubles, or 48 when the per-thread systems live in `gsys`
+// (global scratch of (np + r) * NT doubles per block, for r whose systems do not fit in shared memory; NULL otherwise).
 __global__ void k_als_factor(const double* __restrict__ Xs, const double* __restrict__ LamAll,
                              const double* __restrict__ LtLall, int T, int N, int r, double* __restrict__ Fnew,
-                             double* __restrict__ ssr_part, AlsState* st) {
+                             double* __restrict__ ssr_part, AlsState* st, double* __restrict__ gsys) {
   DFM_SMEM(sm);
   int b = DFM_BY;
   if (st[b].done) return;
   int np = r * (r + 1) / 2;
   int nt = DFM_NT;
-  double* A = sm + DFM_TID;                 // element e at A[e*nt]
-  double* c = sm + (size_t)np * nt + DFM_TID;
-  double* red = sm + (size_t)(np + r) * nt;
+  double* sys = gsys ? gsys + ((size_t)b * DFM_GX + DFM_BX) * (np + r) * nt : sm;
+  double* A = sys + DFM_TID;                // element e at A[e*nt]
+  double* c = sys + (size_t)np * nt + DFM_TID;
+  double* red = gsys ? sm : sm + (size_t)(np + r) * nt;
   const double* X = Xs + (size_t)b * T * N;
   const double* Lam = LamAll + (size_t)b * N * r;
   const double* LtL = LtLall + (size_t)b * r * r;
@@ -847,8 +849,9 @@ __global__ void k_count_active(const AlsState* st, int B, int* out) {
 }
 
 // ---------------------------------------------------------------- a9 loadings + AR  (:391-415, :295-311)
-// One block per series.  data T x ns raw units, F T x r.  Regressors [F 1] (:399).
-// scratch: T doubles per block for the gap-free residual vector.
+// One block per series.  data T x ns raw units, F T x r.  Regressors [F 1] (:399), over the rows where y and every factor
+// are observed (a missing factor row drops that row for every series, as k_var / k_instability / k_fit_corr do).
+// scratch: T doubles per block: y on the usable rows (NaN elsewhere), then the gap-free residual vector.
 __global__ void k_loading(const double* __restrict__ dataAll, const double* __restrict__ Fall, int T, int ns, int r,
                           int nt_min, int n_uarlag, double* __restrict__ lambda, double* __restrict__ r2out,
                           double* __restrict__ uar_coef, double* __restrict__ uar_ser, double* __restrict__ scratch,
@@ -857,9 +860,17 @@ __global__ void k_loading(const double* __restrict__ dataAll, const double* __re
                           double* __restrict__ resid) {
   DFM_SMEM(sm);
   int s_ = DFM_BX, b = DFM_BY;
-  const double* y = dataAll + ((size_t)b * ns + s_) * T;
+  const double* yin = dataAll + ((size_t)b * ns + s_) * T;
   const double* F = Fall + (size_t)b * T * r;
   double* u = scratch + ((size_t)b * ns + s_) * T;
+  // drop_missing_row([y F]) (:396): y_t where y_t and every factor are observed, else NaN; the regression reads this copy
+  for (int t = DFM_TID; t < T; t += DFM_NT) {
+    double v = yin[t];
+    for (int a = 0; a < r && !is_nan(v); ++a) if (is_nan(F[t + (size_t)T * a])) v = DFM_NAN;
+    u[t] = v;
+  }
+  DFM_SYNC();
+  const double* y = u;
   int K = r + 1, np = K * (K + 1) / 2;
   double* A = sm;               // packed K
   double* c = A + np;           // K

@@ -11,7 +11,10 @@
  *  - all matrices are COLUMN-MAJOR Float64 (Julia layout); a panel is T x N, series i
  *    contiguous in t; missing observations are NaN (the Julia shim maps `missing` <-> NaN);
  *  - `batch` = B independent problems stored back to back (panel b at X + b*T*N, every
- *    output likewise); B = 1 is the reference's single-model call;
+ *    output likewise); B = 1 is the reference's single-model call.  dfm_standardize, dfm_pca_score,
+ *    dfm_estimate_factor, dfm_estimate_loading(_ex), dfm_irf, dfm_em_init_from_factors, dfm_em_kalman and
+ *    dfm_kalman_smooth take B <= 65535 (their launches put the batch on the grid's y dimension); a larger
+ *    batch returns DFM_ERR_UNSUPPORTED: split it into several calls;
  *  - `mem` says where the DATA pointers live: DFM_MEM_HOST (the library does the H2D/D2H
  *    copies on the handle's stream) or DFM_MEM_DEVICE (pointers are device pointers on the
  *    handle's device: nothing is copied).  Small option/constraint arrays are always host;
@@ -99,7 +102,8 @@ typedef struct {
 } dfm_factor_stats;
 
 /* X: T x N raw (unstandardized) estimation block with NaN.  F_init: optional T x r starting
- * factors (NULL = PCA of the balanced sub-panel as the reference does, :345-348).
+ * factors (NULL = PCA of the balanced sub-panel as the reference does, :345-348).  r <= 64 with
+ * F_init, r <= 48 with the PCA start (DFM_ERR_UNSUPPORTED past that).
  * Outputs (any may be NULL): F T x r (= m.factor[initperiod:lastperiod,:]); Lambda N x r in
  * standardized units (the loop-local `lambda` of :351, NaN rows for series with < nt_min obs);
  * R2 N (m.fes.R2, NaN = missing); xmean, xstd N; stats [batch]. */
@@ -116,7 +120,8 @@ typedef struct {
   int batch;
   int mem;
 } dfm_loading_opts;
-/* data T x ns (raw units, NaN), F T x r.  Outputs: lambda ns x r, r2 ns, uar_coef ns x n_uarlag,
+/* data T x ns (raw units, NaN), F T x r (NaN = missing).  Each series is fitted on the rows where it and
+ * every factor are observed (drop_missing_row, :396).  Outputs: lambda ns x r, r2 ns, uar_coef ns x n_uarlag,
  * uar_ser ns.  Series with < nt_min usable rows get NaN (the reference leaves them undefined). */
 int dfm_estimate_loading(dfm_handle* h, const double* data, const double* F, const dfm_loading_opts* opts,
                          double* lambda, double* r2, double* uar_coef, double* uar_ser);

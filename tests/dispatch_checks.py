@@ -114,9 +114,9 @@ Case = collections.namedtuple("Case", "id run kernels")
 CASES = []
 
 
-def case(id_, kernels):
+def case(id_, kernels, table=CASES):
     def reg(fn):
-        CASES.append(Case(id_, fn, kernels))
+        table.append(Case(id_, fn, kernels))
         return fn
     return reg
 

@@ -38,13 +38,51 @@ def check_standardize(lib, rng=None):
     assert (np.isnan(gxs) == np.isnan(xs)).all()
 
 
-def check_pca(lib, T=60, N=25, r=4, sizes=None):
+def separated_panel(T, N, decay=0.93, rep=2):
+    """T x N panel U diag(s) V' with s_j = decay^j and a V whose column j has its largest entry in row j, well above the
+    others: distinct singular values and an unambiguous sign rule (see pca_sign_rule)."""
+    rng = np.random.default_rng(rep)
+    n = min(T, N)
+    U, _ = np.linalg.qr(rng.standard_normal((T, n)))
+    M = 0.1 * rng.standard_normal((N, n))
+    M[np.arange(n), np.arange(n)] += rng.choice([-1.0, 1.0], n)
+    V, _ = np.linalg.qr(M)
+    return (U * decay ** np.arange(n)) @ V.T
+
+
+def pca_sign_rule(X, r):
+    """X V_r with numpy's SVD and the library's documented sign rule: the entry of largest magnitude of each right singular
+    vector is positive.  Asserts that the top r + 1 singular values and each column's two largest |entries| are apart, so
+    that the rule and the columns are well defined."""
+    _, s, Vt = np.linalg.svd(X, full_matrices=False)
+    s = np.append(s, 0.0)
+    assert (s[:r] > 1.01 * s[1:r + 1]).all(), "singular values too close"
+    V = Vt[:r].T.copy()
+    a = np.sort(np.abs(V), axis=0)
+    assert (a[-1] - a[-2] > 1e-4).all(), "largest entries too close"      # (the vectors have unit norm)
+    j = np.argmax(np.abs(V), axis=0)
+    V *= np.sign(V[j, np.arange(r)])
+    return X @ V
+
+
+def check_pca(lib, T=60, N=25, r=4, sizes=None, sign_rule=False, batch=1):
+    """sign_rule: raw scores of separated_panel data against pca_sign_rule, no sign alignment; batch > 1: also a batched
+    call against one call per panel."""
     for (t, n) in (sizes or ((T, N), (N, T))):          # both Gram modes (X'X and XX')
-        X, _ = simulate_panel(n, r, t, rep=2)
-        ref = R.pca_score(X, r)
-        got = lib.pca_score(X, r)
-        got, _ = sign_align(got, ref)
-        assert rmse(got, ref) < 1e-10 * max(1.0, np.abs(ref).max())
+        if not sign_rule:
+            X, _ = simulate_panel(n, r, t, rep=2)
+            ref = R.pca_score(X, r)
+            got = lib.pca_score(X, r)
+            got, _ = sign_align(got, ref)
+            assert rmse(got, ref) < 1e-10 * max(1.0, np.abs(ref).max())
+            continue
+        Xb = np.stack([separated_panel(t, n, rep=2 + b) for b in range(batch)])
+        got = lib.pca_score(Xb, r)
+        for b in range(batch):
+            ref = pca_sign_rule(Xb[b], r)
+            assert np.abs(got[b] - ref).max() < 1e-9 * np.abs(ref).max(), np.abs(got[b] - ref).max()
+            if batch > 1:
+                np.testing.assert_allclose(got[b], lib.pca_score(Xb[b], r), rtol=1e-13, atol=1e-13 * np.abs(ref).max())
 
 
 def check_estimate_factor_c1(lib, panels, r=8):
@@ -69,25 +107,37 @@ def check_estimate_factor_c1(lib, panels, r=8):
     return e
 
 
-def check_estimate_factor_same_init(lib, N=30, r=3, T=80, miss=0.08):
-    """Same starting factors on both sides -> no sign ambiguity, tight tolerance; fixed sweeps."""
+def check_estimate_factor_same_init(lib, N=30, r=3, T=80, miss=0.08, iters=(1, 7), short_series=True, constr=None,
+                                    pca_start=False):
+    """Same starting factors on both sides -> no sign ambiguity, tight tolerance; fixed sweeps.  miss = 0 with
+    short_series=False: a balanced panel.  constr = (index, R, r) rows of a :factor constraint (r unstandardized).
+    pca_start: the library starts from its own PCA, the oracle from pca_sign_rule (the sign rule the library documents)."""
     X, _ = simulate_panel(N, r, T, rep=4, standardize=False)
     rng = np.random.default_rng(4)
     hole = rng.uniform(size=(T, N // 2)) < 2 * miss                 # missing data only in half of the columns
     X[:, :N // 2][hole] = np.nan
-    X[:, 0] = np.nan; X[:15, 0] = 1.0 + np.arange(15) * 0.1        # a series with < nt_min obs
+    if short_series:
+        X[:, 0] = np.nan; X[:15, 0] = 1.0 + np.arange(15) * 0.1    # a series with < nt_min obs
     m = R.DFMModel(X, np.ones(N, int), 20, 40, 1, T, 0, r, 1e-8, 4, 2)
     xs, _ = R.standardize_data(X)
-    f0 = R.pca_score(R.drop_missing_col(xs)[0], r)
-    for max_iter in (1, 7):
-        R.estimate_factor(m, max_iter=max_iter, f_init=f0)
-        out = lib.estimate_factor(X, r, nt_min=20, tol=1e-8, max_iter=max_iter, F_init=f0)
+    f0 = (pca_sign_rule if pca_start else R.pca_score)(R.drop_missing_col(xs)[0], r)
+    lc = None
+    if constr is not None:
+        lc = R.LambdaConstraint(np.asarray(constr[0]), np.asarray(constr[1], float), np.asarray(constr[2], float),
+                                np.zeros(len(constr[0])))
+    for max_iter in iters:
+        R.estimate_factor(m, max_iter=max_iter, f_init=f0, lam_constr=lc)
+        out = lib.estimate_factor(X, r, nt_min=20, tol=1e-8, max_iter=max_iter, F_init=None if pca_start else f0, constr=constr)
         assert out["stats"]["iters"] == m.fes.iters
         np.testing.assert_allclose(out["F"], m.factor, rtol=1e-9, atol=1e-10)
         np.testing.assert_allclose(out["Lam"], m.lambda_est, rtol=1e-9, atol=1e-10)
-        assert np.isnan(out["Lam"][0]).all()
+        if short_series:
+            assert np.isnan(out["Lam"][0]).all()
         np.testing.assert_allclose(out["stats"]["ssr"], m.fes.ssr, rtol=1e-11)
         np.testing.assert_allclose(out["R2"], m.fes.R2, rtol=1e-8, atol=1e-10)
+        if constr is not None:                                         # the restriction holds (standardized units)
+            for q, i in enumerate(constr[0]):
+                np.testing.assert_allclose(np.asarray(constr[1])[q] @ out["Lam"][i], constr[2][q] / out["xstd"][i], rtol=1e-9, atol=1e-11)
 
 
 def check_constraint(lib, panels):
@@ -147,20 +197,88 @@ def check_full_nonparametric_c1(lib, panels, r=8):
     return g, m, s
 
 
-def check_var_irf(lib, r=3, p=2, T=120):
+def check_var_irf(lib, r=3, p=2, T=120, withconst=True, shocks=(0, 2), H=12, batch=1, rtol=1e-9):
+    """withconst=False: M, Q, G against a companion form built here (the oracle's fill_matrices assumes a constant).
+    batch > 1: the IRF of a batch of that many perturbed models against one oracle IRF per model."""
     _, tr = simulate_panel(10, r, T, rep=6)
     Fm = np.full((T + 3, r), np.nan); Fm[3:] = tr["F"]
-    v = R.VARModel(Fm, p, True, 4, T + 3); R.estimate_var(v)
-    out = lib.estimate_var(Fm[3:], p, True)
-    np.testing.assert_allclose(out["betahat"], v.betahat, rtol=1e-9, atol=1e-11)
-    np.testing.assert_allclose(out["seps"], v.seps, rtol=1e-9)
-    np.testing.assert_allclose(out["M"], v.M, rtol=1e-9, atol=1e-11)
+    v = R.VARModel(Fm, p, withconst, 4, T + 3); R.estimate_var(v, compute_matrices=withconst)
+    out = lib.estimate_var(Fm[3:], p, withconst)
+    np.testing.assert_allclose(out["betahat"], v.betahat, rtol=rtol, atol=1e-11)
+    np.testing.assert_allclose(out["seps"], v.seps, rtol=rtol)
+    if not withconst:
+        k = r * p
+        v.M = np.zeros((k, k)); v.M[:r] = v.betahat.T; v.M[r:, :k - r] = np.eye(k - r)
+        v.Q = np.zeros((r, k)); v.Q[:, :r] = np.eye(r)
+        v.G = np.zeros((k, r)); v.G[:r] = np.linalg.cholesky(v.seps)
+    np.testing.assert_allclose(out["M"], v.M, rtol=rtol, atol=1e-11)
     np.testing.assert_allclose(out["Q"], v.Q, atol=0)
-    np.testing.assert_allclose(out["G"], v.G, rtol=1e-9, atol=1e-12)
+    np.testing.assert_allclose(out["G"], v.G, rtol=rtol, atol=1e-12)
     np.testing.assert_allclose(out["resid"][p:], v.resid[3 + p:], rtol=1e-8, atol=1e-10)
-    irf_ref = R.impulse_response(v, [0, 2], 12)
-    irf = lib.irf(out["M"], out["Q"], out["G"], 12, [0, 2])
+    assert np.isnan(out["resid"][:p]).all()
+    irf_ref = R.impulse_response(v, list(shocks), H)
+    irf = lib.irf(out["M"], out["Q"], out["G"], H, list(shocks))
     np.testing.assert_allclose(irf, irf_ref, rtol=1e-9, atol=1e-12)
+    if batch > 1:
+        scale = 1.0 - 0.1 * np.arange(batch)                           # damped copies: a different IRF per model
+        Mb = np.stack([out["M"] * s for s in scale]); Qb = np.stack([out["Q"]] * batch); Gb = np.stack([out["G"] * (1 + s) for s in scale])
+        got = lib.irf(Mb, Qb, Gb, H, list(shocks))
+        for b in range(batch):
+            vb = R.VARModel(Fm, p, withconst, 4, T + 3); vb.M, vb.Q, vb.G = Mb[b], Qb[b], Gb[b]
+            np.testing.assert_allclose(got[b], R.impulse_response(vb, list(shocks), H), rtol=1e-9, atol=1e-12)
+
+
+def check_loading(lib, N=12, r=3, T=120, n_uarlag=4, nt_min=40, F_holes=(), edge_series=False, exact=False, batch=1):
+    """estimate_loading (loadings, R2, idiosyncratic AR, constant, residuals) vs oracle.estimate_factor_loading and a
+    numpy OLS of each series on [F 1] over the rows where the series and every factor are observed.  F_holes: rows of F
+    set missing; edge_series: series 1 with exactly nt_min usable rows, series 2 with nt_min - 1; exact: series 3 an exact
+    linear combination of the factors (R2 >= 0.9999: zero AR coefficients, ser 0).  batch > 1: that many panels in one
+    call, each also against a one-panel call."""
+    outs, Xs, Fs = [], [], []
+    for b in range(batch):
+        X, tr = simulate_panel(N, r, T, rep=3 + b, standardize=False)
+        F = tr["F"].copy()
+        F[list(F_holes)] = np.nan
+        X[:10, 2 % N] = np.nan
+        use = ~np.isnan(F).any(axis=1)
+        if edge_series:
+            for i, n_use in ((1, nt_min), (2, nt_min - 1)):
+                rows = np.flatnonzero(use & ~np.isnan(X[:, i]))
+                X[rows[n_use:], i] = np.nan
+        if exact:
+            X[:, 3] = 0.5 + F @ (1.0 + np.arange(r)) / r
+        Xs.append(X); Fs.append(F)
+    got = lib.estimate_loading(np.stack(Xs), np.stack(Fs), nt_min=nt_min, n_uarlag=n_uarlag) if batch > 1 else \
+        lib.estimate_loading(Xs[0], Fs[0], nt_min=nt_min, n_uarlag=n_uarlag)
+    for b in range(batch):
+        X, F = Xs[b], Fs[b]
+        g = {k: (v[b] if batch > 1 else v) for k, v in got.items()}
+        if batch > 1:
+            one = lib.estimate_loading(X, F, nt_min=nt_min, n_uarlag=n_uarlag)
+            for k in ("lam", "r2", "uar_coef", "uar_ser", "constant", "resid"):
+                np.testing.assert_allclose(g[k], one[k], rtol=1e-13, atol=1e-14, err_msg=k)
+        assert g["status"] == 0
+        m = R.DFMModel(X, np.ones(N, int), 20, nt_min, 1, T, 0, r, 1e-8, n_uarlag, 2)
+        m.factor[:] = F
+        R.estimate_factor_loading(m)
+        for k, ref, rt in (("lam", m.lambda_, 1e-9), ("r2", m.r2, 1e-9), ("uar_coef", m.uar_coef, 1e-8), ("uar_ser", m.uar_ser, 1e-8)):
+            assert np.array_equal(np.isnan(g[k]), np.isnan(ref)), k
+            np.testing.assert_allclose(g[k], ref, rtol=rt, atol=1e-10, err_msg=k)
+        use = ~np.isnan(F).any(axis=1)
+        for i in range(N):
+            keep = use & ~np.isnan(X[:, i])
+            if keep.sum() < nt_min:
+                assert np.isnan(g["lam"][i]).all() and np.isnan(g["constant"][i]) and np.isnan(g["resid"][:, i]).all()
+                continue
+            Z = np.column_stack([F[keep], np.ones(keep.sum())])
+            beta = np.linalg.lstsq(Z, X[keep, i], rcond=None)[0]
+            np.testing.assert_allclose(g["constant"][i], beta[-1], rtol=1e-9, atol=1e-10)
+            assert np.array_equal(np.isnan(g["resid"][:, i]), ~keep)
+            np.testing.assert_allclose(g["resid"][keep, i], X[keep, i] - Z @ beta, rtol=1e-8, atol=1e-9)
+        if edge_series:
+            assert np.isfinite(g["lam"][1]).all() and np.isnan(g["lam"][2]).all()
+        if exact:
+            assert g["r2"][3] >= 0.9999 and (g["uar_coef"][3] == 0).all() and g["uar_ser"][3] == 0
 
 
 def check_var_missing_rows(lib, r=3, p=2, T=120):
@@ -270,15 +388,17 @@ def check_em_batch_balanced(lib, B=5, N=16, r=2, T=40, path=0, ll_cell_tol=0.0):
         np.testing.assert_allclose(got["Lam"][b], ref["Lam"], rtol=1e-7, atol=1e-9)
 
 
-def check_als_balanced(lib, N=30, r=3, T=80, B=4):
+def check_als_balanced(lib, N=30, r=3, T=80, B=4, per_panel=False):
     """Balanced panels -> fused ALS kernel (one launch for all sweeps): vs the oracle, from a perturbed
-    start so that several sweeps are needed; also PCA start, iteration cap and batch."""
+    start so that several sweeps are needed; also PCA start, iteration cap and batch.  per_panel: the batched call also
+    against one call per panel, and the panels must stop after different numbers of sweeps."""
     rng = np.random.default_rng(3)
     Xb = np.stack([simulate_panel(N, r, T, rep=60 + b, standardize=False)[0] * (1 + 0.3 * b) + b for b in range(B)])
     f0s = []
     for b in range(B):
         xs, _ = R.standardize_data(Xb[b])
-        f0s.append(R.pca_score(xs, r) @ (np.eye(r) + 0.3 * rng.standard_normal((r, r))) + 0.5 * rng.standard_normal((T, r)))
+        wide = 1 + 3 * b if per_panel else 1                             # per_panel: starts further off, panel by panel
+        f0s.append(R.pca_score(xs, r) @ (np.eye(r) + 0.3 * wide * rng.standard_normal((r, r))) + 0.5 * wide * rng.standard_normal((T, r)))
     f0s = np.stack(f0s)
     for max_iter in (1, 4, 100000):
         got = lib.estimate_factor(Xb, r, nt_min=20, tol=1e-8, max_iter=max_iter, F_init=f0s)
@@ -291,6 +411,12 @@ def check_als_balanced(lib, N=30, r=3, T=80, B=4):
             np.testing.assert_allclose(got["stats"][b]["ssr"], m.fes.ssr, rtol=1e-9)
             np.testing.assert_allclose(got["stats"][b]["tss"], m.fes.tss, rtol=1e-12)
             np.testing.assert_allclose(got["R2"][b], m.fes.R2, rtol=1e-7, atol=1e-9)
+            if per_panel:
+                one = lib.estimate_factor(Xb[b], r, nt_min=20, tol=1e-8, max_iter=max_iter, F_init=f0s[b])
+                assert one["stats"]["iters"] == got["stats"][b]["iters"]
+                np.testing.assert_allclose(got["F"][b], one["F"], rtol=1e-12, atol=1e-13)
+        if per_panel and max_iter == 100000:
+            assert len({s["iters"] for s in got["stats"]}) > 1, [s["iters"] for s in got["stats"]]
     # PCA start (sign-aligned)
     got = lib.estimate_factor(Xb[0], r, nt_min=20, tol=1e-8)
     m = R.DFMModel(Xb[0], np.ones(N, int), 20, 40, 1, T, 0, r, 1e-8, 4, 2); R.estimate_factor(m)
@@ -389,12 +515,20 @@ def check_bootstrap_panels(lib, panels, B=2):
     assert np.array_equal(np.isnan(X[0]) | np.isnan(data), np.isnan(X[0]))                 # original missing pattern re-imposed
 
 
-def check_percentiles(lib, n=37, d=11):
+def check_percentiles(lib, n=37, d=11, q=(5, 16, 50, 84, 95, 0, 100), odd_columns=False):
+    """odd_columns: column 0 all NaN (result NaN) and column d - 1 with one finite record (every percentile is that record)."""
+    import warnings
     rng = np.random.default_rng(3)
-    recs = rng.standard_normal((n, d)); recs[5] = np.nan; recs[20] = np.nan             # two failed replications
-    q = [5, 16, 50, 84, 95, 0, 100]
+    recs = rng.standard_normal((n, d)); recs[5 % n] = np.nan; recs[20 % n] = np.nan      # two failed replications
+    if odd_columns:
+        recs[:, 0] = np.nan
+        recs[:, d - 1] = np.nan; recs[n // 2, d - 1] = 1.25
+    q = list(q)
     got = lib.percentiles(recs, q)
-    ref = np.nanpercentile(recs, q, axis=0)
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)               # (the all-NaN column)
+        ref = np.nanpercentile(recs, q, axis=0)
+    assert np.array_equal(np.isnan(got), np.isnan(ref))
     np.testing.assert_allclose(got, ref, rtol=1e-12, atol=1e-14)
     got1 = lib.percentiles(recs[:1], [50.0])
     np.testing.assert_allclose(got1[0], recs[0])
@@ -416,32 +550,44 @@ def check_em_block_missing(lib, path=1):
     np.testing.assert_allclose(got["A"], ref["A"], rtol=1e-8, atol=1e-10)
 
 
-def check_instability(lib, panels, r=4, series=None):
-    """f4: Chow / QLR statistics (HAC) on the hom_fac_1 panel vs the oracle (pinned on the notebook's Table 4(a))."""
+def check_instability(lib, panels, r=4, series=None, q=6, ccut=0.15, qlr0=False, data=None, factor=None, lastpre=104,
+                      min_obs=80):
+    """f4: Chow / QLR statistics (HAC) on the hom_fac_1 panel vs the oracle (pinned on the notebook's Table 4(a)).
+    data / factor: another panel and its factors instead (no estimation); qlr0: also the q = 0 QLR, against the oracle's
+    QLR with q = 0 over the same break rows."""
     import dynamic_factor_models_b200 as D
-    data, incl = panels["all_bpdata"], panels["all_inclcode"]
-    mo = R.DFMModel(data, incl, 20, 40, 3, 224, 0, r, 1e-8, 4, 4)
-    R.estimate_factor(mo, computeR2=False)
+    if data is None:
+        data, incl = panels["all_bpdata"], panels["all_inclcode"]
+        mo = R.DFMModel(data, incl, 20, 40, 3, 224, 0, r, 1e-8, 4, 4)
+        R.estimate_factor(mo, computeR2=False)
+        factor = mo.factor
     cols = np.arange(data.shape[1]) if series is None else np.asarray(series)
-    sub = R.DFMModel(data[:, cols], np.ones(len(cols), int), 20, 40, 3, 224, 0, r, 1e-8, 4, 4)
-    sub.factor[:] = mo.factor
-    chow_o, qlr_o = R.instability_tests(sub, 104)
-    mg = D.DFMModel(data[:, cols], np.ones(len(cols), int), 20, 40, 3, 224, 0, r, 1e-8, 4, 4)
-    mg.factor[:] = mo.factor                                   # same regressors: the test isolates the instability kernels
-    chow_g, qlr_g = D.instability_tests(mg, 104, lib=lib)
+    sub = type("M", (), {})(); sub.data = data[:, cols]; sub.factor = factor; sub.ns = len(cols)
+    chow_o, qlr_o = R.instability_tests(sub, lastpre, q=q, ccut=ccut, min_obs=min_obs)
+    mg = type("M", (), {})(); mg.data = data[:, cols]; mg.factor = factor   # same regressors: the test isolates the instability kernels
+    got = D.instability_tests(mg, lastpre, q=q, ccut=ccut, min_obs=min_obs, lib=lib, want_q0=qlr0)
+    chow_g, qlr_g = got[:2]
     assert np.array_equal(np.isnan(chow_o), np.isnan(chow_g)) and np.array_equal(np.isnan(qlr_o), np.isnan(qlr_g))
     ok = ~np.isnan(chow_o)
     assert ok.sum() >= 1
     np.testing.assert_allclose(chow_g[ok], chow_o[ok], rtol=1e-8)
     np.testing.assert_allclose(qlr_g[ok], qlr_o[ok], rtol=1e-8)
+    if qlr0:
+        _, qlr0_o = R.instability_tests(sub, lastpre, q=0, ccut=ccut, min_obs=min_obs)
+        assert np.array_equal(np.isnan(qlr0_o), np.isnan(got[2]))
+        np.testing.assert_allclose(got[2][ok], qlr0_o[ok], rtol=1e-8)
 
 
-def check_fit_correlation(lib, panels, r=4):
-    """f4, lower half of Table 4(a): cor(yhat_full, yhat_pre/post) per series vs the oracle (same factors on both sides)."""
-    data, incl = panels["all_bpdata"], panels["all_inclcode"]
-    ms = [R.DFMModel(data, incl, 20, 40, i0, i1, 0, r, 1e-8, 4, 4) for i0, i1 in ((3, 224), (3, 104), (105, 224))]
-    for m in ms:
-        R.estimate_factor(m, computeR2=False)
+def check_fit_correlation(lib, panels, r=4, data=None, factors=None):
+    """f4, lower half of Table 4(a): cor(yhat_full, yhat_pre/post) per series vs the oracle (same factors on both sides).
+    data / factors: another panel and its (full, pre, post) factors instead (no estimation)."""
+    if data is None:
+        data, incl = panels["all_bpdata"], panels["all_inclcode"]
+        ms = [R.DFMModel(data, incl, 20, 40, i0, i1, 0, r, 1e-8, 4, 4) for i0, i1 in ((3, 224), (3, 104), (105, 224))]
+        for m in ms:
+            R.estimate_factor(m, computeR2=False)
+    else:
+        ms = [type("M", (), dict(data=data, factor=f, ns=data.shape[1]))() for f in factors]
     for alt in ms[1:]:
         ref = R.fitted_value_correlations(ms[0], alt, 104)
         got = D.fitted_value_correlations(ms[0], alt, 104, lib=lib)
