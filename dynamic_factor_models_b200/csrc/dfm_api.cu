@@ -86,6 +86,7 @@ struct ProfRec { const char* name;
 struct dfm_handle {
   int device;
   int nsm;                     // streaming multiprocessors of the device: sizes grids and the per-panel CTA plans
+  int l2_bytes;                // L2 cache size: sizes the share of each resident panel the TMA kernels keep in L2
   cudaStream_t stream;
   cudaStream_t copy_stream;    // second stream: the H2D copies of the streaming host path run here, under the EM kernel
   cudaStream_t d2h_stream;     // third stream: results of finished panels go back while the kernel is still running
@@ -255,14 +256,25 @@ static int resident_grid(const dfm_handle* h, K kern, int threads, size_t smem, 
 #endif
 }
 
+// Series-block groups per panel that `grid` CTAs of a TMA kernel keep in L2 at evict-last priority (f2_keep_stages):
+// F2_L2KEEP_PCT of L2 split over the CTAs active in a round; keep[0] for the full rounds, keep[1] for the tail round.
+static void l2_keep_plan(const dfm_handle* h, int grid, int B, int T, int N, int keep[2]) {
+  const long long budget = (long long)h->l2_bytes * F2_L2KEEP_PCT / 100, group = 64LL * F2_SBS * T;   // 64 T bytes per 8 series
+  const long long nsg = (N + 8 * F2_SBS - 1) / (8 * F2_SBS);
+  const int tail = (B % grid) ? B % grid : grid;
+  keep[0] = (int)std::min(nsg, budget / (grid * group));
+  keep[1] = (int)std::min(nsg, budget / (tail * group));
+}
+
 // One launch of the fused EM kernel over all panels of fa (fa.scratch: min(B, nsm * 8) * T * FUSED_SCR(r) doubles):
 // k_em_fused2 (TMA panel ring, even T) when use2, else k_em_fused.
-static int launch_em_fused(dfm_handle* h, const FusedArgs& fa, int r, bool use2) {
+static int launch_em_fused(dfm_handle* h, FusedArgs fa, int r, bool use2) {
   return dispatch<1, 8>(r, [&](auto R) -> int {
     constexpr int RT = decltype(R)::value;
     if (use2) {
       const size_t smem = fused2_smem_doubles<RT>(fa.T, fa.N) * 8;
       const int grid = resident_grid(h, k_em_fused2<RT>, 256, smem, fa.B);
+      l2_keep_plan(h, grid, fa.B, fa.T, fa.N, fa.l2_keep);
       CUtensorMap tm; int rc = make_panel_tmap(h, fa.X, fa.T, (long long)fa.B * fa.N, &tm); if (rc) return rc;
       L(k_em_fused2<RT>, grid, 1, 256, smem, fa, tm);
     } else {
@@ -460,11 +472,12 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
   return DFM_OK;
 }
 
-static int launch_als_fused2(dfm_handle* h, const AlsFusedArgs& fa, int r) {
+static int launch_als_fused2(dfm_handle* h, AlsFusedArgs fa, int r) {
   return dispatch<1, 8>(r, [&](auto R) -> int {
     constexpr int RT = decltype(R)::value;
     const size_t smem = als_fused2_smem_doubles<RT>(fa.T, fa.N) * 8;
     const int grid = resident_grid(h, k_als_fused2<RT>, 256, smem, fa.B);
+    l2_keep_plan(h, grid, fa.B, fa.T, fa.N, fa.l2_keep);
     CUtensorMap tm; int rc = make_panel_tmap(h, fa.Xs, fa.T, (long long)fa.B * fa.N, &tm); if (rc) return rc;
     L(k_als_fused2<RT>, grid, 1, 256, smem, fa, tm);
     return DFM_OK;
@@ -681,12 +694,14 @@ int dfm_create_on_stream(int device, void* cuda_stream, dfm_handle** out) {
   dfm_handle* h = new (std::nothrow) dfm_handle();
   if (!h) return DFM_ERR_CUDA;
   h->device = device; h->ws = nullptr; h->ws_bytes = 0; h->launches = 0; h->err[0] = 0;
-  h->nsm = 132;                // H100 SXM; the CUDA build reads the device's count below (the emulation build has no device)
+  h->nsm = 132;                // H100 SXM; the CUDA build reads the device's values below (the emulation build has no device)
+  h->l2_bytes = 50 << 20;
   h->profile = 0; h->prof = new std::vector<ProfRec>();
   h->stream = nullptr; h->own_stream = false;
   h->copy_stream = nullptr; h->pinned_one = nullptr; h->d2h_stream = nullptr; h->done_host = nullptr; h->done_dev = nullptr; h->done_cap = 0;
 #ifndef DFM_EMU
   if (cudaDeviceGetAttribute(&h->nsm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || h->nsm <= 0) { handle_teardown(h); return DFM_ERR_CUDA; }
+  if (cudaDeviceGetAttribute(&h->l2_bytes, cudaDevAttrL2CacheSize, device) != cudaSuccess) { handle_teardown(h); return DFM_ERR_CUDA; }
   if (cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { h->copy_stream = nullptr; handle_teardown(h); return DFM_ERR_CUDA; }
   if (cudaStreamCreateWithFlags(&h->d2h_stream, cudaStreamNonBlocking) != cudaSuccess) { h->d2h_stream = nullptr; handle_teardown(h); return DFM_ERR_CUDA; }
   if (cudaHostAlloc((void**)&h->pinned_one, sizeof(int), cudaHostAllocDefault) != cudaSuccess) { h->pinned_one = nullptr; handle_teardown(h); return DFM_ERR_CUDA; }

@@ -45,6 +45,9 @@ static_assert(F2_TC % 16 == 4 || F2_TC % 16 == 12, "ring pitch must be 4 or 12 m
 static_assert(F2_TC <= 256 && (F2_TC * 64) % 128 == 0, "TMA box / stage alignment");
 #define F2_NEXS(R_) ((F2_S * F2_STG - 4 * (R_) * (R_)) / FUSED_SCR(R_))   // the last 4 R^2 doubles of the idle ring hold scan matrices
 #define F2_RTAIL(R_) (F2_S * F2_STG - 4 * (R_) * (R_))
+#ifndef F2_L2KEEP_PCT
+#define F2_L2KEEP_PCT 55   // share of L2 the resident panels may keep at evict-last priority (f2_keep_stages); 40 and 55
+#endif                     // tied, 70 was slower, on c5 (H100 SXM 80GB, 700 W, 1980 MHz)
 
 #ifndef DFM_EMU
 __device__ __forceinline__ uint32_t f2_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -54,10 +57,30 @@ __device__ __forceinline__ void f2_mbar_arrive(uint64_t* bar) { asm volatile("mb
 __device__ __forceinline__ void f2_mbar_wait(uint64_t* bar, uint32_t phase) {
   asm volatile("{\n.reg .pred p;\nWAIT_%=:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}" ::"r"(f2_smem_u32(bar)), "r"(phase) : "memory");
 }
-// one 2-D tensor-map copy (SASS UTMALDG): box F2_TS periods x 8 series of the [T, B*N] view of the batch
-__device__ __forceinline__ void f2_tma_2d(void* dst, const CUtensorMap* tmap, int x, int y, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               ::"r"(f2_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(x), "r"(y), "r"(f2_smem_u32(bar)) : "memory");
+// one 2-D tensor-map copy (SASS UTMALDG): box F2_TS periods x 8 series of the [T, B*N] view of the batch, with an L2
+// eviction policy made by createpolicy
+__device__ __forceinline__ void f2_tma_2d(void* dst, const CUtensorMap* tmap, int x, int y, uint64_t* bar, uint64_t policy) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;"
+               ::"r"(f2_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(x), "r"(y), "r"(f2_smem_u32(bar)), "l"(policy) : "memory");
+}
+
+// L2 residency plan.  Each EM iteration (ALS sweep) reads the whole panel twice, but the resident panels are several
+// times larger than L2, so a plain stream evicts every line long before its CTA reads it again.  Instead the series of
+// the first `keep` series-block groups of a panel (keep x 8 F2_SBS series, all periods) are loaded with evict-last
+// priority and stay in L2 across both passes of all iterations of that panel; the rest streams through with
+// evict-first.  The CTAs of one round of panels share a fixed share of L2 (F2_L2KEEP_PCT); the host turns it into
+// keep[0] for the full rounds and keep[1] for the tail round, whose fewer CTAs may each keep more.
+__device__ __forceinline__ int f2_keep_stages(const int* keep, int B, int b) {
+  const int G = (int)gridDim.x;
+  return (b / G < B / G) ? keep[0] : keep[1];
+}
+// Demotes the kept lines of a finished panel (rows [row0, row0 + 8 F2_SBS keep) of the [T, rows] view at X) to normal
+// priority, so that they do not crowd out the next panel's slice or other work on the GPU.  All threads of the CTA.
+__device__ __forceinline__ void f2_release(const double* X, long long row0, int keep, int T, long long rows) {
+  const long long r1 = min(row0 + 8LL * F2_SBS * keep, rows);
+  const uintptr_t a0 = reinterpret_cast<uintptr_t>(X + row0 * T) & ~(uintptr_t)127, a1 = reinterpret_cast<uintptr_t>(X + r1 * T);
+  for (uintptr_t p = a0 + (uintptr_t)threadIdx.x * 128; p < a1; p += (uintptr_t)blockDim.x * 128)
+    asm volatile("applypriority.L2::evict_normal [%0], 128;" ::"l"(p) : "memory");
 }
 #endif
 
@@ -76,18 +99,23 @@ struct F2Ring {
 // [T, B*N] view of the batch (column runs of 800 B; the box is 4 periods wider than the chunk so that the
 // dense row pitch in shared memory is == 4 mod 16, i.e. conflict-free; rows/periods beyond the tensor are
 // zero-filled, rows of the next panel are masked by the consumers).  Eight 1-D bulk copies per stage were
-// issue-bound (requests serialised over the lanes of a warp: tools/bench_stream.cu).
-__device__ __forceinline__ void f2_produce(F2Ring& rg, const CUtensorMap* tmap, int row0, int T, int N, bool c_outer) {
+// issue-bound (requests serialised over the lanes of a warp: tools/bench_stream.cu).  Series-block groups sb < *keep
+// are loaded with evict-last priority, the others with evict-first (f2_keep_stages; *keep is in shared memory).  Both
+// policies are made once per pass: per copy they would lengthen the producer's issue path, which bounds a lone CTA.
+__device__ __forceinline__ void f2_produce(F2Ring& rg, const CUtensorMap* tmap, int row0, int T, int N, bool c_outer, const int* keep) {
   const int lane = threadIdx.x & 31;
   const int nsb = (N + 8 * F2_SBS - 1) / (8 * F2_SBS), nck = (T + F2_TC - 1) / F2_TC;      // (stages per pass: series-block groups x chunks)
-  const int n_out = c_outer ? nck : nsb, n_in = c_outer ? nsb : nck;
+  const int n_out = c_outer ? nck : nsb, n_in = c_outer ? nsb : nck, nkeep = *keep;
+  uint64_t pol_last, pol_first;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_last));
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_first));
   for (int o = 0; o < n_out; ++o)
     for (int i = 0; i < n_in; ++i) {
       const int c = c_outer ? o : i, sb = c_outer ? i : o;
       if (rg.wrap) f2_mbar_wait(&rg.empty[rg.rs], rg.rph ^ 1);
       if (lane == 0) {
         f2_mbar_expect(&rg.full[rg.rs], (uint32_t)(F2_STG * 8));
-        f2_tma_2d(rg.ring + (size_t)rg.rs * F2_STG, tmap, c * F2_TC, row0 + sb * 8 * F2_SBS, &rg.full[rg.rs]);
+        f2_tma_2d(rg.ring + (size_t)rg.rs * F2_STG, tmap, c * F2_TC, row0 + sb * 8 * F2_SBS, &rg.full[rg.rs], sb < nkeep ? pol_last : pol_first);
       }
       __syncwarp();
       rg.advance();
@@ -270,7 +298,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
   double* tmp = Pfprev + RR;               // 2R
   double* red = tmp + 2 * R;               // 40
   double* scal = red + 40;                 // 8: [0]=slr [1]=ld_inf [2]=qsum
-  int* ctl = (int*)(scal + 8);             // [0]=nE [1]=tb [2]=bad [3]=frozen
+  int* ctl = (int*)(scal + 8);             // [0]=nE [1]=tb [2]=bad [3]=frozen [4]=series-block groups kept in L2
   double* bnd = scal + 16;                 // (3*32+1) R + RR: blk_recur workspace for 32 groups
   double* part = bnd;                                // [2][F2_NCW][72] M-pass partial accumulators: ALIASES the scan
                                                      // workspace (used only inside the M pass / only in P3, P5)
@@ -312,6 +340,9 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       M[e] = a.A[(size_t)b * RR + i + R * j]; Q[e] = a.Q[(size_t)b * RR + i + R * j];
     }
     if (DFM_TID == 0) ctl[2] = 0;
+#ifndef DFM_EMU
+    if (DFM_TID == 0) ctl[4] = f2_keep_stages(a.l2_keep, a.B, b);
+#endif
     DFM_SYNC();
     if (a.P0out || a.ready) {
       // initial state covariance in the kernel: P0 = sum_i A^i Q A'^i by doubling (same recursion as k_lyapunov), on
@@ -536,7 +567,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         // TMA pass (see f2_produce / f2_consume_E): warp 0 produces, warps 1..6 consume, warp 7 runs the
         // data-independent covariance chain concurrently
         const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
-        if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true);
+        if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true, &ctl[4]);
         else if (DFM_WARP <= F2_NCW) qacc += f2_consume_E<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, rinv);
         else {
           rg.skip(nitems);                                                   // keep the ring position in step
@@ -817,7 +848,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
         const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
-        if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false);
+        if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false, &ctl[4]);
         else if (DFM_WARP <= F2_NCW) f2_consume_M<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part);
         else {
           rg.skip(nitems);
@@ -857,6 +888,9 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       ll_prev = ll;
       if (conv) { ++it; break; }
     }
+#ifndef DFM_EMU
+    f2_release(a.X, (long long)b * N, ctl[4], T, (long long)a.B * N);    // (every copy of this panel has completed)
+#endif
     // ---- outputs
     for (int e = DFM_TID; e < N * R; e += DFM_NT) { int i = e % N, c = e / N; a.Lam[(size_t)b * N * R + e] = Lam[LI(i, c)]; }
     for (int e = DFM_TID; e < N; e += DFM_NT) a.R[(size_t)b * N + e] = Rv[e];
@@ -908,6 +942,7 @@ struct AlsFusedArgs {
   int B, T, N;
   double tol;
   long long max_iter;
+  int l2_keep[2];       // series-block groups per panel kept in L2: full rounds, tail round (f2_keep_stages)
 };
 
 template <int R>
@@ -922,7 +957,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
   double* FtF = sxx + N;  double* Gi = FtF + RR;  double* LtL = Gi + RR;  double* Hi = LtL + RR;
   double* tmp = Hi + RR;                   // 2R
   double* red = tmp + 2 * R;               // 40
-  int* ctl = (int*)(red + 40);             // [0] = bad
+  int* ctl = (int*)(red + 40);             // [0] = bad, [1] = series-block groups kept in L2
   double* part = red + 48;                 // 2 * F2_NCW * 72
   double* ring = part + 2 * F2_NCW * 72;
 #ifndef DFM_EMU
@@ -940,6 +975,9 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
     DFM_SYNC();
     for (int e = DFM_TID; e < T * R; e += DFM_NT) { int t = e % T, c = e / T; Z[ZI(t, c)] = a.F[(size_t)b * T * R + e]; }
     if (DFM_TID == 0) ctl[0] = 0;
+#ifndef DFM_EMU
+    if (DFM_TID == 0) ctl[1] = f2_keep_stages(a.l2_keep, a.B, b);
+#endif
     DFM_SYNC();
     double ssr = 0.0, ssr_old = 0.0;
     long long it = 0;
@@ -962,7 +1000,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
         sxx[n] = s2;
       }
 #else
-      if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false);
+      if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false, &ctl[1]);
       else if (DFM_WARP <= F2_NCW) f2_consume_M<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part);
       else rg.skip(nitems);
 #endif
@@ -994,7 +1032,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
         for (int n = 0; n < N; ++n) { double x = X[(size_t)n * T + t]; tssp += x * x; for (int c = 0; c < R; ++c) Z[ZI(t, c)] += x * Lam[LI(n, c)]; }
       }
 #else
-      if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true);
+      if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true, &ctl[1]);
       else if (DFM_WARP <= F2_NCW) tssp += f2_consume_E<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, nullptr);
       else rg.skip(nitems);
 #endif
@@ -1019,6 +1057,9 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
       if (!(fabs(ssr_old - ssr) >= a.tol * (double)T * (double)N)) break;            // :367-368
       if (it >= a.max_iter) { status = 4; break; }
     }
+#ifndef DFM_EMU
+    f2_release(a.Xs, (long long)b * N, ctl[1], T, (long long)a.B * N);
+#endif
     for (int e = DFM_TID; e < T * R; e += DFM_NT) { int t = e % T, c = e / T; a.F[(size_t)b * T * R + e] = Z[ZI(t, c)]; }
     for (int e = DFM_TID; e < N * R; e += DFM_NT) { int i = e % N, c = e / N; a.Lam[(size_t)b * N * R + e] = Lam[LI(i, c)]; }
     if (DFM_TID == 0) { a.st[b].ssr_old = ssr_old; a.st[b].ssr = ssr; a.st[b].iters = (int)it; a.st[b].done = 1; a.st[b].status = status; }
