@@ -29,13 +29,15 @@ namespace dfm {
 #define F2_SBS 1        // 8-series blocks per stage (= per tensor-map copy): a copy has a fixed cost whatever its size
 #endif                  // (tools/bench_tma2d.cu), so wider stages raise the rate a single CTA can stream at
 #ifndef F2_S
-#define F2_S (4 / F2_SBS)   // ring stages (the ring keeps its size: F2_S * F2_SBS * 8 * F2_TS doubles)
+#define F2_S (3 / F2_SBS)   // ring stages (the ring keeps its size: F2_S * F2_SBS * 8 * F2_TS doubles)
 #endif
 #define F2_STG (F2_SBS * 8 * F2_TS)   // doubles per stage
 #ifndef F2_TC
-#define F2_TC 132       // periods per stage == row pitch in the ring; must be == 4 or 12 (mod 16) so that the
-#endif                  // DMMA fragment loads are bank-conflict free, and <= 256 (TMA box limit)
-#define F2_TS F2_TC     // (box width == chunk stride: no re-read of periods; T = 500 -> 4 chunks)
+#define F2_TC 172       // periods per stage == row pitch in the ring; must be == 4 or 12 (mod 16) so that the
+#endif                  // DMMA fragment loads are bank-conflict free, and <= 256 (TMA box limit).  A copy costs about
+                        // the same whatever its size, so T = 500 in 3 chunks of 172 (3 stages) beat 4 of 132 (4 stages)
+                        // on c5 by 4 % (H100 SXM 80GB, 700 W, 1980 MHz); 4 chunks of 164 were 7 % slower
+#define F2_TS F2_TC     // (box width == chunk stride: no re-read of periods)
 #define F2_NCW 6        // consumer warps (warps 1..6; warp 0 = producer, warp 7 = chain / solves)
 #define F2_GPARTS_S 4                                    // scalar Gram path: time slices per matrix entry
 #define F2_GPARTS ((R == 8) ? (F2_NCW + 1) : F2_GPARTS_S)   // partial Gram matrices (tensor path: one per warp of P3-P5)
