@@ -68,6 +68,15 @@ class SsOut(C.Structure):
 SS_OUTPUTS = ("F", "PF", "common", "xhat", "xvar")
 
 
+class SimOpts(C.Structure):
+    _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("n_draw", C.c_longlong),
+                ("draw0", C.c_longlong), ("seed", C.c_ulonglong), ("mem", C.c_int)]
+
+
+class SimOut(C.Structure):
+    _fields_ = [("F", C.c_void_p), ("X", C.c_void_p), ("status", C.c_void_p)]
+
+
 def default_library_path():
     return os.path.join(HERE, "lib", "libdfm_b200.so")
 
@@ -75,7 +84,8 @@ def default_library_path():
 EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stream", "dfm_destroy", "dfm_sync",
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
-           "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_kalman_smooth", "dfm_em_init_from_factors",
+           "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_kalman_smooth", "dfm_simulation_smoother",
+           "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -143,6 +153,7 @@ class Library:
                               C.c_int, C.c_int, C.c_void_p]
         L.dfm_em_kalman.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(EmOpts), C.POINTER(EmInit), C.POINTER(EmOut)]
         L.dfm_kalman_smooth.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsOpts), C.POINTER(EmInit), C.POINTER(SsOut)]
+        L.dfm_simulation_smoother.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SimOpts), C.POINTER(EmInit), C.POINTER(SimOut)]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p]
         L.dfm_bootstrap_panels.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 8
@@ -213,6 +224,15 @@ class Library:
         ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
         ou = SsOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
         self.check(self.lib.dfm_kalman_smooth(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_kalman_smooth")
+
+    def simulation_smoother_raw(self, X, T, N, r, p, H, n_draw, draw0, seed, params, out, mem):
+        """Pointer-level dfm_simulation_smoother (ints = device or host addresses).  params: dict Lam, R, A, Q[, P0]; out: dict
+        of F, X, status (missing or 0 = NULL)."""
+        o = SimOpts(T=T, N=N, r=r, p=p, H=H, n_draw=n_draw, draw0=draw0, seed=seed, mem=mem)
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
+        ou = SimOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
+        self.check(self.lib.dfm_simulation_smoother(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)),
+                   "dfm_simulation_smoother")
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)
@@ -444,4 +464,22 @@ class Library:
                 res[n] = pf if b else pf[0]
             else:
                 res[n] = from_cm(a_, Tp, r if n == "F" else N, b)
+        return res
+
+    def simulation_smoother(self, X, Lam, R, A, Q, p=1, P0=None, H=0, n_draw=1, seed=0, draw0=0, outputs=("F", "X")):
+        """Draws draw0 .. draw0 + n_draw - 1 from the joint posterior of the factor path and the missing cells at FIXED
+        parameters (dfm_simulation_smoother).  X (T, N) standardized with NaN, one model; parameters as kalman_smooth.  Returns
+        F (n_draw, T+H, r) and X (n_draw, T+H, N) -- those named in `outputs` -- and status."""
+        X = np.asarray(X, float); T, N = X.shape; r = np.asarray(Lam).shape[-1]; Tp = T + H
+        bufs = dict(X=to_cm(X), Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float), A=to_cm(A), Q=to_cm(Q),
+                    P0=to_cm(P0) if P0 is not None else None)
+        size = dict(F=Tp * r, X=Tp * N)
+        outs = {n: np.empty(n_draw * size[n]) for n in outputs}
+        ost = np.empty(1, dtype=np.int32)
+        self.simulation_smoother_raw(bufs["X"].ctypes.data, T, N, r, p, H, n_draw, draw0, seed,
+                                     {n: (bufs[n].ctypes.data if bufs[n] is not None else 0) for n in ("Lam", "R", "A", "Q", "P0")},
+                                     {**{n: a_.ctypes.data for n, a_ in outs.items()}, "status": ost.ctypes.data}, MEM_HOST)
+        res = dict(status=int(ost[0]))
+        for n, a_ in outs.items():
+            res[n] = from_cm(a_, Tp, r if n == "F" else N, n_draw)
         return res

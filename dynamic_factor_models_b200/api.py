@@ -213,8 +213,22 @@ def forecast(m, H, lib=None):
       common (T+H, ns) the common component lambda_i' E[f_t | data] in data units (xmean + xstd * common, as compute_series);
       loglik           log-likelihood of the observed cells at m.em's parameters.
     Series left out of the model (too few observations for the ALS step) have NaN columns."""
+    b = _state_space_block(m, H, lib, "forecast")
+    lib, e = b["lib"], b["em"]
+    o = lib.kalman_smooth(b["Xs"], b["Lam"], e["R"], e["A"], e["Q"], p=b["p"], P0=e["P0"], H=H)
+    if o["status"] != 0:
+        raise RuntimeError(f"forecast: device status {o['status']}")
+    xmean, xstd = b["xmean"], b["xstd"]
+    return dict(periods=b["periods"], series=b["series"], factor=o["F"], factor_var=o["PF"],
+                xhat=xmean + xstd * o["xhat"], xvar=xstd ** 2 * o["xvar"], common=xmean + xstd * o["common"],
+                loglik=o["loglik"])
+
+
+def _state_space_block(m, H, lib, what):
+    """The estimation block of a model estimated with Parametric(), standardized as `estimate` standardizes it, with the
+    series left out of the model (NaN ALS loadings) set to NaN, and the EM estimates with those series' loadings NaN."""
     if m.em is None:
-        raise ValueError("forecast needs a model estimated with Parametric()")
+        raise ValueError(f"{what} needs a model estimated with Parametric()")
     if H < 0:
         raise ValueError("H must be >= 0")
     lib = lib or get_library()
@@ -225,14 +239,41 @@ def forecast(m, H, lib=None):
     out_model = np.isnan(m.lambda_est[:, 0])
     Xs = np.where(out_model[None, :], np.nan, Xs)
     e = m.em
-    r = e["Lam"].shape[1]; p = e["A"].shape[1] // r
-    Lam = np.where(out_model[:, None], np.nan, e["Lam"])
-    o = lib.kalman_smooth(Xs, Lam, e["R"], e["A"], e["Q"], p=p, P0=e["P0"], H=H)
+    r = e["Lam"].shape[1]
+    return dict(lib=lib, periods=np.arange(i0, i1 + H + 1), series=incl, Xs=Xs, xmean=xmean, xstd=xstd, em=e, p=e["A"].shape[1] // r,
+                Lam=np.where(out_model[:, None], np.nan, e["Lam"]))
+
+
+def posterior_draws(m, H, n_draw, seed, draw0=0, lib=None):
+    """Draws from the JOINT posterior of the factor path and the missing / forecast values of a model estimated with
+    `estimate(m, Parametric())`, at its EM estimates (simulation smoother, dfm_simulation_smoother).
+
+    Same block as `forecast(m, H)` (rows `periods`, columns `series`).  Returns a dict with
+      factor (n_draw, T+H, r)  draws of f_t (standardized units, as m.factor);
+      x (n_draw, T+H, ns)      draws of the panel in data units: the data where observed, a draw where missing or forecast;
+    draw j is draw id draw0 + j of stream `seed` (any split of a draw range gives the same draws).  Functions of a path --
+    growth rates, averages, threshold probabilities -- take their posterior distribution from these draws; forecast's
+    xhat / xvar are their means / variances cell by cell.  Series left out of the model have NaN columns."""
+    b = _state_space_block(m, H, lib, "posterior_draws")
+    lib, e = b["lib"], b["em"]
+    o = lib.simulation_smoother(b["Xs"], b["Lam"], e["R"], e["A"], e["Q"], p=b["p"], P0=e["P0"], H=H, n_draw=n_draw, seed=seed,
+                                draw0=draw0)
     if o["status"] != 0:
-        raise RuntimeError(f"forecast: device status {o['status']}")
-    return dict(periods=np.arange(i0, i1 + H + 1), series=incl, factor=o["F"], factor_var=o["PF"],
-                xhat=xmean + xstd * o["xhat"], xvar=xstd ** 2 * o["xvar"], common=xmean + xstd * o["common"],
-                loglik=o["loglik"])
+        raise RuntimeError(f"posterior_draws: device status {o['status']}")
+    return dict(periods=b["periods"], series=b["series"], factor=o["F"], x=b["xmean"] + b["xstd"] * o["X"])
+
+
+def forecast_bands(m, H, q, n_draw, seed, lib=None):
+    """Percentile bands (numpy.percentile's linear interpolation, on the device through dfm_percentiles) of the panel draws
+    of `posterior_draws(m, H, n_draw, seed)`, cell by cell.  Returns a dict with bands (len(q), T+H, ns) in data units, rows
+    `periods`, columns `series` as forecast(m, H), and q.  n_draw <= 16384."""
+    if not 1 <= n_draw <= 16384:
+        raise ValueError("forecast_bands: n_draw must be in [1, 16384]")
+    lib = lib or get_library()
+    d = posterior_draws(m, H, n_draw, seed, lib=lib)
+    x = d["x"]
+    bands = lib.percentiles(x.reshape(n_draw, -1), q)
+    return dict(periods=d["periods"], series=d["series"], q=np.asarray(q, float), bands=bands.reshape((len(q),) + x.shape[1:]))
 
 
 def em_init_from_factors(Xs, F, p=1, lib=None):

@@ -12,6 +12,7 @@
 #include "dfm_kernels_als_masked.cuh"
 #include "dfm_kernels_rep.cuh"
 #include "dfm_kernels_inst.cuh"
+#include "dfm_kernels_sim.cuh"
 #include <algorithm>
 #include <new>
 #include <thread>
@@ -1215,78 +1216,117 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
 }
 
 // ------------------------------------------------------------------------------------ a'': smoothing / nowcasting / forecasting
-// One E-step of the general path at fixed parameters on panels padded with H all-missing periods, then k_ss_project.
-// Nothing here writes the parameter buffers: k_em_prep runs only in its opening mode (W, log R, C), k_em_filter_smooth's
-// transition M-step goes to scratch, and no measurement M-step or closing step is launched.
+// One E-step of the general path at fixed parameters on panels padded with H all-missing periods (ss_estep), shared by
+// dfm_kalman_smooth (then k_ss_project) and dfm_simulation_smoother (then the k_sim_* kernels).  Nothing here writes the
+// parameter buffers: k_em_prep runs only in its opening mode (W, log R, C), k_em_filter_smooth's transition M-step goes to
+// scratch, and no measurement M-step or closing step is launched.
+
+// Shapes and options both entry points accept (`what`: the entry point, for the error message).
+static int ss_check(dfm_handle* h, const char* what, int T, int N, int r, int p, int H, int batch, int mem) {
+  char msg[128];
+  if (T <= 0 || N <= 0 || r <= 0 || r > 64 || p <= 0 || H < 0 || batch <= 0 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE) ||
+      (long long)T + H < 2) {
+    snprintf(msg, sizeof(msg), "%s: bad shape/options", what);
+    return fail(h, DFM_ERR_ARG, msg);
+  }
+  if (batch > kMaxGridBatch) { snprintf(msg, sizeof(msg), "%s: batch > 65535", what); return fail(h, DFM_ERR_UNSUPPORTED, msg); }
+  const int stgT = fs_stage_periods(h->nsm, batch, r, p);
+  if (r * p > 48 || em_fs_smem_doubles(r, p, stgT) * 8 > kMaxSmem) {
+    snprintf(msg, sizeof(msg), "%s: state dimension r*p too large for the general path", what);
+    return fail(h, DFM_ERR_UNSUPPORTED, msg);
+  }
+  return DFM_OK;
+}
+
+// Device buffers of the fixed-parameter E-step over B panels of Tp = T + H periods, and the device views of its inputs.
+struct SsStage {
+  double *Xp, *L, *R, *A, *Q, *P0, *Fs, *PsF, *ll;
+  EmState* st;
+  int *it, *stat;
+  GenBufs g;
+  const double *x, *pL, *pR, *pA, *pQ;            // padded panels and parameters on the device (set by ss_estep)
+};
+static SsStage ss_bufs(Arena& a, int mem, int H, size_t B, int Tp, int N, int r, int p) {
+  const size_t TN = (size_t)Tp * N; const int k = r * p, kk = k * k, rr = r * r, rk = r * k, np = r * (r + 1) / 2;
+  SsStage s{};
+  // padded panel: needed unless the input is already on the device with nothing to pad
+  s.Xp = (mem == DFM_MEM_HOST || H > 0) ? a.get<double>(B * TN) : nullptr;
+  s.L = mem == DFM_MEM_HOST ? a.get<double>(B * N * r) : nullptr;
+  s.R = mem == DFM_MEM_HOST ? a.get<double>(B * N) : nullptr;
+  s.A = mem == DFM_MEM_HOST ? a.get<double>(B * rk) : nullptr;
+  s.Q = mem == DFM_MEM_HOST ? a.get<double>(B * rr) : nullptr;
+  s.P0 = a.get<double>(B * kk);
+  s.Fs = a.get<double>(B * Tp * r); s.PsF = a.get<double>(B * Tp * np);
+  s.ll = a.get<double>(B); s.st = a.get<EmState>(B);
+  s.it = a.get<int>(B); s.stat = a.get<int>(B);
+  s.g = gen_bufs(a, EmbPlan{}, B, Tp, N, r, p);
+  return s;
+}
+
+// Staging (padded panels, parameters, P0) and one E-step of the general path's kernels; k_em_prep in its opening mode only
+// reads Lam, R.  Leaves the smoothed moments in s.Fs / s.PsF / s.ll, the per-panel status in s.stat, and the filter's
+// covariances, b_t, C_t and src in s.g.
+static int ss_estep(dfm_handle* h, SsStage& s, const double* X, const dfm_em_init* params, int T, int N, int r, int p, int H, int batch,
+                    int mem) {
+  const size_t B = batch, TN = (size_t)(T + H) * N; const int Tp = T + H;
+  const int k = r * p, kk = k * k, rr = r * r, rk = r * k, np = r * (r + 1) / 2;
+  const int ntC = tpt_threads(np + r), nblkC = (Tp + ntC - 1) / ntC;
+  int rc = DFM_OK;
+  s.x = X;
+  if (mem == DFM_MEM_HOST) {
+    if (H > 0) {
+      CK(cudaMemcpy2DAsync(s.Xp, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, B * N, cudaMemcpyHostToDevice, h->stream));
+      long long n = (long long)B * N * H;
+      L(k_ss_pad, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)nullptr, T, Tp, (long long)B * N, s.Xp);
+    } else CK(cudaMemcpyAsync(s.Xp, X, B * TN * 8, cudaMemcpyHostToDevice, h->stream));
+    s.x = s.Xp;
+  } else if (H > 0) {
+    long long n = (long long)B * TN;
+    L(k_ss_pad, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, X, T, Tp, (long long)B * N, s.Xp);
+    s.x = s.Xp;
+  }
+  rc = stage_in(h, params->Lam, s.L, B * N * r, mem, &s.pL); if (rc) return rc;
+  rc = stage_in(h, params->R, s.R, B * N, mem, &s.pR); if (rc) return rc;
+  rc = stage_in(h, params->A, s.A, B * rk, mem, &s.pA); if (rc) return rc;
+  rc = stage_in(h, params->Q, s.Q, B * rr, mem, &s.pQ); if (rc) return rc;
+  if (params->P0) CK(cudaMemcpyAsync(s.P0, params->P0, B * kk * 8, mem == DFM_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+  else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, s.pA, s.pQ, r, p, s.P0, 12);
+  L(k_em_state_init, batch, 1, 1, 0, s.st);
+  L(k_em_scan, N, batch, 64, 0, s.x, s.pL, Tp, N, r, s.st);
+  L(k_em_prep, batch, 1, 128, 0, s.pL, s.pR, N, r, p, s.g.W, s.g.logR, s.g.C, (double*)nullptr, (const double*)nullptr, (double*)nullptr,
+    (const double*)nullptr, s.st, 1, 0, 0);
+  L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, s.x, s.pL, s.g.W, s.pR, s.g.logR, s.g.C, Tp, N, r, s.g.Bt, s.g.qt,
+    s.g.slr, s.g.nt, s.g.Ct, s.st);
+  L(k_em_contract_bal, (Tp + 31) / 32, batch, 256, 8 * 32 * 3 * 8, s.x, s.g.W, s.pR, s.g.logR, Tp, N, r, s.g.Bt, s.g.qt, s.g.slr, s.g.nt, s.st);
+  int ncl = fs_cluster_size(h, batch, s.g.xch);
+  rc = launch_filter_smooth(h, ncl, s.g, batch, Tp, r, p, s.pA, s.pQ, s.P0, s.Fs, s.PsF, s.ll, s.st, 1, 0.0, 1);
+  if (rc) return rc;
+  L(k_em_collect, batch, 1, 1, 0, s.st, s.it, s.stat);
+  return DFM_OK;
+}
+
 int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, const dfm_em_init* params, const dfm_ss_out* out) {
   if (!h || !X || !o || !params || !out || !params->Lam || !params->R || !params->A || !params->Q)
     return fail(h, DFM_ERR_ARG, "dfm_kalman_smooth: null argument");
   const int T = o->T, N = o->N, r = o->r, p = o->p, H = o->H, batch = o->batch, mem = o->mem;
-  if (T <= 0 || N <= 0 || r <= 0 || r > 64 || p <= 0 || H < 0 || batch <= 0 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE) ||
-      (long long)T + H < 2)
-    return fail(h, DFM_ERR_ARG, "dfm_kalman_smooth: bad shape/options");
-  if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_kalman_smooth: batch > 65535");
+  int rc = ss_check(h, "dfm_kalman_smooth", T, N, r, p, H, batch, mem);
+  if (rc) return rc;
   const int Tp = T + H;
-  const int stgT = fs_stage_periods(h->nsm, batch, r, p);
-  const size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
-  if (r * p > 48 || smFS > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_kalman_smooth: state dimension r*p too large for the general path");
   const size_t smP = ss_project_smem_doubles(r) * 8;
   CK(cudaSetDevice(h->device));
-  const size_t B = batch, TN = (size_t)Tp * N; const int k = r * p, kk = k * k, rr = r * r, rk = r * k, np = r * (r + 1) / 2;
-  const int ntC = tpt_threads(np + r), nblkC = (Tp + ntC - 1) / ntC;
+  const size_t B = batch, TN = (size_t)Tp * N; const int rr = r * r;
   const bool dev_out = mem == DFM_MEM_DEVICE;
   for (int pass = 0; pass < 2; ++pass) {
     Arena a(pass ? h->ws : nullptr);
-    // padded panel: needed unless the input is already on the device with nothing to pad
-    double* dXp = (mem == DFM_MEM_HOST || H > 0) ? a.get<double>(B * TN) : nullptr;
-    double* dL = mem == DFM_MEM_HOST ? a.get<double>(B * N * r) : nullptr;
-    double* dR = mem == DFM_MEM_HOST ? a.get<double>(B * N) : nullptr;
-    double* dA = mem == DFM_MEM_HOST ? a.get<double>(B * rk) : nullptr;
-    double* dQ = mem == DFM_MEM_HOST ? a.get<double>(B * rr) : nullptr;
-    double* dP0 = a.get<double>(B * kk);
-    double* dFs = a.get<double>(B * Tp * r); double* dPsF = a.get<double>(B * Tp * np);
-    double* dll = a.get<double>(B); EmState* st = a.get<EmState>(B);
-    int* dit = a.get<int>(B); int* dstat = a.get<int>(B);
-    const GenBufs g = gen_bufs(a, EmbPlan{}, B, Tp, N, r, p);
+    SsStage s = ss_bufs(a, mem, H, B, Tp, N, r, p);
     double* dPFfull = (out->PF && !dev_out) ? a.get<double>(B * Tp * rr) : nullptr;
     double* dcom = (out->common && !dev_out) ? a.get<double>(B * TN) : nullptr;
     double* dxh = (out->xhat && !dev_out) ? a.get<double>(B * TN) : nullptr;
     double* dxv = (out->xvar && !dev_out) ? a.get<double>(B * TN) : nullptr;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    int rc = DFM_OK;
-    // ---- staging: padded panels and parameters
-    const double* x = X;
-    if (mem == DFM_MEM_HOST) {
-      if (H > 0) {
-        CK(cudaMemcpy2DAsync(dXp, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, B * N, cudaMemcpyHostToDevice, h->stream));
-        long long n = (long long)B * N * H;
-        L(k_ss_pad, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)nullptr, T, Tp, (long long)B * N, dXp);
-      } else CK(cudaMemcpyAsync(dXp, X, B * TN * 8, cudaMemcpyHostToDevice, h->stream));
-      x = dXp;
-    } else if (H > 0) {
-      long long n = (long long)B * TN;
-      L(k_ss_pad, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, X, T, Tp, (long long)B * N, dXp);
-      x = dXp;
-    }
-    const double *pL, *pR, *pA, *pQ;
-    rc = stage_in(h, params->Lam, dL, B * N * r, mem, &pL); if (rc) return rc;
-    rc = stage_in(h, params->R, dR, B * N, mem, &pR); if (rc) return rc;
-    rc = stage_in(h, params->A, dA, B * rk, mem, &pA); if (rc) return rc;
-    rc = stage_in(h, params->Q, dQ, B * rr, mem, &pQ); if (rc) return rc;
-    if (params->P0) CK(cudaMemcpyAsync(dP0, params->P0, B * kk * 8, dev_out ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
-    else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, pA, pQ, r, p, dP0, 12);
-    // ---- one E-step (the general path's kernels; k_em_prep in its opening mode only reads Lam, R)
-    L(k_em_state_init, batch, 1, 1, 0, st);
-    L(k_em_scan, N, batch, 64, 0, x, pL, Tp, N, r, st);
-    L(k_em_prep, batch, 1, 128, 0, pL, pR, N, r, p, g.W, g.logR, g.C, (double*)nullptr, (const double*)nullptr, (double*)nullptr,
-      (const double*)nullptr, st, 1, 0, 0);
-    L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, pL, g.W, pR, g.logR, g.C, Tp, N, r, g.Bt, g.qt, g.slr, g.nt, g.Ct, st);
-    L(k_em_contract_bal, (Tp + 31) / 32, batch, 256, 8 * 32 * 3 * 8, x, g.W, pR, g.logR, Tp, N, r, g.Bt, g.qt, g.slr, g.nt, st);
-    int ncl = fs_cluster_size(h, batch, g.xch);
-    rc = launch_filter_smooth(h, ncl, g, batch, Tp, r, p, pA, pQ, dP0, dFs, dPsF, dll, st, 1, 0.0, 1);
+    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    rc = ss_estep(h, s, X, params, T, N, r, p, H, batch, mem);
     if (rc) return rc;
-    L(k_em_collect, batch, 1, 1, 0, st, dit, dstat);
-    L(k_ss_nan_failed, batch, 1, 256, 0, (const EmState*)st, Tp, r, dFs, dPsF, dll);
+    L(k_ss_nan_failed, batch, 1, 256, 0, (const EmState*)s.st, Tp, r, s.Fs, s.PsF, s.ll);
     // ---- projection onto the series
     double* ocom = dev_out ? out->common : dcom;
     double* oxh = dev_out ? out->xhat : dxh;
@@ -1297,16 +1337,16 @@ int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, cons
       const int per = std::max(1, 65535 / nst);            // panels per launch (grid.y limit)
       for (int b0 = 0; b0 < batch; b0 += per) {
         const int nb = std::min(per, batch - b0);
-        L(k_ss_project, ntt, nst * nb, 256, smP, x, (const double*)dFs, (const double*)dPsF, pL, pR, (const EmState*)st, Tp, N, r, b0,
-          ocom, oxh, oxv);
+        L(k_ss_project, ntt, nst * nb, 256, smP, s.x, (const double*)s.Fs, (const double*)s.PsF, s.pL, s.pR, (const EmState*)s.st, Tp, N, r,
+          b0, ocom, oxh, oxv);
       }
     }
     // ---- results
-    rc = copy_out(h, out->F, dFs, B * Tp * r, mem); if (rc) return rc;
+    rc = copy_out(h, out->F, s.Fs, B * Tp * r, mem); if (rc) return rc;
     if (out->PF) {
       long long n = (long long)Tp * rr;
       double* dst = dev_out ? out->PF : dPFfull;
-      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, dPsF, Tp, r, dst);
+      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, s.PsF, Tp, r, dst);
       if (!dev_out) { rc = copy_out(h, out->PF, dPFfull, B * Tp * rr, mem); if (rc) return rc; }
     }
     if (!dev_out) {
@@ -1314,8 +1354,73 @@ int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, cons
       rc = copy_out(h, out->xhat, dxh, B * TN, mem); if (rc) return rc;
       rc = copy_out(h, out->xvar, dxv, B * TN, mem); if (rc) return rc;
     }
-    rc = copy_out(h, out->loglik, dll, B, mem); if (rc) return rc;
-    rc = copy_out(h, out->status, dstat, B, mem); if (rc) return rc;
+    rc = copy_out(h, out->loglik, s.ll, B, mem); if (rc) return rc;
+    rc = copy_out(h, out->status, s.stat, B, mem); if (rc) return rc;
+  }
+  return finish(h, mem);
+}
+
+// ------------------------------------------------------------------------------------ simulation smoother
+// Draws per chunk: the per-draw scratch of k_sim_paths (zf_t and f+_t of every period) and, for host outputs, the staging of
+// one chunk's draws stay within kSimChunkBytes whatever n_draw; k_sim_project's grid.y (<= 65535) bounds the chunk as well.
+static const size_t kSimChunkBytes = (size_t)512 << 20;
+static long long sim_chunk(long long n_draw, int Tp, int N, int r, int k, bool stageF, bool stageX) {
+  const size_t per = (size_t)Tp * (k + r + (stageF ? r : 0) + (stageX ? N : 0)) * 8;
+  long long c = (long long)std::max<size_t>(SIM_ND, kSimChunkBytes / per);
+  c = std::min<long long>(c, (long long)(65535 / ((N + SS_NS - 1) / SS_NS)) * SIM_PD);
+  return std::min(c, n_draw);
+}
+
+// The E-step of dfm_kalman_smooth (one model), k_sim_gains once, then k_sim_paths (and k_sim_project when panel draws are
+// requested) per chunk of draws.
+int dfm_simulation_smoother(dfm_handle* h, const double* X, const dfm_sim_opts* o, const dfm_em_init* params, const dfm_sim_out* out) {
+  if (!h || !X || !o || !params || !out || !params->Lam || !params->R || !params->A || !params->Q)
+    return fail(h, DFM_ERR_ARG, "dfm_simulation_smoother: null argument");
+  const int T = o->T, N = o->N, r = o->r, p = o->p, H = o->H, mem = o->mem;
+  if (o->n_draw < 1 || o->draw0 < 0) return fail(h, DFM_ERR_ARG, "dfm_simulation_smoother: n_draw < 1 or draw0 < 0");
+  int rc = ss_check(h, "dfm_simulation_smoother", T, N, r, p, H, 1, mem);
+  if (rc) return rc;
+  const int Tp = T + H, k = r * p;
+  const size_t smG = sim_gains_smem_doubles(r, p) * 8, smS = sim_paths_smem_doubles(r, p) * 8, smP = sim_project_smem_doubles(r) * 8;
+  CK(cudaSetDevice(h->device));
+  const bool dev_out = mem == DFM_MEM_DEVICE;
+  const long long nch = sim_chunk(o->n_draw, Tp, N, r, k, out->F && !dev_out, out->X && !dev_out);
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    SsStage s = ss_bufs(a, mem, H, 1, Tp, N, r, p);
+    double* gains = a.get<double>(sim_gains_doubles(Tp, k, r));
+    int* sstat = a.get<int>(1);
+    double* zfS = a.get<double>((size_t)nch * Tp * k);
+    double* fS = a.get<double>((size_t)nch * Tp * r);
+    double* dF = (out->F && !dev_out) ? a.get<double>((size_t)nch * Tp * r) : nullptr;
+    double* dX = (out->X && !dev_out) ? a.get<double>((size_t)nch * Tp * N) : nullptr;
+    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    rc = ss_estep(h, s, X, params, T, N, r, p, H, 1, mem);
+    if (rc) return rc;
+    const int* src = s.g.nt + Tp;                        // src[t] of k_em_filter_smooth (g.nt: n_t, then src_t)
+    CK(cudaMemsetAsync(sstat, 0, sizeof(int), h->stream));
+    DFM_SET_SMEM(k_sim_gains, smG);
+    L(k_sim_gains, Tp + 1, 1, 256, smG, s.pA, s.pQ, (const double*)s.P0, (const double*)s.g.C, (const double*)s.g.Ct, (const double*)s.g.Bt,
+      (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const int*)s.g.nt, (const EmState*)s.st, Tp, r, p, gains, sstat);
+    DFM_SET_SMEM(k_sim_paths, smS);
+    DFM_SET_SMEM(k_sim_project, smP);
+    const int nst = (N + SS_NS - 1) / SS_NS, ntt = (Tp + SS_TP - 1) / SS_TP;
+    for (long long j0 = 0; j0 < o->n_draw; j0 += nch) {
+      const int nd = (int)std::min(nch, o->n_draw - j0);
+      const long long id0 = o->draw0 + j0;
+      double* Fo = out->F ? (dev_out ? out->F + (size_t)j0 * Tp * r : dF) : nullptr;
+      double* Xo = out->X ? (dev_out ? out->X + (size_t)j0 * Tp * N : dX) : nullptr;
+      L(k_sim_paths, (nd + SIM_ND - 1) / SIM_ND, 1, SIM_NT, smS, (const double*)gains, src, Tp, r, p, o->seed, id0, nd, (const int*)sstat,
+        zfS, fS, Fo);
+      if (Xo)
+        L(k_sim_project, ntt, nst * ((nd + SIM_PD - 1) / SIM_PD), 256, smP, s.x, s.pL, s.pR, (const double*)fS, Tp, N, r, o->seed, id0, nd,
+          (const int*)sstat, Xo);
+      if (!dev_out) {
+        if (out->F) { rc = copy_out(h, out->F + (size_t)j0 * Tp * r, dF, (size_t)nd * Tp * r, mem); if (rc) return rc; }
+        if (out->X) { rc = copy_out(h, out->X + (size_t)j0 * Tp * N, dX, (size_t)nd * Tp * N, mem); if (rc) return rc; }
+      }
+    }
+    rc = copy_out(h, out->status, sstat, 1, mem); if (rc) return rc;
   }
   return finish(h, mem);
 }

@@ -234,6 +234,42 @@ typedef struct {              /* any pointer may be NULL (not computed); per pan
  * (k = r*p <= 48); H < 0 is DFM_ERR_ARG.  The parameter arrays are only read.  Synchronous for host memory. */
 int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* opts, const dfm_em_init* params, const dfm_ss_out* out);
 
+/* ---- simulation smoother: draws from the JOINT posterior of the factor path and the missing cells ---------------------
+ * dfm_kalman_smooth gives marginals (one period, one cell at a time).  This call draws (f_1 .. f_{T+H}, x_missing) given the
+ * observed cells at fixed parameters, so that any function of a path -- a 4-quarter growth rate, an annual average, the
+ * probability of staying below a threshold, a ratio of imputed cells -- gets its posterior distribution from the draws; one
+ * draw per sweep is also the factor step of a Gibbs sampler.  Mean-corrected simulation smoother (Durbin & Koopman 2002) on
+ * the E-step of dfm_kalman_smooth; a draw costs O((T+H) k^2) whatever N (the spec is tests/simsmooth_oracle.py).
+ * Random numbers: the Philox4x32-10 stream of the replication generators (below) with replication id = draw id and four
+ * streams (element indices; Tp = T + H, k = r p):
+ *    7  z+_0 = L_P0 nu                                  element a        (a < k)
+ *    8  state shocks eta_t of periods t >= 1            element t r + a  (a < r)
+ *    9  xi_t, the N(0, C_t) term of the observations    element t r + a  (a < r)
+ *   10  eps_it, the idiosyncratic draw of a missing cell element i Tp + t (drawn for missing cells only)
+ * Draw j of a call is draw id draw0 + j, a pure function of (seed, draw id): any split of a draw range over calls or GPUs
+ * (dfm_shard_range) gives bit-identical draws.  oracle/dgp.py restates the stream; tests/simsmooth_oracle.py the four tags. */
+typedef struct {
+  int T, N, r, p;             /* in-sample panel T x N, STANDARDIZED, NaN = missing (as dfm_kalman_smooth); ONE model per call */
+  int H;                      /* periods T+1 .. T+H after the panel */
+  long long n_draw;           /* >= 1 */
+  long long draw0;            /* draw id of the first draw, >= 0 */
+  unsigned long long seed;
+  int mem;
+} dfm_sim_opts;
+
+typedef struct {              /* any of F / X may be NULL (not computed); all column-major, draw after draw */
+  double* F;                  /* n_draw x ((T+H) x r)   factor path draws f~_t */
+  double* X;                  /* n_draw x ((T+H) x N)   panel draws: x_it where observed, lambda_i' f~_t + sqrt(R_i) eps_it where
+                                                        missing (the H periods after the panel included), NaN columns for series
+                                                        out of the model */
+  int* status;                /* [1]  0, or DFM_ERR_NOT_PD (a covariance not positive definite or R_i <= 0: the draws are NaN) */
+} dfm_sim_out;
+
+/* X: T x N standardized panel; params: (Lam, R, A, Q[, P0]) of one model as dfm_kalman_smooth's.  Size limits and error codes
+ * as dfm_kalman_smooth; n_draw < 1 or draw0 < 0 is DFM_ERR_ARG.  The device workspace does not grow with n_draw (the draws
+ * are made in chunks).  Synchronous for host memory. */
+int dfm_simulation_smoother(dfm_handle* h, const double* X, const dfm_sim_opts* opts, const dfm_em_init* params, const dfm_sim_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

@@ -217,4 +217,24 @@ function kalman_smooth(Xs::Matrix{Float64}, em, H::Integer)
     return (F = F, PF = PF, common = common, xhat = xhat, xvar = xvar, loglik = ll[], status = st[])
 end
 
+struct SimOpts; T::Cint; N::Cint; r::Cint; p::Cint; H::Cint; n_draw::Clonglong; draw0::Clonglong; seed::Culonglong; mem::Cint; end
+struct SimOut; F::Ptr{Cdouble}; X::Ptr{Cdouble}; status::Ptr{Cint}; end
+
+"""Draws `draw0 .. draw0+n_draw-1` (stream `seed`) from the JOINT posterior of the factor path and the missing / forecast
+cells of the standardized panel `Xs` at the parameters `em` of `estimate!(m, Parametric())` (dfm_simulation_smoother).
+F: (T+H) x r x n_draw, X: (T+H) x N x n_draw (standardized units; the data where observed)."""
+function simulation_smoother(Xs::Matrix{Float64}, em, H::Integer, n_draw::Integer, seed::Integer; draw0::Integer = 0)
+    h = gethandle()
+    T, N = size(Xs); r = size(em.Lam, 2); p = size(em.A, 2) ÷ r; Tp = T + H
+    F = Array{Float64}(undef, Tp, r, n_draw); X = Array{Float64}(undef, Tp, N, n_draw); st = Ref{Cint}(0)
+    GC.@preserve Xs em F X begin
+        opts = Ref(SimOpts(T, N, r, p, H, n_draw, draw0, seed, MEM_HOST))
+        init = Ref(EmInit(pointer(em.Lam), pointer(em.R), pointer(em.A), pointer(em.Q), C_NULL))
+        out = Ref(SimOut(pointer(F), pointer(X), Base.unsafe_convert(Ptr{Cint}, st)))
+        check(ccall((:dfm_simulation_smoother, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ref{SimOpts}, Ref{EmInit}, Ref{SimOut}),
+                    h, Xs, opts, init, out), "dfm_simulation_smoother")
+    end
+    return (F = F, X = X, status = st[])
+end
+
 end # module
