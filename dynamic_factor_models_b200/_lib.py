@@ -77,6 +77,19 @@ class SimOut(C.Structure):
     _fields_ = [("F", C.c_void_p), ("X", C.c_void_p), ("status", C.c_void_p)]
 
 
+class NewsOpts(C.Structure):
+    _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("news_rows", C.c_int),
+                ("n_target", C.c_int), ("target_series", c_ip), ("target_period", c_ip), ("batch", C.c_int), ("mem", C.c_int)]
+
+
+class NewsOut(C.Structure):
+    _fields_ = [("old_est", C.c_void_p), ("new_est", C.c_void_p), ("news", C.c_void_p), ("weight", C.c_void_p),
+                ("contrib", C.c_void_p), ("status", C.c_void_p)]
+
+
+NEWS_OUTPUTS = ("old_est", "new_est", "news", "weight", "contrib")
+
+
 def default_library_path():
     return os.path.join(HERE, "lib", "libdfm_b200.so")
 
@@ -85,7 +98,7 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_kalman_smooth", "dfm_simulation_smoother",
-           "dfm_em_init_from_factors",
+           "dfm_news", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -154,6 +167,7 @@ class Library:
         L.dfm_em_kalman.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(EmOpts), C.POINTER(EmInit), C.POINTER(EmOut)]
         L.dfm_kalman_smooth.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsOpts), C.POINTER(EmInit), C.POINTER(SsOut)]
         L.dfm_simulation_smoother.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SimOpts), C.POINTER(EmInit), C.POINTER(SimOut)]
+        L.dfm_news.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(NewsOpts), C.POINTER(EmInit), C.POINTER(NewsOut)]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p]
         L.dfm_bootstrap_panels.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 8
@@ -233,6 +247,17 @@ class Library:
         ou = SimOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
         self.check(self.lib.dfm_simulation_smoother(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)),
                    "dfm_simulation_smoother")
+
+    def news_raw(self, X_old, X_new, T, N, r, p, H, B, news_rows, targets, params, out, mem):
+        """Pointer-level dfm_news (ints = device or host addresses).  targets: (series, period) pairs, 0-based; params: dict
+        Lam, R, A, Q[, P0]; out: dict of old_est, new_est, news, weight, contrib, status (missing or 0 = NULL)."""
+        ts = np.ascontiguousarray([t[0] for t in targets], dtype=np.int32)
+        tp = np.ascontiguousarray([t[1] for t in targets], dtype=np.int32)
+        o = NewsOpts(T=T, N=N, r=r, p=p, H=H, news_rows=news_rows, n_target=len(ts), target_series=ts.ctypes.data_as(c_ip),
+                     target_period=tp.ctypes.data_as(c_ip), batch=B, mem=mem)
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
+        ou = NewsOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
+        self.check(self.lib.dfm_news(self.h, C.c_void_p(X_old), C.c_void_p(X_new), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_news")
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)
@@ -482,4 +507,31 @@ class Library:
         res = dict(status=int(ost[0]))
         for n, a_ in outs.items():
             res[n] = from_cm(a_, Tp, r if n == "F" else N, n_draw)
+        return res
+
+    def news(self, X_old, X_new, Lam, R, A, Q, p=1, P0=None, H=0, targets=(), news_rows=1, outputs=NEWS_OUTPUTS):
+        """News decomposition of the revision of each target between two vintages at FIXED parameters (dfm_news).  X_old,
+        X_new (T, N) or (B, T, N) standardized with NaN, the new vintage only adding cells in the last `news_rows` rows;
+        parameters as kalman_smooth; targets: (series, period) pairs, 0-based, period < T + H.  Returns old_est, new_est
+        (n_target), news (news_rows, N), weight / contrib (news_rows, N, n_target) -- those named in `outputs` -- and status
+        (per pair for batched input)."""
+        X_old = np.asarray(X_old, float); b = X_old.shape[0] if X_old.ndim == 3 else None
+        T, N = X_old.shape[-2:]; r = np.asarray(Lam).shape[-1]; B = b or 1; nq = len(targets)
+        bufs = dict(Xo=to_cm(X_old), Xn=to_cm(X_new), Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float), A=to_cm(A), Q=to_cm(Q),
+                    P0=to_cm(P0) if P0 is not None else None)
+        size = dict(old_est=nq, new_est=nq, news=news_rows * N, weight=news_rows * N * nq, contrib=news_rows * N * nq)
+        outs = {n: np.empty(B * size[n]) for n in outputs}
+        ost = np.empty(B, dtype=np.int32)
+        self.news_raw(bufs["Xo"].ctypes.data, bufs["Xn"].ctypes.data, T, N, r, p, H, B, news_rows, list(targets),
+                      {n: (bufs[n].ctypes.data if bufs[n] is not None else 0) for n in ("Lam", "R", "A", "Q", "P0")},
+                      {**{n: a_.ctypes.data for n, a_ in outs.items()}, "status": ost.ctypes.data}, MEM_HOST)
+        res = dict(status=ost if b else int(ost[0]))
+        for n, a_ in outs.items():
+            if n in ("old_est", "new_est"):
+                v = a_.reshape(B, nq)
+            elif n == "news":
+                v = a_.reshape(B, N, news_rows).transpose(0, 2, 1)
+            else:
+                v = a_.reshape(B, nq, N, news_rows).transpose(0, 3, 2, 1)
+            res[n] = np.ascontiguousarray(v if b else v[0])
         return res

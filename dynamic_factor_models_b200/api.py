@@ -263,6 +263,71 @@ def posterior_draws(m, H, n_draw, seed, draw0=0, lib=None):
     return dict(periods=b["periods"], series=b["series"], factor=o["F"], x=b["xmean"] + b["xstd"] * o["X"])
 
 
+def news(m, data_new, targets, H=0, lib=None):
+    """Why the nowcast moved: the news decomposition (Banbura & Modugno 2014) of the revision of each target between the
+    data of a model estimated with `estimate(m, Parametric())` and a new vintage `data_new` (the shape of m.data), at the
+    EM estimates m.em (dfm_news).
+
+    targets: (column of m.data, 1-based period) pairs, period in initperiod .. lastperiod + H.  Both vintages are
+    standardized with the mean and std of the estimation block of m.data, as `forecast` standardizes it.  The release window
+    starts at the first row that holds a new cell.  Cells observed in both vintages with different values (data revisions)
+    are handled first: `revision_effect` is the change of the estimate when the old cells take their new values, and the
+    decomposition runs from that revised vintage.  A cell that disappears from the new vintage raises ValueError.
+    Returns a dict, in data units:
+      old, new (n_target)                E[y | old data], E[y | new data];
+      revision_effect (n_target)         the part of new - old due to revised cells;
+      news (news_rows, ns)               x_j - E[x_j | old] at the released cells, NaN elsewhere;
+      weights, contributions (n_target, news_rows, ns)   w_qj (scaled by xstd_target / xstd_j) and w_qj news_j;
+      by_series (n_target, ns)           contributions summed over the window rows:  by_series.sum(1) + revision_effect
+                                         = new - old;
+    and periods (the window rows, 1-based), series (columns of m.data), targets."""
+    b = _state_space_block(m, H, lib, "news")
+    lib, e = b["lib"], b["em"]
+    i0, i1 = m.initperiod, m.lastperiod
+    incl, xmean, xstd, Xs = b["series"], b["xmean"], b["xstd"], b["Xs"]
+    data_new = np.asarray(data_new, float)
+    if data_new.shape != m.data.shape:
+        raise ValueError(f"news: data_new has shape {data_new.shape}, m.data {m.data.shape}")
+    T, ns = Xs.shape
+    col = {int(c): j for j, c in enumerate(incl)}
+    tg = []
+    for c, t in targets:
+        if int(c) not in col:
+            raise ValueError(f"news: target column {c} is not an estimation series")
+        if not i0 <= t <= i1 + H:
+            raise ValueError(f"news: target period {t} outside {i0} .. {i1 + H}")
+        tg.append((col[int(c)], int(t) - i0))
+    Xold = m.data[:, incl][i0 - 1:i1]
+    Xnew = data_new[:, incl][i0 - 1:i1]
+    inm = ~np.isnan(Xs)                                                 # old cells in the model
+    if (inm & np.isnan(Xnew)).any():
+        raise ValueError("news: a cell observed in m.data is missing in data_new")
+    revised = inm & (Xnew != Xold)
+    Xn_std = (Xnew - xmean) / xstd
+    Xrev = np.where(revised, Xn_std, Xs)                                # the old cells at their new values
+    out_model = np.isnan(b["Lam"][:, 0])
+    Xn = np.where(inm, Xrev, np.where(out_model[None, :], np.nan, Xn_std))
+    added = np.isnan(Xrev) & ~np.isnan(Xn)
+    rows = np.flatnonzero(added.any(1))
+    nr = T - int(rows[0]) if len(rows) else 1
+    o = lib.news(Xrev, Xn, b["Lam"], e["R"], e["A"], e["Q"], p=b["p"], P0=e["P0"], H=H, targets=tg, news_rows=nr)
+    if o["status"] != 0:
+        raise RuntimeError(f"news: device status {o['status']}")
+    ti = np.array([j for j, _ in tg], int)
+    sd_t, mu_t = xstd[ti], xmean[ti]
+    base = o["old_est"]
+    if revised.any():
+        ks = lib.kalman_smooth(Xs, b["Lam"], e["R"], e["A"], e["Q"], p=b["p"], P0=e["P0"], H=H, outputs=("xhat",))
+        if ks["status"] != 0:
+            raise RuntimeError(f"news: device status {ks['status']}")
+        base = ks["xhat"][[t for _, t in tg], ti]
+    w = np.transpose(o["weight"], (2, 0, 1)) * sd_t[:, None, None] / xstd[None, None, :]
+    c = np.transpose(o["contrib"], (2, 0, 1)) * sd_t[:, None, None]
+    return dict(old=mu_t + sd_t * base, new=mu_t + sd_t * o["new_est"], revision_effect=sd_t * (o["old_est"] - base),
+                news=xstd[None, :] * o["news"], weights=w, contributions=c, by_series=c.sum(1),
+                periods=np.arange(i0 + T - nr, i1 + 1), series=incl, targets=list(targets))
+
+
 def forecast_bands(m, H, q, n_draw, seed, lib=None):
     """Percentile bands (numpy.percentile's linear interpolation, on the device through dfm_percentiles) of the panel draws
     of `posterior_draws(m, H, n_draw, seed)`, cell by cell.  Returns a dict with bands (len(q), T+H, ns) in data units, rows

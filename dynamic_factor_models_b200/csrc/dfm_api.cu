@@ -13,6 +13,7 @@
 #include "dfm_kernels_rep.cuh"
 #include "dfm_kernels_inst.cuh"
 #include "dfm_kernels_sim.cuh"
+#include "dfm_kernels_news.cuh"
 #include <algorithm>
 #include <new>
 #include <thread>
@@ -1421,6 +1422,112 @@ int dfm_simulation_smoother(dfm_handle* h, const double* X, const dfm_sim_opts* 
       }
     }
     rc = copy_out(h, out->status, sstat, 1, mem); if (rc) return rc;
+  }
+  return finish(h, mem);
+}
+
+// ------------------------------------------------------------------------------------ news decomposition
+// The E-step of dfm_kalman_smooth on the old vintage (ss_estep), then k_news_window, k_news_cov, k_news_project and
+// k_news_finish.  Only the release window of X_new is staged; for host memory the rows above it are compared with X_old
+// here, so that the rest of the new panel never crosses PCIe.
+int dfm_news(dfm_handle* h, const double* X_old, const double* X_new, const dfm_news_opts* o, const dfm_em_init* params,
+             const dfm_news_out* out) {
+  if (!h || !X_old || !X_new || !o || !params || !out || !params->Lam || !params->R || !params->A || !params->Q || !o->target_series ||
+      !o->target_period)
+    return fail(h, DFM_ERR_ARG, "dfm_news: null argument");
+  const int T = o->T, N = o->N, r = o->r, p = o->p, H = o->H, batch = o->batch, mem = o->mem, nr = o->news_rows, nq = o->n_target;
+  int rc = ss_check(h, "dfm_news", T, N, r, p, H, batch, mem);
+  if (rc) return rc;
+  if (nr < 1 || nr > T || nq < 1 || nq > NEWS_MAXQ) return fail(h, DFM_ERR_ARG, "dfm_news: news_rows or n_target out of range");
+  const int Tp = T + H;
+  std::vector<int> tg(2 * (size_t)nq), outside;        // target series, then periods; target periods outside the window
+  for (int q = 0; q < nq; ++q) {
+    const int i = o->target_series[q], t = o->target_period[q];
+    if (i < 0 || i >= N || t < 0 || t >= Tp) return fail(h, DFM_ERR_ARG, "dfm_news: target series or period out of range");
+    tg[q] = i; tg[nq + q] = t;
+    if (t < T - nr || t >= T) outside.push_back(t);
+  }
+  std::sort(outside.begin(), outside.end());
+  const int Wmax = nr + (int)(std::unique(outside.begin(), outside.end()) - outside.begin());
+  if ((long long)Wmax * r > NEWS_MAXN) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_news: W r > 128 (too many periods in the window and targets)");
+  const bool dev = mem == DFM_MEM_DEVICE;
+  const size_t B = batch, onr = (size_t)nr * N;
+  std::vector<int> hbad;
+  if (!dev) {                                          // the rows above the window: X_new must repeat X_old there
+    hbad.assign(B, 0);
+    const size_t na = (size_t)(T - nr);
+    for (size_t c = 0; c < B * N && na > 0; ++c) {
+      const double* x0 = X_old + c * T; const double* x1 = X_new + c * T;
+      if (memcmp(x0, x1, na * sizeof(double)) == 0) continue;
+      for (size_t t = 0; t < na; ++t)
+        if (std::isnan(x0[t]) != std::isnan(x1[t]) || (!std::isnan(x0[t]) && x0[t] != x1[t])) { hbad[c / N] = 1; break; }
+    }
+  }
+  const int nmax = Wmax * r;
+  const size_t smW = news_window_smem_bytes(nr, nq);
+  const size_t smallC = news_cov_small_doubles(r, p), bigC = news_cov_big_doubles(r, p, nmax, nq);
+  const bool big_in_smem = (smallC + bigC) * 8 <= kMaxSmem;
+  const size_t smC = (big_in_smem ? smallC + bigC : smallC) * 8, smP = news_project_smem_doubles(r) * 8;
+  const int nst = (N + NEWS_NS - 1) / NEWS_NS, ntw = (nr + NEWS_TP - 1) / NEWS_TP, ntile = nst * ntw;
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    SsStage s = ss_bufs(a, mem, H, B, Tp, N, r, p);
+    double* dXn = dev ? nullptr : a.get<double>(B * onr);
+    int* dtg = a.get<int>(2 * (size_t)nq);
+    unsigned char* dmask = a.get<unsigned char>(B * onr);
+    int* dpl = a.get<int>(B * (Wmax + 1));
+    int* drowp = a.get<int>(B * nr);
+    int* dpst = a.get<int>(B);
+    int* dkind = a.get<int>(B * nq);
+    double* dold = a.get<double>(B * nq);
+    double* dgv = a.get<double>(B * nq * nmax);
+    double* dpart = a.get<double>(B * ntile * nq);
+    double* dbig = big_in_smem ? nullptr : a.get<double>(B * bigC);
+    double* hOld = (out->old_est && !dev) ? a.get<double>(B * nq) : nullptr;
+    double* hNew = (out->new_est && !dev) ? a.get<double>(B * nq) : nullptr;
+    double* hNews = (out->news && !dev) ? a.get<double>(B * onr) : nullptr;
+    double* hW = (out->weight && !dev) ? a.get<double>(B * onr * nq) : nullptr;
+    double* hC = (out->contrib && !dev) ? a.get<double>(B * onr * nq) : nullptr;
+    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    rc = ss_estep(h, s, X_old, params, T, N, r, p, H, batch, mem);
+    if (rc) return rc;
+    const int* src = s.g.nt + B * Tp;                  // src[t] of k_em_filter_smooth (g.nt: n_t, then src_t), per pair
+    CK(cudaMemcpyAsync(dtg, tg.data(), tg.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    const double* xn = X_new; int ldn = T, row0 = T - nr;
+    if (dev) CK(cudaMemsetAsync(dpst, 0, B * sizeof(int), h->stream));
+    else {
+      CK(cudaMemcpyAsync(dpst, hbad.data(), B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpy2DAsync(dXn, (size_t)nr * 8,X_new + (T - nr), (size_t)T * 8, (size_t)nr * 8, B * N, cudaMemcpyHostToDevice, h->stream));
+      xn = dXn; ldn = nr; row0 = 0;
+    }
+    L(k_news_window, batch, 1, 256, smW, s.x, xn, ldn, row0, dev ? X_new : (const double*)nullptr, s.pL, s.pR, (const int*)dtg + nq, nq,
+      (const int*)s.stat, T, Tp, N, r, nr, Wmax, dmask, dpl, drowp, dpst);
+    DFM_SET_SMEM(k_news_cov, smC);
+    L(k_news_cov, batch, 1, 256, smC, s.pA, (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const double*)s.Fs, s.x, s.pL, s.pR,
+      (const unsigned char*)dmask, (const int*)dpl, (const int*)dtg, (const int*)dtg + nq, nq, (const int*)dpst, T, Tp, N, r, p, nr, Wmax,
+      dbig, dgv, dkind, dold);
+    double* oNews = out->news ? (dev ? out->news : hNews) : nullptr;
+    double* oW = out->weight ? (dev ? out->weight : hW) : nullptr;
+    double* oC = out->contrib ? (dev ? out->contrib : hC) : nullptr;
+    DFM_SET_SMEM(k_news_project, smP);
+    const int per = std::max(1, 65535 / nst);          // pairs per launch (grid.y limit)
+    for (int b0 = 0; b0 < batch; b0 += per) {
+      const int nb = std::min(per, batch - b0);
+      L(k_news_project, ntw, nst * nb, 256, smP, (const double*)s.Fs, xn, ldn, row0, s.pL, s.pR, (const unsigned char*)dmask,
+        (const int*)drowp, (const double*)dgv, (const int*)dkind, (const int*)dtg, (const int*)dtg + nq, nq, (const int*)dpst, T, Tp, N, r,
+        nr, Wmax, b0, oNews, oW, oC, dpart);
+    }
+    L(k_news_finish, batch, 1, 64, 0, (const double*)dpart, ntile, (const double*)dold, (const int*)dpst, nq,
+      out->old_est ? (dev ? out->old_est : hOld) : (double*)nullptr, out->new_est ? (dev ? out->new_est : hNew) : (double*)nullptr);
+    if (!dev) {
+      rc = copy_out(h, out->old_est, hOld, B * nq, mem); if (rc) return rc;
+      rc = copy_out(h, out->new_est, hNew, B * nq, mem); if (rc) return rc;
+      rc = copy_out(h, out->news, hNews, B * onr, mem); if (rc) return rc;
+      rc = copy_out(h, out->weight, hW, B * onr * nq, mem); if (rc) return rc;
+      rc = copy_out(h, out->contrib, hC, B * onr * nq, mem); if (rc) return rc;
+    }
+    rc = copy_out(h, out->status, dpst, B, mem); if (rc) return rc;
   }
   return finish(h, mem);
 }

@@ -270,6 +270,42 @@ typedef struct {              /* any of F / X may be NULL (not computed); all co
  * are made in chunks).  Synchronous for host memory. */
 int dfm_simulation_smoother(dfm_handle* h, const double* X, const dfm_sim_opts* opts, const dfm_em_init* params, const dfm_sim_out* out);
 
+/* ---- news decomposition: why the nowcast moved between two data vintages -------------------------------------------------
+ * At fixed parameters, the revision of a target y = x_{i*, t*} between an old vintage and a new one that only ADDS cells is
+ * a sum over the released cells j (Banbura & Modugno 2014; Banbura, Giannone, Modugno & Reichlin 2013):
+ *     E[y | new] - E[y | old] = sum_j w_j I_j,   I_j = x_j - E[x_j | old] (the news),   w = Cov(y, I | old) Var(I | old)^-1.
+ * The weights come from the joint covariance of the factors of the periods that hold a news cell or a target (W of them)
+ * given the old vintage, through a Woodbury solve of size W r (no n_news x n_news matrix); the spec is tests/news_oracle.py.
+ * A target observed in the old vintage has revision 0 and weights 0; a released target has weight 1 on its own cell; a
+ * target in a series out of the model (NaN loading or R) is NaN.  A new cell of a series out of the model is not news. */
+typedef struct {
+  int T, N, r, p, H;          /* as dfm_ss_opts; both panels STANDARDIZED with the same means / stds, NaN = missing */
+  int news_rows;              /* news cells may lie only in rows T - news_rows .. T - 1 (the release window); 1 <= news_rows <= T */
+  int n_target;               /* 1 .. 64 */
+  const int* target_series;   /* HOST [n_target], 0-based column */
+  const int* target_period;   /* HOST [n_target], 0-based row in 0 .. T+H-1 (rows >= T: forecasts) */
+  int batch, mem;             /* batch = vintage pairs, each with its own parameters (as dfm_kalman_smooth) */
+} dfm_news_opts;
+
+typedef struct {              /* any pointer may be NULL (not computed); per pair back to back; column-major */
+  double* old_est;            /* [n_target]                    E[y_q | old] (the data where y_q is observed in the old vintage) */
+  double* new_est;            /* [n_target]                    old_est + the sum of the contributions (fixed summation order) */
+  double* news;               /* news_rows x N                 I_j at the news cells, NaN elsewhere */
+  double* weight;             /* news_rows x N x n_target      w_qj at the news cells, 0 elsewhere */
+  double* contrib;            /* news_rows x N x n_target      w_qj I_j at the news cells, 0 elsewhere */
+  int* status;                /* [batch]  0; DFM_ERR_NOT_PD (the E-step failed: a covariance not positive definite or
+                                 R_i <= 0); DFM_ERR_ARG (this pair's vintages are inconsistent: an old cell missing or changed
+                                 in the new one, or a new cell above the window).  A failed pair's outputs are NaN; the other
+                                 pairs are unaffected. */
+} dfm_news_out;
+
+/* X_old, X_new: T x N standardized panels, pairs back to back; params: (Lam, R, A, Q[, P0]) per pair as dfm_kalman_smooth's.
+ * Size limits as dfm_kalman_smooth.  W r <= 128, with W bounded by the number of distinct rows of the window and the target
+ * periods (checked here, before any data is read; DFM_ERR_UNSUPPORTED past it).  Bad targets or options: DFM_ERR_ARG.
+ * Synchronous for host memory. */
+int dfm_news(dfm_handle* h, const double* X_old, const double* X_new, const dfm_news_opts* opts, const dfm_em_init* params,
+             const dfm_news_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

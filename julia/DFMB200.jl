@@ -237,4 +237,29 @@ function simulation_smoother(Xs::Matrix{Float64}, em, H::Integer, n_draw::Intege
     return (F = F, X = X, status = st[])
 end
 
+struct NewsOpts; T::Cint; N::Cint; r::Cint; p::Cint; H::Cint; news_rows::Cint; n_target::Cint
+                 target_series::Ptr{Cint}; target_period::Ptr{Cint}; batch::Cint; mem::Cint; end
+struct NewsOut; old_est::Ptr{Cdouble}; new_est::Ptr{Cdouble}; news::Ptr{Cdouble}; weight::Ptr{Cdouble}; contrib::Ptr{Cdouble}
+                status::Ptr{Cint}; end
+
+"""News decomposition (dfm_news) of the revision of each target between the standardized vintages `Xold` and `Xnew` (NaN =
+missing; `Xnew` only adds cells, in its last `news_rows` rows) at the parameters `em` of `estimate!(m, Parametric())`.
+`targets`: (series, period) pairs, 1-based, period <= T+H.  Returns old / new estimates, news (news_rows x N) and weights /
+contributions (news_rows x N x n_target), all in standardized units."""
+function news(Xold::Matrix{Float64}, Xnew::Matrix{Float64}, em, H::Integer, targets, news_rows::Integer)
+    h = gethandle()
+    T, N = size(Xold); r = size(em.Lam, 2); p = size(em.A, 2) ÷ r; nq = length(targets)
+    ts = Cint[t[1] - 1 for t in targets]; tp = Cint[t[2] - 1 for t in targets]
+    old = Vector{Float64}(undef, nq); new = similar(old); nw = Matrix{Float64}(undef, news_rows, N)
+    w = Array{Float64}(undef, news_rows, N, nq); c = similar(w); st = Ref{Cint}(0)
+    GC.@preserve Xold Xnew em ts tp old new nw w c begin
+        opts = Ref(NewsOpts(T, N, r, p, H, news_rows, nq, pointer(ts), pointer(tp), 1, MEM_HOST))
+        init = Ref(EmInit(pointer(em.Lam), pointer(em.R), pointer(em.A), pointer(em.Q), C_NULL))
+        out = Ref(NewsOut(pointer(old), pointer(new), pointer(nw), pointer(w), pointer(c), Base.unsafe_convert(Ptr{Cint}, st)))
+        check(ccall((:dfm_news, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ptr{Cdouble}, Ref{NewsOpts}, Ref{EmInit}, Ref{NewsOut}),
+                    h, Xold, Xnew, opts, init, out), "dfm_news")
+    end
+    return (old = old, new = new, news = nw, weights = w, contributions = c, status = st[])
+end
+
 end # module
