@@ -258,14 +258,13 @@ static int resident_grid(const dfm_handle* h, K kern, int threads, size_t smem, 
 #endif
 }
 
-// Series-block groups per panel that `grid` CTAs of a TMA kernel keep in L2 at evict-last priority (f2_keep_stages):
-// F2_L2KEEP_PCT of L2 split over the CTAs active in a round; keep[0] for the full rounds, keep[1] for the tail round.
-static void l2_keep_plan(const dfm_handle* h, int grid, int B, int T, int N, int keep[2]) {
-  const long long budget = (long long)h->l2_bytes * F2_L2KEEP_PCT / 100, group = 64LL * F2_SBS * T;   // 64 T bytes per 8 series
-  const long long nsg = (N + 8 * F2_SBS - 1) / (8 * F2_SBS);
+// Turn window of the `grid` CTAs of a TMA kernel (f2_produce): F2_L2WIN_PCT of L2 split over the CTAs active in a round,
+// in copies per pass turn; win[0] for the full rounds, win[1] for the tail round.
+static void l2_turn_plan(const dfm_handle* h, int grid, int B, int N, int win[2]) {
+  const long long copy = 64LL * F2_SBS * F2_TC, nsg = (N + 8 * F2_SBS - 1) / (8 * F2_SBS);   // bytes of one copy, groups per panel
   const int tail = (B % grid) ? B % grid : grid;
-  keep[0] = (int)std::min(nsg, budget / (grid * group));
-  keep[1] = (int)std::min(nsg, budget / (tail * group));
+  win[0] = (int)std::min(nsg, (long long)h->l2_bytes * F2_L2WIN_PCT / 100 / (grid * copy));
+  win[1] = (int)std::min(nsg, (long long)h->l2_bytes * F2_L2WIN_PCT / 100 / (tail * copy));
 }
 
 // One launch of the fused EM kernel over all panels of fa (fa.scratch: min(B, nsm * 8) * T * FUSED_SCR(r) doubles):
@@ -276,7 +275,7 @@ static int launch_em_fused(dfm_handle* h, FusedArgs fa, int r, bool use2) {
     if (use2) {
       const size_t smem = fused2_smem_doubles<RT>(fa.T, fa.N) * 8;
       const int grid = resident_grid(h, k_em_fused2<RT>, 256, smem, fa.B);
-      l2_keep_plan(h, grid, fa.B, fa.T, fa.N, fa.l2_keep);
+      l2_turn_plan(h, grid, fa.B, fa.N, fa.l2_win);
       CUtensorMap tm; int rc = make_panel_tmap(h, fa.X, fa.T, (long long)fa.B * fa.N, &tm); if (rc) return rc;
       L(k_em_fused2<RT>, grid, 1, 256, smem, fa, tm);
     } else {
@@ -479,7 +478,7 @@ static int launch_als_fused2(dfm_handle* h, AlsFusedArgs fa, int r) {
     constexpr int RT = decltype(R)::value;
     const size_t smem = als_fused2_smem_doubles<RT>(fa.T, fa.N) * 8;
     const int grid = resident_grid(h, k_als_fused2<RT>, 256, smem, fa.B);
-    l2_keep_plan(h, grid, fa.B, fa.T, fa.N, fa.l2_keep);
+    l2_turn_plan(h, grid, fa.B, fa.N, fa.l2_win);
     CUtensorMap tm; int rc = make_panel_tmap(h, fa.Xs, fa.T, (long long)fa.B * fa.N, &tm); if (rc) return rc;
     L(k_als_fused2<RT>, grid, 1, 256, smem, fa, tm);
     return DFM_OK;

@@ -49,7 +49,7 @@ struct FusedArgs {
   int* done;                 // streaming host path: done[b] = 1 (mapped pinned host memory) once panel b's results are in device memory
   double* P0out;             // non-NULL: compute P0 in the kernel (Lyapunov doubling of (A, Q), p0_steps steps, as k_lyapunov)
   int p0_steps;              //           and store it here ([B][r*r]).  With ready or P0out set the kernel also pre-fills its loglik rows.
-  int l2_keep[2];            // k_em_fused2: series-block groups per panel kept in L2: full rounds, tail round (f2_keep_stages)
+  int l2_win[2];             // k_em_fused2: turn window per panel pass (copies): full rounds, tail round (f2_round_win)
 };
 #define FUSED_SCR(R_) (5 * (R_) * (R_) + 1)
 

@@ -47,9 +47,9 @@ static_assert(F2_TC % 16 == 4 || F2_TC % 16 == 12, "ring pitch must be 4 or 12 m
 static_assert(F2_TC <= 256 && (F2_TC * 64) % 128 == 0, "TMA box / stage alignment");
 #define F2_NEXS(R_) ((F2_S * F2_STG - 4 * (R_) * (R_)) / FUSED_SCR(R_))   // the last 4 R^2 doubles of the idle ring hold scan matrices
 #define F2_RTAIL(R_) (F2_S * F2_STG - 4 * (R_) * (R_))
-#ifndef F2_L2KEEP_PCT
-#define F2_L2KEEP_PCT 55   // share of L2 the resident panels may keep at evict-last priority (f2_keep_stages); 40 and 55
-#endif                     // tied, 70 was slower, on c5 (H100 SXM 80GB, 700 W, 1980 MHz)
+#ifndef F2_L2WIN_PCT
+#define F2_L2WIN_PCT 67    // share of L2 for the turn windows of the resident panels (f2_produce; DESIGN.md section 7)
+#endif
 
 #ifndef DFM_EMU
 __device__ __forceinline__ uint32_t f2_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -66,23 +66,18 @@ __device__ __forceinline__ void f2_tma_2d(void* dst, const CUtensorMap* tmap, in
                ::"r"(f2_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(x), "r"(y), "r"(f2_smem_u32(bar)), "l"(policy) : "memory");
 }
 
-// L2 residency plan.  Each EM iteration (ALS sweep) reads the whole panel twice, but the resident panels are several
-// times larger than L2, so a plain stream evicts every line long before its CTA reads it again.  Instead the series of
-// the first `keep` series-block groups of a panel (keep x 8 F2_SBS series, all periods) are loaded with evict-last
-// priority and stay in L2 across both passes of all iterations of that panel; the rest streams through with
-// evict-first.  The CTAs of one round of panels share a fixed share of L2 (F2_L2KEEP_PCT); the host turns it into
-// keep[0] for the full rounds and keep[1] for the tail round, whose fewer CTAs may each keep more.
-__device__ __forceinline__ int f2_keep_stages(const int* keep, int B, int b) {
+// L2 turn plan.  Each EM iteration (ALS sweep) reads the whole panel twice, but the resident panels are several times
+// larger than L2, so a plain stream evicts every line long before its CTA reads it again.  The passes are therefore
+// ordered so that each one starts where the previous one ended: the E pass ends on the last period chunk of the high
+// series-block groups, and the M pass, which runs backwards over the groups, starts there; the M pass ends on the first
+// chunk of the low groups, where the E pass starts.  The last `win` copies of a pass that the next pass re-reads first
+// (the turn window) are loaded evict-normal, so that they outlive the evict-first stream until that re-read, a few
+// microseconds and one serial phase later; the re-read and every other copy load evict-first (f2_produce).  The host
+// splits F2_L2WIN_PCT of L2 over the CTAs of one round of panels (l2_turn_plan): win[0] for the full rounds, win[1] for
+// the tail round, whose fewer CTAs may each hold more.
+__device__ __forceinline__ int f2_round_win(const int* win, int B, int b) {
   const int G = (int)gridDim.x;
-  return (b / G < B / G) ? keep[0] : keep[1];
-}
-// Demotes the kept lines of a finished panel (rows [row0, row0 + 8 F2_SBS keep) of the [T, rows] view at X) to normal
-// priority, so that they do not crowd out the next panel's slice or other work on the GPU.  All threads of the CTA.
-__device__ __forceinline__ void f2_release(const double* X, long long row0, int keep, int T, long long rows) {
-  const long long r1 = min(row0 + 8LL * F2_SBS * keep, rows);
-  const uintptr_t a0 = reinterpret_cast<uintptr_t>(X + row0 * T) & ~(uintptr_t)127, a1 = reinterpret_cast<uintptr_t>(X + r1 * T);
-  for (uintptr_t p = a0 + (uintptr_t)threadIdx.x * 128; p < a1; p += (uintptr_t)blockDim.x * 128)
-    asm volatile("applypriority.L2::evict_normal [%0], 128;" ::"l"(p) : "memory");
+  return (b / G < B / G) ? win[0] : win[1];
 }
 #endif
 
@@ -101,23 +96,27 @@ struct F2Ring {
 // [T, B*N] view of the batch (column runs of 800 B; the box is 4 periods wider than the chunk so that the
 // dense row pitch in shared memory is == 4 mod 16, i.e. conflict-free; rows/periods beyond the tensor are
 // zero-filled, rows of the next panel are masked by the consumers).  Eight 1-D bulk copies per stage were
-// issue-bound (requests serialised over the lanes of a warp: tools/bench_stream.cu).  Series-block groups sb < *keep
-// are loaded with evict-last priority, the others with evict-first (f2_keep_stages; *keep is in shared memory).  Both
-// policies are made once per pass: per copy they would lengthen the producer's issue path, which bounds a lone CTA.
-__device__ __forceinline__ void f2_produce(F2Ring& rg, const CUtensorMap* tmap, int row0, int T, int N, bool c_outer, const int* keep) {
+// issue-bound (requests serialised over the lanes of a warp: tools/bench_stream.cu).  The E pass (c_outer) runs over the
+// series-block groups in ascending order, the M pass in descending order, so that each pass starts on the copies the
+// previous one read last.  The turn window (L2 turn plan above; *win is in shared memory) is the last *win groups of
+// the last chunk (E pass) or of the first chunk (M pass): it loads evict-normal, the rest evict-first.  Both policies
+// are made once per pass: per copy they would lengthen the producer's issue path, which bounds a lone CTA.
+__device__ __forceinline__ void f2_produce(F2Ring& rg, const CUtensorMap* tmap, int row0, int T, int N, bool c_outer, const int* win) {
   const int lane = threadIdx.x & 31;
   const int nsb = (N + 8 * F2_SBS - 1) / (8 * F2_SBS), nck = (T + F2_TC - 1) / F2_TC;      // (stages per pass: series-block groups x chunks)
-  const int n_out = c_outer ? nck : nsb, n_in = c_outer ? nsb : nck, nkeep = *keep;
-  uint64_t pol_last, pol_first;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_last));
+  const int n_out = c_outer ? nck : nsb, n_in = c_outer ? nsb : nck, nw = *win;
+  const int wc = c_outer ? nck - 1 : 0, w0 = c_outer ? nsb - nw : 0, w1 = c_outer ? nsb : nw;   // turn window: chunk wc, groups [w0, w1)
+  uint64_t pol_win, pol_first;
+  asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol_win));
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_first));
   for (int o = 0; o < n_out; ++o)
     for (int i = 0; i < n_in; ++i) {
-      const int c = c_outer ? o : i, sb = c_outer ? i : o;
+      const int c = c_outer ? o : i, sb = c_outer ? i : nsb - 1 - o;
       if (rg.wrap) f2_mbar_wait(&rg.empty[rg.rs], rg.rph ^ 1);
       if (lane == 0) {
         f2_mbar_expect(&rg.full[rg.rs], (uint32_t)(F2_STG * 8));
-        f2_tma_2d(rg.ring + (size_t)rg.rs * F2_STG, tmap, c * F2_TC, row0 + sb * 8 * F2_SBS, &rg.full[rg.rs], sb < nkeep ? pol_last : pol_first);
+        f2_tma_2d(rg.ring + (size_t)rg.rs * F2_STG, tmap, c * F2_TC, row0 + sb * 8 * F2_SBS, &rg.full[rg.rs],
+                  (c == wc && sb >= w0 && sb < w1) ? pol_win : pol_first);
       }
       __syncwarp();
       rg.advance();
@@ -187,8 +186,9 @@ __device__ __forceinline__ double f2_consume_E(F2Ring& rg, int cw, int T, int N,
 }
 
 // M pass, consumer warp cw:  Lam[n][:] <- sum_t x[t,n] Z[t][:]  (S_xf) and sxx[n] <- sum_t x[t,n]^2.
-// Series-block outer / period-chunk inner; two accumulator pairs per warp; deterministic cross-warp
-// reduction of the F2_NCW partial tiles at the end of every series block (named barrier 1).
+// Series-block outer in descending order (f2_produce) / period-chunk inner; two accumulator pairs per warp;
+// deterministic cross-warp reduction of the F2_NCW partial tiles at the end of every series block (named barrier 1).
+// A block's sums depend on its own chunks only, so the block order does not change any result.
 template <int R>
 __device__ __forceinline__ void f2_consume_M(F2Ring& rg, int cw, int T, int N, int Tp, int Np, const double* Z, double* Lam,
                                              double* sxx, double* part) {
@@ -202,7 +202,7 @@ __device__ __forceinline__ void f2_consume_M(F2Ring& rg, int cw, int T, int N, i
 #pragma unroll
     for (int j = 0; j < F2_NKC; ++j) { d[sub][j][0] = 0.0; d[sub][j][1] = 0.0; }
   }
-  for (int sg = 0; sg < nsg; ++sg)
+  for (int sg = nsg - 1; sg >= 0; --sg)
     for (int c = 0; c < nck; ++c) {
       f2_mbar_wait(&rg.full[rg.rs], rg.rph);
       const double* stage = rg.ring + (size_t)rg.rs * F2_STG;
@@ -300,7 +300,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
   double* tmp = Pfprev + RR;               // 2R
   double* red = tmp + 2 * R;               // 40
   double* scal = red + 40;                 // 8: [0]=slr [1]=ld_inf [2]=qsum
-  int* ctl = (int*)(scal + 8);             // [0]=nE [1]=tb [2]=bad [3]=frozen [4]=series-block groups kept in L2
+  int* ctl = (int*)(scal + 8);             // [0]=nE [1]=tb [2]=bad [3]=frozen [4]=turn window of the panel (f2_produce)
   double* bnd = scal + 16;                 // (3*32+1) R + RR: blk_recur workspace for 32 groups
   double* part = bnd;                                // [2][F2_NCW][72] M-pass partial accumulators: ALIASES the scan
                                                      // workspace (used only inside the M pass / only in P3, P5)
@@ -324,7 +324,9 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
   const double eps = 1e-14;
 
   for (int b = DFM_BX; b < a.B; b += DFM_GX) {
+#ifdef DFM_EMU
     const double* X = a.X + (size_t)b * T * N;
+#endif
 #ifndef DFM_EMU
     if (a.ready) {                             // streaming host path: wait until this panel's chunk has landed
       if (threadIdx.x == 0) {
@@ -343,7 +345,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
     }
     if (DFM_TID == 0) ctl[2] = 0;
 #ifndef DFM_EMU
-    if (DFM_TID == 0) ctl[4] = f2_keep_stages(a.l2_keep, a.B, b);
+    if (DFM_TID == 0) ctl[4] = f2_round_win(a.l2_win, a.B, b);
 #endif
     DFM_SYNC();
     if (a.P0out || a.ready) {
@@ -890,9 +892,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       ll_prev = ll;
       if (conv) { ++it; break; }
     }
-#ifndef DFM_EMU
-    f2_release(a.X, (long long)b * N, ctl[4], T, (long long)a.B * N);    // (every copy of this panel has completed)
-#endif
     // ---- outputs
     for (int e = DFM_TID; e < N * R; e += DFM_NT) { int i = e % N, c = e / N; a.Lam[(size_t)b * N * R + e] = Lam[LI(i, c)]; }
     for (int e = DFM_TID; e < N; e += DFM_NT) a.R[(size_t)b * N + e] = Rv[e];
@@ -944,7 +943,7 @@ struct AlsFusedArgs {
   int B, T, N;
   double tol;
   long long max_iter;
-  int l2_keep[2];       // series-block groups per panel kept in L2: full rounds, tail round (f2_keep_stages)
+  int l2_win[2];        // turn window per panel pass (copies): full rounds, tail round (f2_round_win)
 };
 
 template <int R>
@@ -959,7 +958,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
   double* FtF = sxx + N;  double* Gi = FtF + RR;  double* LtL = Gi + RR;  double* Hi = LtL + RR;
   double* tmp = Hi + RR;                   // 2R
   double* red = tmp + 2 * R;               // 40
-  int* ctl = (int*)(red + 40);             // [0] = bad, [1] = series-block groups kept in L2
+  int* ctl = (int*)(red + 40);             // [0] = bad, [1] = turn window of the panel (f2_produce)
   double* part = red + 48;                 // 2 * F2_NCW * 72
   double* ring = part + 2 * F2_NCW * 72;
 #ifndef DFM_EMU
@@ -972,13 +971,15 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
   const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
 #endif
   for (int b = DFM_BX; b < a.B; b += DFM_GX) {
+#ifdef DFM_EMU
     const double* X = a.Xs + (size_t)b * T * N;
+#endif
     for (int e = DFM_TID; e < FZ * Tp; e += DFM_NT) Z[e] = 0.0;
     DFM_SYNC();
     for (int e = DFM_TID; e < T * R; e += DFM_NT) { int t = e % T, c = e / T; Z[ZI(t, c)] = a.F[(size_t)b * T * R + e]; }
     if (DFM_TID == 0) ctl[0] = 0;
 #ifndef DFM_EMU
-    if (DFM_TID == 0) ctl[1] = f2_keep_stages(a.l2_keep, a.B, b);
+    if (DFM_TID == 0) ctl[1] = f2_round_win(a.l2_win, a.B, b);
 #endif
     DFM_SYNC();
     double ssr = 0.0, ssr_old = 0.0;
@@ -1059,9 +1060,6 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
       if (!(fabs(ssr_old - ssr) >= a.tol * (double)T * (double)N)) break;            // :367-368
       if (it >= a.max_iter) { status = 4; break; }
     }
-#ifndef DFM_EMU
-    f2_release(a.Xs, (long long)b * N, ctl[1], T, (long long)a.B * N);
-#endif
     for (int e = DFM_TID; e < T * R; e += DFM_NT) { int t = e % T, c = e / T; a.F[(size_t)b * T * R + e] = Z[ZI(t, c)]; }
     for (int e = DFM_TID; e < N * R; e += DFM_NT) { int i = e % N, c = e / N; a.Lam[(size_t)b * N * R + e] = Lam[LI(i, c)]; }
     if (DFM_TID == 0) { a.st[b].ssr_old = ssr_old; a.st[b].ssr = ssr; a.st[b].iters = (int)it; a.st[b].done = 1; a.st[b].status = status; }
