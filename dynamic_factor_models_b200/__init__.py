@@ -13,6 +13,6 @@ from .api import (  # noqa: F401
     construct_constraint, estimate, estimate_factor, estimate_factor_loading, estimate_var,
     impulse_response, bai_ng_criterion, amengual_watson_test, estimate_factor_numbers,
     standardize_data, pca_score, em_kalman, em_init_from_factors, set_default_library, get_library,
-    kalman_smooth, forecast, posterior_draws, forecast_bands, news,
+    kalman_smooth, forecast, posterior_draws, forecast_bands, news, parametric_irf, parametric_bootstrap,
 )
 from . import ingest  # noqa: F401   (host-side panel ingestion: the step before the path)

@@ -90,6 +90,20 @@ class NewsOut(C.Structure):
 NEWS_OUTPUTS = ("old_est", "new_est", "news", "weight", "contrib")
 
 
+class SsbOpts(C.Structure):
+    _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H_irf", C.c_int), ("H_fc", C.c_int),
+                ("fc_rows", C.c_int), ("max_iter", C.c_int), ("tol", C.c_double), ("n_rep", C.c_longlong), ("rep0", C.c_longlong),
+                ("seed", C.c_ulonglong), ("mem", C.c_int)]
+
+
+class SsbOut(C.Structure):
+    _fields_ = [("Lam", C.c_void_p), ("R", C.c_void_p), ("A", C.c_void_p), ("Q", C.c_void_p), ("irf", C.c_void_p),
+                ("xhat", C.c_void_p), ("xvar", C.c_void_p), ("loglik", C.c_void_p), ("iters", C.c_void_p), ("status", C.c_void_p)]
+
+
+SSB_OUTPUTS = ("Lam", "R", "A", "Q", "irf", "xhat", "xvar")
+
+
 def default_library_path():
     return os.path.join(HERE, "lib", "libdfm_b200.so")
 
@@ -98,7 +112,7 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_kalman_smooth", "dfm_simulation_smoother",
-           "dfm_news", "dfm_em_init_from_factors",
+           "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -168,6 +182,9 @@ class Library:
         L.dfm_kalman_smooth.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsOpts), C.POINTER(EmInit), C.POINTER(SsOut)]
         L.dfm_simulation_smoother.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SimOpts), C.POINTER(EmInit), C.POINTER(SimOut)]
         L.dfm_news.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(NewsOpts), C.POINTER(EmInit), C.POINTER(NewsOut)]
+        L.dfm_ss_simulate_panels.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(EmInit), C.c_ulonglong,
+                                             C.c_longlong, C.c_int, C.c_int, C.c_void_p]
+        L.dfm_ss_bootstrap.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsbOpts), C.POINTER(EmInit), C.POINTER(SsbOut)]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p]
         L.dfm_bootstrap_panels.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 8
@@ -258,6 +275,21 @@ class Library:
         ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
         ou = NewsOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
         self.check(self.lib.dfm_news(self.h, C.c_void_p(X_old), C.c_void_p(X_new), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_news")
+
+    def ss_simulate_panels_raw(self, X, T, N, r, p, params, seed, rep0, B, Xout, mem):
+        """Pointer-level dfm_ss_simulate_panels (ints = device or host addresses).  params: dict Lam, R, A, Q, P0."""
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
+        self.check(self.lib.dfm_ss_simulate_panels(self.h, C.c_void_p(X), T, N, r, p, C.byref(ini), seed, rep0, B, mem, C.c_void_p(Xout)),
+                   "dfm_ss_simulate_panels")
+
+    def ss_bootstrap_raw(self, X, T, N, r, p, params, out, mem, n_rep, rep0=0, seed=0, H_irf=24, H_fc=0, fc_rows=0, max_iter=50, tol=0.0):
+        """Pointer-level dfm_ss_bootstrap (ints = device or host addresses).  params: dict Lam, R, A, Q, P0; out: dict of Lam, R,
+        A, Q, irf, xhat, xvar, loglik, iters, status (missing or 0 = NULL)."""
+        o = SsbOpts(T=T, N=N, r=r, p=p, H_irf=H_irf, H_fc=H_fc, fc_rows=fc_rows, max_iter=max_iter, tol=tol, n_rep=n_rep, rep0=rep0,
+                    seed=seed, mem=mem)
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
+        ou = SsbOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
+        self.check(self.lib.dfm_ss_bootstrap(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_ss_bootstrap")
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)
@@ -507,6 +539,42 @@ class Library:
         res = dict(status=int(ost[0]))
         for n, a_ in outs.items():
             res[n] = from_cm(a_, Tp, r if n == "F" else N, n_draw)
+        return res
+
+    def ss_simulate_panels(self, X, Lam, R, A, Q, P0, p=1, n_rep=1, seed=0, rep0=0):
+        """(n_rep, T, N) panels drawn from the state-space model at (Lam, R, A, Q, P0) (dfm_ss_simulate_panels), replication ids
+        rep0 .. rep0 + n_rep - 1, NaN where the template X (T, N) is missing or the series is out of the model."""
+        X = np.asarray(X, float); T, N = X.shape; r = np.asarray(Lam).shape[-1]
+        bufs = dict(X=to_cm(X), Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float), A=to_cm(A), Q=to_cm(Q), P0=to_cm(P0))
+        out = np.empty(n_rep * T * N)
+        self.ss_simulate_panels_raw(bufs["X"].ctypes.data, T, N, r, p, {n: bufs[n].ctypes.data for n in ("Lam", "R", "A", "Q", "P0")},
+                                    seed, rep0, n_rep, out.ctypes.data, MEM_HOST)
+        return from_cm(out, T, N, n_rep)
+
+    def ss_bootstrap(self, X, Lam, R, A, Q, P0, p=1, n_rep=1, seed=0, rep0=0, H_irf=24, H_fc=0, fc_rows=0, max_iter=50, tol=0.0,
+                     outputs=SSB_OUTPUTS):
+        """Parametric bootstrap of the state-space model at (Lam, R, A, Q, P0) fitted to the standardized panel X (T, N)
+        (dfm_ss_bootstrap): replicates rep0 .. rep0 + n_rep - 1 simulated, re-estimated by EM from the fitted parameters and
+        aligned with them.  Returns Lam (n_rep, N, r), R (n_rep, N), A (n_rep, r, k), Q (n_rep, r, r), irf (n_rep, r, H_irf, r)
+        [variable, horizon, shock], xhat / xvar (n_rep, fc_rows, N) -- those named in `outputs` -- and loglik, iters, status."""
+        X = np.asarray(X, float); T, N = X.shape; r = np.asarray(Lam).shape[-1]; k = r * p
+        bufs = dict(X=to_cm(X), Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float), A=to_cm(A), Q=to_cm(Q), P0=to_cm(P0))
+        size = dict(Lam=N * r, R=N, A=r * k, Q=r * r, irf=r * H_irf * r, xhat=fc_rows * N, xvar=fc_rows * N)
+        outs = {n: np.full(max(n_rep * size[n], 0), np.nan) for n in outputs}           # (bad sizes: the library refuses them)
+        ll = np.empty(max(n_rep, 0)); it = np.empty(max(n_rep, 0), np.int32); st = np.empty(max(n_rep, 0), np.int32)
+        self.ss_bootstrap_raw(bufs["X"].ctypes.data, T, N, r, p, {n: bufs[n].ctypes.data for n in ("Lam", "R", "A", "Q", "P0")},
+                              {**{n: a_.ctypes.data for n, a_ in outs.items()}, "loglik": ll.ctypes.data, "iters": it.ctypes.data,
+                               "status": st.ctypes.data}, MEM_HOST, n_rep, rep0=rep0, seed=seed, H_irf=H_irf, H_fc=H_fc, fc_rows=fc_rows,
+                              max_iter=max_iter, tol=tol)
+        res = dict(loglik=ll, iters=it, status=st)
+        shape = dict(Lam=(N, r), A=(r, k), Q=(r, r), xhat=(fc_rows, N), xvar=(fc_rows, N))
+        for n, a_ in outs.items():
+            if n == "R":
+                res[n] = a_.reshape(n_rep, N)
+            elif n == "irf":
+                res[n] = np.ascontiguousarray(a_.reshape(n_rep, r, H_irf, r).transpose(0, 3, 2, 1))
+            else:
+                res[n] = from_cm(a_, shape[n][0], shape[n][1], n_rep)
         return res
 
     def news(self, X_old, X_new, Lam, R, A, Q, p=1, P0=None, H=0, targets=(), news_rows=1, outputs=NEWS_OUTPUTS):

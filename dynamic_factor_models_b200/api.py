@@ -341,6 +341,69 @@ def forecast_bands(m, H, q, n_draw, seed, lib=None):
     return dict(periods=d["periods"], series=d["series"], q=np.asarray(q, float), bands=bands.reshape((len(q),) + x.shape[1:]))
 
 
+def parametric_irf(m, H, lib=None):
+    """Impulse responses of a model estimated with `estimate(m, Parametric())` at its EM estimates m.em, through dfm_irf:
+    irf[:, h, j] = E M^h G e_j with M the companion matrix of m.em["A"] and G = [chol(Q); 0] (orthogonalized shocks).
+    Returns (r, H, r) [variable, horizon, shock] in standardized factor units, as impulse_response.  The centre of the bands of
+    parametric_bootstrap."""
+    if m.em is None:
+        raise ValueError("parametric_irf needs a model estimated with Parametric()")
+    if H <= 0:
+        raise ValueError("H must be > 0")
+    lib = lib or get_library()
+    A, Q = m.em["A"], m.em["Q"]
+    r = Q.shape[0]; k = A.shape[1]
+    M = np.zeros((k, k)); M[:r] = A; M[r:, :k - r] = np.eye(k - r)
+    Qs = np.zeros((r, k)); Qs[:, :r] = np.eye(r)
+    G = np.zeros((k, r)); G[:r] = np.linalg.cholesky(Q)
+    return lib.irf(M, Qs, G, H, list(range(r)))
+
+
+def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
+                         lib=None):
+    """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn
+    from the state-space model at m.em (with the estimation block's missing pattern and ragged edge), the EM re-runs on all of
+    them from m.em (max_iter / tol as Parametric), and every replicate is rotated back onto m.em's factors.  Bands over the
+    replicates carry the estimation uncertainty of the parameters, which forecast / forecast_bands / posterior_draws leave out.
+
+    Same block as `forecast(m, H_fc)`.  fc_rows: trailing rows of the T + H_fc forecast rows returned per replicate (default
+    H_fc; more rows include the ragged edge).  Returns a dict:
+      Lam (n_rep, ns, r), R (n_rep, ns), A (n_rep, r, k), Q (n_rep, r, r)   aligned parameter draws (standardized units);
+      irf (n_rep, r, H_irf, r)          impulse responses [variable, horizon, shock];  irf_point = parametric_irf(m, H_irf);
+      irf_bands (len(q), r, H_irf, r)   percentiles of irf over the replicates (device, dfm_percentiles; failed replicates
+                                        ignored);
+      xhat (n_rep, fc_rows, ns)         E[x | data] at each replicate's parameters, data units;  xhat_bands (len(q), fc_rows, ns);
+      xvar (n_rep, fc_rows, ns)         Var[x | data] at each replicate's parameters, data units;
+      total_var (fc_rows, ns)           mean_b xvar_b + var_b xhat_b (law of total variance: filtering and parameter uncertainty);
+      loglik, iters, status (n_rep)     the replicates' EM results (status != 0: failed, NaN records);
+    and periods (the fc_rows rows, 1-based), series, q.  Series left out of the model have NaN columns.  n_rep <= 16384."""
+    if not 1 <= n_rep <= 16384:
+        raise ValueError("parametric_bootstrap: n_rep must be in [1, 16384]")
+    if H_irf <= 0:
+        raise ValueError("parametric_bootstrap: H_irf must be > 0")
+    b = _state_space_block(m, H_fc, lib, "parametric_bootstrap")
+    lib, e = b["lib"], b["em"]
+    T = b["Xs"].shape[0]
+    fc_rows = H_fc if fc_rows is None else int(fc_rows)
+    if not 0 <= fc_rows <= T + H_fc:
+        raise ValueError(f"parametric_bootstrap: fc_rows must be in [0, {T + H_fc}]")
+    o = lib.ss_bootstrap(b["Xs"], b["Lam"], e["R"], e["A"], e["Q"], e["P0"], p=b["p"], n_rep=n_rep, seed=seed, rep0=rep0, H_irf=H_irf,
+                         H_fc=H_fc, fc_rows=fc_rows, max_iter=max_iter, tol=tol)
+    qq = np.asarray(q, float)
+    r = e["Q"].shape[0]
+    out = dict(Lam=o["Lam"], R=o["R"], A=o["A"], Q=o["Q"], irf=o["irf"], irf_point=parametric_irf(m, H_irf, lib=lib),
+               irf_bands=lib.percentiles(o["irf"].reshape(n_rep, -1), qq).reshape(len(qq), r, H_irf, r),
+               loglik=o["loglik"], iters=o["iters"], status=o["status"], periods=b["periods"][len(b["periods"]) - fc_rows:],
+               series=b["series"], q=qq)
+    if fc_rows > 0:
+        xstd, ok = b["xstd"], o["status"] == 0
+        xh = b["xmean"] + xstd * o["xhat"]
+        xv = xstd ** 2 * o["xvar"]
+        out.update(xhat=xh, xvar=xv, xhat_bands=lib.percentiles(xh.reshape(n_rep, -1), qq).reshape((len(qq),) + xh.shape[1:]),
+                   total_var=xv[ok].mean(0) + xh[ok].var(0) if ok.any() else np.full(xh.shape[1:], np.nan))
+    return out
+
+
 def em_init_from_factors(Xs, F, p=1, lib=None):
     return (lib or get_library()).em_init_from_factors(Xs, F, p)
 

@@ -14,6 +14,7 @@
 #include "dfm_kernels_inst.cuh"
 #include "dfm_kernels_sim.cuh"
 #include "dfm_kernels_news.cuh"
+#include "dfm_kernels_ssb.cuh"
 #include <algorithm>
 #include <new>
 #include <thread>
@@ -97,6 +98,8 @@ struct dfm_handle {
   bool own_stream;
   char* ws;
   size_t ws_bytes;
+  char* rws;                   // second workspace: temporaries of entry points that call other entry points (which use ws and
+  size_t rws_bytes;            //   may regrow it), kept across calls like ws
   long long launches;
   int profile;                 // 1: bracket every kernel launch with CUDA events (dfm_profile_*)
   std::vector<ProfRec>* prof;
@@ -157,6 +160,16 @@ int ensure_ws(dfm_handle* h, size_t bytes) {
   void* p = nullptr;
   CK(cudaMalloc(&p, want));
   h->ws = (char*)p; h->ws_bytes = want;
+  return DFM_OK;
+}
+
+// the second workspace (dfm_handle::rws), grown as ensure_ws grows ws
+int ensure_rws(dfm_handle* h, size_t bytes) {
+  if (bytes <= h->rws_bytes) return DFM_OK;
+  if (h->rws) { CK(cudaStreamSynchronize(h->stream)); CK(cudaFree(h->rws)); h->rws = nullptr; h->rws_bytes = 0; }
+  void* p = nullptr;
+  CK(cudaMalloc(&p, bytes));
+  h->rws = (char*)p; h->rws_bytes = bytes;
   return DFM_OK;
 }
 
@@ -674,6 +687,7 @@ static void handle_teardown(dfm_handle* h) {
   if (!h) return;
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->ws) cudaFree(h->ws);
+  if (h->rws) cudaFree(h->rws);
   if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
 #ifndef DFM_EMU
   if (h->copy_stream) { cudaStreamSynchronize(h->copy_stream); cudaStreamDestroy(h->copy_stream); }
@@ -694,7 +708,7 @@ int dfm_create_on_stream(int device, void* cuda_stream, dfm_handle** out) {
   if (cudaSetDevice(device) != cudaSuccess) return DFM_ERR_CUDA;
   dfm_handle* h = new (std::nothrow) dfm_handle();
   if (!h) return DFM_ERR_CUDA;
-  h->device = device; h->ws = nullptr; h->ws_bytes = 0; h->launches = 0; h->err[0] = 0;
+  h->device = device; h->ws = nullptr; h->ws_bytes = 0; h->rws = nullptr; h->rws_bytes = 0; h->launches = 0; h->err[0] = 0;
   h->nsm = 132;                // H100 SXM; the CUDA build reads the device's values below (the emulation build has no device)
   h->l2_bytes = 50 << 20;
   h->profile = 0; h->prof = new std::vector<ProfRec>();
@@ -1635,6 +1649,183 @@ int dfm_bootstrap_irf(dfm_handle* h, const dfm_boot_opts* o, const double* F0, c
   cudaError_t e = cudaStreamSynchronize(h->stream);
   cudaFree(base);
 #undef BI_FAIL
+  CK(e);
+  return DFM_OK;
+}
+
+// ------------------------------------------------------------------------------------ parametric bootstrap (state-space model)
+// k_ss_simulate, then k_ss_sim_project in launches of at most 65535 / ceil(N / SS_NS) tiles of SIM_PD replicates (grid.y).
+// g: the factors of k_ss_sim_chol; fS: nb * T * r scratch; Xout: nb panels.
+static void ssb_simulate(dfm_handle* h, const double* xt, const double* Lam, const double* Rv, const double* g, int T, int N, int r, int p,
+                         unsigned long long seed, long long rep0, int nb, double* fS, double* Xout) {
+  const size_t smS = ssb_sim_smem_doubles(r, p) * 8, smP = ssb_project_smem_doubles(r) * 8;
+  DFM_SET_SMEM(k_ss_simulate, smS);
+  DFM_SET_SMEM(k_ss_sim_project, smP);
+  L(k_ss_simulate, (nb + SSB_ND - 1) / SSB_ND, 1, SSB_NT, smS, g, T, r, p, seed, rep0, nb, fS);
+  const int nst = (N + SS_NS - 1) / SS_NS, ntt = (T + SS_TP - 1) / SS_TP;
+  const int per = std::max(1, 65535 / nst) * SIM_PD;
+  for (int j0 = 0; j0 < nb; j0 += per) {
+    const int n = std::min(per, nb - j0);
+    L(k_ss_sim_project, ntt, nst * ((n + SIM_PD - 1) / SIM_PD), 256, smP, xt, Lam, Rv, (const double*)(fS + (size_t)j0 * T * r), T, N, r,
+      seed, rep0 + j0, n, Xout + (size_t)j0 * T * N);
+  }
+}
+
+int dfm_ss_simulate_panels(dfm_handle* h, const double* X, int T, int N, int r, int p, const dfm_em_init* params, unsigned long long seed,
+                           long long rep0, int batch, int mem, double* Xout) {
+  if (!h || !X || !params || !Xout || !params->Lam || !params->R || !params->A || !params->Q || !params->P0)
+    return fail(h, DFM_ERR_ARG, "dfm_ss_simulate_panels: null argument (P0 is required)");
+  if (T <= 1 || N <= 0 || r <= 0 || p <= 0 || batch <= 0 || rep0 < 0 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_ss_simulate_panels: bad shape/options");
+  if (r * p > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_ss_simulate_panels: state dimension r*p > 48");
+  CK(cudaSetDevice(h->device));
+  const size_t B = batch, TN = (size_t)T * N; const int k = r * p;
+  const bool hst = mem == DFM_MEM_HOST;
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    double* dX = hst ? a.get<double>(TN) : nullptr;
+    double* dL = hst ? a.get<double>((size_t)N * r) : nullptr; double* dR = hst ? a.get<double>(N) : nullptr;
+    double* dA = hst ? a.get<double>((size_t)r * k) : nullptr; double* dQ = hst ? a.get<double>((size_t)r * r) : nullptr;
+    double* dP = hst ? a.get<double>((size_t)k * k) : nullptr;
+    double* g = a.get<double>(ssb_chol_doubles(r, p));
+    double* fS = a.get<double>(B * T * r);
+    double* dO = hst ? a.get<double>(B * TN) : Xout;
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    const double *x, *l, *rv, *am, *q, *p0;
+    int rc = stage_in(h, X, dX, TN, mem, &x); if (rc) return rc;
+    rc = stage_in(h, params->Lam, dL, (size_t)N * r, mem, &l); if (rc) return rc;
+    rc = stage_in(h, params->R, dR, (size_t)N, mem, &rv); if (rc) return rc;
+    rc = stage_in(h, params->A, dA, (size_t)r * k, mem, &am); if (rc) return rc;
+    rc = stage_in(h, params->Q, dQ, (size_t)r * r, mem, &q); if (rc) return rc;
+    rc = stage_in(h, params->P0, dP, (size_t)k * k, mem, &p0); if (rc) return rc;
+    L(k_ss_sim_chol, 1, 1, 128, ssb_chol_smem_doubles(r, p) * 8, am, q, p0, r, p, g);
+    ssb_simulate(h, x, l, rv, g, T, N, r, p, seed, rep0, batch, fS, dO);
+    if (hst) { rc = copy_out(h, Xout, dO, B * TN, mem); if (rc) return rc; }
+  }
+  return finish(h, mem);
+}
+
+// Replicates per sub-batch of dfm_ss_bootstrap: a function of the model's shape and the device only, never of n_rep, rep0 or
+// the outputs asked for.  dfm_em_kalman and dfm_kalman_smooth choose their launch plan (thread-block cluster, threads, staging
+// tile, multi-CTA contraction split) from their batch, and plans sum in different orders; every sub-batch therefore has
+// exactly this many replicates (the last one is filled with the replication ids that follow), so that a replicate's results
+// are the same bits whatever n_rep, the shard split or the number of calls.  At most two waves of the fused kernels' grid
+// (2 CTAs per SM), and the device memory an estimate of a sub-batch needs (panel, factors, parameter copies and the EM's
+// general-path workspace per replicate) within kSimChunkBytes.
+static int ssb_batch(const dfm_handle* h, int T, int N, int r, int p) {
+  const size_t k = (size_t)r * p, kk = k * k, rk = r * k, np = (size_t)r * (r + 1) / 2;
+  const size_t par = (size_t)N * r + N + rk + (size_t)r * r;
+  const size_t per = 8 * ((size_t)T * N + (size_t)T * r + 8 * par + 3 * kk + (size_t)T * (2 * kk + 2 * k + 2 * np + 4 * r + 4) + 64 * k +
+                          16 * (kk + rk));
+  const long long cap = std::max<long long>(1, (long long)(kSimChunkBytes / per));
+  return (int)std::min<long long>(cap, std::min(2 * h->nsm, kMaxGridBatch));
+}
+
+// The whole parametric bootstrap, per sub-batch of ssb_batch() replicates: k_ss_simulate (+ k_ss_sim_project) -> dfm_em_kalman
+// from the fitted parameters -> k_ss_align -> dfm_irf -> (forecasts) copies of the panel, dfm_kalman_smooth at the aligned
+// parameters and k_ss_fc_rows.  The stages are the public entry points run on temporaries of this call, which live in the
+// handle's second workspace (the stages use and may regrow the first); the device memory does not grow with n_rep.
+int dfm_ss_bootstrap(dfm_handle* h, const double* X, const dfm_ssb_opts* o, const dfm_em_init* params, const dfm_ssb_out* out) {
+  if (!h || !X || !o || !params || !out || !params->Lam || !params->R || !params->A || !params->Q || !params->P0)
+    return fail(h, DFM_ERR_ARG, "dfm_ss_bootstrap: null argument (P0 is required)");
+  const int T = o->T, N = o->N, r = o->r, p = o->p, Hi = o->H_irf, Hf = o->H_fc, fr = o->fc_rows, mi = o->max_iter, mem = o->mem;
+  const long long n_rep = o->n_rep;
+  if (T <= 1 || N <= 0 || r <= 0 || p <= 0 || Hi <= 0 || Hf < 0 || fr < 0 || (long long)fr > (long long)T + Hf || mi <= 0 ||
+      !(o->tol >= 0) || n_rep < 1 || o->rep0 < 0 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_ss_bootstrap: bad shape/options");
+  const int k = r * p;
+  if (k > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_ss_bootstrap: state dimension r*p > 48");
+  const bool fc = fr > 0 && (out->xhat || out->xvar);
+  const int Tp = T + Hf;
+  const int nc = ssb_batch(h, T, N, r, p);
+  if (em_fs_smem_doubles(r, p, fs_stage_periods(h->nsm, nc, r, p)) * 8 > kMaxSmem)
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_ss_bootstrap: state dimension r*p too large for the general path");
+  CK(cudaSetDevice(h->device));
+  const size_t B = nc, TN = (size_t)T * N, kk = (size_t)k * k, rr = (size_t)r * r, rk = (size_t)r * k, Nr = (size_t)N * r;
+  const size_t nirf = (size_t)r * Hi * r;
+  // temporaries of this call, in the second workspace (the stages' own scratch lives in the first, which they may regrow)
+  size_t tot = 0;
+  auto take = [&](size_t n) { size_t o_ = tot; tot += (n * 8 + 255) & ~(size_t)255; return o_; };
+  const bool hst = mem == DFM_MEM_HOST;
+  const size_t oXs = take(hst ? TN : 0), oLh = take(hst ? Nr : 0), oRh = take(hst ? N : 0), oAh = take(hst ? rk : 0), oQh = take(hst ? rr : 0),
+               oPh = take(hst ? kk : 0), og = take(ssb_chol_doubles(r, p));
+  const size_t oX = take(B * TN), ofS = take(B * T * r), oiL = take(B * Nr), oiR = take(B * N), oiA = take(B * rk), oiQ = take(B * rr),
+               oiP = take(B * kk), oeL = take(B * Nr), oeR = take(B * N), oeA = take(B * rk), oeQ = take(B * rr), oell = take(B * mi),
+               oeit = take(B), oest = take(B), ooL = take(B * Nr), ooR = take(B * N), ooA = take(B * rk), ooQ = take(B * rr),
+               opL = take(fc ? B * Nr : 0), opR = take(fc ? B * N : 0), opA = take(fc ? B * rk : 0), opQ = take(fc ? B * rr : 0),
+               oM = take(B * kk), oQs = take(B * rk), oG = take(B * rk), ollf = take(B), ost = take(B), oI = take(B * nirf),
+               oxh = take(fc ? B * Tp * N : 0), oxv = take(fc ? B * Tp * N : 0), ofh = take(fc ? B * fr * N : 0), ofv = take(fc ? B * fr * N : 0);
+  { int rc = ensure_rws(h, tot); if (rc) return rc; }
+  char* const base = h->rws;
+  auto D = [&](size_t o_) { return reinterpret_cast<double*>(base + o_); };
+  auto I = [&](size_t o_) { return reinterpret_cast<int*>(base + o_); };
+#define SSB_FAIL(rc_) do { int r__ = (rc_); if (r__) { cudaStreamSynchronize(h->stream); return r__; } } while (0)
+#define SSB_CK(call) SSB_FAIL((call) == cudaSuccess ? DFM_OK : fail(h, DFM_ERR_CUDA, "dfm_ss_bootstrap: copy failed"))
+  const double *xs = X, *Lh = params->Lam, *Rh = params->R, *Ah = params->A, *Qh = params->Q, *Ph = params->P0;
+  if (hst) {
+    const double* src[6] = {X, params->Lam, params->R, params->A, params->Q, params->P0};
+    const size_t dst[6] = {oXs, oLh, oRh, oAh, oQh, oPh}, n[6] = {TN, Nr, (size_t)N, rk, rr, kk};
+    for (int i = 0; i < 6; ++i) SSB_CK(cudaMemcpyAsync(D(dst[i]), src[i], n[i] * 8, cudaMemcpyHostToDevice, h->stream));
+    xs = D(oXs); Lh = D(oLh); Rh = D(oRh); Ah = D(oAh); Qh = D(oQh); Ph = D(oPh);
+  }
+  L(k_ss_sim_chol, 1, 1, 128, ssb_chol_smem_doubles(r, p) * 8, Ah, Qh, Ph, r, p, D(og));
+  std::vector<int> ids(r);
+  for (int j = 0; j < r; ++j) ids[j] = j;
+  const size_t smA = ssb_align_smem_doubles(r, p) * 8;
+  DFM_SET_SMEM(k_ss_align, smA);
+  auto bcast = [&](const double* src, size_t n, double* dst, int nb) {
+    L(k_ss_bcast, (int)std::min<size_t>((n + 255) / 256, 1024), nb, 256, 0, src, (long long)n, dst);
+  };
+  const cudaMemcpyKind kout = hst ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  for (long long j0 = 0; j0 < n_rep; j0 += nc) {
+    const int nb = nc;                                              // replicates computed (a full sub-batch, see ssb_batch)
+    const int nkeep = (int)std::min<long long>(nc, n_rep - j0);     // ... and returned
+    // 1. panels
+    ssb_simulate(h, xs, Lh, Rh, D(og), T, N, r, p, o->seed, o->rep0 + j0, nb, D(ofS), D(oX));
+    // 2. EM from the fitted parameters (P0 held fixed)
+    bcast(Lh, Nr, D(oiL), nb); bcast(Rh, N, D(oiR), nb); bcast(Ah, rk, D(oiA), nb); bcast(Qh, rr, D(oiQ), nb); bcast(Ph, kk, D(oiP), nb);
+    dfm_em_opts eo{}; eo.T = T; eo.N = N; eo.r = r; eo.p = p; eo.max_iter = mi; eo.tol = o->tol; eo.batch = nb; eo.mem = DFM_MEM_DEVICE; eo.path = 0;
+    dfm_em_init ei{D(oiL), D(oiR), D(oiA), D(oiQ), D(oiP)};
+    dfm_em_out eout{}; eout.Lam = D(oeL); eout.R = D(oeR); eout.A = D(oeA); eout.Q = D(oeQ); eout.loglik = D(oell); eout.iters = I(oeit);
+    eout.status = I(oest);
+    SSB_FAIL(dfm_em_kalman(h, D(oX), &eo, &ei, &eout));
+    // 3. alignment
+    SsbAlignArgs aa{};
+    aa.Lh = Lh; aa.Rh = Rh; aa.Ah = Ah; aa.Qh = Qh;
+    aa.Ls = D(oeL); aa.Rs = D(oeR); aa.As = D(oeA); aa.Qs = D(oeQ); aa.ll = D(oell); aa.it = I(oeit); aa.em_status = I(oest);
+    aa.Lo = D(ooL); aa.Ro = D(ooR); aa.Ao = D(ooA); aa.Qo = D(ooQ);
+    if (fc) { aa.Le = D(opL); aa.Re = D(opR); aa.Ae = D(opA); aa.Qe = D(opQ); }
+    aa.M = D(oM); aa.Qsel = D(oQs); aa.G = D(oG); aa.llf = D(ollf); aa.status = I(ost);
+    aa.N = N; aa.r = r; aa.p = p; aa.max_iter = mi;
+    L(k_ss_align, nb, 1, SSB_NT, smA, aa);
+    // 4. impulse responses of all r shocks
+    SSB_FAIL(dfm_irf(h, D(oM), D(oQs), D(oG), k, r, Hi, r, ids.data(), nb, DFM_MEM_DEVICE, D(oI)));
+    // 5. forecasts: the original panel at every replicate's aligned parameters
+    if (fc) {
+      bcast(xs, TN, D(oX), nb);
+      dfm_ss_opts so{}; so.T = T; so.N = N; so.r = r; so.p = p; so.H = Hf; so.batch = nb; so.mem = DFM_MEM_DEVICE;
+      dfm_em_init sp{D(opL), D(opR), D(opA), D(opQ), D(oiP)};
+      dfm_ss_out sout{}; sout.xhat = D(oxh); sout.xvar = D(oxv);
+      SSB_FAIL(dfm_kalman_smooth(h, D(oX), &so, &sp, &sout));
+      const long long n = (long long)nb * N * fr;
+      L(k_ss_fc_rows, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)D(oxh), (const double*)D(oxv), Tp, N, fr, nb,
+        (const int*)I(ost), out->xhat ? D(ofh) : (double*)nullptr, out->xvar ? D(ofv) : (double*)nullptr);
+    }
+    // 6. records
+    const size_t b0 = (size_t)j0;
+    cudaError_t ce = cudaSuccess;
+    auto put = [&](void* dst, size_t o_, size_t per_rep, size_t elt) {
+      if (dst && ce == cudaSuccess) ce = cudaMemcpyAsync((char*)dst + b0 * per_rep * elt, base + o_, (size_t)nkeep * per_rep * elt, kout, h->stream);
+    };
+    put(out->Lam, ooL, Nr, 8); put(out->R, ooR, N, 8); put(out->A, ooA, rk, 8); put(out->Q, ooQ, rr, 8); put(out->irf, oI, nirf, 8);
+    if (fc) { put(out->xhat, ofh, (size_t)fr * N, 8); put(out->xvar, ofv, (size_t)fr * N, 8); }
+    put(out->loglik, ollf, 1, 8); put(out->iters, oeit, 1, 4); put(out->status, ost, 1, 4);
+    SSB_CK(ce);
+    SSB_CK(cudaGetLastError());
+  }
+  cudaError_t e = cudaStreamSynchronize(h->stream);
+#undef SSB_CK
+#undef SSB_FAIL
   CK(e);
   return DFM_OK;
 }

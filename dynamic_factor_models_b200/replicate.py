@@ -96,3 +96,32 @@ def bootstrap_irf(lib, m, n_rep, H=24, rank=0, world=1, seed=SEED):
     pb = lib.percentiles(allrec, BAND_PERCENTILES)                           # device sort per statistic
     bands = {q: pb[k].reshape(r, H, r) for k, q in enumerate(BAND_PERCENTILES)}
     return irfs, bands
+
+
+def ss_bootstrap(lib, m, n_rep, H_irf=24, H_fc=0, fc_rows=0, max_iter=50, tol=0.0, rank=0, world=1, seed=SEED):
+    """Parametric bootstrap of a model estimated with `estimate(m, Parametric())`, sharded over ranks: rank g runs ONE
+    dfm_ss_bootstrap call on replication ids dfm_shard_range(n_rep, g, world) (simulate -> EM from m.em -> align -> IRF, device
+    resident), then one all-gather of the records.  A replicate's panel is a pure function of (seed, replication id), so the
+    result does not depend on the number of ranks.  Record per replicate: [irf (r * H_irf * r), loglik, iters, status, xhat
+    (fc_rows * ns)].  Returns (irfs (n_rep, r, H_irf, r) [variable, horizon, shock], bands dict of 5/16/50/84/95 percentiles,
+    records (n_rep, d))."""
+    from .api import _state_space_block
+    blk = _state_space_block(m, H_fc, lib, "ss_bootstrap")
+    e = blk["em"]
+    r = e["Q"].shape[0]; ns = blk["Xs"].shape[1]
+    nirf = r * H_irf * r
+    b, en = lib.shard_range(n_rep, rank, world)
+    rec = np.full((en - b, nirf + 3 + fc_rows * ns), np.nan)
+    if en > b:
+        o = lib.ss_bootstrap(blk["Xs"], blk["Lam"], e["R"], e["A"], e["Q"], e["P0"], p=blk["p"], n_rep=en - b, seed=seed, rep0=b,
+                             H_irf=H_irf, H_fc=H_fc, fc_rows=fc_rows, max_iter=max_iter, tol=tol,
+                             outputs=("irf", "xhat") if fc_rows > 0 else ("irf",))
+        rec[:, :nirf] = o["irf"].transpose(0, 3, 2, 1).reshape(en - b, -1)      # dfm_irf's record layout [shock][horizon][variable]
+        rec[:, nirf] = o["loglik"]; rec[:, nirf + 1] = o["iters"]; rec[:, nirf + 2] = o["status"]
+        if fc_rows > 0:
+            rec[:, nirf + 3:] = o["xhat"].reshape(en - b, -1)
+    allrec = gather_records(rec, n_rep, rank, world, lib)
+    irfs = np.ascontiguousarray(allrec[:, :nirf].reshape(n_rep, r, H_irf, r).transpose(0, 3, 2, 1))
+    pb = lib.percentiles(allrec[:, :nirf], BAND_PERCENTILES)
+    bands = {q: pb[k].reshape(r, H_irf, r).transpose(2, 1, 0) for k, q in enumerate(BAND_PERCENTILES)}
+    return irfs, bands, allrec

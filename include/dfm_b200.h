@@ -306,6 +306,68 @@ typedef struct {              /* any pointer may be NULL (not computed); per pai
 int dfm_news(dfm_handle* h, const double* X_old, const double* X_new, const dfm_news_opts* opts, const dfm_em_init* params,
              const dfm_news_out* out);
 
+/* ---- parametric bootstrap of a fitted state-space model: bands with parameter uncertainty ------------------------------
+ * Forecasts, posterior draws and news condition on the EM estimates theta^ = (Lam, R, A, Q).  This call draws B panels from
+ * the model at theta^, re-runs the EM on all of them from theta^, brings every replicate back into the rotation of theta^
+ * and returns its parameters, impulse responses and (optionally) forecasts, so that bands over the replicates carry the
+ * estimation uncertainty of theta (the spec is tests/ss_bootstrap_oracle.py).
+ * Panels (standardized model units, not re-standardized):  z_1 = L_P0 nu,  z_t = M z_{t-1} + [L_Q eta_t; 0],
+ * x_it = lam_i' f_t + sqrt(R_i) eps_it where the template panel is observed, NaN where it is missing (the original missing
+ * pattern and ragged edge) and in the columns of series out of the model (NaN Lam row or R_i).  L_P0, L_Q: lower Cholesky
+ * factors, a pivot <= 1e-12 max diag counting as a zero column (the simulation smoother's rule).
+ * Random numbers: the Philox4x32-10 stream of the replication generators with replication id = rep0 + b and three streams
+ * (element indices; k = r p), after the simulation smoother's 7-10:
+ *   11  nu, z_1 = L_P0 nu                              element a        (a < k)
+ *   12  state shocks eta_t of periods t >= 1           element t r + a  (a < r)
+ *   13  eps_it, the idiosyncratic draw of a cell        element i T + t  (drawn for cells the template observes)
+ * so replicate b is a pure function of (seed, rep0 + b): any split of a replication range (dfm_shard_range) gives
+ * bit-identical panels, and dfm_ss_bootstrap's replicate b re-estimates exactly dfm_ss_simulate_panels' panel b. */
+/* X: T x N template (standardized; only its NaN pattern is read); params: (Lam, R, A, Q, P0) of ONE model, P0 required
+ * (e.g. the EM's P0 output).  Xout: batch panels T x N column-major, replication ids rep0 .. rep0 + batch - 1.
+ * k = r p > 48: DFM_ERR_UNSUPPORTED.  Synchronous for host memory. */
+int dfm_ss_simulate_panels(dfm_handle* h, const double* X, int T, int N, int r, int p, const dfm_em_init* params, unsigned long long seed,
+                           long long rep0, int batch, int mem, double* Xout);
+
+typedef struct {
+  int T, N, r, p;             /* the fitted model's panel T x N (STANDARDIZED, NaN = missing) and state shape */
+  int H_irf;                  /* > 0: impulse-response horizons 0 .. H_irf - 1 */
+  int H_fc;                   /* >= 0: periods after the panel for the forecasts */
+  int fc_rows;                /* 0 .. T + H_fc: trailing rows of the padded (T + H_fc) x N forecast panel returned per replicate
+                                 (so that the ragged edge can be included); 0 = no forecasts */
+  int max_iter; double tol;   /* EM of every replicate, as dfm_em_opts (tol = 0: run max_iter iterations) */
+  long long n_rep;            /* >= 1 replicates */
+  long long rep0;             /* replication id of the first replicate, >= 0 */
+  unsigned long long seed;
+  int mem;
+} dfm_ssb_opts;
+
+typedef struct {              /* any pointer may be NULL (not computed / not returned); per replicate back to back; column-major */
+  double* Lam;                /* N x r     aligned loadings (NaN rows for series out of the model) */
+  double* R;                  /* N         idiosyncratic variances */
+  double* A;                  /* r x k     aligned [A_1 .. A_p] */
+  double* Q;                  /* r x r     aligned state-shock covariance */
+  double* irf;                /* r x H_irf x r records [shock j][horizon h][variable i] as dfm_bootstrap_irf's: Q M^h G e_j with
+                                 G = [chol(Q~); 0] (orthogonalized shocks of the aligned model) */
+  double* xhat;               /* fc_rows x N   E[x_it | data] at the replicate's parameters (last fc_rows rows of T + H_fc) */
+  double* xvar;               /* fc_rows x N   Var[x_it | data] at the replicate's parameters */
+  double* loglik;             /* [n_rep]   log-likelihood of the parameters entering the replicate's last EM iteration */
+  int* iters;                 /* [n_rep]   EM iterations */
+  int* status;                /* [n_rep]   0; the EM status when not 0; DFM_ERR_NOT_PD when the alignment fails (Lam*' W Lam* or
+                                 X singular, or Q~ not positive definite; see DESIGN.md 4.9).  A failed replicate has NaN
+                                 parameters, impulse responses and forecasts; loglik / iters stay the EM's. */
+} dfm_ssb_out;
+
+/* Alignment (rotation f -> K f of the EM estimates Lam*, R*, A*, Q* onto theta^), W = diag(1 / R^_i) over the series in the model:
+ *   X = (Lam*' W Lam*)^-1 Lam*' W Lam^,  K = X^-1,  Lam~ = Lam* X,  A~_l = K A*_l X,  Q~ = K Q* K',  R~ = R*.
+ * X: T x N standardized panel of the fitted model; params: theta^ (Lam, R, A, Q, P0), P0 required (the EM holds it fixed; every
+ * replicate's EM starts from theta^ with it).  Balanced panels with p = 1, r <= 8 and even T re-estimate on dfm_em_kalman's
+ * fused path, everything else on its general path.  Bad shapes / options (H_irf <= 0, n_rep < 1, fc_rows > T + H_fc, ...):
+ * DFM_ERR_ARG; k = r p > 48: DFM_ERR_UNSUPPORTED; per-replicate failures go to status only.  The replicates run in
+ * sub-batches whose size depends only on (T, N, r, p) and the device (the last one filled up with the following replication
+ * ids, whose results are discarded), so the device memory of a call does not grow with n_rep and replicate rep0 + b has the
+ * same bits whatever n_rep, the shard split or the number of calls.  Synchronous. */
+int dfm_ss_bootstrap(dfm_handle* h, const double* X, const dfm_ssb_opts* opts, const dfm_em_init* params, const dfm_ssb_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

@@ -262,4 +262,33 @@ function news(Xold::Matrix{Float64}, Xnew::Matrix{Float64}, em, H::Integer, targ
     return (old = old, new = new, news = nw, weights = w, contributions = c, status = st[])
 end
 
+struct SsbOpts; T::Cint; N::Cint; r::Cint; p::Cint; H_irf::Cint; H_fc::Cint; fc_rows::Cint; max_iter::Cint; tol::Cdouble
+                n_rep::Clonglong; rep0::Clonglong; seed::Culonglong; mem::Cint; end
+struct SsbOut; Lam::Ptr{Cdouble}; R::Ptr{Cdouble}; A::Ptr{Cdouble}; Q::Ptr{Cdouble}; irf::Ptr{Cdouble}; xhat::Ptr{Cdouble}
+               xvar::Ptr{Cdouble}; loglik::Ptr{Cdouble}; iters::Ptr{Cint}; status::Ptr{Cint}; end
+
+"""Parametric bootstrap (dfm_ss_bootstrap) of the state-space model `em` (the result of `estimate!(m, Parametric())`, P0
+included) fitted to the standardized panel `Xs`: replicates `rep0 .. rep0+n_rep-1` (stream `seed`) are simulated, re-estimated
+by EM from `em` and rotated back onto it.  Returns the aligned Lam (N x r x n_rep), R, A, Q, the impulse responses
+irf (r x H_irf x r x n_rep, [shock, horizon, variable] as `dfm_irf`), xhat / xvar (fc_rows x N x n_rep: the last fc_rows of
+the T+H_fc rows), loglik, iters, status (standardized units; status != 0: a failed replicate with NaN records)."""
+function ss_bootstrap(Xs::Matrix{Float64}, em, n_rep::Integer, seed::Integer; H_irf::Integer = 24, H_fc::Integer = 0,
+                      fc_rows::Integer = H_fc, max_iter::Integer = 50, tol::Real = 0.0, rep0::Integer = 0)
+    h = gethandle()
+    T, N = size(Xs); r = size(em.Lam, 2); k = size(em.A, 2); p = k ÷ r
+    Lam = Array{Float64}(undef, N, r, n_rep); R = Matrix{Float64}(undef, N, n_rep); A = Array{Float64}(undef, r, k, n_rep)
+    Q = Array{Float64}(undef, r, r, n_rep); irf = Array{Float64}(undef, r, H_irf, r, n_rep)
+    xhat = Array{Float64}(undef, fc_rows, N, n_rep); xvar = similar(xhat)
+    ll = Vector{Float64}(undef, n_rep); it = Vector{Cint}(undef, n_rep); st = Vector{Cint}(undef, n_rep)
+    GC.@preserve Xs em Lam R A Q irf xhat xvar ll it st begin
+        opts = Ref(SsbOpts(T, N, r, p, H_irf, H_fc, fc_rows, max_iter, tol, n_rep, rep0, seed, MEM_HOST))
+        init = Ref(EmInit(pointer(em.Lam), pointer(em.R), pointer(em.A), pointer(em.Q), pointer(em.P0)))
+        out = Ref(SsbOut(pointer(Lam), pointer(R), pointer(A), pointer(Q), pointer(irf), pointer(xhat), pointer(xvar), pointer(ll),
+                         pointer(it), pointer(st)))
+        check(ccall((:dfm_ss_bootstrap, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ref{SsbOpts}, Ref{EmInit}, Ref{SsbOut}), h, Xs, opts, init, out),
+              "dfm_ss_bootstrap")
+    end
+    return (Lam = Lam, R = R, A = A, Q = Q, irf = irf, xhat = xhat, xvar = xvar, loglik = ll, iters = it, status = st)
+end
+
 end # module
