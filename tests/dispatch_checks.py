@@ -290,7 +290,7 @@ def _als_masked(r):
 
 for _r, _N, _T in ((2, 16, 150), (4, 21, 150), (6, 31, 151), (7, 40, 150)):
     _fused(_r, _N, _T)
-for _r, _N, _T in ((2, 16, 264), (6, 27, 150), (7, 40, 302)):            # N % 8 = 3 and T % 132 = 18 at r = 6
+for _r, _N, _T in ((2, 16, 264), (6, 27, 150), (7, 40, 302)):            # N % 8 = 3 and one short chunk (150 < 172) at r = 6
     _fused2(_r, _N, _T)
 for _r in (1, 2, 4, 5, 6, 7):
     _als_fused(_r)

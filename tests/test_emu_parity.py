@@ -104,7 +104,7 @@ def test_table5_through_kernel_source(lib, panels, notebook_tables, vset):
 
 @pytest.mark.parametrize("N,r,T", [(19, 5, 62), (33, 2, 44), (27, 7, 150), (50, 6, 36)])
 def test_fused2_em_ragged_shapes(lib, N, r, T):
-    """Shapes that are not multiples of the 8-series / 132-period stage geometry or of the scan chunking, and the
+    """Shapes that are not multiples of the 8-series / 172-period stage geometry or of the scan chunking, and the
     template instantiations the other tests do not touch (r = 2, 5, 6, 7)."""
     P.check_em(lib, N=N, r=r, T=T, p=1, miss=0.0, path=3, iters=4)
 

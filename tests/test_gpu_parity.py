@@ -162,10 +162,10 @@ def test_fused_rejects_missing(lib):
 def test_fused2_em_r3(lib): P.check_em(lib, p=1, miss=0.0, path=3)
 def test_fused2_em_r8(lib): P.check_em(lib, N=40, r=8, T=90, p=1, miss=0.0, path=3, iters=5)
 def test_fused2_em_r1(lib): P.check_em(lib, N=12, r=1, T=50, p=1, miss=0.0, path=3, iters=4)
-def test_fused2_em_r5_ragged(lib): P.check_em(lib, N=37, r=5, T=102, p=1, miss=0.0, path=3, iters=4)   # N % 8 != 0, short chunks
-def test_fused2_em_long(lib): P.check_em(lib, N=24, r=4, T=300, p=1, miss=0.0, path=3, iters=3)        # several ring wraps, 3 period chunks
-def test_fused2_em_ragged_long(lib): P.check_em(lib, N=45, r=8, T=278, p=1, miss=0.0, path=3, iters=3)   # tail chunk 14 periods (len % 4 == 2), N % 8 == 5
-def test_fused2_em_exact_chunks(lib): P.check_em(lib, N=16, r=8, T=264, p=1, miss=0.0, path=3, iters=3)   # T == 2 full chunks: overlapped last row block everywhere
+def test_fused2_em_r5_ragged(lib): P.check_em(lib, N=37, r=5, T=102, p=1, miss=0.0, path=3, iters=4)   # N % 8 != 0, one short period chunk
+def test_fused2_em_long(lib): P.check_em(lib, N=24, r=4, T=300, p=1, miss=0.0, path=3, iters=3)        # several ring wraps, 2 period chunks
+def test_fused2_em_ragged_long(lib): P.check_em(lib, N=45, r=8, T=278, p=1, miss=0.0, path=3, iters=3)   # tail chunk 106 periods (len % 4 == 2), N % 8 == 5
+def test_fused2_em_exact_chunks(lib): P.check_em(lib, N=16, r=8, T=264, p=1, miss=0.0, path=3, iters=3)   # a full chunk + a 92-period tail (T = 2 x 132 fitted the former box)
 def test_fused2_em_convergence_rule(lib): P.check_em_convergence_rule(lib, path=3)
 def test_fused2_em_batch(lib): P.check_em_batch_balanced(lib, B=7, path=3)
 def test_fused2_matches_general_c2(lib):
