@@ -56,6 +56,10 @@ class EmOut(C.Structure):
                 ("F", C.c_void_p), ("PF", C.c_void_p), ("loglik", C.c_void_p), ("iters", C.c_void_p), ("status", C.c_void_p)]
 
 
+class LamConstr(C.Structure):
+    _fields_ = [("n_constr", C.c_int), ("index", c_ip), ("H", c_dp), ("h", c_dp)]
+
+
 class SsOpts(C.Structure):
     _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("batch", C.c_int), ("mem", C.c_int)]
 
@@ -111,7 +115,7 @@ def default_library_path():
 EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stream", "dfm_destroy", "dfm_sync",
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
-           "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_kalman_smooth", "dfm_simulation_smoother",
+           "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
            "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
@@ -140,6 +144,19 @@ def from_cm(buf, rows, cols, batch=None):
     if batch is None:
         return np.ascontiguousarray(buf.reshape(cols, rows).T)
     return np.ascontiguousarray(buf.reshape(batch, cols, rows).transpose(0, 2, 1))
+
+
+def _lam_constr(constr, r):
+    """(index, H (n_c x r), h) -> (LamConstr, the arrays it points to).  None entries become NULL pointers (the library refuses
+    them when n_c > 0)."""
+    idx, H, h = constr
+    n = len(idx) if idx is not None else (len(h) if h is not None else 0)
+    ia = np.ascontiguousarray(idx, dtype=np.int32) if idx is not None else None
+    Hm = to_cm(np.asarray(H, float).reshape(n, r)) if H is not None else None
+    hv = np.ascontiguousarray(h, dtype=np.float64) if h is not None else None
+    lc = LamConstr(n_constr=n, index=ia.ctypes.data_as(c_ip) if ia is not None else None,
+                   H=Hm.ctypes.data_as(c_dp) if Hm is not None else None, h=hv.ctypes.data_as(c_dp) if hv is not None else None)
+    return lc, (ia, Hm, hv)
 
 
 class Library:
@@ -179,6 +196,8 @@ class Library:
         L.dfm_irf.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_ip,
                               C.c_int, C.c_int, C.c_void_p]
         L.dfm_em_kalman.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(EmOpts), C.POINTER(EmInit), C.POINTER(EmOut)]
+        L.dfm_em_kalman_constrained.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(EmOpts), C.POINTER(EmInit), C.POINTER(LamConstr),
+                                                C.POINTER(EmOut)]
         L.dfm_kalman_smooth.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsOpts), C.POINTER(EmInit), C.POINTER(SsOut)]
         L.dfm_simulation_smoother.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SimOpts), C.POINTER(EmInit), C.POINTER(SimOut)]
         L.dfm_news.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(NewsOpts), C.POINTER(EmInit), C.POINTER(NewsOut)]
@@ -240,13 +259,19 @@ class Library:
             i += 1
         return out
 
-    def em_kalman_raw(self, X, T, N, r, p, B, max_iter, tol, init, out, mem, path=0):
+    def em_kalman_raw(self, X, T, N, r, p, B, max_iter, tol, init, out, mem, path=0, constr=None):
         """Pointer-level call (ints = device or pinned-host addresses).  init/out: dicts of
-        name -> address (missing = NULL)."""
+        name -> address (missing = NULL).  constr: as em_kalman (host arrays)."""
         o = EmOpts(T=T, N=N, r=r, p=p, max_iter=max_iter, tol=tol, batch=B, mem=mem, path=path)
         ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in init.items()})
         ou = EmOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
-        self.check(self.lib.dfm_em_kalman(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_em_kalman")
+        if constr is None:
+            self.check(self.lib.dfm_em_kalman(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_em_kalman")
+            return
+        lc, keep = _lam_constr(constr, r)
+        self.check(self.lib.dfm_em_kalman_constrained(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(lc), C.byref(ou)),
+                   "dfm_em_kalman_constrained")
+        del keep
 
     def kalman_smooth_raw(self, X, T, N, r, p, H, B, params, out, mem):
         """Pointer-level dfm_kalman_smooth (ints = device or host addresses).  params: dict Lam, R, A, Q[, P0]; out: dict of
@@ -478,7 +503,9 @@ class Library:
                                                      _ptr(R), _ptr(A), _ptr(Q)), "dfm_em_init_from_factors")
         return from_cm(Lam, N, r, b), (R.reshape(B, N) if b else R), from_cm(A, r, k, b), from_cm(Q, r, r, b)
 
-    def em_kalman(self, X, Lam, R, A, Q, p=1, P0=None, max_iter=50, tol=0.0, path=0, want_PF=True):
+    def em_kalman(self, X, Lam, R, A, Q, p=1, P0=None, max_iter=50, tol=0.0, path=0, want_PF=True, constr=None):
+        """State-space EM (dfm_em_kalman).  constr = (index[int], H[n_c x r], h[n_c]) in STANDARDIZED units, or None: the EM under
+        H[q] @ Lam[index[q]] = h[q] (dfm_em_kalman_constrained), the same restriction for every panel of a batch."""
         X = np.asarray(X, float); b = X.shape[0] if X.ndim == 3 else None
         T, N = X.shape[-2:]; r = np.asarray(Lam).shape[-1]; B = b or 1; k = r * p
         o = EmOpts(T=T, N=N, r=r, p=p, max_iter=max_iter, tol=tol, batch=B, mem=MEM_HOST, path=path)
@@ -490,7 +517,13 @@ class Library:
         oit = np.empty(B, dtype=np.int32); ost = np.empty(B, dtype=np.int32)
         out = EmOut(Lam=_ptr(oL), R=_ptr(oR), A=_ptr(oA), Q=_ptr(oQ), P0=_ptr(oP0), F=_ptr(oF), PF=_ptr(oPF), loglik=_ptr(oll),
                     iters=_ptr(oit), status=_ptr(ost))
-        self.check(self.lib.dfm_em_kalman(self.h, _ptr(bufs["X"]), C.byref(o), C.byref(ini), C.byref(out)), "dfm_em_kalman")
+        if constr is None:
+            self.check(self.lib.dfm_em_kalman(self.h, _ptr(bufs["X"]), C.byref(o), C.byref(ini), C.byref(out)), "dfm_em_kalman")
+        else:
+            lc, keep = _lam_constr(constr, r)
+            self.check(self.lib.dfm_em_kalman_constrained(self.h, _ptr(bufs["X"]), C.byref(o), C.byref(ini), C.byref(lc), C.byref(out)),
+                       "dfm_em_kalman_constrained")
+            del keep
         res = dict(Lam=from_cm(oL, N, r, b), R=oR.reshape(B, N) if b else oR, A=from_cm(oA, r, k, b), Q=from_cm(oQ, r, r, b),
                    P0=from_cm(oP0, k, k, b), F=from_cm(oF, T, r, b), loglik=oll.reshape(B, max_iter) if b else oll,
                    iters=oit if b else int(oit[0]), status=ost if b else int(ost[0]))

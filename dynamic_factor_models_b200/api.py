@@ -169,27 +169,37 @@ def impulse_response(varm, shock_ids, T, lib=None):
     return lib.irf(varm.M, varm.Q, varm.G, T, [i - 1 for i in ids])
 
 
-def estimate(m, method=None, lam_constr_f=None, lam_constr_fl=None, lib=None):
-    """estimate!(m, ::NonParametric) :530-543;  estimate!(m, ::Parametric) = the slot of :23."""
+def estimate(m, method=None, lam_constr_f=None, lam_constr_fl=None, lam_constr_em=None, lib=None):
+    """estimate!(m, ::NonParametric) :530-543;  estimate!(m, ::Parametric) = the slot of :23.
+
+    lam_constr_em (Parametric only): a LambdaConstraint on the estimation series (indices as lam_constr_f's, r in data units)
+    under which the state-space EM runs, e.g. the named-factor normalisation of Figure 7.  Its r is divided by the estimation
+    block's xstd (standardize_constraint!); the standardized restriction is kept in m.em["lam_constr"]."""
     method = method or NonParametric()
     estimate_factor(m, lam_constr=lam_constr_f, lib=lib)
     estimate_factor_loading(m, lam_constr=lam_constr_fl, lib=lib)
     estimate_var(m.factor_var_model, lib=lib)
     if isinstance(method, Parametric):
-        _estimate_parametric(m, method, lib or get_library())
+        _estimate_parametric(m, method, lib or get_library(), lam_constr_em)
     return None
 
 
-def _estimate_parametric(m, method, lib):
-    """State-space EM initialised by the non-parametric estimates (SURVEY.md section 8 row a')."""
+def _estimate_parametric(m, method, lib, lam_constr_em=None):
+    """State-space EM initialised by the non-parametric estimates (SURVEY.md section 8 row a'), restricted by lam_constr_em."""
     i0, i1 = m.initperiod, m.lastperiod
     p = method.n_factorlag or m.n_factorlag
     X = m.data[:, m.inclcode == 1][i0 - 1:i1]
-    Xs, _, _ = lib.standardize(X)
+    Xs, _, xstd = lib.standardize(X)
     Xs = np.where(np.isnan(m.lambda_est[:, :1].T), np.nan, Xs)      # series dropped by nt_min stay out of the model
     F0 = m.factor[i0 - 1:i1]
     Lam, R, A, Q = lib.em_init_from_factors(Xs, F0, p)
-    m.em = lib.em_kalman(Xs, Lam, R, A, Q, p=p, max_iter=method.max_iter, tol=method.tol)
+    constr = None
+    if lam_constr_em is not None:
+        idx = np.asarray(lam_constr_em.indices, dtype=np.int32)
+        constr = (idx, np.asarray(lam_constr_em.R, float).reshape(len(idx), -1), np.asarray(lam_constr_em.r, float) / xstd[idx])
+    m.em = lib.em_kalman(Xs, Lam, R, A, Q, p=p, max_iter=method.max_iter, tol=method.tol, constr=constr)
+    if constr is not None:
+        m.em["lam_constr"] = constr
     m.factor[i0 - 1:i1] = m.em["F"]
     return None
 
@@ -359,6 +369,22 @@ def parametric_irf(m, H, lib=None):
     return lib.irf(M, Qs, G, H, list(range(r)))
 
 
+def series_irf(m, H, lib=None):
+    """Responses of the estimation series to the orthogonalised factor shocks of `parametric_irf(m, H)`, in data units:
+    (ns, H, r) [series, horizon, shock], out[i, h, j] = xstd_i lam_i' irf[:, h, j] with lam_i = m.em["Lam"][i] (series in the
+    order of forecast's `series`; NaN for series out of the model).
+
+    Identification: the factors of a state-space DFM are identified only up to f -> K f (Lam -> Lam K^-1, A_l -> K A_l K^-1,
+    Q -> K Q K').  Under a named-factor restriction (lam_constr_em pinning some series' loadings to e_1', as Figure 7's oil
+    series) the rotations left free have K's first row e_1'.  Then (K Q K')_11 = Q_11 and (K Q K') e_1 = K Q e_1, so the first
+    column of chol(K Q K') is K times that of chol(Q): the factor responses to shock 1 become K times the old ones and the series
+    responses lam_i' K^-1 K irf do not change.  The column of shock 1 is identified even though factors 2..r are not; the other
+    shocks' columns depend on the rotation."""
+    irf = parametric_irf(m, H, lib=lib)
+    b = _state_space_block(m, 0, lib, "series_irf")
+    return b["xstd"][:, None, None] * np.einsum("ia,ahj->ihj", b["Lam"], irf)
+
+
 def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
                          lib=None):
     """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn
@@ -377,6 +403,9 @@ def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922
       total_var (fc_rows, ns)           mean_b xvar_b + var_b xhat_b (law of total variance: filtering and parameter uncertainty);
       loglik, iters, status (n_rep)     the replicates' EM results (status != 0: failed, NaN records);
     and periods (the fc_rows rows, 1-based), series, q.  Series left out of the model have NaN columns.  n_rep <= 16384."""
+    if m.em is not None and m.em.get("lam_constr") is not None:
+        raise ValueError("parametric_bootstrap: the EM of m ran under restrictions on the loadings (lam_constr_em); the bootstrap "
+                         "re-estimates without them and its rotation onto m.em would undo them")
     if not 1 <= n_rep <= 16384:
         raise ValueError("parametric_bootstrap: n_rep must be in [1, 16384]")
     if H_irf <= 0:

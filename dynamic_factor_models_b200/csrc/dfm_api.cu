@@ -16,6 +16,7 @@
 #include "dfm_kernels_news.cuh"
 #include "dfm_kernels_ssb.cuh"
 #include <algorithm>
+#include <cmath>
 #include <new>
 #include <thread>
 #include <type_traits>
@@ -336,10 +337,18 @@ static void emb_launch_E(dfm_handle* h, const EmbPlan& e, const double* x, const
       dBt, dqt, dslr, dnt, st);
   });
 }
+// cs.off != nullptr (restrictions on the loadings): k_emb_mstep_constr with its scratch for the correction.
 static void emb_launch_M(dfm_handle* h, const EmbPlan& e, const double* x, const double* dFs, const double* dSff, int T, int N, int r, int batch,
-                         double* dL, double* dR, double* dW, double* dlogR, EmState* st) {
+                         double* dL, double* dR, double* dW, double* dlogR, EmState* st, EmConstr cs = EmConstr{}) {
   dispatch<1, 4>(e.ncb, [&](auto C) {
     constexpr int NCB = decltype(C)::value;
+    if (cs.off) {
+      const size_t sm = e.smM + (size_t)em_constr_scratch(r) * 8;
+      DFM_SET_SMEM(k_emb_mstep_constr<NCB>, sm);
+      L(k_emb_mstep_constr<NCB>, e.ntM, e.tsM * batch, 256, sm, x, dFs, dSff, T, N, r, e.tsM, e.tper, batch, e.Spart, e.sxxpart,
+        e.counters + (size_t)batch * e.ntE, dL, dR, dW, dlogR, e.Cpart, st, cs);
+      return;
+    }
     DFM_SET_SMEM(k_emb_mstep<NCB>, e.smM);
     L(k_emb_mstep<NCB>, e.ntM, e.tsM * batch, 256, e.smM, x, dFs, dSff, T, N, r, e.tsM, e.tper, batch, e.Spart, e.sxxpart,
       e.counters + (size_t)batch * e.ntE, dL, dR, dW, dlogR, e.Cpart, st);
@@ -438,8 +447,10 @@ static int launch_filter_smooth(dfm_handle* h, int& ncl, const GenBufs& g, int b
   return DFM_OK;
 }
 
-// General multi-kernel EM path on device-resident data (any r, p, missing data).
-static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, const EmBufs& d, const GenBufs& g, int want_psf) {
+// General multi-kernel EM path on device-resident data (any r, p, missing data).  cs: restrictions on the loadings (the
+// device CSR of em_kalman_impl; off == nullptr: none), applied by the two measurement M-step kernels.
+static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, const EmBufs& d, const GenBufs& g, int want_psf,
+                          EmConstr cs) {
   const int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mi = o->max_iter;
   const int np = r * (r + 1) / 2;
   const int ntC = tpt_threads(np + r), nblkC = (T + ntC - 1) / ntC;
@@ -470,9 +481,13 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
       else emb_launch_E(h, emb, x, g.W, d.R, g.logR, T, N, r, batch, g.Bt, g.qt, g.slr, g.nt, d.st);
     }
     launch_filter_smooth(h, ncl, g, batch, T, r, p, d.A, d.Q, d.P0, d.Fs, d.PsF, d.ll, d.st, mi, o->tol, want_psf);
-    if (any_missing || !emb.on) L(k_em_mstep_series, N, batch, 64, (size_t)(2 * np + r + 8) * 8, x, d.Fs, d.PsF, g.Sff, T, N, r, d.L, d.R, d.st, emb_on);
+    if (any_missing || !emb.on) {
+      const size_t smS = (size_t)(2 * np + r + 8 + (cs.off ? em_constr_scratch(r) : 0)) * 8;
+      if (cs.off) DFM_SET_SMEM(k_em_mstep_series, smS);
+      L(k_em_mstep_series, N, batch, 64, smS, x, d.Fs, d.PsF, g.Sff, T, N, r, d.L, d.R, d.st, emb_on, cs);
+    }
     if (any_bal && emb.on) {
-      emb_launch_M(h, emb, x, d.Fs, g.Sff, T, N, r, batch, d.L, d.R, g.W, g.logR, d.st);
+      emb_launch_M(h, emb, x, d.Fs, g.Sff, T, N, r, batch, d.L, d.R, g.W, g.logR, d.st, cs);
       L(k_emb_close, batch, 1, 256, 0, N, r, p, emb.ntM, emb.Cpart, g.C, d.A, g.An, d.Q, g.Qn, d.st, mi, 1);
     }
     if (any_missing || !emb.on) L(k_em_prep, batch, 1, 128, 0, d.L, d.R, N, r, p, g.W, g.logR, g.C, d.A, g.An, d.Q, g.Qn, d.st, mi, 1, emb_on);
@@ -1139,12 +1154,41 @@ int dfm_em_init_from_factors(dfm_handle* h, const double* Xs, const double* F, i
 }
 
 // ------------------------------------------------------------------------------------ a'
-int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const dfm_em_init* init, const dfm_em_out* out) {
+// dfm_em_kalman and dfm_em_kalman_constrained.  con == nullptr or con->n_constr == 0: the unrestricted EM (same dispatch, same
+// bits).  Otherwise the restriction is checked, uploaded once as a per-series CSR (rows grouped by series in their given order)
+// and the call runs the general path, whatever the shape.
+static int em_kalman_impl(dfm_handle* h, const double* X, const dfm_em_opts* o, const dfm_em_init* init, const dfm_lam_constr* con,
+                          const dfm_em_out* out) {
   if (!h || !X || !o || !init || !out || !init->Lam || !init->R || !init->A || !init->Q)
     return fail(h, DFM_ERR_ARG, "dfm_em_kalman: null argument");
   int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mem = o->mem, mi = o->max_iter;
   if (T <= 1 || N <= 0 || r <= 0 || r > 64 || p <= 0 || batch <= 0 || mi <= 0 || o->tol < 0)
     return fail(h, DFM_ERR_ARG, "dfm_em_kalman: bad shape/options");
+  const int nc = con ? con->n_constr : 0;
+  std::vector<int> coff;                  // host CSR of the restriction: offsets [N+1], rows [nc x r] row-major, values [nc]
+  std::vector<double> cH, ch;
+  if (nc < 0) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: n_constr < 0");
+  if (nc > 0) {
+    if (!con->index || !con->H || !con->h) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: null restriction array");
+    coff.assign((size_t)N + 1, 0);
+    for (int q = 0; q < nc; ++q) {
+      const int i = con->index[q];
+      if (i < 0 || i >= N) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: restriction index outside [0, N)");
+      if (!std::isfinite(con->h[q])) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: non-finite restriction value");
+      for (int a = 0; a < r; ++a)
+        if (!std::isfinite(con->H[q + (size_t)nc * a])) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: non-finite restriction row");
+      if (++coff[i + 1] > r) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: more than r restriction rows on one series");
+    }
+    for (int i = 0; i < N; ++i) coff[i + 1] += coff[i];
+    cH.resize((size_t)nc * r); ch.resize(nc);
+    std::vector<int> fill(coff.begin(), coff.end() - 1);
+    for (int q = 0; q < nc; ++q) {
+      const int dst = fill[con->index[q]]++;
+      for (int a = 0; a < r; ++a) cH[(size_t)dst * r + a] = con->H[q + (size_t)nc * a];
+      ch[dst] = con->h[q];
+    }
+    if (o->path == 2 || o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman_constrained: the fused paths take no restrictions");
+  }
   if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: batch > 65535");
   const int stgT = fs_stage_periods(h->nsm, batch, r, p);
   size_t smFS = em_fs_smem_doubles(r, p, stgT) * 8;
@@ -1155,8 +1199,8 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
   if (o->path == 2 && !fused_ok) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs p = 1, r <= 8 and a panel that fits shared memory");
   const bool fused2_ok = fused2_shape_ok(T, N, r, p);
   if (o->path == 3 && !fused2_ok) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: TMA fused path needs p = 1, r <= 8, even T and a panel that fits shared memory");
-  const bool try_fused = (fused_ok || fused2_ok) && o->path != 1;      // the path is only chosen after the NaN scan
-  const bool use2 = fused2_ok && (o->path == 0 || o->path == 3);
+  const bool try_fused = (fused_ok || fused2_ok) && o->path != 1 && nc == 0;      // the path is only chosen after the NaN scan
+  const bool use2 = fused2_ok && (o->path == 0 || o->path == 3) && nc == 0;
   const EmbPlan emb = emb_plan(T, N, r, batch, h->nsm);
   for (int pass = 0; pass < 2; ++pass) {
     Arena a(pass ? h->ws : nullptr);
@@ -1172,7 +1216,14 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
     d.ready = a.get<int>(kMaxReadyChunks);
     d.scratch = try_fused ? a.get<double>((size_t)std::min(batch, h->nsm * 8) * T * FUSED_SCR(r)) : nullptr;
     const GenBufs g = gen_bufs(a, emb, B, T, N, r, p);        // also the fallback when the scan finds missing data
+    EmConstr cs{};
+    if (nc) { cs.off = a.get<int>((size_t)N + 1); cs.H = a.get<double>((size_t)nc * r); cs.h = a.get<double>(nc); }
     if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    if (nc) {                             // (pageable sources: each copy returns once its source has been staged)
+      CK(cudaMemcpyAsync((void*)cs.off, coff.data(), coff.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync((void*)cs.H, cH.data(), cH.size() * 8, cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync((void*)cs.h, ch.data(), ch.size() * 8, cudaMemcpyHostToDevice, h->stream));
+    }
     int rc = DFM_OK;
     bool fused = try_fused;
     bool uploaded = false;                // the streaming host path found missing data: the panels are on the device already
@@ -1209,7 +1260,7 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
       }
     }
     if (fused) rc = launch_em_fused(h, fused_args(d, o, x), r, use2);
-    else rc = run_em_general(h, x, o, d, g, out->PF ? 1 : 0);
+    else rc = run_em_general(h, x, o, d, g, out->PF ? 1 : 0, cs);
     if (rc) return rc;
     rc = copy_out(h, out->Lam, d.L, B * N * r, mem); if (rc) return rc;
     rc = copy_out(h, out->R, d.R, B * N, mem); if (rc) return rc;
@@ -1227,6 +1278,15 @@ int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const df
     rc = copy_out(h, out->status, d.stat, B, mem); if (rc) return rc;
   }
   return finish(h, mem);
+}
+
+int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* o, const dfm_em_init* init, const dfm_em_out* out) {
+  return em_kalman_impl(h, X, o, init, nullptr, out);
+}
+
+int dfm_em_kalman_constrained(dfm_handle* h, const double* X, const dfm_em_opts* o, const dfm_em_init* init, const dfm_lam_constr* constr,
+                              const dfm_em_out* out) {
+  return em_kalman_impl(h, X, o, init, constr, out);
 }
 
 // ------------------------------------------------------------------------------------ a'': smoothing / nowcasting / forecasting

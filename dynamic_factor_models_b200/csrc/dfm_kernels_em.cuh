@@ -1048,11 +1048,55 @@ __global__ void EM_FS_BOUNDS k_em_filter_smooth(const double* __restrict__ Aall,
   }
 }
 
+// Linear restrictions on the loadings (LambdaConstraint, standardized units), uploaded once per call as a per-series CSR:
+// the rows of series i are off[i] .. off[i+1]-1, row q is H[q*r .. q*r+r) (row-major) with value h[q].  off == nullptr: none.
+struct EmConstr { const int* off; const double* H; const double* h; };
+#define EM_CONSTR_PIVOT_RTOL 1e-12     // G pivot <= this * G_jj: dependent restriction rows
+
+// shared scratch of lam_constr_correct (doubles): Y r x r, G packed, d r
+__host__ __device__ inline int em_constr_scratch(int r) { return r * r + r * (r + 1) / 2 + r; }
+
+// Restricted M-step of one series, one thread:  lam (in: lu = S^-1 s, out: lu - Y G^-1 (H lu - h)) with Y = S^-1 H',
+// G = H Y; solve(v) overwrites v (r) with S^-1 v using the caller's Cholesky factor of S.  m rows, m <= r.
+// ws: em_constr_scratch(r) doubles.  Returns 1 when G is singular (lam unchanged then).
+template <class Solve>
+__device__ inline int lam_constr_correct(double* lam, int r, const double* H, const double* h, int m, double* ws, Solve solve) {
+  double* Y = ws; double* G = Y + r * r; double* d = G + r * (r + 1) / 2;
+  for (int j = 0; j < m; ++j) {
+    const double* hj = H + (size_t)j * r;
+    for (int a = 0; a < r; ++a) Y[a + r * j] = hj[a];
+    solve(Y + r * j);
+    double v = -h[j];
+    for (int a = 0; a < r; ++a) v += hj[a] * lam[a];
+    d[j] = v;
+    for (int l = 0; l <= j; ++l) { double g = 0.0; for (int a = 0; a < r; ++a) g += hj[a] * Y[a + r * l]; G[pidx(j, l)] = g; }
+  }
+  for (int j = 0; j < m; ++j) {                       // packed Cholesky of G with a relative pivot test
+    double p = G[pidx(j, j)];
+    const double g0 = p;
+    for (int c = 0; c < j; ++c) p -= G[pidx(j, c)] * G[pidx(j, c)];
+    if (!(p > EM_CONSTR_PIVOT_RTOL * g0)) return 1;
+    p = sqrt(p);
+    G[pidx(j, j)] = p;
+    for (int i = j + 1; i < m; ++i) {
+      double s = G[pidx(i, j)];
+      for (int c = 0; c < j; ++c) s -= G[pidx(i, c)] * G[pidx(j, c)];
+      G[pidx(i, j)] = s / p;
+    }
+  }
+  chol_resolve_packed(G, d, m, 1);
+  for (int a = 0; a < r; ++a) { double v = lam[a]; for (int j = 0; j < m; ++j) v -= Y[a + r * j] * d[j]; lam[a] = v; }
+  return 0;
+}
+
 // Measurement M-step: one block per series.  S_ff^(i) = SffAll - sum_{t missing} E_t.
 // Lam_i = S_ff^(i)^-1 S_xf^(i);  R_i = (S_xx - 2 lam'S_xf + lam' S_ff lam) / T_i.   grid (N, B).
+// With restrictions (cs.off != nullptr) a restricted series' Lam_i is corrected (lam_constr_correct) with the packed Cholesky
+// factor of S_ff^(i) before R_i is formed; shared memory then holds em_constr_scratch(r) more doubles.
 __global__ void k_em_mstep_series(const double* __restrict__ Xall, const double* __restrict__ Fs_,
                                   const double* __restrict__ PsF_, const double* __restrict__ SffAll_, int T, int N,
-                                  int r, double* __restrict__ LamAll, double* __restrict__ Rall, EmState* st, int skip_bal) {
+                                  int r, double* __restrict__ LamAll, double* __restrict__ Rall, EmState* st, int skip_bal,
+                                  EmConstr cs) {
   DFM_SMEM(sm);
   int i = DFM_BX, b = DFM_BY;
   if (st[b].done) return;
@@ -1086,6 +1130,11 @@ __global__ void k_em_mstep_series(const double* __restrict__ Xall, const double*
   double sxf[64];
   for (int a = 0; a < r; ++a) sxf[a] = c[a];
   if (chol_solve_packed(A, c, r, 1)) { st[b].status = 3; return; }
+  if (cs.off) {
+    const int q0 = cs.off[i], m = cs.off[i + 1] - q0;
+    if (m > 0 && lam_constr_correct(c, r, cs.H + (size_t)q0 * r, cs.h + q0, m, A0 + np,
+                                    [&](double* v) { chol_resolve_packed(A, v, r, 1); })) { st[b].status = 3; return; }
+  }
   double q1 = 0.0, q2 = 0.0;
   for (int a = 0; a < r; ++a) {
     q1 += c[a] * sxf[a];

@@ -131,15 +131,41 @@ __global__ void k_emb_contract(const double* __restrict__ Xall, const double* __
   if (DFM_TID == 0) counters[b * ntiles + tile] = 0;
 }
 
+// R_i, W_i = Lam_i / R_i, log R_i of a restricted series i from its corrected loadings li[0..r) (S0: S_ff); li[r] = 1/R_i.
+// The same arithmetic as the unrestricted thread-per-series loop of emb_mstep_body, which keeps its own inline copy so that
+// the unrestricted kernel compiles exactly as before.
+__device__ __forceinline__ void emb_series_finish(double* li, const double* sx, const double* S0, int r, int T, int N, int i, double* Lam,
+                                                  double* R, double* W, double* logR, int* bad) {
+  const double sxx = sx[r];
+  double q1 = 0.0, q2 = 0.0;
+  for (int a = 0; a < r; ++a) {
+    q1 += li[a] * sx[a];
+    double v = 0.0;
+    for (int c = 0; c < r; ++c) v += S0[a + r * c] * li[c];
+    q2 += li[a] * v;
+  }
+  const double Ri = (sxx - 2.0 * q1 + q2) / (double)T;
+  R[i] = Ri;
+  const double rinv = 1.0 / Ri;
+  if (!(Ri > 0.0)) *bad = 1;
+  for (int a = 0; a < r; ++a) { Lam[i + (size_t)N * a] = li[a]; W[i + (size_t)N * a] = li[a] * rinv; }
+  logR[i] = log(Ri);
+  li[r] = rinv;
+}
+
 // M contraction + measurement M-step.  grid (ceil(N/64), tsplit * B), 256 threads.
-// Shared: 2 r*r + 2 * 64*(r+1) + 96 doubles.  Spart [tsplit][B][N x r], sxxpart [tsplit][B][N]; counters [B][ceil(N/64)].
-// Cpart [B][ceil(N/64)][r x r]: this tile's share of C = Lam' R^-1 Lam (summed by k_emb_close).
-template <int NCB>
-__global__ void k_emb_mstep(const double* __restrict__ Xall, const double* __restrict__ Fs_, const double* __restrict__ SffAll_,
-                            int T, int N, int r, int tsplit, int tper, int Bn, double* __restrict__ Spart,
-                            double* __restrict__ sxxpart, int* __restrict__ counters, double* __restrict__ LamAll,
-                            double* __restrict__ Rall, double* __restrict__ Wall, double* __restrict__ logRall,
-                            double* __restrict__ Cpart, EmState* st) {
+// Shared: 2 r*r + 2 * 64*(r+1) + 96 doubles (+ em_constr_scratch(r) when CON).  Spart [tsplit][B][N x r], sxxpart [tsplit][B][N];
+// counters [B][ceil(N/64)].  Cpart [B][ceil(N/64)][r x r]: this tile's share of C = Lam' R^-1 Lam (summed by k_emb_close).
+// k_emb_mstep_constr (the call has restrictions on the loadings, CON): the thread-per-series loop leaves the restricted series
+// of the tile at Lam_i = S_ff^-1 S_xf,i; thread 0 then corrects them one by one (lam_constr_correct with the shared Cholesky
+// factor of S_ff, scratch in shared memory) before their R_i, W_i, log R_i and the tile's share of C are formed.  Both
+// kernels are the one body below; without CON it compiles to the unrestricted kernel alone.
+template <int NCB, bool CON>
+__device__ __forceinline__ void emb_mstep_body(const double* __restrict__ Xall, const double* __restrict__ Fs_,
+                                               const double* __restrict__ SffAll_, int T, int N, int r, int tsplit, int tper, int Bn,
+                                               double* __restrict__ Spart, double* __restrict__ sxxpart, int* __restrict__ counters,
+                                               double* __restrict__ LamAll, double* __restrict__ Rall, double* __restrict__ Wall,
+                                               double* __restrict__ logRall, double* __restrict__ Cpart, EmState* st, EmConstr cs) {
   DFM_SMEM(sm);
   const int tile = DFM_BX, s = DFM_BY % tsplit, b = DFM_BY / tsplit;
   if (st[b].done || st[b].has_missing) return;
@@ -235,6 +261,7 @@ __global__ void k_emb_mstep(const double* __restrict__ Xall, const double* __res
     // L y = sxf ; L' lam = y   (y and lam overwrite li)
     for (int a = 0; a < r; ++a) { double v = li[a]; for (int c = 0; c < a; ++c) v -= S[a + r * c] * li[c]; li[a] = v / S[a + r * a]; }
     for (int a = r - 1; a >= 0; --a) { double v = li[a]; for (int c = a + 1; c < r; ++c) v -= S[c + r * a] * li[c]; li[a] = v / S[a + r * a]; }
+    if constexpr (CON) { if (cs.off[i + 1] > cs.off[i]) continue; }     // restricted: corrected and finished below
     for (int a = 0; a < r; ++a) {
       q1 += li[a] * sx[a];
       double v = 0.0;
@@ -250,6 +277,22 @@ __global__ void k_emb_mstep(const double* __restrict__ Xall, const double* __res
     li[r] = rinv;
   }
   DFM_SYNC();
+  if constexpr (CON) if (DFM_TID == 0) {
+    double* ws = sxf + (size_t)EMB_TILE * (r + 1);
+    for (int il = 0; il < EMB_TILE; ++il) {
+      const int i = tile * EMB_TILE + il;
+      if (i >= N) break;
+      const int q0 = cs.off[i], m = cs.off[i + 1] - q0;
+      if (m == 0 || is_nan(Lam[i]) || is_nan(R[i])) continue;
+      double* li = lamt + (size_t)il * (r + 1);
+      if (lam_constr_correct(li, r, cs.H + (size_t)q0 * r, cs.h + q0, m, ws, [&](double* v) {
+            for (int a = 0; a < r; ++a) { double u = v[a]; for (int c = 0; c < a; ++c) u -= S[a + r * c] * v[c]; v[a] = u / S[a + r * a]; }
+            for (int a = r - 1; a >= 0; --a) { double u = v[a]; for (int c = a + 1; c < r; ++c) u -= S[c + r * a] * v[c]; v[a] = u / S[a + r * a]; }
+          })) flag[1] = 1;
+      emb_series_finish(li, sxf + (size_t)il * (r + 1), S0, r, T, N, i, Lam, R, Wall + (size_t)b * N * r, logRall + (size_t)b * N, &flag[1]);
+    }
+  }
+  if constexpr (CON) DFM_SYNC();
   for (int e = DFM_TID; e < r * r; e += DFM_NT) {
     const int a = e % r, c = e / r;
     double v = 0.0;
@@ -257,6 +300,26 @@ __global__ void k_emb_mstep(const double* __restrict__ Xall, const double* __res
     Cpart[((size_t)b * ntiles + tile) * r * r + e] = v;
   }
   if (DFM_TID == 0) { counters[b * ntiles + tile] = 0; if (flag[1]) st[b].status = 3; }
+}
+
+template <int NCB>
+__global__ void k_emb_mstep(const double* __restrict__ Xall, const double* __restrict__ Fs_, const double* __restrict__ SffAll_,
+                            int T, int N, int r, int tsplit, int tper, int Bn, double* __restrict__ Spart,
+                            double* __restrict__ sxxpart, int* __restrict__ counters, double* __restrict__ LamAll,
+                            double* __restrict__ Rall, double* __restrict__ Wall, double* __restrict__ logRall,
+                            double* __restrict__ Cpart, EmState* st) {
+  emb_mstep_body<NCB, false>(Xall, Fs_, SffAll_, T, N, r, tsplit, tper, Bn, Spart, sxxpart, counters, LamAll, Rall, Wall, logRall,
+                             Cpart, st, EmConstr{nullptr, nullptr, nullptr});
+}
+
+template <int NCB>
+__global__ void k_emb_mstep_constr(const double* __restrict__ Xall, const double* __restrict__ Fs_, const double* __restrict__ SffAll_,
+                                   int T, int N, int r, int tsplit, int tper, int Bn, double* __restrict__ Spart,
+                                   double* __restrict__ sxxpart, int* __restrict__ counters, double* __restrict__ LamAll,
+                                   double* __restrict__ Rall, double* __restrict__ Wall, double* __restrict__ logRall,
+                                   double* __restrict__ Cpart, EmState* st, EmConstr cs) {
+  emb_mstep_body<NCB, true>(Xall, Fs_, SffAll_, T, N, r, tsplit, tper, Bn, Spart, sxxpart, counters, LamAll, Rall, Wall, logRall,
+                            Cpart, st, cs);
 }
 
 // Closing step of an iteration on the balanced multi-CTA path: commit the transition M-step, iteration count /

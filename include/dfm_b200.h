@@ -207,6 +207,31 @@ typedef struct {            /* outputs; any pointer may be NULL */
 int dfm_em_kalman(dfm_handle* h, const double* X, const dfm_em_opts* opts, const dfm_em_init* init,
                   const dfm_em_out* out);
 
+/* The same EM under linear restrictions on the loadings (the reference's LambdaConstraint, :1063-1186, e.g. the named-factor
+ * normalisation of Stock & Watson's Figure 7): row q says  H[q,:] lam_{index[q]} = h[q].  Host arrays, STANDARDIZED units
+ * (divide the reference's r by the series' xstd, as standardize_constraint! does); H is n_constr x r column-major.  The same
+ * restriction applies to every panel of the batch.  The measurement M-step of a restricted series i (rows H_i, values h_i) is
+ * the exact constrained maximiser
+ *     lu = S_i^-1 s_i,  Y = S_i^-1 H_i',  G = H_i Y,  lam_i = lu - Y G^-1 (H_i lu - h_i),  R_i as the unrestricted formula
+ * (S_i = sum_{t obs} E[f f'], s_i = sum_{t obs} x_it E[f]), so the log-likelihood stays monotone.  loglik[0] belongs to the
+ * initial parameters as given (they may violate the restriction); from iteration 1 on the parameters satisfy it.
+ *   constr == NULL or n_constr == 0: exactly dfm_em_kalman (same dispatch, same bits).
+ *   With rows, the call always runs the general multi-kernel path (never the fused kernels or the streaming host path);
+ *   opts->path 2 or 3 -> DFM_ERR_UNSUPPORTED.
+ *   DFM_ERR_ARG: an index outside [0, N), more than r rows on one series, a non-finite H or h entry, a NULL array with
+ *   n_constr > 0, n_constr < 0.
+ *   Dependent rows on a series (singular G, relative Cholesky pivot <= 1e-12) -> that panel's status is DFM_ERR_NOT_PD, as a
+ *   failed unrestricted solve.  Rows on a series out of the model (NaN Lam row or R) are ignored. */
+typedef struct {
+  int n_constr;             /* rows; 0 = none */
+  const int* index;         /* [n_constr] 0-based series of each row */
+  const double* H;          /* [n_constr x r] column-major */
+  const double* h;          /* [n_constr] */
+} dfm_lam_constr;
+
+int dfm_em_kalman_constrained(dfm_handle* h, const double* X, const dfm_em_opts* opts, const dfm_em_init* init,
+                              const dfm_lam_constr* constr, const dfm_em_out* out);
+
 /* ---- a'': smoothing, nowcasting and forecasting with a fitted state-space model --------- */
 /* The model of dfm_em_kalman at GIVEN parameters (no M-step): one Kalman filter + RTS smoother pass over the panel and H
  * periods after it.  A forecast period is one in which no series is observed, so the same pass gives the smoothed

@@ -38,6 +38,7 @@ struct EmOut
     Lam::Ptr{Cdouble}; R::Ptr{Cdouble}; A::Ptr{Cdouble}; Q::Ptr{Cdouble}; P0::Ptr{Cdouble}
     F::Ptr{Cdouble}; PF::Ptr{Cdouble}; loglik::Ptr{Cdouble}; iters::Ptr{Cint}; status::Ptr{Cint}
 end
+struct LamConstr; n_constr::Cint; index::Ptr{Cint}; H::Ptr{Cdouble}; h::Ptr{Cdouble}; end
 
 const handle = Ref{Ptr{Cvoid}}(C_NULL)
 function gethandle(device::Integer = 0)
@@ -157,8 +158,10 @@ function fitted_value_correlations(m, m_alt, lastpre::Integer; min_obs::Integer 
     return frommissing(cor)
 end
 
-"""`estimate!(m, ::NonParametric)` (dfm_functions.ipynb:530-543) and the `Parametric` slot of :23."""
-function estimate!(m, method = Main.NonParametric(); lam_constr_f = nothing, lam_constr_fl = nothing,
+"""`estimate!(m, ::NonParametric)` (dfm_functions.ipynb:530-543) and the `Parametric` slot of :23.
+`lam_constr_em` (Parametric only): a LambdaConstraint on the estimation series (as `lam_constr_f`) under which the state-space
+EM runs (dfm_em_kalman_constrained); its `r` is divided by the block's standard deviations, as standardize_constraint! does."""
+function estimate!(m, method = Main.NonParametric(); lam_constr_f = nothing, lam_constr_fl = nothing, lam_constr_em = nothing,
                    max_iter::Integer = 50, tol::Real = 1e-6)
     estimate_factor!(m, lam_constr = lam_constr_f)
     estimate_factor_loading!(m, lam_constr = lam_constr_fl)
@@ -182,13 +185,24 @@ function estimate!(m, method = Main.NonParametric(); lam_constr_f = nothing, lam
                 (Ptr{Cvoid}, Ptr{Cdouble}, Ptr{Cdouble}, Cint, Cint, Cint, Cint, Cint, Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cdouble}),
                 h, Xs, F0, T, N, r, p, 1, MEM_HOST, Lam, R, A, Q), "dfm_em_init_from_factors")
     F = Matrix{Float64}(undef, T, r); ll = fill(NaN, max_iter); it = Ref{Cint}(0); st = Ref{Cint}(0)
-    GC.@preserve Lam R A Q F ll begin
+    nc = lam_constr_em === nothing ? 0 : length(lam_constr_em.indices)
+    cidx = nc == 0 ? Cint[] : Cint.(lam_constr_em.indices .- 1)
+    cH = nc == 0 ? Float64[] : Matrix{Float64}(lam_constr_em.R)
+    ch = nc == 0 ? Float64[] : Vector{Float64}(lam_constr_em.r) ./ sd[lam_constr_em.indices]
+    GC.@preserve Lam R A Q F ll cidx cH ch begin
         opts = Ref(EmOpts(T, N, r, p, max_iter, tol, 1, MEM_HOST, 0))
         init = Ref(EmInit(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL))
         out = Ref(EmOut(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL, pointer(F), C_NULL, pointer(ll),
                         Base.unsafe_convert(Ptr{Cint}, it), Base.unsafe_convert(Ptr{Cint}, st)))
-        check(ccall((:dfm_em_kalman, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ref{EmOpts}, Ref{EmInit}, Ref{EmOut}), h, Xs, opts, init, out),
-              "dfm_em_kalman")
+        if nc == 0
+            check(ccall((:dfm_em_kalman, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ref{EmOpts}, Ref{EmInit}, Ref{EmOut}), h, Xs, opts, init, out),
+                  "dfm_em_kalman")
+        else
+            con = Ref(LamConstr(nc, pointer(cidx), pointer(cH), pointer(ch)))
+            check(ccall((:dfm_em_kalman_constrained, LIB), Cint,
+                        (Ptr{Cvoid}, Ptr{Cdouble}, Ref{EmOpts}, Ref{EmInit}, Ref{LamConstr}, Ref{EmOut}), h, Xs, opts, init, con, out),
+                  "dfm_em_kalman_constrained")
+        end
     end
     m.factor[m.initperiod:m.lastperiod, :] = F
     return (loglik = ll[1:it[]], iters = it[], Lam = Lam, R = R, A = A, Q = Q)
