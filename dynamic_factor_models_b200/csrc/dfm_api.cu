@@ -110,10 +110,11 @@ struct dfm_handle {
 namespace {
 
 const size_t kMaxSmem = 220 * 1024;
-const int kMaxReadyChunks = 4096;
 // Entry points whose launches put the batch on gridDim.y (at most 65535 blocks) refuse larger batches with
 // DFM_ERR_UNSUPPORTED; callers split such batches.
 const int kMaxGridBatch = 65535;
+const int kReadyChunk = 32;                                    // panels per upload chunk of the streaming host path
+const int kMaxReadyChunks = (kMaxGridBatch + kReadyChunk - 1) / kReadyChunk;   // "landed" flags of the largest batch
 
 struct Arena {
   char* base; size_t off;
@@ -204,7 +205,7 @@ int tpt_threads(int ws_doubles) {
 
 }  // namespace
 
-// any NaN in the panel / parameters?  (the fused path handles balanced panels only)
+// any NaN in the panel / parameters?  (the fused path handles balanced panels only)  Lam == nullptr: the panel only.
 namespace dfm {
 __global__ void k_em_scan_fused(const double* __restrict__ X, const double* __restrict__ Lam, const double* __restrict__ R,
                                 int T, int N, int r, int* flag) {
@@ -212,7 +213,7 @@ __global__ void k_em_scan_fused(const double* __restrict__ X, const double* __re
   const double* x = X + ((size_t)b * N + i) * T;
   int bad = 0;
   for (int t = DFM_TID; t < T; t += DFM_NT) if (is_nan(x[t])) bad = 1;
-  if (DFM_TID == 0) { for (int a = 0; a < r; ++a) if (is_nan(Lam[(size_t)b * N * r + i + (size_t)N * a])) bad = 1; if (is_nan(R[(size_t)b * N + i])) bad = 1; }
+  if (Lam && DFM_TID == 0) { for (int a = 0; a < r; ++a) if (is_nan(Lam[(size_t)b * N * r + i + (size_t)N * a])) bad = 1; if (is_nan(R[(size_t)b * N + i])) bad = 1; }
   if (bad) *flag = 1;
 }
 }  // namespace dfm
@@ -576,8 +577,7 @@ static int em_streaming(dfm_handle* h, const double* X, const dfm_em_opts* o, co
   const int T = o->T, N = o->N, r = o->r, batch = o->batch, mi = o->max_iter;
   const size_t B = batch, TN = (size_t)T * N; const int k = r * o->p, kk = k * k, rr = r * r, rk = r * k;
   *fallback = false;
-  int chunk = 32;                                              // ~25 MB of C2-shaped panels: the first CTAs start early
-  while ((batch + chunk - 1) / chunk > kMaxReadyChunks) chunk *= 2;
+  const int chunk = kReadyChunk;                               // ~25 MB of C2-shaped panels: the first CTAs start early
   const int nch = (batch + chunk - 1) / chunk;
   cudaStream_t cs = h->copy_stream;
   cudaEvent_t ev0 = nullptr, ev_k = nullptr;
@@ -667,12 +667,22 @@ static int em_streaming(dfm_handle* h, const double* X, const dfm_em_opts* o, co
   bool failed = false;
   for (size_t bb = 0; bb < B; ++bb) failed = failed || hstat[bb] == 3;
   if (failed) {                                                // NaN log-likelihood somewhere: missing data or a numerical failure?
-    CK(cudaMemsetAsync(d.flag, 0, sizeof(int), h->stream));
-    L(k_em_scan_fused, N, batch, 64, 0, d.X, d.L, d.R, T, N, r, d.flag);      // (X only matters: Lam/R of failed panels are NaN anyway)
-    int hflag = 0;
-    CK(cudaMemcpyAsync(&hflag, d.flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    *fallback = hflag != 0;
+    // The question is whether the CALLER passed a NaN (a missing cell; a series out of the model), as in the scan the
+    // other host path runs before the kernel.  d.L / d.R hold what the kernel wrote by now, and a panel that failed
+    // numerically on clean data leaves NaNs there: scanning them would send the whole batch through the general path
+    // for one bad panel.  So: the caller's Lam and R on the host, X on the device.
+    bool nan_in = false;
+    for (size_t e = 0; e < B * N * r && !nan_in; ++e) nan_in = std::isnan(init->Lam[e]);
+    for (size_t e = 0; e < B * N && !nan_in; ++e) nan_in = std::isnan(init->R[e]);
+    if (!nan_in) {
+      CK(cudaMemsetAsync(d.flag, 0, sizeof(int), h->stream));
+      L(k_em_scan_fused, N, batch, 64, 0, d.X, (const double*)nullptr, (const double*)nullptr, T, N, r, d.flag);
+      int hflag = 0;
+      CK(cudaMemcpyAsync(&hflag, d.flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+      CK(cudaStreamSynchronize(h->stream));
+      nan_in = hflag != 0;
+    }
+    *fallback = nan_in;
   }
   if (!*fallback) CK(cudaGetLastError());
   return DFM_OK;
