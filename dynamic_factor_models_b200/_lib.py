@@ -108,6 +108,30 @@ class SsbOut(C.Structure):
 SSB_OUTPUTS = ("Lam", "R", "A", "Q", "irf", "xhat", "xvar")
 
 
+class GibbsPrior(C.Structure):
+    _fields_ = [("kap_lam", C.c_double), ("a_R", C.c_double), ("b_R", C.c_double), ("kap_A", C.c_double), ("nu_Q", C.c_double),
+                ("s_Q", C.c_double)]
+
+
+class GibbsOpts(C.Structure):
+    _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H_irf", C.c_int), ("H_fc", C.c_int),
+                ("fc_rows", C.c_int), ("n_chain", C.c_int), ("chain0", C.c_longlong), ("sweep0", C.c_longlong), ("n_burn", C.c_int),
+                ("n_keep", C.c_int), ("thin", C.c_int), ("seed", C.c_ulonglong), ("mem", C.c_int), ("prior", GibbsPrior)]
+
+
+class GibbsOut(C.Structure):
+    _fields_ = [("Lam", C.c_void_p), ("R", C.c_void_p), ("A", C.c_void_p), ("Q", C.c_void_p), ("irf", C.c_void_p), ("F", C.c_void_p),
+                ("X", C.c_void_p), ("loglik", C.c_void_p), ("status", C.c_void_p)]
+
+
+GIBBS_OUTPUTS = ("Lam", "R", "A", "Q", "irf", "F", "X")
+
+
+def gibbs_default_prior(r):
+    """The API's weak conjugate prior (standardized units): kap_lam = kap_A = 0.01, a_R = 3, b_R = 1, nu_Q = r + 2, s_Q = 1."""
+    return dict(kap_lam=0.01, a_R=3.0, b_R=1.0, kap_A=0.01, nu_Q=r + 2.0, s_Q=1.0)
+
+
 def default_library_path():
     return os.path.join(HERE, "lib", "libdfm_b200.so")
 
@@ -116,7 +140,7 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
-           "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_em_init_from_factors",
+           "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -204,6 +228,7 @@ class Library:
         L.dfm_ss_simulate_panels.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(EmInit), C.c_ulonglong,
                                              C.c_longlong, C.c_int, C.c_int, C.c_void_p]
         L.dfm_ss_bootstrap.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsbOpts), C.POINTER(EmInit), C.POINTER(SsbOut)]
+        L.dfm_gibbs.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GibbsOpts), C.POINTER(EmInit), C.POINTER(EmInit), C.POINTER(GibbsOut)]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p]
         L.dfm_bootstrap_panels.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 8
@@ -315,6 +340,63 @@ class Library:
         ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in params.items()})
         ou = SsbOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
         self.check(self.lib.dfm_ss_bootstrap(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_ss_bootstrap")
+
+    def gibbs_raw(self, X, T, N, r, p, init, ref, out, mem, n_chain, chain0=0, sweep0=0, n_burn=0, n_keep=1, thin=1, seed=0, H_irf=0,
+                  H_fc=0, fc_rows=0, prior=None):
+        """Pointer-level dfm_gibbs (ints = device or host addresses).  init: dict Lam, R, A, Q, P0 (n_chain models back to back);
+        ref: dict Lam, R, A, Q or None; out: dict of Lam, R, A, Q, irf, F, X, loglik, status (missing or 0 = NULL); prior: dict
+        (gibbs_default_prior(r) when None)."""
+        pr = dict(gibbs_default_prior(r)); pr.update(prior or {})
+        o = GibbsOpts(T=T, N=N, r=r, p=p, H_irf=H_irf, H_fc=H_fc, fc_rows=fc_rows, n_chain=n_chain, chain0=chain0, sweep0=sweep0,
+                      n_burn=n_burn, n_keep=n_keep, thin=thin, seed=seed, mem=mem, prior=GibbsPrior(**pr))
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in init.items()})
+        rf = EmInit(**{k: C.c_void_p(v) if v else None for k, v in ref.items()}) if ref is not None else None
+        ou = GibbsOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
+        self.check(self.lib.dfm_gibbs(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(rf) if rf is not None else None, C.byref(ou)),
+                   "dfm_gibbs")
+
+    def gibbs(self, X, init, p=1, n_chain=None, chain0=0, sweep0=0, n_burn=0, n_keep=1, thin=1, seed=0, H_irf=0, H_fc=0, fc_rows=0,
+              prior=None, ref=None, outputs=GIBBS_OUTPUTS):
+        """Gibbs chains of the state-space model on the standardized panel X (T, N) (dfm_gibbs).  init: dict Lam (n_chain, N, r),
+        R (n_chain, N), A (n_chain, r, k), Q (n_chain, r, r), P0 (n_chain, k, k) -- or one model (2-D arrays), copied to every
+        chain; ref: dict Lam, R, A, Q (the model the impulse responses are aligned onto).  Returns Lam (n_chain, n_keep, N, r),
+        R (n_chain, n_keep, N), A, Q, irf (n_chain, n_keep, r, H_irf, r) [variable, horizon, shock], F (n_chain, n_keep, T + H_fc,
+        r), X (n_chain, n_keep, fc_rows, N) -- those named in `outputs` -- loglik (n_chain, n_sweep) and status (n_chain)."""
+        X = np.asarray(X, float); T, N = X.shape
+        Lam = np.asarray(init["Lam"], float); r = Lam.shape[-1]; k = r * p
+        if n_chain is None:
+            n_chain = Lam.shape[0] if Lam.ndim == 3 else 1
+        ini = {}
+        for n_, shp in (("Lam", (N, r)), ("R", (N,)), ("A", (r, k)), ("Q", (r, r)), ("P0", (k, k))):
+            a_ = np.asarray(init[n_], float)
+            if a_.ndim == len(shp):
+                a_ = np.broadcast_to(a_, (n_chain,) + shp)
+            ini[n_] = to_cm(a_) if len(shp) == 2 else np.ascontiguousarray(a_, dtype=float).ravel()
+        rf = None
+        if ref is not None:
+            rf = {n_: (to_cm(ref[n_]) if n_ != "R" else np.ascontiguousarray(ref[n_], dtype=float)) for n_ in ("Lam", "R", "A", "Q")}
+        n_sweep = n_burn + n_keep * thin; Tp = T + H_fc
+        size = dict(Lam=N * r, R=N, A=r * k, Q=r * r, irf=r * H_irf * r, F=Tp * r, X=fc_rows * N)
+        outs = {n_: np.full(max(n_chain * n_keep * size[n_], 0), np.nan) for n_ in outputs}
+        ll = np.full(max(n_chain * n_sweep, 0), np.nan); st = np.zeros(max(n_chain, 0), np.int32)
+        xin = to_cm(X)
+        self.gibbs_raw(xin.ctypes.data, T, N, r, p, {n_: a_.ctypes.data for n_, a_ in ini.items()},
+                       {n_: a_.ctypes.data for n_, a_ in rf.items()} if rf is not None else None,
+                       {**{n_: a_.ctypes.data for n_, a_ in outs.items()}, "loglik": ll.ctypes.data, "status": st.ctypes.data}, MEM_HOST,
+                       n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin, seed=seed, H_irf=H_irf, H_fc=H_fc,
+                       fc_rows=fc_rows, prior=prior)
+        res = dict(loglik=ll.reshape(n_chain, n_sweep), status=st)
+        shape = dict(Lam=(N, r), A=(r, k), Q=(r, r), F=(Tp, r), X=(fc_rows, N))
+        nb = n_chain * n_keep
+        for n_, a_ in outs.items():
+            if n_ == "R":
+                v = a_.reshape(nb, N)
+            elif n_ == "irf":
+                v = a_.reshape(nb, r, H_irf, r).transpose(0, 3, 2, 1)
+            else:
+                v = from_cm(a_, shape[n_][0], shape[n_][1], nb)
+            res[n_] = np.ascontiguousarray(v).reshape((n_chain, n_keep) + v.shape[1:])
+        return res
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)

@@ -9,7 +9,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from ._lib import Library
+from ._lib import Library, gibbs_default_prior as _gibbs_default_prior
 
 _default = None
 
@@ -430,6 +430,73 @@ def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922
         xv = xstd ** 2 * o["xvar"]
         out.update(xhat=xh, xvar=xv, xhat_bands=lib.percentiles(xh.reshape(n_rep, -1), qq).reshape((len(qq),) + xh.shape[1:]),
                    total_var=xv[ok].mean(0) + xh[ok].var(0) if ok.any() else np.full(xh.shape[1:], np.nan))
+    return out
+
+
+def split_rhat(draws):
+    """Split-R^ (Gelman et al. 2013, Bayesian Data Analysis 3rd ed., section 11.4) of draws (n_chain, n, ...): every chain cut in
+    two halves, R^ = sqrt(((n'-1)/n' W + B/n') / W) over the 2 n_chain half-chains of length n'.  NaN when n < 4 or a chain
+    failed (NaN draws)."""
+    d = np.asarray(draws, float)
+    h = d.shape[1] // 2
+    if h < 2:
+        return np.full(d.shape[2:], np.nan)
+    s = np.concatenate([d[:, :h], d[:, h:2 * h]], axis=0)
+    W = s.var(axis=1, ddof=1).mean(axis=0)
+    B = h * s.mean(axis=1).var(axis=0, ddof=1)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.sqrt(((h - 1) / h * W + B / h) / W)
+
+
+def gibbs(m, n_chain=4, n_burn=500, n_keep=1000, thin=1, H_irf=24, H_fc=0, fc_rows=None, prior=None, seed=20260922,
+          q=(5, 16, 50, 84, 95), chain0=0, sweep0=0, lib=None):
+    """Bayesian estimation of a model estimated with `estimate(m, Parametric())` by Gibbs sampling (dfm_gibbs): n_chain chains,
+    all started at m.em, alternate a joint draw of the factor path (the simulation smoother) with conjugate draws of the
+    parameters.  Prior (standardized units; `prior` overrides entries of the default, which is weak next to T of a few hundred):
+      lam_i | R_i ~ N(0, R_i / kap_lam I),  R_i ~ IG(a_R, b_R),  A' | Q ~ MN(0, I / kap_A, Q),  Q ~ IW(nu_Q, s_Q I);
+      defaults kap_lam = kap_A = 0.01, a_R = 3, b_R = 1, nu_Q = r + 2, s_Q = 1.  P0 stays at m.em's; A is not restricted to be
+      stationary.
+    Same block as `forecast(m, H_fc)`; fc_rows: trailing rows of the T + H_fc rows whose predictive draws are returned (default
+    H_fc).  Returns a dict:
+      Lam (n_chain, n_keep, ns, r), R (.., ns), A (.., r, k), Q (.., r, r)   raw parameter draws (standardized units);
+      irf (n_chain, n_keep, r, H_irf, r)   impulse responses [variable, horizon, shock] of each draw rotated onto m.em
+                                           (parametric_bootstrap's alignment);  irf_bands (len(q), r, H_irf, r);
+      x (n_chain, n_keep, fc_rows, ns)     predictive draws in data units (the data where observed);  x_bands (len(q), fc_rows, ns);
+      loglik (n_chain, n_burn + n_keep thin)  log-likelihood of the parameters entering each sweep;  status (n_chain);
+      rhat dict(loglik, R (ns), x (fc_rows, ns))  split-R^ over the kept draws (the loglik of kept sweeps);
+    and periods (the fc_rows rows, 1-based), series, q.  Bands through dfm_percentiles (n_chain n_keep <= 16384)."""
+    if m.em is not None and m.em.get("lam_constr") is not None:
+        raise ValueError("gibbs: the EM of m ran under restrictions on the loadings (lam_constr_em); the sampler draws unrestricted "
+                         "loadings")
+    if not 1 <= n_chain * n_keep <= 16384:
+        raise ValueError("gibbs: n_chain * n_keep must be in [1, 16384]")
+    b = _state_space_block(m, H_fc, lib, "gibbs")
+    lib, e = b["lib"], b["em"]
+    T = b["Xs"].shape[0]
+    fc_rows = H_fc if fc_rows is None else int(fc_rows)
+    if not 0 <= fc_rows <= T + H_fc:
+        raise ValueError(f"gibbs: fc_rows must be in [0, {T + H_fc}]")
+    r = e["Q"].shape[0]
+    pr = dict(_gibbs_default_prior(r)); pr.update(prior or {})
+    init = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"], P0=e["P0"])
+    ref = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"])
+    outs = ("Lam", "R", "A", "Q") + (("irf",) if H_irf > 0 else ()) + (("X",) if fc_rows > 0 else ())
+    o = lib.gibbs(b["Xs"], init, p=b["p"], n_chain=n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin,
+                  seed=seed, H_irf=H_irf, H_fc=H_fc, fc_rows=fc_rows, prior=pr, ref=ref if H_irf > 0 else None, outputs=outs)
+    qq = np.asarray(q, float)
+    n = n_chain * n_keep
+    kept = n_burn + thin * np.arange(1, n_keep + 1) - 1
+    out = dict(Lam=o["Lam"], R=o["R"], A=o["A"], Q=o["Q"], loglik=o["loglik"], status=o["status"], prior=pr,
+               periods=b["periods"][len(b["periods"]) - fc_rows:], series=b["series"], q=qq,
+               rhat=dict(loglik=float(split_rhat(o["loglik"][:, kept])), R=split_rhat(o["R"])))
+    if H_irf > 0:
+        out["irf"] = o["irf"]
+        out["irf_bands"] = lib.percentiles(o["irf"].reshape(n, -1), qq).reshape((len(qq),) + o["irf"].shape[2:])
+    if fc_rows > 0:
+        x = b["xmean"] + b["xstd"] * o["X"]
+        out["x"] = x
+        out["x_bands"] = lib.percentiles(x.reshape(n, -1), qq).reshape((len(qq),) + x.shape[2:])
+        out["rhat"]["x"] = split_rhat(x)
     return out
 
 

@@ -15,6 +15,7 @@
 #include "dfm_kernels_sim.cuh"
 #include "dfm_kernels_news.cuh"
 #include "dfm_kernels_ssb.cuh"
+#include "dfm_kernels_gibbs.cuh"
 #include <algorithm>
 #include <cmath>
 #include <new>
@@ -1498,7 +1499,7 @@ int dfm_simulation_smoother(dfm_handle* h, const double* X, const dfm_sim_opts* 
         zfS, fS, Fo);
       if (Xo)
         L(k_sim_project, ntt, nst * ((nd + SIM_PD - 1) / SIM_PD), 256, smP, s.x, s.pL, s.pR, (const double*)fS, Tp, N, r, o->seed, id0, nd,
-          (const int*)sstat, Xo);
+          (const int*)sstat, Xo, 0, 1LL);
       if (!dev_out) {
         if (out->F) { rc = copy_out(h, out->F + (size_t)j0 * Tp * r, dF, (size_t)nd * Tp * r, mem); if (rc) return rc; }
         if (out->X) { rc = copy_out(h, out->X + (size_t)j0 * Tp * N, dX, (size_t)nd * Tp * N, mem); if (rc) return rc; }
@@ -1898,6 +1899,191 @@ int dfm_ss_bootstrap(dfm_handle* h, const double* X, const dfm_ssb_opts* o, cons
 #undef SSB_FAIL
   CK(e);
   return DFM_OK;
+}
+
+// ------------------------------------------------------------------------------------ Gibbs sampler
+// Per sub-batch of ssb_batch() chains (the bootstrap's rule: a size fixed by the model's shape and the device, so that chain c
+// has the same bits whatever n_chain or chain0), the sweeps run device-resident with no host synchronisation between them
+// (records going to pageable host memory are staged per kept sweep):
+//   ss_estep (one padded panel copy per chain, k_ss_bcast once per call) -> k_sim_gains (grid.y = chain) -> k_gibbs_paths ->
+//   [kept: k_sim_project + k_ss_fc_rows] -> k_gibbs_stats -> k_gibbs_draw -> [kept: records, k_ss_align + k_irf].
+int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm_em_init* init, const dfm_em_init* ref,
+              const dfm_gibbs_out* out) {
+  if (!h || !X || !o || !init || !out || !init->Lam || !init->R || !init->A || !init->Q || !init->P0)
+    return fail(h, DFM_ERR_ARG, "dfm_gibbs: null argument (P0 is required)");
+  const int T = o->T, N = o->N, r = o->r, p = o->p, Hi = o->H_irf, Hf = o->H_fc, fr = o->fc_rows, mem = o->mem;
+  const long long nch = o->n_chain;
+  const dfm_gibbs_prior& pr = o->prior;
+  if (T <= 1 || N <= 0 || r <= 0 || p <= 0 || Hi < 0 || Hf < 0 || fr < 0 || (long long)fr > (long long)T + Hf || nch < 1 ||
+      o->chain0 < 0 || o->chain0 + nch > (1LL << 16) || o->sweep0 < 0 || o->n_burn < 0 || o->n_keep < 1 || o->thin < 1 ||
+      (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_gibbs: bad shape/options");
+  const long long n_sweep = (long long)o->n_burn + (long long)o->n_keep * o->thin;
+  if (o->sweep0 + n_sweep > (1LL << 24)) return fail(h, DFM_ERR_ARG, "dfm_gibbs: sweep indices must stay below 2^24");
+  if (!(pr.kap_lam > 0) || !(pr.a_R >= 1) || !(pr.b_R > 0) || !(pr.kap_A > 0) || !(pr.s_Q > 0) || !(pr.nu_Q + T - r >= 2) ||
+      !std::isfinite(pr.kap_lam + pr.a_R + pr.b_R + pr.kap_A + pr.nu_Q + pr.s_Q))
+    return fail(h, DFM_ERR_ARG, "dfm_gibbs: bad prior (kappas, b_R, s_Q > 0, a_R >= 1, nu_Q + T - r >= 2)");
+  if (Hi > 0 && out->irf && (!ref || !ref->Lam || !ref->R || !ref->A || !ref->Q))
+    return fail(h, DFM_ERR_ARG, "dfm_gibbs: ref is required for impulse responses");
+  const int k = r * p, Tp = T + Hf;
+  if (k > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: state dimension r*p > 48");
+  const int C = ssb_batch(h, T, N, r, p);
+  int rc = ss_check(h, "dfm_gibbs", Tp, N, r, p, 0, C, DFM_MEM_DEVICE);
+  if (rc) return rc;
+  const size_t smG = sim_gains_smem_doubles(r, p) * 8, smPa = gibbs_paths_smem_doubles(r, p) * 8, smSt = gibbs_stats_smem_doubles() * 8,
+               smD = gibbs_draw_smem_doubles(r, p) * 8, smP = sim_project_smem_doubles(r) * 8, smA = ssb_align_smem_doubles(r, p) * 8;
+  if (smD > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: state too large for the parameter-draw kernel");
+  const int nst = (N + SS_NS - 1) / SS_NS;
+  if ((long long)nst * ((C + SIM_PD - 1) / SIM_PD) > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: N too large");
+  CK(cudaSetDevice(h->device));
+  const size_t B = C, Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nirf = (size_t)r * Hi * r;
+  const bool wantX = out->X && fr > 0, wantI = out->irf && Hi > 0;
+  const bool hst = mem == DFM_MEM_HOST;
+  const cudaMemcpyKind kin = hst ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, kout = hst ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  const long long nk = o->n_keep;
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    SsStage s = ss_bufs(a, DFM_MEM_DEVICE, 0, B, Tp, N, r, p);
+    double* Xpad = a.get<double>(B * Tp * N);
+    double *dL = a.get<double>(B * Nr), *dR = a.get<double>(B * N), *dA = a.get<double>(B * rk), *dQ = a.get<double>(B * rr),
+           *dP = a.get<double>(B * kk);
+    double* gains = a.get<double>(B * sim_gains_doubles(Tp, k, r));
+    int* cst = a.get<int>(B);
+    double *zfS = a.get<double>(B * Tp * k), *fS = a.get<double>(B * Tp * r), *z0 = a.get<double>(B * k), *sv = a.get<double>(B * Nr);
+    double* wk = a.get<double>(B * gibbs_draw_wk_doubles(N, r));
+    int *nobs = a.get<int>(N), *mcnt = a.get<int>(N), *midx = a.get<int>((size_t)N * T);
+    double* qv = a.get<double>(N);
+    double* Fk = out->F ? a.get<double>(B * Tp * r) : nullptr;
+    double* Xproj = wantX ? a.get<double>(B * Tp * N) : nullptr;
+    double* Xrow = wantX ? a.get<double>(B * fr * N) : nullptr;
+    double *sL = a.get<double>(B * Nr), *sR = a.get<double>(B * N), *sA = a.get<double>(B * rk), *sQ = a.get<double>(B * rr),
+           *sll = a.get<double>(B);
+    int* sst = a.get<int>(B);
+    double *rL = wantI ? a.get<double>(Nr) : nullptr, *rR = wantI ? a.get<double>(N) : nullptr, *rA = wantI ? a.get<double>(rk) : nullptr,
+           *rQ = wantI ? a.get<double>(rr) : nullptr;
+    double *aL = wantI ? a.get<double>(B * Nr) : nullptr, *aR = wantI ? a.get<double>(B * N) : nullptr,
+           *aA = wantI ? a.get<double>(B * rk) : nullptr, *aQ = wantI ? a.get<double>(B * rr) : nullptr,
+           *aM = wantI ? a.get<double>(B * kk) : nullptr, *aS = wantI ? a.get<double>(B * rk) : nullptr,
+           *aG = wantI ? a.get<double>(B * rk) : nullptr, *allf = wantI ? a.get<double>(B) : nullptr,
+           *adum = wantI ? a.get<double>(B + 4) : nullptr, *dI = wantI ? a.get<double>(B * nirf) : nullptr;
+    int* ast = wantI ? a.get<int>(B) : nullptr;
+    int* ids = wantI ? a.get<int>(r) : nullptr;
+    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    // ---- once per call: the padded panel, its copies, the per-series counts; the reference model and shock ids
+    if (hst) {
+      CK(cudaMemcpy2DAsync(Xpad, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, N, cudaMemcpyHostToDevice, h->stream));
+      if (Hf > 0) L(k_ss_pad, (int)std::min<long long>(((long long)N * Hf + 255) / 256, 4096), 1, 256, 0, (const double*)nullptr, T, Tp, (long long)N, Xpad);
+    } else {
+      L(k_ss_pad, (int)std::min<long long>(((long long)N * Tp + 255) / 256, 4096), 1, 256, 0, X, T, Tp, (long long)N, Xpad);
+    }
+    auto bcast = [&](const double* src, size_t n, double* dst, int nb) {
+      if (nb > 0) L(k_ss_bcast, (int)std::min<size_t>((n + 255) / 256, 1024), nb, 256, 0, src, (long long)n, dst);
+    };
+    bcast(Xpad, (size_t)Tp * N, Xpad + (size_t)Tp * N, C - 1);
+    L(k_gibbs_scan, (N + 127) / 128, 1, 128, 0, (const double*)Xpad, T, Tp, N, nobs, qv, mcnt, midx);
+    if (wantI) {
+      CK(cudaMemcpyAsync(rL, ref->Lam, Nr * 8, kin, h->stream)); CK(cudaMemcpyAsync(rR, ref->R, (size_t)N * 8, kin, h->stream));
+      CK(cudaMemcpyAsync(rA, ref->A, rk * 8, kin, h->stream)); CK(cudaMemcpyAsync(rQ, ref->Q, rr * 8, kin, h->stream));
+      std::vector<int> hid(r);
+      for (int j = 0; j < r; ++j) hid[j] = j;
+      CK(cudaMemcpyAsync(ids, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaStreamSynchronize(h->stream));                  // (hid is a local)
+      DFM_SET_SMEM(k_ss_align, smA);
+    }
+    DFM_SET_SMEM(k_sim_gains, smG);
+    DFM_SET_SMEM(k_gibbs_paths, smPa);
+    DFM_SET_SMEM(k_gibbs_stats, smSt);
+    DFM_SET_SMEM(k_gibbs_draw, smD);
+    DFM_SET_SMEM(k_sim_project, smP);
+    const int* src = s.g.nt + (size_t)C * Tp;
+    const long long idstride = 1LL << 24;
+    GibbsDrawArgs da{};
+    da.X = Xpad; da.fS = fS; da.z0 = z0; da.sv = sv; da.q = qv; da.nobs = nobs; da.mcnt = mcnt; da.midx = midx;
+    da.Lam = dL; da.R = dR; da.A = dA; da.Q = dQ; da.wk = wk; da.cst = cst;
+    da.pr = GbPrior{pr.kap_lam, pr.a_R, pr.b_R, pr.kap_A, pr.nu_Q, pr.s_Q};
+    da.T = T; da.Tp = Tp; da.N = N; da.r = r; da.p = p; da.C = C; da.seed = o->seed; da.idstride = idstride;
+    for (long long j0 = 0; j0 < nch; j0 += C) {
+      const int nkeep = (int)std::min<long long>(C, nch - j0);       // chains returned (a full sub-batch is computed)
+      // ---- initial parameters: the sub-batch's chains, then copies of the last chain's for the fill-up
+      const double* isrc[5] = {init->Lam, init->R, init->A, init->Q, init->P0};
+      double* idst[5] = {dL, dR, dA, dQ, dP};
+      const size_t isz[5] = {Nr, (size_t)N, rk, rr, kk};
+      for (int q = 0; q < 5; ++q) {
+        CK(cudaMemcpyAsync(idst[q], isrc[q] + (size_t)j0 * isz[q], (size_t)nkeep * isz[q] * 8, kin, h->stream));
+        bcast(idst[q] + (size_t)(nkeep - 1) * isz[q], isz[q], idst[q] + (size_t)nkeep * isz[q], C - nkeep);
+      }
+      CK(cudaMemsetAsync(cst, 0, B * sizeof(int), h->stream));
+      // ---- records: rows [j0, j0 + nkeep) of an output with `per` elements per chain, at element offset `off` of each row
+      cudaError_t ce = cudaSuccess;
+      auto put = [&](void* dst, const void* srcd, size_t n, size_t esz, size_t per, size_t off) {
+        if (dst && ce == cudaSuccess)
+          ce = cudaMemcpy2DAsync((char*)dst + ((size_t)j0 * per + off) * esz, per * esz, srcd, n * esz, n * esz, nkeep, kout, h->stream);
+      };
+      const long long cid0 = o->chain0 + j0;
+      for (long long sw = 0; sw < n_sweep; ++sw) {
+        const bool kept = sw >= o->n_burn && (sw - o->n_burn + 1) % o->thin == 0;
+        const long long jk = kept ? (sw - o->n_burn + 1) / o->thin - 1 : -1;
+        const long long id0 = (cid0 << 24) + o->sweep0 + sw;
+        dfm_em_init ep{dL, dR, dA, dQ, dP};
+        rc = ss_estep(h, s, Xpad, &ep, Tp, N, r, p, 0, C, DFM_MEM_DEVICE);
+        if (rc) return rc;
+        L(k_sim_gains, Tp + 1, C, 256, smG, s.pA, s.pQ, (const double*)s.P0, (const double*)s.g.C, (const double*)s.g.Ct,
+          (const double*)s.g.Bt, (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const int*)s.g.nt, (const EmState*)s.st, Tp, r, p,
+          gains, cst);
+        L(k_gibbs_paths, (C + GB_PW - 1) / GB_PW, 1, 32 * GB_PW, smPa, (const double*)gains, Tp, r, p, C, o->seed, id0, idstride,
+          (const int*)cst, zfS, fS, z0, kept ? Fk : (double*)nullptr);
+        if (out->loglik) {
+          L(k_gibbs_rec, 1, C, 32, 0, (const double*)s.ll, 1LL, 1LL, (const int*)cst, sll, 1LL);
+          put(out->loglik, sll, 1, 8, (size_t)n_sweep, (size_t)sw);
+        }
+        if (kept && wantX) {
+          L(k_sim_project, (Tp + SS_TP - 1) / SS_TP, nst * ((C + SIM_PD - 1) / SIM_PD), 256, smP, (const double*)Xpad, (const double*)dL,
+            (const double*)dR, (const double*)fS, Tp, N, r, o->seed, id0, C, (const int*)cst, Xproj, 1, idstride);
+          const long long n = (long long)C * N * fr;
+          L(k_ss_fc_rows, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)Xproj, (const double*)nullptr, Tp, N,
+            fr, C, (const int*)cst, Xrow, (double*)nullptr);
+        }
+        L(k_gibbs_stats, (N + GB_NS - 1) / GB_NS, (C * r + GB_NC - 1) / GB_NC, 128, smSt, (const double*)Xpad, (const double*)fS, T, Tp, N,
+          r, C, sv);
+        da.id0 = id0;
+        L(k_gibbs_draw, C, 1, GB_NT, smD, da);
+        if (kept) {
+          const double* psrc[4] = {dL, dR, dA, dQ};
+          double* pst[4] = {sL, sR, sA, sQ};
+          double* pdst[4] = {out->Lam, out->R, out->A, out->Q};
+          for (int q = 0; q < 4; ++q) {
+            if (!pdst[q]) continue;
+            L(k_gibbs_rec, (int)std::min<size_t>((isz[q] + 255) / 256, 64), C, 256, 0, psrc[q], (long long)isz[q], (long long)isz[q],
+              (const int*)cst, pst[q], (long long)isz[q]);
+            put(pdst[q], pst[q], isz[q], 8, (size_t)nk * isz[q], (size_t)jk * isz[q]);
+          }
+          if (out->F) put(out->F, Fk, (size_t)Tp * r, 8, (size_t)nk * Tp * r, (size_t)jk * Tp * r);
+          if (wantX) put(out->X, Xrow, (size_t)fr * N, 8, (size_t)nk * fr * N, (size_t)jk * fr * N);
+          if (wantI) {
+            SsbAlignArgs aa{};
+            aa.Lh = rL; aa.Rh = rR; aa.Ah = rA; aa.Qh = rQ;
+            aa.Ls = dL; aa.Rs = dR; aa.As = dA; aa.Qs = dQ;
+            aa.ll = adum; aa.it = cst; aa.em_status = cst;        // (it = status in {0, 3}: llf reads adum[b + 2] at most)
+            aa.Lo = aL; aa.Ro = aR; aa.Ao = aA; aa.Qo = aQ;
+            aa.M = aM; aa.Qsel = aS; aa.G = aG; aa.llf = allf; aa.status = ast;
+            aa.N = N; aa.r = r; aa.p = p; aa.max_iter = 1;
+            L(k_ss_align, C, 1, SSB_NT, smA, aa);
+            L(k_irf, r, C, 64, (size_t)(2 * k + 8) * 8, (const double*)aM, (const double*)aS, (const double*)aG, k, r, Hi, r, (const int*)ids, dI);
+            put(out->irf, dI, nirf, 8, (size_t)nk * nirf, (size_t)jk * nirf);
+          }
+        }
+        if (ce != cudaSuccess) { cudaStreamSynchronize(h->stream); return fail(h, DFM_ERR_CUDA, "dfm_gibbs: copy failed"); }
+      }
+      if (out->status) {
+        L(k_gibbs_status, 1, 1, 256, 0, (const int*)cst, C, sst);
+        put(out->status, sst, 1, 4, 1, 0);
+      }
+      if (ce != cudaSuccess) { cudaStreamSynchronize(h->stream); return fail(h, DFM_ERR_CUDA, "dfm_gibbs: copy failed"); }
+      CK(cudaGetLastError());
+    }
+  }
+  CK(cudaStreamSynchronize(h->stream));
+  return finish(h, mem);
 }
 
 // ------------------------------------------------------------------------------------ (f)3: percentile bands

@@ -82,7 +82,10 @@ __host__ __device__ inline size_t sim_gains_smem_doubles(int r, int p) {
 // (~1e-16 |C|) where nothing is observed; its square root would be ~1e-8 |C|^1/2, so C_t of a period with n_t = 0 (a forecast
 // period) is taken as exactly 0.  status: 0 on entry; set to the E-step's status, or to 3 if some P_{t+1|t} is not positive
 // definite.
-// grid (Tp + 1): CTA t < Tp builds period t, CTA Tp the period-independent factors.
+// grid (Tp + 1, models): CTA t < Tp builds period t, CTA Tp the period-independent factors.  Model c = DFM_BY of a batch of
+// E-steps (dfm_gibbs: one model per chain) reads and writes at the per-model strides of the E-step's buffers (A r x k, Q and C
+// r x r, P0 k x k, Ct Tp x r(r+1)/2, Bt Tp x r, Pp / Pf Tp x k x k, src / nobs Tp, st 1) and of the gain table
+// (sim_gains_doubles), and status[c]; one model (grid.y = 1) is dfm_simulation_smoother's call.
 __global__ void k_sim_gains(const double* __restrict__ A, const double* __restrict__ Q, const double* __restrict__ P0,
                             const double* __restrict__ Cg, const double* __restrict__ Ct, const double* __restrict__ Bt,
                             const double* __restrict__ Ppg, const double* __restrict__ Pfg, const int* __restrict__ src,
@@ -90,6 +93,12 @@ __global__ void k_sim_gains(const double* __restrict__ A, const double* __restri
                             int* status) {
   DFM_SMEM(sm);
   const int t = DFM_BX, k = r * p, kk = k * k, rr = r * r, rk = r * k;
+  if (DFM_BY > 0) {
+    const size_t c = DFM_BY;
+    A += c * rk; Q += c * rr; P0 += c * kk; Cg += c * rr; Ct += c * Tp * (size_t)(r * (r + 1) / 2); Bt += c * Tp * r;
+    Ppg += c * Tp * kk; Pfg += c * Tp * kk; src += c * Tp; nobs += c * Tp; st += c; gains += c * sim_gains_doubles(Tp, k, r);
+    status += c;
+  }
   if (st->status != 0) { if (DFM_TID == 0) atomicMax(status, st->status); return; }
   double* M = sm;      double* Pf = M + kk;   double* Pp = Pf + kk;  double* T1 = Pp + kk;  double* T2 = T1 + kk;
   double* Cs = T2 + kk; double* LC = Cs + rr; double* KC = LC + rr;  double* KL = KC + rk;
@@ -280,10 +289,12 @@ __host__ __device__ inline size_t sim_project_smem_doubles(int r) {
 // factor draws [Tp][nd][r] of k_sim_paths; Xout[d]: Tp x N column-major per draw.  The data where observed,
 // lam_i' f~_t + sqrt(R_i) eps_it where missing, NaN for a series out of the model and everywhere when status != 0.  Writes
 // are staged through shared memory so that consecutive threads store consecutive periods of one series.
+// pstride = 0: one model (Lam, R, *status) for every draw, draw j has id id0 + j (dfm_simulation_smoother).  pstride = 1: draw j
+// has its own model (Lam + j N r, R + j N, status[j]) and id id0 + j idstride (dfm_gibbs: one draw per chain).
 // grid (ceil(Tp / SS_TP), ceil(N / SS_NS) * ceil(nd / SIM_PD)), 256 threads.
 __global__ void k_sim_project(const double* __restrict__ X, const double* __restrict__ Lam, const double* __restrict__ R,
                               const double* __restrict__ fS, int Tp, int N, int r, unsigned long long seed, long long id0, int nd,
-                              const int* __restrict__ status, double* __restrict__ Xout) {
+                              const int* __restrict__ status, double* __restrict__ Xout, int pstride, long long idstride) {
   DFM_SMEM(sm);
   const int nst = (N + SS_NS - 1) / SS_NS;
   const int i0 = (DFM_BY % nst) * SS_NS, d0 = (DFM_BY / nst) * SIM_PD, t0 = DFM_BX * SS_TP;
@@ -295,20 +306,27 @@ __global__ void k_sim_project(const double* __restrict__ X, const double* __rest
   double* Xs = Fsh + (size_t)SS_TP * ld;               // [SS_NS][ldv]  the data
   double* Cs = Xs + (size_t)SS_NS * ldv;               // [SS_NS][ldv]  lam_i' f~_t
   double* Sd = Cs + (size_t)SS_NS * ldv;               // [SS_NS]       sqrt(R_i), NaN for a series out of the model
-  const bool failed = *status != 0;
-  for (int e = DFM_TID; e < SS_NS * r; e += DFM_NT) {
-    const int i = e % SS_NS, a = e / SS_NS;
-    Ls[i * ld + a] = (i < ni) ? Lam[i0 + i + (size_t)N * a] : 0.0;
-  }
-  for (int i = DFM_TID; i < SS_NS; i += DFM_NT) Sd[i] = (i < ni && !is_nan(Lam[i0 + i])) ? sqrt(R[i0 + i]) : DFM_NAN;
+  bool failed = *status != 0;
+  auto load_model = [&](const double* Lm, const double* Rm) {
+    for (int e = DFM_TID; e < SS_NS * r; e += DFM_NT) {
+      const int i = e % SS_NS, a = e / SS_NS;
+      Ls[i * ld + a] = (i < ni) ? Lm[i0 + i + (size_t)N * a] : 0.0;
+    }
+    for (int i = DFM_TID; i < SS_NS; i += DFM_NT) Sd[i] = (i < ni && !is_nan(Lm[i0 + i])) ? sqrt(Rm[i0 + i]) : DFM_NAN;
+  };
+  if (!pstride) load_model(Lam, R);
   for (int e = DFM_TID; e < ni * SS_TP; e += DFM_NT) {
     const int i = e / SS_TP, t = e - i * SS_TP;
     if (t < nt) Xs[i * ldv + t] = X[(size_t)(i0 + i) * Tp + t0 + t];
   }
   for (int d = 0; d < dn; ++d) {
     const int j = d0 + d;
-    const unsigned long long id = (unsigned long long)(id0 + j);
+    const unsigned long long id = pstride ? (unsigned long long)(id0 + (long long)j * idstride) : (unsigned long long)(id0 + j);
     DFM_SYNC();
+    if (pstride) {
+      load_model(Lam + (size_t)j * N * r, R + (size_t)j * N);
+      failed = status[j] != 0;
+    }
     for (int e = DFM_TID; e < nt * r; e += DFM_NT) { const int t = e / r, a = e - t * r; Fsh[t * ld + a] = fS[((size_t)(t0 + t) * nd + j) * r + a]; }
     DFM_SYNC();
     wt_gemm(Fsh, ld, 1, Ls, ld, 1, nt, ni, r, [&](int t, int i, double v) { Cs[i * ldv + t] = v; });

@@ -393,6 +393,71 @@ typedef struct {              /* any pointer may be NULL (not computed / not ret
  * same bits whatever n_rep, the shard split or the number of calls.  Synchronous. */
 int dfm_ss_bootstrap(dfm_handle* h, const double* X, const dfm_ssb_opts* opts, const dfm_em_init* params, const dfm_ssb_out* out);
 
+/* ---- Bayesian estimation of the state-space model: batched Gibbs chains ----------------------------------------------
+ * The model of dfm_em_kalman (standardized panel, NaN = missing, P0 HELD FIXED) with a conjugate proper prior, standardized units:
+ *   lam_i | R_i ~ N(0, (R_i / kap_lam) I_r),  R_i ~ IG(a_R, b_R);   A' | Q ~ MN(0, I_k / kap_A, Q),  Q ~ IW(nu_Q, s_Q I_r).
+ * Sweep s of chain c at theta = (Lam, R, A, Q), id = gibbs_id(c, s) = c 2^24 + s, Tp = T + H_fc (the spec is tests/gibbs_oracle.py):
+ *   1. factor step: (z~_0 .. z~_{Tp-1}, x~_missing) exactly as dfm_simulation_smoother's draw `id` at theta;
+ *   2. per series in the model, over its observed in-sample periods: L_i = chol(kap_lam I + S_i), m_i = L_i^-T L_i^-1 s_i,
+ *      R_i = (b_R + (q_i - s_i' m_i) / 2) / Gamma(a_R + n_i / 2),  lam_i = m_i + sqrt(R_i) L_i^-T nu_i
+ *      (S_i = sum f~ f~', s_i = sum x f~, q_i = sum x^2);  series out of the model (NaN Lam row or R_i) stay NaN;
+ *   3. regression of f~_t on z~_{t-1}, t = 1 .. T-1 (the lag block of z~_0 gives the pre-sample lags):
+ *      Q ~ IW(nu_Q + T - 1, s_Q I + Y'Y - B^' Z'Y) by Bartlett,  A' = B^ + L_Z^-T Xi L_Q',  B^ = (kap_A I + Z'Z)^-1 Z'Y;
+ *   4. the forecast periods t >= T are drawn in step 1 for the predictive output only.
+ * Draws of A are kept as drawn (no stationarity restriction).
+ * Random numbers: the Philox4x32-10 stream with replication id gibbs_id(c, s); the factor step uses the simulation smoother's
+ * tags 7-10 unchanged, the parameter step (element indices; Gamma number e = i for R_i, N + j for the Bartlett diagonal B_jj):
+ *   14  nu_i                                       element i r + a          (a < r)
+ *   15  Bartlett B_ij (i > j), then Xi (k x r)     element i + r j;  r^2 + a + k b
+ *   16  normals of the Gamma sampler               element 64 e + j         (attempt j < 64 of Gamma number e)
+ *   17  uniforms of the Gamma sampler              element 64 e + j
+ * Gamma(alpha >= 1) is Marsaglia & Tsang; if all 64 attempts of a number are rejected (probability < 1e-80) it is d = alpha - 1/3.
+ * Chain c is a pure function of (seed, c, its initial theta, sweep0). */
+typedef struct {
+  double kap_lam, a_R, b_R;   /* loadings / idiosyncratic variances: kap_lam > 0, a_R >= 1, b_R > 0 */
+  double kap_A, nu_Q, s_Q;    /* transition: kap_A > 0, s_Q > 0, nu_Q + T - r >= 2 */
+} dfm_gibbs_prior;
+
+typedef struct {
+  int T, N, r, p;             /* panel T x N (STANDARDIZED, NaN = missing) and state shape, k = r p <= 48 */
+  int H_irf;                  /* >= 0: impulse-response horizons 0 .. H_irf - 1 (0 = none) */
+  int H_fc;                   /* >= 0: periods after the panel drawn for the predictive panel */
+  int fc_rows;                /* 0 .. T + H_fc: trailing rows of the (T + H_fc) x N predictive panel returned per kept draw */
+  int n_chain;                /* >= 1 */
+  long long chain0;           /* chain id of the first chain; chain ids < 2^16 */
+  long long sweep0;           /* index of the first sweep; sweep indices < 2^24 */
+  int n_burn, n_keep, thin;   /* >= 0, >= 1, >= 1: n_sweep = n_burn + n_keep thin per chain */
+  unsigned long long seed;
+  int mem;
+  dfm_gibbs_prior prior;
+} dfm_gibbs_opts;
+
+typedef struct {              /* any pointer may be NULL; per chain back to back (chain-major, then kept draw); column-major */
+  double* Lam;                /* n_keep x (N x r)      kept draws (NaN rows for series out of the model) */
+  double* R;                  /* n_keep x N */
+  double* A;                  /* n_keep x (r x k) */
+  double* Q;                  /* n_keep x (r x r) */
+  double* irf;                /* n_keep x (r x H_irf x r)  records [shock][horizon][variable] of dfm_irf at the draw aligned onto ref
+                                 (dfm_ss_bootstrap's rotation and G = [chol(Q~); 0]); NaN where the alignment fails */
+  double* F;                  /* n_keep x (Tp x r)     factor path of the kept sweep */
+  double* X;                  /* n_keep x (fc_rows x N) predictive panel of the kept sweep (last fc_rows rows of Tp): the data where
+                                 observed, lam_i' f~_t + sqrt(R_i) eps_it where missing or after the panel (at the theta entering
+                                 the sweep, as the factor draw), NaN for series out of the model */
+  double* loglik;             /* n_sweep               log-likelihood of the parameters entering each sweep */
+  int* status;                /* [n_chain] 0, or 3: an E-step failed or a P_{t+1|t} or Cholesky factor was not positive definite
+                                 (the chain's records from that sweep on are NaN) */
+} dfm_gibbs_out;
+
+/* X: T x N standardized panel; init: (Lam, R, A, Q, P0) of every chain, back to back (P0 required, e.g. the EM's); ref: theta^
+ * (Lam, R, A, Q) that the impulse responses are aligned onto (may be NULL when H_irf = 0).  Kept draw j of a chain is the state
+ * after sweep sweep0 + n_burn + (j + 1) thin - 1, so a call with init = the last kept draw and sweep0 advanced by n_sweep
+ * continues the chains.  The chains run in sub-batches whose size depends only on (T, N, r, p) and the device (the last one
+ * filled with the chain ids that follow, started from copies of the last chain's init, their results discarded): chain c has
+ * the same bits whatever n_chain, chain0 or the shard split, and the device memory does not grow with n_chain, n_keep or the
+ * number of sweeps.  Bad options: DFM_ERR_ARG; k > 48: DFM_ERR_UNSUPPORTED.  Synchronous. */
+int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* opts, const dfm_em_init* init, const dfm_em_init* ref,
+              const dfm_gibbs_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

@@ -305,4 +305,41 @@ function ss_bootstrap(Xs::Matrix{Float64}, em, n_rep::Integer, seed::Integer; H_
     return (Lam = Lam, R = R, A = A, Q = Q, irf = irf, xhat = xhat, xvar = xvar, loglik = ll, iters = it, status = st)
 end
 
+struct GibbsPrior; kap_lam::Cdouble; a_R::Cdouble; b_R::Cdouble; kap_A::Cdouble; nu_Q::Cdouble; s_Q::Cdouble; end
+struct GibbsOpts; T::Cint; N::Cint; r::Cint; p::Cint; H_irf::Cint; H_fc::Cint; fc_rows::Cint; n_chain::Cint; chain0::Clonglong
+                  sweep0::Clonglong; n_burn::Cint; n_keep::Cint; thin::Cint; seed::Culonglong; mem::Cint; prior::GibbsPrior; end
+struct GibbsOut; Lam::Ptr{Cdouble}; R::Ptr{Cdouble}; A::Ptr{Cdouble}; Q::Ptr{Cdouble}; irf::Ptr{Cdouble}; F::Ptr{Cdouble}
+                 X::Ptr{Cdouble}; loglik::Ptr{Cdouble}; status::Ptr{Cint}; end
+
+"""Gibbs sampler (dfm_gibbs) of the state-space model on the standardized panel `Xs`: `n_chain` chains (ids chain0 ..), all
+started at `em` (the result of `estimate!(m, Parametric())`, P0 included and held fixed), `n_burn` burn-in sweeps then `n_keep`
+kept draws every `thin` sweeps, conjugate prior `prior` (standardized units; default kap_lam = kap_A = 0.01, a_R = 3, b_R = 1,
+nu_Q = r + 2, s_Q = 1).  Returns the raw draws Lam (N x r x n_keep x n_chain), R, A, Q, the impulse responses of each draw
+aligned onto `em` (irf: r x H_irf x r x n_keep x n_chain, [shock, horizon, variable] as `dfm_irf`), the factor paths
+F ((T+H_fc) x r x ..), the predictive panel X (fc_rows x N x ..: the last fc_rows of the T+H_fc rows), loglik (n_sweep x
+n_chain) and status (n_chain)."""
+function gibbs(Xs::Matrix{Float64}, em, n_chain::Integer, seed::Integer; n_burn::Integer = 500, n_keep::Integer = 1000,
+               thin::Integer = 1, H_irf::Integer = 24, H_fc::Integer = 0, fc_rows::Integer = H_fc, chain0::Integer = 0,
+               sweep0::Integer = 0, prior = nothing)
+    h = gethandle()
+    T, N = size(Xs); r = size(em.Lam, 2); k = size(em.A, 2); p = k ÷ r; Tp = T + H_fc; ns = n_burn + n_keep * thin
+    pr = prior === nothing ? GibbsPrior(0.01, 3.0, 1.0, 0.01, r + 2.0, 1.0) : prior
+    rep(a) = repeat(vec(a), n_chain)
+    iL = rep(em.Lam); iR = rep(em.R); iA = rep(em.A); iQ = rep(em.Q); iP = rep(em.P0)
+    Lam = Array{Float64}(undef, N, r, n_keep, n_chain); R = Array{Float64}(undef, N, n_keep, n_chain)
+    A = Array{Float64}(undef, r, k, n_keep, n_chain); Q = Array{Float64}(undef, r, r, n_keep, n_chain)
+    irf = Array{Float64}(undef, r, max(H_irf, 0), r, n_keep, n_chain); F = Array{Float64}(undef, Tp, r, n_keep, n_chain)
+    X = Array{Float64}(undef, fc_rows, N, n_keep, n_chain); ll = Matrix{Float64}(undef, ns, n_chain); st = Vector{Cint}(undef, n_chain)
+    GC.@preserve Xs em iL iR iA iQ iP Lam R A Q irf F X ll st begin
+        opts = Ref(GibbsOpts(T, N, r, p, H_irf, H_fc, fc_rows, n_chain, chain0, sweep0, n_burn, n_keep, thin, seed, MEM_HOST, pr))
+        init = Ref(EmInit(pointer(iL), pointer(iR), pointer(iA), pointer(iQ), pointer(iP)))
+        ref = Ref(EmInit(pointer(em.Lam), pointer(em.R), pointer(em.A), pointer(em.Q), C_NULL))
+        out = Ref(GibbsOut(pointer(Lam), pointer(R), pointer(A), pointer(Q), H_irf > 0 ? pointer(irf) : C_NULL, pointer(F),
+                           fc_rows > 0 ? pointer(X) : C_NULL, pointer(ll), pointer(st)))
+        check(ccall((:dfm_gibbs, LIB), Cint, (Ptr{Cvoid}, Ptr{Cdouble}, Ref{GibbsOpts}, Ref{EmInit}, Ref{EmInit}, Ref{GibbsOut}),
+                    h, Xs, opts, init, ref, out), "dfm_gibbs")
+    end
+    return (Lam = Lam, R = R, A = A, Q = Q, irf = irf, F = F, X = X, loglik = ll, status = st)
+end
+
 end # module
