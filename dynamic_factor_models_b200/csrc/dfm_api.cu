@@ -45,13 +45,13 @@ static inline void emu_set_smem(const void* kern, size_t bytes) {
   g_emu_smem_attr[kern] = bytes;
 }
 static inline bool emu_launch_ok(const void* kern, long long gx, long long gy, long long nt, size_t smem) {
-  size_t attr = 0;
+  size_t attr = 48 * 1024;                                    // the attribute's default; a set value replaces it, up or down
   {
     std::lock_guard<std::mutex> lk(g_emu_attr_mu);
     auto it = g_emu_smem_attr.find(kern);
     if (it != g_emu_smem_attr.end()) attr = it->second;
   }
-  const bool ok = smem <= std::max<size_t>(48 * 1024, attr) && nt >= 1 && nt <= 1024 && gx >= 1 && gx <= 2147483647LL && gy >= 1 &&
+  const bool ok = smem <= attr && nt >= 1 && nt <= 1024 && gx >= 1 && gx <= 2147483647LL && gy >= 1 &&
                   gy <= 65535;
   if (!ok) emu_set_error(cudaErrorInvalidConfiguration);
   return ok;
@@ -475,6 +475,10 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
   }
   const bool any_missing = n_missing > 0, any_bal = emb.on ? (n_missing < batch) : true;
   const int emb_on = emb.on ? 1 : 0;
+  // k_em_mstep_series' shared memory is set on every call: a call with restrictions sets a size for its r, and the
+  // attribute (per kernel, per process) would otherwise cap the launches of later calls at a larger r
+  const size_t smS = (size_t)(2 * np + r + 8 + (cs.off ? em_constr_scratch(r) : 0)) * 8;
+  if (any_missing || !emb.on) DFM_SET_SMEM(k_em_mstep_series, smS);
   int h_active = batch;
   for (int it = 0; it < mi && h_active > 0; ++it) {
     if (any_missing) L(k_em_contract, nblkC, batch, ntC, ((size_t)(np + r) * ntC + 8) * 8, x, d.L, g.W, d.R, g.logR, g.C, T, N, r, g.Bt, g.qt, g.slr, g.nt, g.Ct, d.st);
@@ -484,8 +488,6 @@ static int run_em_general(dfm_handle* h, const double* x, const dfm_em_opts* o, 
     }
     launch_filter_smooth(h, ncl, g, batch, T, r, p, d.A, d.Q, d.P0, d.Fs, d.PsF, d.ll, d.st, mi, o->tol, want_psf);
     if (any_missing || !emb.on) {
-      const size_t smS = (size_t)(2 * np + r + 8 + (cs.off ? em_constr_scratch(r) : 0)) * 8;
-      if (cs.off) DFM_SET_SMEM(k_em_mstep_series, smS);
       L(k_em_mstep_series, N, batch, 64, smS, x, d.Fs, d.PsF, g.Sff, T, N, r, d.L, d.R, d.st, emb_on, cs);
     }
     if (any_bal && emb.on) {
