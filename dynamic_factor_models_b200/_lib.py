@@ -140,7 +140,8 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_launch_count", "dfm_last_error", "dfm_profile_enable", "dfm_profile_query", "dfm_profile_reset",
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
-           "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_em_init_from_factors",
+           "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_gibbs_constrained",
+           "dfm_series_responses", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -229,6 +230,10 @@ class Library:
                                              C.c_longlong, C.c_int, C.c_int, C.c_void_p]
         L.dfm_ss_bootstrap.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SsbOpts), C.POINTER(EmInit), C.POINTER(SsbOut)]
         L.dfm_gibbs.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GibbsOpts), C.POINTER(EmInit), C.POINTER(EmInit), C.POINTER(GibbsOut)]
+        L.dfm_gibbs_constrained.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GibbsOpts), C.POINTER(EmInit), C.POINTER(EmInit),
+                                            C.POINTER(LamConstr), C.POINTER(GibbsOut)]
+        L.dfm_series_responses.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                           C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p]
         L.dfm_bootstrap_panels.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 8
@@ -342,26 +347,34 @@ class Library:
         self.check(self.lib.dfm_ss_bootstrap(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(ou)), "dfm_ss_bootstrap")
 
     def gibbs_raw(self, X, T, N, r, p, init, ref, out, mem, n_chain, chain0=0, sweep0=0, n_burn=0, n_keep=1, thin=1, seed=0, H_irf=0,
-                  H_fc=0, fc_rows=0, prior=None):
+                  H_fc=0, fc_rows=0, prior=None, constr=None):
         """Pointer-level dfm_gibbs (ints = device or host addresses).  init: dict Lam, R, A, Q, P0 (n_chain models back to back);
         ref: dict Lam, R, A, Q or None; out: dict of Lam, R, A, Q, irf, F, X, loglik, status (missing or 0 = NULL); prior: dict
-        (gibbs_default_prior(r) when None)."""
+        (gibbs_default_prior(r) when None); constr: (index, H (n_c x r), h) host arrays in standardized units, or None: the
+        chains under H[q] @ lam_{index[q]} = h[q] (dfm_gibbs_constrained)."""
         pr = dict(gibbs_default_prior(r)); pr.update(prior or {})
         o = GibbsOpts(T=T, N=N, r=r, p=p, H_irf=H_irf, H_fc=H_fc, fc_rows=fc_rows, n_chain=n_chain, chain0=chain0, sweep0=sweep0,
                       n_burn=n_burn, n_keep=n_keep, thin=thin, seed=seed, mem=mem, prior=GibbsPrior(**pr))
         ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in init.items()})
         rf = EmInit(**{k: C.c_void_p(v) if v else None for k, v in ref.items()}) if ref is not None else None
         ou = GibbsOut(**{k: C.c_void_p(v) if v else None for k, v in out.items()})
-        self.check(self.lib.dfm_gibbs(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), C.byref(rf) if rf is not None else None, C.byref(ou)),
-                   "dfm_gibbs")
+        rfp = C.byref(rf) if rf is not None else None
+        if constr is None:
+            self.check(self.lib.dfm_gibbs(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), rfp, C.byref(ou)), "dfm_gibbs")
+            return
+        lc, keep = _lam_constr(constr, r)
+        self.check(self.lib.dfm_gibbs_constrained(self.h, C.c_void_p(X), C.byref(o), C.byref(ini), rfp, C.byref(lc), C.byref(ou)),
+                   "dfm_gibbs_constrained")
+        del keep
 
     def gibbs(self, X, init, p=1, n_chain=None, chain0=0, sweep0=0, n_burn=0, n_keep=1, thin=1, seed=0, H_irf=0, H_fc=0, fc_rows=0,
-              prior=None, ref=None, outputs=GIBBS_OUTPUTS):
+              prior=None, ref=None, outputs=GIBBS_OUTPUTS, constr=None):
         """Gibbs chains of the state-space model on the standardized panel X (T, N) (dfm_gibbs).  init: dict Lam (n_chain, N, r),
         R (n_chain, N), A (n_chain, r, k), Q (n_chain, r, r), P0 (n_chain, k, k) -- or one model (2-D arrays), copied to every
         chain; ref: dict Lam, R, A, Q (the model the impulse responses are aligned onto).  Returns Lam (n_chain, n_keep, N, r),
         R (n_chain, n_keep, N), A, Q, irf (n_chain, n_keep, r, H_irf, r) [variable, horizon, shock], F (n_chain, n_keep, T + H_fc,
-        r), X (n_chain, n_keep, fc_rows, N) -- those named in `outputs` -- loglik (n_chain, n_sweep) and status (n_chain)."""
+        r), X (n_chain, n_keep, fc_rows, N) -- those named in `outputs` -- loglik (n_chain, n_sweep) and status (n_chain).
+        constr: restrictions on the loadings as gibbs_raw's (dfm_gibbs_constrained; no irf then)."""
         X = np.asarray(X, float); T, N = X.shape
         Lam = np.asarray(init["Lam"], float); r = Lam.shape[-1]; k = r * p
         if n_chain is None:
@@ -384,7 +397,7 @@ class Library:
                        {n_: a_.ctypes.data for n_, a_ in rf.items()} if rf is not None else None,
                        {**{n_: a_.ctypes.data for n_, a_ in outs.items()}, "loglik": ll.ctypes.data, "status": st.ctypes.data}, MEM_HOST,
                        n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin, seed=seed, H_irf=H_irf, H_fc=H_fc,
-                       fc_rows=fc_rows, prior=prior)
+                       fc_rows=fc_rows, prior=prior, constr=constr)
         res = dict(loglik=ll.reshape(n_chain, n_sweep), status=st)
         shape = dict(Lam=(N, r), A=(r, k), Q=(r, r), F=(Tp, r), X=(fc_rows, N))
         nb = n_chain * n_keep
@@ -396,6 +409,34 @@ class Library:
             else:
                 v = from_cm(a_, shape[n_][0], shape[n_][1], nb)
             res[n_] = np.ascontiguousarray(v).reshape((n_chain, n_keep) + v.shape[1:])
+        return res
+
+    def series_responses_raw(self, models, N, r, p, n_model, H, n_shock, scale, mem, resp=0, fevd=0, status=0):
+        """Pointer-level dfm_series_responses (ints = device or host addresses).  models: dict Lam, R, A, Q (n_model models back to
+        back); scale: address or 0 (= 1)."""
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in models.items()})
+        vp = lambda a: C.c_void_p(a) if a else None
+        self.check(self.lib.dfm_series_responses(self.h, C.byref(ini), N, r, p, n_model, H, n_shock, vp(scale), mem, vp(resp), vp(fevd),
+                                                 vp(status)), "dfm_series_responses")
+
+    def series_responses(self, Lam, R, A, Q, H, n_shock=None, scale=None, outputs=("resp", "fevd")):
+        """Series responses and variance decompositions of models (Lam (B, N, r), R (B, N), A (B, r, k), Q (B, r, r)), or of one
+        model (2-D Lam) (dfm_series_responses): resp / fevd (B, N, H, n_shock) -- those named in `outputs` -- and status (B),
+        without the batch axis for one model.  scale: (N,) per-series scale of resp (None = 1)."""
+        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
+        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        n_shock = r if n_shock is None else int(n_shock)
+        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
+        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
+        outs = {n_: np.full(max(B * N * H * n_shock, 0), np.nan) for n_ in outputs}
+        st = np.zeros(B, np.int32)
+        self.series_responses_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, N, r, p, B, H, n_shock,
+                                  sc.ctypes.data if sc is not None else 0, MEM_HOST, resp=outs["resp"].ctypes.data if "resp" in outs else 0,
+                                  fevd=outs["fevd"].ctypes.data if "fevd" in outs else 0, status=st.ctypes.data)
+        res = dict(status=st if b else int(st[0]))
+        for n_, a_ in outs.items():
+            v = a_.reshape(B, n_shock, H, N).transpose(0, 3, 2, 1)
+            res[n_] = np.ascontiguousarray(v if b else v[0])
         return res
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):

@@ -385,6 +385,107 @@ def series_irf(m, H, lib=None):
     return b["xstd"][:, None, None] * np.einsum("ia,ahj->ihj", b["Lam"], irf)
 
 
+def variance_decomposition(m, H, lib=None):
+    """Series responses and forecast-error variance decompositions of a model estimated with `estimate(m, Parametric())` at its
+    EM estimates m.em (dfm_series_responses).  With L = chol(Q), Psi_h = [M^h]_{1:r,1:r} L and c_{i,h} = lam_i' Psi_h:
+      resp (ns, H, r)   xstd_i c_{i,h,j}: the response of series i in data units to the orthogonalised shock j (= series_irf);
+      fevd (ns, H, r)   sum_{l<=h} c_{i,l,j}^2 / (sum_{l<=h} |c_{i,l}|^2 + R_i): the share of the (h+1)-step forecast-error
+                        variance of series i due to shock j; 1 - fevd.sum(-1) is the idiosyncratic share;
+    and series (the order of forecast's `series`; NaN rows for series out of the model).
+
+    Identification: as series_irf.  The factors are identified only up to f -> K f; under a named-factor restriction
+    (lam_constr_em pinning some series' loadings to e_1') the columns of shock 1 of resp and fevd do not depend on the rotation
+    left free, the other shocks' columns do (their sum, and so the idiosyncratic share, does not)."""
+    if H <= 0:
+        raise ValueError("H must be > 0")
+    b = _state_space_block(m, 0, lib, "variance_decomposition")
+    lib, e = b["lib"], b["em"]
+    o = lib.series_responses(b["Lam"], e["R"], e["A"], e["Q"], H, scale=b["xstd"])
+    if o["status"] != 0:
+        raise RuntimeError(f"variance_decomposition: device status {o['status']}")
+    return dict(resp=o["resp"], fevd=o["fevd"], series=b["series"])
+
+
+def _named_factors(m):
+    """The factors j (0-based) that m.em["lam_constr"] names: some series in the model has full-rank rows whose solution is
+    c e_j, c != 0."""
+    c = m.em.get("lam_constr") if m.em is not None else None
+    if c is None:
+        return set()
+    idx, Hm, hv = c
+    Lam = m.em["Lam"]
+    r = Lam.shape[1]
+    named = set()
+    for i in set(int(v) for v in idx):
+        if np.isnan(Lam[i]).any() or np.isnan(m.em["R"][i]) or np.isnan(m.lambda_est[i, 0]):
+            continue
+        sel = np.flatnonzero(np.asarray(idx) == i)
+        Hi, hi = np.asarray(Hm, float)[sel], np.asarray(hv, float)[sel]
+        if len(sel) < r or np.linalg.matrix_rank(Hi) < r:
+            continue
+        lam = np.linalg.lstsq(Hi, hi, rcond=None)[0]
+        nz = np.flatnonzero(np.abs(lam) > 1e-12 * np.abs(lam).max()) if np.abs(lam).max() > 0 else []
+        if len(nz) == 1:
+            named.add(int(nz[0]))
+    return named
+
+
+def identified_responses(m, H, shocks=1, n_chain=4, n_burn=500, n_keep=1000, thin=1, prior=None, seed=20260922,
+                         q=(5, 16, 50, 84, 95), chain0=0, sweep0=0, lib=None):
+    """Posterior bands of the series responses and variance decompositions of the named shocks 1..`shocks` of a model estimated
+    with `estimate(m, Parametric(), lam_constr_em=...)`, whose restriction names factors 1..shocks (factor j is named when some
+    series in the model has r independent rows whose solution is c e_j, c != 0, as Figure 7's oil series).  Those columns are
+    the ones the rotation left free by the restriction does not change (series_irf, variance_decomposition).
+
+    Gibbs chains under the restriction (dfm_gibbs_constrained: the prior of gibbs with each restricted series' loadings
+    conditioned on its rows) start at m.em; every kept draw's responses and decompositions come from dfm_series_responses.
+    Returns a dict:
+      resp, fevd (ns, H, shocks)                            at m.em (variance_decomposition's first `shocks` columns);
+      resp_draws, fevd_draws (n_chain, n_keep, ns, H, shocks)  of every kept draw (NaN for a failed chain);
+      resp_bands, fevd_bands (len(q), ns, H, shocks)        percentiles over the draws (dfm_percentiles; failed chains ignored);
+      Lam, R, A, Q (n_chain, n_keep, ...)                   raw parameter draws (standardized units);
+      loglik (n_chain, n_burn + n_keep thin), status (n_chain);
+      rhat dict(loglik, resp (ns, H, shocks))               split-R^ over the kept draws;
+    and prior, series, shocks, q.  n_chain n_keep <= 16384."""
+    if m.em is None or m.em.get("lam_constr") is None:
+        raise ValueError("identified_responses needs a model estimated with Parametric() under lam_constr_em")
+    r = m.em["Q"].shape[0]
+    if not 1 <= shocks <= r:
+        raise ValueError(f"identified_responses: shocks must be in [1, {r}]")
+    named = _named_factors(m)
+    missing = [j + 1 for j in range(shocks) if j not in named]
+    if missing:
+        raise ValueError(f"identified_responses: the restriction of m does not name factor(s) {missing} (no series in the model "
+                         "has r independent rows whose solution is a multiple of e_j), so their shocks are not identified")
+    if H <= 0:
+        raise ValueError("H must be > 0")
+    if not 1 <= n_chain * n_keep <= 16384:
+        raise ValueError("identified_responses: n_chain * n_keep must be in [1, 16384]")
+    b = _state_space_block(m, 0, lib, "identified_responses")
+    lib, e = b["lib"], b["em"]
+    pr = dict(_gibbs_default_prior(r)); pr.update(prior or {})
+    init = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"], P0=e["P0"])
+    o = lib.gibbs(b["Xs"], init, p=b["p"], n_chain=n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin,
+                  seed=seed, prior=pr, outputs=("Lam", "R", "A", "Q"), constr=e["lam_constr"])
+    n = n_chain * n_keep
+    ns = b["Xs"].shape[1]
+    sh = lambda a_: a_.reshape((n,) + a_.shape[2:])
+    d = lib.series_responses(sh(o["Lam"]), sh(o["R"]), sh(o["A"]), sh(o["Q"]), H, n_shock=shocks, scale=b["xstd"])
+    pt = lib.series_responses(b["Lam"], e["R"], e["A"], e["Q"], H, n_shock=shocks, scale=b["xstd"])
+    if pt["status"] != 0:
+        raise RuntimeError(f"identified_responses: device status {pt['status']}")
+    qq = np.asarray(q, float)
+    out = dict(resp=pt["resp"], fevd=pt["fevd"], Lam=o["Lam"], R=o["R"], A=o["A"], Q=o["Q"], loglik=o["loglik"], status=o["status"],
+               prior=pr, series=b["series"], shocks=shocks, q=qq)
+    kept = n_burn + thin * np.arange(1, n_keep + 1) - 1
+    for nm in ("resp", "fevd"):
+        dr = d[nm].reshape((n_chain, n_keep, ns, H, shocks))
+        out[nm + "_draws"] = dr
+        out[nm + "_bands"] = lib.percentiles(d[nm].reshape(n, -1), qq).reshape((len(qq), ns, H, shocks))
+    out["rhat"] = dict(loglik=float(split_rhat(o["loglik"][:, kept])), resp=split_rhat(out["resp_draws"]))
+    return out
+
+
 def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
                          lib=None):
     """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn

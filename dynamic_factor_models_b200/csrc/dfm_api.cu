@@ -16,6 +16,7 @@
 #include "dfm_kernels_news.cuh"
 #include "dfm_kernels_ssb.cuh"
 #include "dfm_kernels_gibbs.cuh"
+#include "dfm_kernels_resp.cuh"
 #include <algorithm>
 #include <cmath>
 #include <new>
@@ -1167,6 +1168,54 @@ int dfm_em_init_from_factors(dfm_handle* h, const double* Xs, const double* F, i
 }
 
 // ------------------------------------------------------------------------------------ a'
+// Restrictions on the loadings (dfm_lam_constr) as a host CSR grouped by series in their given order: offsets [N+1], rows
+// [nc x r] row-major, values [nc].  `what`: the entry point, for the error messages.
+struct ConstrCsr { int nc = 0; std::vector<int> off; std::vector<double> H, h; };
+
+static int constr_csr(dfm_handle* h, const char* what, const dfm_lam_constr* con, int N, int r, ConstrCsr* cc) {
+  char msg[160];
+  auto bad = [&](const char* why) { snprintf(msg, sizeof(msg), "%s: %s", what, why); return fail(h, DFM_ERR_ARG, msg); };
+  const int nc = con ? con->n_constr : 0;
+  cc->nc = nc;
+  if (nc < 0) return bad("n_constr < 0");
+  if (nc == 0) return DFM_OK;
+  if (!con->index || !con->H || !con->h) return bad("null restriction array");
+  std::vector<int>& coff = cc->off;
+  coff.assign((size_t)N + 1, 0);
+  for (int q = 0; q < nc; ++q) {
+    const int i = con->index[q];
+    if (i < 0 || i >= N) return bad("restriction index outside [0, N)");
+    if (!std::isfinite(con->h[q])) return bad("non-finite restriction value");
+    for (int a = 0; a < r; ++a)
+      if (!std::isfinite(con->H[q + (size_t)nc * a])) return bad("non-finite restriction row");
+    if (++coff[i + 1] > r) return bad("more than r restriction rows on one series");
+  }
+  for (int i = 0; i < N; ++i) coff[i + 1] += coff[i];
+  cc->H.resize((size_t)nc * r); cc->h.resize(nc);
+  std::vector<int> fill(coff.begin(), coff.end() - 1);
+  for (int q = 0; q < nc; ++q) {
+    const int dst = fill[con->index[q]]++;
+    for (int a = 0; a < r; ++a) cc->H[(size_t)dst * r + a] = con->H[q + (size_t)nc * a];
+    cc->h[dst] = con->h[q];
+  }
+  return DFM_OK;
+}
+
+// The device copy of a CSR: cs's arrays from the arena (N + 1 ints, nc r and nc doubles); upload on the handle's stream.
+static EmConstr constr_bufs(Arena& a, const ConstrCsr& cc, int N, int r) {
+  EmConstr cs{};
+  if (cc.nc) { cs.off = a.get<int>((size_t)N + 1); cs.H = a.get<double>((size_t)cc.nc * r); cs.h = a.get<double>(cc.nc); }
+  return cs;
+}
+
+static int constr_upload(dfm_handle* h, const ConstrCsr& cc, const EmConstr& cs) {
+  if (!cc.nc) return DFM_OK;              // (pageable sources: each copy returns once its source has been staged)
+  CK(cudaMemcpyAsync((void*)cs.off, cc.off.data(), cc.off.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync((void*)cs.H, cc.H.data(), cc.H.size() * 8, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync((void*)cs.h, cc.h.data(), cc.h.size() * 8, cudaMemcpyHostToDevice, h->stream));
+  return DFM_OK;
+}
+
 // dfm_em_kalman and dfm_em_kalman_constrained.  con == nullptr or con->n_constr == 0: the unrestricted EM (same dispatch, same
 // bits).  Otherwise the restriction is checked, uploaded once as a per-series CSR (rows grouped by series in their given order)
 // and the call runs the general path, whatever the shape.
@@ -1177,29 +1226,10 @@ static int em_kalman_impl(dfm_handle* h, const double* X, const dfm_em_opts* o, 
   int T = o->T, N = o->N, r = o->r, p = o->p, batch = o->batch, mem = o->mem, mi = o->max_iter;
   if (T <= 1 || N <= 0 || r <= 0 || r > 64 || p <= 0 || batch <= 0 || mi <= 0 || o->tol < 0)
     return fail(h, DFM_ERR_ARG, "dfm_em_kalman: bad shape/options");
-  const int nc = con ? con->n_constr : 0;
-  std::vector<int> coff;                  // host CSR of the restriction: offsets [N+1], rows [nc x r] row-major, values [nc]
-  std::vector<double> cH, ch;
-  if (nc < 0) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: n_constr < 0");
+  ConstrCsr cc;
+  { int rc = constr_csr(h, "dfm_em_kalman_constrained", con, N, r, &cc); if (rc) return rc; }
+  const int nc = cc.nc;
   if (nc > 0) {
-    if (!con->index || !con->H || !con->h) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: null restriction array");
-    coff.assign((size_t)N + 1, 0);
-    for (int q = 0; q < nc; ++q) {
-      const int i = con->index[q];
-      if (i < 0 || i >= N) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: restriction index outside [0, N)");
-      if (!std::isfinite(con->h[q])) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: non-finite restriction value");
-      for (int a = 0; a < r; ++a)
-        if (!std::isfinite(con->H[q + (size_t)nc * a])) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: non-finite restriction row");
-      if (++coff[i + 1] > r) return fail(h, DFM_ERR_ARG, "dfm_em_kalman_constrained: more than r restriction rows on one series");
-    }
-    for (int i = 0; i < N; ++i) coff[i + 1] += coff[i];
-    cH.resize((size_t)nc * r); ch.resize(nc);
-    std::vector<int> fill(coff.begin(), coff.end() - 1);
-    for (int q = 0; q < nc; ++q) {
-      const int dst = fill[con->index[q]]++;
-      for (int a = 0; a < r; ++a) cH[(size_t)dst * r + a] = con->H[q + (size_t)nc * a];
-      ch[dst] = con->h[q];
-    }
     if (o->path == 2 || o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman_constrained: the fused paths take no restrictions");
   }
   if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: batch > 65535");
@@ -1229,15 +1259,10 @@ static int em_kalman_impl(dfm_handle* h, const double* X, const dfm_em_opts* o, 
     d.ready = a.get<int>(kMaxReadyChunks);
     d.scratch = try_fused ? a.get<double>((size_t)std::min(batch, h->nsm * 8) * T * FUSED_SCR(r)) : nullptr;
     const GenBufs g = gen_bufs(a, emb, B, T, N, r, p);        // also the fallback when the scan finds missing data
-    EmConstr cs{};
-    if (nc) { cs.off = a.get<int>((size_t)N + 1); cs.H = a.get<double>((size_t)nc * r); cs.h = a.get<double>(nc); }
+    const EmConstr cs = constr_bufs(a, cc, N, r);
     if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    if (nc) {                             // (pageable sources: each copy returns once its source has been staged)
-      CK(cudaMemcpyAsync((void*)cs.off, coff.data(), coff.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync((void*)cs.H, cH.data(), cH.size() * 8, cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync((void*)cs.h, ch.data(), ch.size() * 8, cudaMemcpyHostToDevice, h->stream));
-    }
-    int rc = DFM_OK;
+    int rc = constr_upload(h, cc, cs);
+    if (rc) return rc;
     bool fused = try_fused;
     bool uploaded = false;                // the streaming host path found missing data: the panels are on the device already
 #ifndef DFM_EMU
@@ -1909,8 +1934,11 @@ int dfm_ss_bootstrap(dfm_handle* h, const double* X, const dfm_ssb_opts* o, cons
 // (records going to pageable host memory are staged per kept sweep):
 //   ss_estep (one padded panel copy per chain, k_ss_bcast once per call) -> k_sim_gains (grid.y = chain) -> k_gibbs_paths ->
 //   [kept: k_sim_project + k_ss_fc_rows] -> k_gibbs_stats -> k_gibbs_draw -> [kept: records, k_ss_align + k_irf].
-int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm_em_init* init, const dfm_em_init* ref,
-              const dfm_gibbs_out* out) {
+// dfm_gibbs and dfm_gibbs_constrained.  con == nullptr or con->n_constr == 0: the unrestricted sampler (same launches, same
+// bits).  Otherwise the rows are checked as dfm_em_kalman_constrained's, uploaded once as a per-series CSR, and the parameter
+// step is k_gibbs_draw_constr.
+static int gibbs_impl(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm_em_init* init, const dfm_em_init* ref,
+                      const dfm_lam_constr* con, const dfm_gibbs_out* out) {
   if (!h || !X || !o || !init || !out || !init->Lam || !init->R || !init->A || !init->Q || !init->P0)
     return fail(h, DFM_ERR_ARG, "dfm_gibbs: null argument (P0 is required)");
   const int T = o->T, N = o->N, r = o->r, p = o->p, Hi = o->H_irf, Hf = o->H_fc, fr = o->fc_rows, mem = o->mem;
@@ -1927,6 +1955,10 @@ int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm
     return fail(h, DFM_ERR_ARG, "dfm_gibbs: bad prior (kappas, b_R, s_Q > 0, a_R >= 1, nu_Q + T - r >= 2)");
   if (Hi > 0 && out->irf && (!ref || !ref->Lam || !ref->R || !ref->A || !ref->Q))
     return fail(h, DFM_ERR_ARG, "dfm_gibbs: ref is required for impulse responses");
+  ConstrCsr cc;
+  { int rc = constr_csr(h, "dfm_gibbs_constrained", con, N, r, &cc); if (rc) return rc; }
+  if (cc.nc && out->irf)
+    return fail(h, DFM_ERR_ARG, "dfm_gibbs_constrained: no impulse responses with restrictions (the rotation onto ref would undo them)");
   const int k = r * p, Tp = T + Hf;
   if (k > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: state dimension r*p > 48");
   const int C = ssb_batch(h, T, N, r, p);
@@ -1935,6 +1967,8 @@ int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm
   const size_t smG = sim_gains_smem_doubles(r, p) * 8, smPa = gibbs_paths_smem_doubles(r, p) * 8, smSt = gibbs_stats_smem_doubles() * 8,
                smD = gibbs_draw_smem_doubles(r, p) * 8, smP = sim_project_smem_doubles(r) * 8, smA = ssb_align_smem_doubles(r, p) * 8;
   if (smD > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: state too large for the parameter-draw kernel");
+  const size_t smDc = smD + gibbs_constr_smem_doubles(r) * 8;          // k_gibbs_draw_constr
+  if (cc.nc && smDc > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs_constrained: state too large for the parameter-draw kernel");
   const int nst = (N + SS_NS - 1) / SS_NS;
   if ((long long)nst * ((C + SIM_PD - 1) / SIM_PD) > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: N too large");
   CK(cudaSetDevice(h->device));
@@ -1970,7 +2004,10 @@ int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm
            *adum = wantI ? a.get<double>(B + 4) : nullptr, *dI = wantI ? a.get<double>(B * nirf) : nullptr;
     int* ast = wantI ? a.get<int>(B) : nullptr;
     int* ids = wantI ? a.get<int>(r) : nullptr;
+    const EmConstr cs = constr_bufs(a, cc, N, r);
     if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    rc = constr_upload(h, cc, cs);
+    if (rc) return rc;
     // ---- once per call: the padded panel, its copies, the per-series counts; the reference model and shock ids
     if (hst) {
       CK(cudaMemcpy2DAsync(Xpad, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, N, cudaMemcpyHostToDevice, h->stream));
@@ -1995,7 +2032,8 @@ int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm
     DFM_SET_SMEM(k_sim_gains, smG);
     DFM_SET_SMEM(k_gibbs_paths, smPa);
     DFM_SET_SMEM(k_gibbs_stats, smSt);
-    DFM_SET_SMEM(k_gibbs_draw, smD);
+    if (cc.nc) DFM_SET_SMEM(k_gibbs_draw_constr, smDc);
+    else DFM_SET_SMEM(k_gibbs_draw, smD);
     DFM_SET_SMEM(k_sim_project, smP);
     const int* src = s.g.nt + (size_t)C * Tp;
     const long long idstride = 1LL << 24;
@@ -2048,7 +2086,8 @@ int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm
         L(k_gibbs_stats, (N + GB_NS - 1) / GB_NS, (C * r + GB_NC - 1) / GB_NC, 128, smSt, (const double*)Xpad, (const double*)fS, T, Tp, N,
           r, C, sv);
         da.id0 = id0;
-        L(k_gibbs_draw, C, 1, GB_NT, smD, da);
+        if (cc.nc) L(k_gibbs_draw_constr, C, 1, GB_NT, smDc, da, cs);
+        else L(k_gibbs_draw, C, 1, GB_NT, smD, da);
         if (kept) {
           const double* psrc[4] = {dL, dR, dA, dQ};
           double* pst[4] = {sL, sR, sA, sQ};
@@ -2085,6 +2124,77 @@ int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm
     }
   }
   CK(cudaStreamSynchronize(h->stream));
+  return finish(h, mem);
+}
+
+int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm_em_init* init, const dfm_em_init* ref,
+              const dfm_gibbs_out* out) {
+  return gibbs_impl(h, X, o, init, ref, nullptr, out);
+}
+
+int dfm_gibbs_constrained(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, const dfm_em_init* init, const dfm_em_init* ref,
+                          const dfm_lam_constr* constr, const dfm_gibbs_out* out) {
+  return gibbs_impl(h, X, o, init, ref, constr, out);
+}
+
+// ------------------------------------------------------------------------------------ series responses / FEVD
+// Per chunk of models (a size fixed by the shapes, so that device memory does not grow with n_model): k_sr_prep -> k_irf (all r
+// shocks) -> k_series_resp.  Host arrays are staged per chunk; device outputs are written in place.
+int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r, int p, int n_model, int H, int n_shock,
+                         const double* scale, int mem, double* resp, double* fevd, int* status) {
+  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || N <= 0 || r <= 0 || r > 64 || p <= 0 ||
+      n_model <= 0 || H <= 0 || n_shock <= 0 || n_shock > r || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_series_responses: bad argument");
+  const int k = r * p;
+  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nout = (size_t)N * H * n_shock;
+  const size_t sm0 = series_resp_smem_doubles(r, n_shock, 0);
+  if ((sm0 + rr) * 8 > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: r too large");
+  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
+  const size_t smR = series_resp_smem_doubles(r, n_shock, hc) * 8;
+  const bool hst = mem == DFM_MEM_HOST;
+  const size_t per = 8 * (kk + 2 * rk + rr * H + (hst ? Nr + N + rk + rr + (resp ? nout : 0) + (fevd ? nout : 0) : 0)) + 8;
+  const int nb = (int)std::min<long long>({(long long)n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)), 65535LL});
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    const size_t B = nb;
+    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
+           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
+           *dS = hst && scale ? a.get<double>(N) : nullptr;
+    double *dRe = hst && resp ? a.get<double>(B * nout) : nullptr, *dFe = hst && fevd ? a.get<double>(B * nout) : nullptr;
+    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H);
+    int* dst = a.get<int>(B);
+    int* ids = a.get<int>(r);
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    std::vector<int> hid(r);
+    for (int j = 0; j < r; ++j) hid[j] = j;
+    CK(cudaMemcpyAsync(ids, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    const double* sc = scale;
+    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
+    DFM_SET_SMEM(k_series_resp, smR);
+    for (long long j0 = 0; j0 < n_model; j0 += nb) {
+      const int nm = (int)std::min<long long>(nb, n_model - j0);
+      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr;
+      int rc = DFM_OK;
+      if (hst) {
+        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
+        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
+        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
+        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
+      }
+      double* oR = resp ? (hst ? dRe : resp + j0 * nout) : nullptr;
+      double* oF = fevd ? (hst ? dFe : fevd + j0 * nout) : nullptr;
+      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
+      L(k_irf, r, nm, 64, (size_t)(2 * k + 8) * 8, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)ids, dI);
+      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm, SR_NS, smR, L_, R_, sc, (const double*)dI, (const int*)dst, N, r, H, n_shock, hc, oR, oF);
+      if (hst) {
+        rc = copy_out(h, resp ? resp + j0 * nout : nullptr, dRe, nm * nout, mem); if (rc) return rc;
+        rc = copy_out(h, fevd ? fevd + j0 * nout : nullptr, dFe, nm * nout, mem); if (rc) return rc;
+      }
+      rc = copy_out(h, status ? status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
+      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+    }
+  }
   return finish(h, mem);
 }
 

@@ -18,8 +18,14 @@
 //   RNG_GB_GN   16  normals of the Gamma sampler                 element 64 e + j (attempt j of Gamma number e)
 //   RNG_GB_GU   17  uniforms of the Gamma sampler                element 64 e + j
 // Gamma numbers: e = i for R_i (series i < N), e = N + j for the Bartlett diagonal j < r.
+// dfm_gibbs_constrained (k_gibbs_draw_constr): a series with restriction rows H_i lam_i = h_i draws from the exact conditional
+// under the prior N(0, R_i / kap_lam I) conditioned on the rows, with the same random numbers (tag 14 elements i r + a, Gamma
+// number i):  lam*_i = the EM's correction of m_i (S~ = kap_lam I + S_i in place of S), h0 = H_i' (H_i H_i')^-1 h_i,
+//   R_i = (b_R + (q_i - 2 s_i' lam*_i + lam*_i' S~ lam*_i - kap_lam |h0|^2) / 2) / Gamma(a_R + n_i / 2),
+//   lam_i = the EM's correction of the unrestricted draw m_i + sqrt(R_i) L_i^-T nu_i.
 #pragma once
 #include "dfm_common.cuh"
+#include "dfm_kernels_em.cuh"
 #include "dfm_kernels_rep.cuh"
 #include "dfm_kernels_sim.cuh"
 
@@ -240,9 +246,17 @@ struct GibbsDrawArgs {
   unsigned long long seed; long long id0, idstride;
 };
 
+// Shared scratch of k_gibbs_draw_constr's restricted pass (doubles, after gibbs_draw_smem_doubles): lam_constr_correct's
+// scratch, then three r-vectors.
+__host__ __device__ inline size_t gibbs_constr_smem_doubles(int r) { return (size_t)em_constr_scratch(r) + 3 * (size_t)r; }
+
 // One CTA per chain (GB_NT threads): the parameter step of the sweep at the path of k_gibbs_paths (steps 2-3 of the spec).
 // A chain whose status is not 0 keeps its parameters; a Cholesky factor that is not positive definite sets status 3.
-__global__ void k_gibbs_draw(GibbsDrawArgs a) {
+// CON (k_gibbs_draw_constr, the call has restriction rows cs): the thread-per-series loop leaves the restricted series after
+// their Cholesky solve (L_i and m_i stay in wk); thread 0 then draws them one by one (header comment), with the scratch of
+// gibbs_constr_smem_doubles in shared memory.  Dependent rows set status 3.  Without CON the body is the unrestricted kernel.
+template <bool CON>
+__device__ __forceinline__ void gibbs_draw_body(GibbsDrawArgs a, EmConstr cs) {
   DFM_SMEM(sm);
   const int c = DFM_BX, r = a.r, p = a.p, k = r * p, T = a.T, N = a.N, C = a.C, kk = k * k, rr = r * r, rk = r * k;
   const int np = r * (r + 1) / 2;
@@ -302,6 +316,7 @@ __global__ void k_gibbs_draw(GibbsDrawArgs a) {
       }
     for (int x = 0; x < r; ++x) { const double v = sv[i + (size_t)N * x]; bv[(size_t)x * N] = v; s0[(size_t)x * N] = v; }
     if (chol_solve_packed(Ap, bv, r, N)) { atomicMax(&info[1], 1); continue; }
+    if constexpr (CON) { if (cs.off[i + 1] > cs.off[i]) continue; }     // restricted: drawn below
     double sm_ = 0.0;
     for (int x = 0; x < r; ++x) sm_ += s0[(size_t)x * N] * bv[(size_t)x * N];
     const double al = a.pr.a_R + 0.5 * a.nobs[i], be = a.pr.b_R + 0.5 * (a.q[i] - sm_);
@@ -315,6 +330,62 @@ __global__ void k_gibbs_draw(GibbsDrawArgs a) {
     }
     Rv[i] = Ri;
     for (int x = 0; x < r; ++x) Lam[i + (size_t)N * x] = bv[(size_t)x * N] + sr * s0[(size_t)x * N];
+  }
+  if constexpr (CON) {
+    DFM_SYNC();
+    if (DFM_TID == 0) {
+      double* ws = zc + 2 * k + 8;                     // (info occupies the 8 doubles after zc)
+      double* lv = ws + em_constr_scratch(r);          // lam*, then the draw
+      double* h0 = lv + r;                             // H_i' (H_i H_i')^-1 h_i
+      double* uv = h0 + r;
+      for (int i = 0; i < N && !info[1]; ++i) {
+        const int q0 = cs.off[i], m = cs.off[i + 1] - q0;
+        bool in = m > 0 && !is_nan(Rv[i]);
+        for (int b = 0; b < r && in; ++b) if (is_nan(Lam[i + (size_t)N * b])) in = false;
+        if (!in) continue;
+        const double* Ap = wk + i;                     // L_i (packed, stride N)
+        const double* bv = wk + (size_t)np * N + i;    // m_i
+        const double* s0 = wk + (size_t)(np + r) * N + i;
+        const double* Hq = cs.H + (size_t)q0 * r;
+        const double* hq = cs.h + q0;
+        auto solve = [&](double* v) {                  // v <- S~^-1 v
+          for (int x = 0; x < r; ++x) {
+            double s = v[x];
+            for (int y = 0; y < x; ++y) s -= Ap[(size_t)pidx(x, y) * N] * v[y];
+            v[x] = s / Ap[(size_t)pidx(x, x) * N];
+          }
+          for (int x = r - 1; x >= 0; --x) {
+            double s = v[x];
+            for (int y = x + 1; y < r; ++y) s -= Ap[(size_t)pidx(y, x) * N] * v[y];
+            v[x] = s / Ap[(size_t)pidx(x, x) * N];
+          }
+        };
+        for (int x = 0; x < r; ++x) { h0[x] = 0.0; lv[x] = bv[(size_t)x * N]; }
+        if (lam_constr_correct(h0, r, Hq, hq, m, ws, [](double*) {}) || lam_constr_correct(lv, r, Hq, hq, m, ws, solve)) {
+          info[1] = 1;
+          break;
+        }
+        double sl = 0.0, q2 = 0.0, n0 = 0.0;
+        for (int x = 0; x < r; ++x) {
+          double v = 0.0;                              // (L_i' lam*)_x
+          for (int y = x; y < r; ++y) v += Ap[(size_t)pidx(y, x) * N] * lv[y];
+          q2 += v * v; sl += s0[(size_t)x * N] * lv[x]; n0 += h0[x] * h0[x];
+        }
+        const double al = a.pr.a_R + 0.5 * a.nobs[i];
+        const double be = a.pr.b_R + 0.5 * (a.q[i] - 2.0 * sl + q2 - a.pr.kap_lam * n0);
+        const double Ri = be / gb_gamma(al, a.seed, id, (unsigned long long)i);
+        const double sr = sqrt(Ri);
+        for (int x = r - 1; x >= 0; --x) {              // L_i^-T nu_i
+          double s = rng_normal(a.seed, id, RNG_GB_NU, (unsigned long long)i * r + x);
+          for (int y = x + 1; y < r; ++y) s -= Ap[(size_t)pidx(y, x) * N] * uv[y];
+          uv[x] = s / Ap[(size_t)pidx(x, x) * N];
+        }
+        for (int x = 0; x < r; ++x) uv[x] = bv[(size_t)x * N] + sr * uv[x];
+        if (lam_constr_correct(uv, r, Hq, hq, m, ws, solve)) { info[1] = 1; break; }
+        Rv[i] = Ri;
+        for (int x = 0; x < r; ++x) Lam[i + (size_t)N * x] = uv[x];
+      }
+    }
   }
   // ---- transition step
   for (int e = DFM_TID; e < kk; e += DFM_NT) { const int x = e % k, y = e / k; LZ[e] = ZZ[e] + (x == y ? a.pr.kap_A : 0.0); }
@@ -354,6 +425,9 @@ __global__ void k_gibbs_draw(GibbsDrawArgs a) {
   for (int e = DFM_TID; e < rk; e += DFM_NT) { const int x = e % r, y = e / r; Ao[e] = At[y + k * x]; }
   for (int e = DFM_TID; e < rr; e += DFM_NT) Qo[e] = Qn[e];
 }
+
+__global__ void k_gibbs_draw(GibbsDrawArgs a) { gibbs_draw_body<false>(a, EmConstr{nullptr, nullptr, nullptr}); }
+__global__ void k_gibbs_draw_constr(GibbsDrawArgs a, EmConstr cs) { gibbs_draw_body<true>(a, cs); }
 
 // dst[c * dstride + e] = src[c * sstride + e] for e < n, NaN where cst[c] != 0 (the records of a kept sweep).  grid (.., C).
 __global__ void k_gibbs_rec(const double* __restrict__ src, long long sstride, long long n, const int* __restrict__ cst,

@@ -458,6 +458,35 @@ typedef struct {              /* any pointer may be NULL; per chain back to back
 int dfm_gibbs(dfm_handle* h, const double* X, const dfm_gibbs_opts* opts, const dfm_em_init* init, const dfm_em_init* ref,
               const dfm_gibbs_out* out);
 
+/* The same sampler under linear restrictions on the loadings (dfm_lam_constr, STANDARDIZED units, as dfm_em_kalman_constrained),
+ * e.g. the named-factor normalisation of Stock & Watson's Figure 7.  For a restricted series i (rows H_i, values h_i, m_i <= r)
+ * the prior on lam_i is N(0, R_i / kap_lam I) CONDITIONED on H_i lam_i = h_i, so its conditional posterior is exact: with
+ * S~ = kap_lam I + S_i (L_i = chol(S~)), Y = S~^-1 H_i', G = H_i Y, m_i = S~^-1 s_i,
+ *     lam*_i = m_i - Y G^-1 (H_i m_i - h_i)                      (the EM's correction, S~ in place of S)
+ *     R_i    = (b_R + (q_i - 2 s_i' lam*_i + lam*_i' S~ lam*_i - kap_lam h_i' (H_i H_i')^-1 h_i) / 2) / Gamma(a_R + n_i / 2)
+ *     lam_i  = the same correction applied to the unrestricted draw m_i + sqrt(R_i) L_i^-T nu_i
+ * (the r - m_i free dimensions cancel from the shape).  A restricted series uses the unrestricted series' random numbers (tag
+ * 14 elements i r + a, Gamma number i); unrestricted series, the factor step and the transition step are unchanged.
+ *   constr == NULL or n_constr == 0: exactly dfm_gibbs (same bits).
+ *   DFM_ERR_ARG: the restriction errors of dfm_em_kalman_constrained, and out->irf != NULL with rows (the rotation onto ref
+ *   would rotate the draws off the restriction).  Rows on a series out of the model are ignored.  Dependent rows on a series
+ *   (relative pivot of G <= 1e-12) give that chain status 3. */
+int dfm_gibbs_constrained(dfm_handle* h, const double* X, const dfm_gibbs_opts* opts, const dfm_em_init* init, const dfm_em_init* ref,
+                          const dfm_lam_constr* constr, const dfm_gibbs_out* out);
+
+/* ---- series responses and forecast-error variance decompositions of many models --------------------------------------
+ * models: n_model models (Lam N x r, R N, A r x k, Q r x r; P0 unused) back to back as dfm_em_init's batch layout, k = r p.
+ * Per model, L = chol(Q), Psi_h = [M^h]_{1:r,1:r} L (h = 0 .. H-1, M the companion matrix of A), c_{i,h} = lam_i' Psi_h (1 x r):
+ *   resp[i,h,j] = scale_i c_{i,h,j}                                           (n_shock = r: api.series_irf)
+ *   fevd[i,h,j] = sum_{l<=h} c_{i,l,j}^2 / (sum_{l<=h} |c_{i,l}|^2 + R_i)    (share of the (h+1)-step forecast-error variance of
+ *                                                                             x_i due to shock j, idiosyncratic part included)
+ * for the leading n_shock shocks (1 <= n_shock <= r); outputs N x H x n_shock per model, column-major, either may be NULL.
+ * scale: N (e.g. xstd; NULL = 1).  Series out of the model (NaN Lam row or R_i) get NaN columns.  status [n_model] (may be
+ * NULL): 0, or DFM_ERR_NOT_PD when Q is not positive definite or A / Q hold a NaN (a failed chain): that model's outputs are
+ * NaN.  All arrays in `mem`.  r <= 64; bad arguments: DFM_ERR_ARG.  Synchronous for host memory. */
+int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r, int p, int n_model, int H, int n_shock,
+                         const double* scale, int mem, double* resp, double* fevd, int* status);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

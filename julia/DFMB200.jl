@@ -342,4 +342,47 @@ function gibbs(Xs::Matrix{Float64}, em, n_chain::Integer, seed::Integer; n_burn:
     return (Lam = Lam, R = R, A = A, Q = Q, irf = irf, F = F, X = X, loglik = ll, status = st)
 end
 
+"""Gibbs sampler under linear restrictions on the loadings (dfm_gibbs_constrained): as `gibbs` without impulse responses, with
+`index` (0-based series), `Hc` (n_constr x r) and `hc` (n_constr) in STANDARDIZED units (em.lam_constr of a restricted fit)."""
+function gibbs_constrained(Xs::Matrix{Float64}, em, index::Vector{Cint}, Hc::Matrix{Float64}, hc::Vector{Float64}, n_chain::Integer,
+                           seed::Integer; n_burn::Integer = 500, n_keep::Integer = 1000, thin::Integer = 1, chain0::Integer = 0,
+                           sweep0::Integer = 0, prior = nothing)
+    h = gethandle()
+    T, N = size(Xs); r = size(em.Lam, 2); k = size(em.A, 2); p = k ÷ r; ns = n_burn + n_keep * thin; nc = length(index)
+    pr = prior === nothing ? GibbsPrior(0.01, 3.0, 1.0, 0.01, r + 2.0, 1.0) : prior
+    rep(a) = repeat(vec(a), n_chain)
+    iL = rep(em.Lam); iR = rep(em.R); iA = rep(em.A); iQ = rep(em.Q); iP = rep(em.P0)
+    Lam = Array{Float64}(undef, N, r, n_keep, n_chain); R = Array{Float64}(undef, N, n_keep, n_chain)
+    A = Array{Float64}(undef, r, k, n_keep, n_chain); Q = Array{Float64}(undef, r, r, n_keep, n_chain)
+    ll = Matrix{Float64}(undef, ns, n_chain); st = Vector{Cint}(undef, n_chain)
+    GC.@preserve Xs em iL iR iA iQ iP Lam R A Q ll st index Hc hc begin
+        opts = Ref(GibbsOpts(T, N, r, p, 0, 0, 0, n_chain, chain0, sweep0, n_burn, n_keep, thin, seed, MEM_HOST, pr))
+        init = Ref(EmInit(pointer(iL), pointer(iR), pointer(iA), pointer(iQ), pointer(iP)))
+        con = Ref(LamConstr(nc, pointer(index), pointer(Hc), pointer(hc)))
+        out = Ref(GibbsOut(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL, C_NULL, C_NULL, pointer(ll), pointer(st)))
+        check(ccall((:dfm_gibbs_constrained, LIB), Cint,
+                    (Ptr{Cvoid}, Ptr{Cdouble}, Ref{GibbsOpts}, Ref{EmInit}, Ptr{Cvoid}, Ref{LamConstr}, Ref{GibbsOut}),
+                    h, Xs, opts, init, C_NULL, con, out), "dfm_gibbs_constrained")
+    end
+    return (Lam = Lam, R = R, A = A, Q = Q, loglik = ll, status = st)
+end
+
+"""Series responses and forecast-error variance decompositions (dfm_series_responses) of B models Lam (N x r x B), R (N x B),
+A (r x k x B), Q (r x r x B): resp, fevd (N x H x n_shock x B) and status (B); `scale` (N) multiplies resp (e.g. xstd)."""
+function series_responses(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{Float64,3}, Q::Array{Float64,3}, H::Integer;
+                          n_shock::Integer = size(Lam, 2), scale = nothing)
+    h = gethandle()
+    N, r, B = size(Lam); p = size(A, 2) ÷ r
+    resp = Array{Float64}(undef, N, H, n_shock, B); fevd = similar(resp); st = Vector{Cint}(undef, B)
+    sc = scale === nothing ? Float64[] : Vector{Float64}(scale)
+    GC.@preserve Lam R A Q resp fevd st sc begin
+        models = Ref(EmInit(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL))
+        check(ccall((:dfm_series_responses, LIB), Cint,
+                    (Ptr{Cvoid}, Ref{EmInit}, Cint, Cint, Cint, Cint, Cint, Cint, Ptr{Cdouble}, Cint, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Cint}),
+                    h, models, N, r, p, B, H, n_shock, scale === nothing ? C_NULL : pointer(sc), MEM_HOST, resp, fevd, st),
+              "dfm_series_responses")
+    end
+    return (resp = resp, fevd = fevd, status = st)
+end
+
 end # module
