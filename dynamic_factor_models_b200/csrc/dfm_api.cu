@@ -1089,6 +1089,8 @@ int dfm_irf(dfm_handle* h, const double* M, const double* Q, const double* G, in
     return fail(h, DFM_ERR_ARG, "dfm_irf: bad argument");
   for (int j = 0; j < n_shock; ++j) if (shock_ids[j] < 0 || shock_ids[j] >= r) return fail(h, DFM_ERR_ARG, "dfm_irf: shock id out of range");
   if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_irf: batch > 65535");
+  const size_t smI = irf_smem_doubles(k) * 8;
+  if (smI > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_irf: state dimension k too large (k > 14076)");
   CK(cudaSetDevice(h->device));
   size_t B = batch;
   for (int pass = 0; pass < 2; ++pass) {
@@ -1104,7 +1106,8 @@ int dfm_irf(dfm_handle* h, const double* M, const double* Q, const double* G, in
     rc = stage_in(h, Q, dQ, B * r * k, mem, &q); if (rc) return rc;
     rc = stage_in(h, G, dG, B * k * r, mem, &g); if (rc) return rc;
     CK(cudaMemcpyAsync(ids, shock_ids, n_shock * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    L(k_irf, n_shock, batch, 64, (size_t)(2 * k + 8) * 8, m, q, g, k, r, H, n_shock, ids, dI);
+    DFM_SET_SMEM(k_irf, smI);                                // (every call: a lower value from an earlier call may be in place)
+    L(k_irf, n_shock, batch, 64, smI, m, q, g, k, r, H, n_shock, ids, dI);
     if (mem == DFM_MEM_HOST) { rc = copy_out(h, irf, dI, B * r * H * n_shock, mem); if (rc) return rc; }
   }
   return finish(h, mem);
@@ -1965,7 +1968,8 @@ static int gibbs_impl(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, c
   int rc = ss_check(h, "dfm_gibbs", Tp, N, r, p, 0, C, DFM_MEM_DEVICE);
   if (rc) return rc;
   const size_t smG = sim_gains_smem_doubles(r, p) * 8, smPa = gibbs_paths_smem_doubles(r, p) * 8, smSt = gibbs_stats_smem_doubles() * 8,
-               smD = gibbs_draw_smem_doubles(r, p) * 8, smP = sim_project_smem_doubles(r) * 8, smA = ssb_align_smem_doubles(r, p) * 8;
+               smD = gibbs_draw_smem_doubles(r, p) * 8, smP = sim_project_smem_doubles(r) * 8, smA = ssb_align_smem_doubles(r, p) * 8,
+               smI = irf_smem_doubles(k) * 8;
   if (smD > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs: state too large for the parameter-draw kernel");
   const size_t smDc = smD + gibbs_constr_smem_doubles(r) * 8;          // k_gibbs_draw_constr
   if (cc.nc && smDc > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_gibbs_constrained: state too large for the parameter-draw kernel");
@@ -2028,6 +2032,7 @@ static int gibbs_impl(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, c
       CK(cudaMemcpyAsync(ids, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
       CK(cudaStreamSynchronize(h->stream));                  // (hid is a local)
       DFM_SET_SMEM(k_ss_align, smA);
+      DFM_SET_SMEM(k_irf, smI);
     }
     DFM_SET_SMEM(k_sim_gains, smG);
     DFM_SET_SMEM(k_gibbs_paths, smPa);
@@ -2109,7 +2114,7 @@ static int gibbs_impl(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, c
             aa.M = aM; aa.Qsel = aS; aa.G = aG; aa.llf = allf; aa.status = ast;
             aa.N = N; aa.r = r; aa.p = p; aa.max_iter = 1;
             L(k_ss_align, C, 1, SSB_NT, smA, aa);
-            L(k_irf, r, C, 64, (size_t)(2 * k + 8) * 8, (const double*)aM, (const double*)aS, (const double*)aG, k, r, Hi, r, (const int*)ids, dI);
+            L(k_irf, r, C, 64, smI, (const double*)aM, (const double*)aS, (const double*)aG, k, r, Hi, r, (const int*)ids, dI);
             put(out->irf, dI, nirf, 8, (size_t)nk * nirf, (size_t)jk * nirf);
           }
         }
@@ -2151,6 +2156,8 @@ int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r,
   if ((sm0 + rr) * 8 > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: r too large");
   const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
   const size_t smR = series_resp_smem_doubles(r, n_shock, hc) * 8;
+  const size_t smI = irf_smem_doubles(k) * 8;
+  if (smI > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: state dimension r*p too large (r*p > 14076)");
   const bool hst = mem == DFM_MEM_HOST;
   const size_t per = 8 * (kk + 2 * rk + rr * H + (hst ? Nr + N + rk + rr + (resp ? nout : 0) + (fevd ? nout : 0) : 0)) + 8;
   const int nb = (int)std::min<long long>({(long long)n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)), 65535LL});
@@ -2172,6 +2179,7 @@ int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r,
     const double* sc = scale;
     if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
     DFM_SET_SMEM(k_series_resp, smR);
+    DFM_SET_SMEM(k_irf, smI);
     for (long long j0 = 0; j0 < n_model; j0 += nb) {
       const int nm = (int)std::min<long long>(nb, n_model - j0);
       const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr;
@@ -2185,7 +2193,7 @@ int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r,
       double* oR = resp ? (hst ? dRe : resp + j0 * nout) : nullptr;
       double* oF = fevd ? (hst ? dFe : fevd + j0 * nout) : nullptr;
       L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
-      L(k_irf, r, nm, 64, (size_t)(2 * k + 8) * 8, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)ids, dI);
+      L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)ids, dI);
       L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm, SR_NS, smR, L_, R_, sc, (const double*)dI, (const int*)dst, N, r, H, n_shock, hc, oR, oF);
       if (hst) {
         rc = copy_out(h, resp ? resp + j0 * nout : nullptr, dRe, nm * nout, mem); if (rc) return rc;

@@ -1094,7 +1094,9 @@ __global__ void k_var(const double* __restrict__ Fall, int T, int r, int p, int 
 }
 
 // ---------------------------------------------------------------- a11 IRF (:793-816)
-// grid (n_shock, B), one block per shock; shared 2k doubles.
+// grid (n_shock, B), one block per shock; shared irf_smem_doubles(k) (x and x2, 2k doubles, and 8 spare).
+__host__ __device__ inline size_t irf_smem_doubles(int k) { return 2 * (size_t)k + 8; }
+
 __global__ void k_irf(const double* __restrict__ Mall, const double* __restrict__ Qall, const double* __restrict__ Gall,
                       int k, int r, int H, int n_shock, const int* __restrict__ shock_ids, double* __restrict__ irf) {
   DFM_SMEM(sm);

@@ -163,7 +163,8 @@ int dfm_fit_correlation(dfm_handle* h, const double* data, const double* F, cons
                         int min_obs, int mem, double* cor /*ns*/, int* status /*ns or NULL*/);
 
 /* ---- a11: impulse_response / compute_irf_single_shock!, :793-825 ----------------------- */
-/* irf[:, h, j] = Q M^h G[:, shock_ids[j]],  h = 0..H-1;  irf is r x H x n_shock column-major. */
+/* irf[:, h, j] = Q M^h G[:, shock_ids[j]],  h = 0..H-1;  irf is r x H x n_shock column-major.
+ * k <= 14076 (the two k-vectors of a shock live in shared memory); larger k: DFM_ERR_UNSUPPORTED. */
 int dfm_irf(dfm_handle* h, const double* M, const double* Q, const double* G, int k, int r, int H,
             int n_shock, const int* shock_ids /*host, 0-based*/, int batch, int mem, double* irf);
 
@@ -483,7 +484,8 @@ int dfm_gibbs_constrained(dfm_handle* h, const double* X, const dfm_gibbs_opts* 
  * for the leading n_shock shocks (1 <= n_shock <= r); outputs N x H x n_shock per model, column-major, either may be NULL.
  * scale: N (e.g. xstd; NULL = 1).  Series out of the model (NaN Lam row or R_i) get NaN columns.  status [n_model] (may be
  * NULL): 0, or DFM_ERR_NOT_PD when Q is not positive definite or A / Q hold a NaN (a failed chain): that model's outputs are
- * NaN.  All arrays in `mem`.  r <= 64; bad arguments: DFM_ERR_ARG.  Synchronous for host memory. */
+ * NaN.  All arrays in `mem`.  r <= 64; bad arguments: DFM_ERR_ARG; r p > 14076 (dfm_irf's bound): DFM_ERR_UNSUPPORTED.
+ * Synchronous for host memory. */
 int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r, int p, int n_model, int H, int n_shock,
                          const double* scale, int mem, double* resp, double* fevd, int* status);
 
