@@ -14,6 +14,7 @@ from .api import (  # noqa: F401
     impulse_response, bai_ng_criterion, amengual_watson_test, estimate_factor_numbers,
     standardize_data, pca_score, em_kalman, em_init_from_factors, set_default_library, get_library,
     kalman_smooth, forecast, posterior_draws, forecast_bands, news, parametric_irf, parametric_bootstrap,
-    series_irf, gibbs, split_rhat, variance_decomposition, identified_responses,
+    series_irf, gibbs, split_rhat, variance_decomposition, identified_responses, historical_decomposition,
+    identified_history,
 )
 from . import ingest  # noqa: F401   (host-side panel ingestion: the step before the path)

@@ -72,6 +72,18 @@ class SsOut(C.Structure):
 SS_OUTPUTS = ("F", "PF", "common", "xhat", "xvar")
 
 
+class HdOpts(C.Structure):
+    _fields_ = [("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("Tp", C.c_int), ("t0", C.c_int), ("n_shock", C.c_int),
+                ("n_model", C.c_int), ("mem", C.c_int)]
+
+
+class HdOut(C.Structure):
+    _fields_ = [("shocks", C.c_void_p), ("contrib", C.c_void_p), ("rest", C.c_void_p), ("base", C.c_void_p), ("status", C.c_void_p)]
+
+
+HD_OUTPUTS = ("shocks", "contrib", "rest", "base")
+
+
 class SimOpts(C.Structure):
     _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("n_draw", C.c_longlong),
                 ("draw0", C.c_longlong), ("seed", C.c_ulonglong), ("mem", C.c_int)]
@@ -141,7 +153,7 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
            "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_gibbs_constrained",
-           "dfm_series_responses", "dfm_em_init_from_factors",
+           "dfm_series_responses", "dfm_historical_decomposition", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -232,6 +244,8 @@ class Library:
         L.dfm_gibbs.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GibbsOpts), C.POINTER(EmInit), C.POINTER(EmInit), C.POINTER(GibbsOut)]
         L.dfm_gibbs_constrained.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GibbsOpts), C.POINTER(EmInit), C.POINTER(EmInit),
                                             C.POINTER(LamConstr), C.POINTER(GibbsOut)]
+        L.dfm_historical_decomposition.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.POINTER(HdOpts),
+                                                   C.POINTER(HdOut)]
         L.dfm_series_responses.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -437,6 +451,44 @@ class Library:
         for n_, a_ in outs.items():
             v = a_.reshape(B, n_shock, H, N).transpose(0, 3, 2, 1)
             res[n_] = np.ascontiguousarray(v if b else v[0])
+        return res
+
+    def historical_decomposition_raw(self, models, F, N, r, p, Tp, t0, n_shock, n_model, scale, mem, shocks=0, contrib=0, rest=0, base=0,
+                                     status=0):
+        """Pointer-level dfm_historical_decomposition (ints = device or host addresses).  models: dict Lam, R, A, Q (n_model models
+        back to back); F: the n_model paths (Tp x r each); t0: the 0-based base row; scale: address or 0 (= 1)."""
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in models.items()})
+        vp = lambda a: C.c_void_p(a) if a else None
+        o = HdOpts(N=N, r=r, p=p, Tp=Tp, t0=t0, n_shock=n_shock, n_model=n_model, mem=mem)
+        ou = HdOut(shocks=vp(shocks), contrib=vp(contrib), rest=vp(rest), base=vp(base), status=vp(status))
+        self.check(self.lib.dfm_historical_decomposition(self.h, C.byref(ini), vp(F), vp(scale), C.byref(o), C.byref(ou)),
+                   "dfm_historical_decomposition")
+
+    def historical_decomposition(self, Lam, R, A, Q, F, t0, n_shock=None, scale=None, outputs=HD_OUTPUTS):
+        """Historical decompositions of models (Lam (B, N, r), R (B, N), A (B, r, k), Q (B, r, r)) along their factor paths F
+        (B, Tp, r), or of one model (2-D Lam, F (Tp, r)) (dfm_historical_decomposition), from the 0-based base row t0: shocks
+        (B, Tp, r), contrib (B, N, Tp, n_shock), rest, base (B, N, Tp) -- those named in `outputs` -- and status (B), without the
+        batch axis for one model.  scale: (N,) per-series scale (None = 1).  The arrays are views of the column-major buffers the
+        library wrote (no copy: the draws of a long Gibbs run take gigabytes)."""
+        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
+        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        F = np.asarray(F, float); Tp = F.shape[-2]
+        n_shock = r if n_shock is None else int(n_shock)
+        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
+        Fb = to_cm(F)
+        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
+        size = dict(shocks=Tp * r, contrib=N * Tp * n_shock, rest=N * Tp, base=N * Tp)
+        outs = {n_: np.full(B * size[n_], np.nan) for n_ in outputs}
+        st = np.zeros(B, np.int32)
+        self.historical_decomposition_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, Fb.ctypes.data, N, r, p, Tp, t0, n_shock, B,
+                                          sc.ctypes.data if sc is not None else 0, MEM_HOST,
+                                          status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        res = dict(status=st if b else int(st[0]))
+        shape = dict(shocks=(B, r, Tp), contrib=(B, n_shock, Tp, N), rest=(B, Tp, N), base=(B, Tp, N))
+        for n_, a_ in outs.items():
+            v = a_.reshape(shape[n_])
+            v = v.transpose(0, 3, 2, 1) if v.ndim == 4 else v.transpose(0, 2, 1)
+            res[n_] = v if b else v[0]
         return res
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):

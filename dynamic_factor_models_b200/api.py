@@ -486,6 +486,120 @@ def identified_responses(m, H, shocks=1, n_chain=4, n_burn=500, n_keep=1000, thi
     return out
 
 
+def _history_rows(m, b, t0, what):
+    """(t0 as a 1-based period, its row in the estimation block, the smoothed path F (T, r) at m.em)."""
+    lo = m.initperiod + b["p"] - 1
+    t0 = lo if t0 is None else int(t0)
+    if not lo <= t0 <= m.lastperiod:
+        raise ValueError(f"{what}: t0 must be a period in {lo} .. {m.lastperiod} (initperiod + p - 1 .. lastperiod)")
+    e = b["em"]
+    o = b["lib"].kalman_smooth(b["Xs"], b["Lam"], e["R"], e["A"], e["Q"], p=b["p"], P0=e["P0"], H=0, outputs=("F",))
+    if o["status"] != 0:
+        raise RuntimeError(f"{what}: device status {o['status']}")
+    return t0, t0 - m.initperiod, o["F"]
+
+
+def historical_decomposition(m, t0=None, lib=None):
+    """Historical decomposition of a model estimated with `estimate(m, Parametric())` at its EM estimates m.em
+    (dfm_historical_decomposition): each series' common component split, period by period, into the contributions of the r
+    orthogonalised factor shocks since the base period t0 and the part carried over from the factors at t0.
+
+    The path is the smoothed factor path E[f_t | data] at m.em (kalman_smooth over the estimation block, as forecast(m, 0)); all
+    the pieces are linear in the path, so they are their own expectations given the data at m.em.  With L = chol(Q),
+    Psi_h = [M^h]_{1:r,1:r} L (series_irf's responses) and the structural shocks eps_t = L^-1 (f_t - sum_l A_l f_{t-l}):
+      contrib (ns, T, r)  xstd_i lam_i' sum_{s=t0+1..t} Psi_{t-s} e_j eps_{j,s}: the part of series i at period t due to shock
+                          j since t0 (0 up to t0);
+      base (ns, T)        xstd_i lam_i' [M^{t-t0} z_t0]_{1:r}: the path the factors at t0 and before would have taken without
+                          shocks (the common component itself up to t0);
+      resid (ns, T)       data - xmean - xstd_i lam_i' f_t (NaN where the data is missing);
+      shocks (T, r)       eps_t (standardized; NaN for the first p periods, which have no lags in the sample);
+    so xmean + base + contrib.sum(-1) + resid is the data at every observed cell.  Rows are the periods initperiod ..
+    lastperiod (1-based, `periods`), columns the estimation series (`series`); series out of the model have NaN columns.
+    t0: a 1-based period in initperiod + p - 1 .. lastperiod (default initperiod + p - 1, the first period whose p lags lie in
+    the sample; returned as `t0`).
+
+    Identification: as series_irf.  Under a named-factor restriction (lam_constr_em pinning some series' loadings to e_1') the
+    rotations f -> K f left free have K's first row e_1'; then eps_1 and the column of shock 1 of contrib do not change, and
+    neither do base and the sum of the other columns; the other shocks' individual columns do."""
+    b = _state_space_block(m, 0, lib, "historical_decomposition")
+    lib, e = b["lib"], b["em"]
+    r = e["Q"].shape[0]
+    t0, row, F = _history_rows(m, b, t0, "historical_decomposition")
+    o = lib.historical_decomposition(b["Lam"], e["R"], e["A"], e["Q"], F, row, n_shock=r, scale=b["xstd"],
+                                     outputs=("shocks", "contrib", "base"))
+    if o["status"] != 0:
+        raise RuntimeError(f"historical_decomposition: device status {o['status']}")
+    X = m.data[:, b["series"]][m.initperiod - 1:m.lastperiod]
+    resid = (X - b["xmean"] - b["xstd"] * (F @ b["Lam"].T)).T
+    return dict(contrib=np.ascontiguousarray(o["contrib"]), base=np.ascontiguousarray(o["base"]), resid=np.ascontiguousarray(resid),
+                shocks=np.ascontiguousarray(o["shocks"]), periods=b["periods"], series=b["series"], t0=t0)
+
+
+def identified_history(m, shocks=1, t0=None, n_chain=4, n_burn=500, n_keep=1000, thin=1, prior=None, seed=20260922,
+                       q=(5, 16, 50, 84, 95), chain0=0, sweep0=0, return_draws=False, lib=None):
+    """Posterior bands of the historical decomposition by the named shocks 1..`shocks` of a model estimated with
+    `estimate(m, Parametric(), lam_constr_em=...)`, whose restriction names factors 1..shocks (as identified_responses, whose
+    preconditions and errors apply).  Those are the columns that the rotation left free by the restriction does not change
+    (historical_decomposition).
+
+    Gibbs chains under the restriction (dfm_gibbs_constrained, as identified_responses) start at m.em.  Kept draw j records the
+    factor path drawn in its sweep at the parameters entering that sweep and the parameters drawn given that path: a joint
+    posterior draw, decomposed as recorded (one dfm_historical_decomposition over all kept draws, n_shock = shocks).  Returns a
+    dict, in data units, rows `periods`, columns `series`, t0 as historical_decomposition:
+      contrib (ns, T, shocks), rest (ns, T), base (ns, T), shocks (T, shocks)   at m.em along the smoothed path
+                          (historical_decomposition's; rest = the other shocks' columns summed);
+      contrib_bands, rest_bands, base_bands, shocks_bands (len(q), ...)         percentiles over the kept draws
+                          (dfm_percentiles; failed chains, whose draws are NaN, are ignored);
+      contrib_draws, rest_draws, base_draws, shocks_draws (n_chain, n_keep, ...) only with return_draws=True: at the defaults
+                          each is about 0.5 GB for Stock & Watson's Figure 7 block (139 series, 120 periods);
+      rhat dict(loglik, contrib (ns, T, shocks))   split-R^ over the kept draws (NaN up to t0, where contrib is 0 in every draw);
+      status (n_chain), loglik (n_chain, n_burn + n_keep thin);
+    and prior, q, periods, series, t0.  n_chain n_keep <= 16384."""
+    if m.em is None or m.em.get("lam_constr") is None:
+        raise ValueError("identified_history needs a model estimated with Parametric() under lam_constr_em")
+    r = m.em["Q"].shape[0]
+    if not 1 <= shocks <= r:
+        raise ValueError(f"identified_history: shocks must be in [1, {r}]")
+    named = _named_factors(m)
+    missing = [j + 1 for j in range(shocks) if j not in named]
+    if missing:
+        raise ValueError(f"identified_history: the restriction of m does not name factor(s) {missing} (no series in the model "
+                         "has r independent rows whose solution is a multiple of e_j), so their shocks are not identified")
+    if not 1 <= n_chain * n_keep <= 16384:
+        raise ValueError("identified_history: n_chain * n_keep must be in [1, 16384]")
+    b = _state_space_block(m, 0, lib, "identified_history")
+    lib, e = b["lib"], b["em"]
+    t0, row, F = _history_rows(m, b, t0, "identified_history")
+    pt = lib.historical_decomposition(b["Lam"], e["R"], e["A"], e["Q"], F, row, n_shock=shocks, scale=b["xstd"])
+    if pt["status"] != 0:
+        raise RuntimeError(f"identified_history: device status {pt['status']}")
+    pr = dict(_gibbs_default_prior(r)); pr.update(prior or {})
+    init = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"], P0=e["P0"])
+    o = lib.gibbs(b["Xs"], init, p=b["p"], n_chain=n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin,
+                  seed=seed, prior=pr, outputs=("Lam", "R", "A", "Q", "F"), constr=e["lam_constr"])
+    n = n_chain * n_keep
+    sh = lambda a_: a_.reshape((n,) + a_.shape[2:])
+    d = lib.historical_decomposition(sh(o["Lam"]), sh(o["R"]), sh(o["A"]), sh(o["Q"]), sh(o["F"]), row, n_shock=shocks,
+                                     scale=b["xstd"])
+    qq = np.asarray(q, float)
+    out = dict(contrib=np.ascontiguousarray(pt["contrib"]), rest=np.ascontiguousarray(pt["rest"]),
+               base=np.ascontiguousarray(pt["base"]), shocks=np.ascontiguousarray(pt["shocks"][:, :shocks]), status=o["status"],
+               loglik=o["loglik"], prior=pr, q=qq, periods=b["periods"], series=b["series"], t0=t0)
+    # the records in the library's column-major layout, (n, d) row-major for dfm_percentiles, and back
+    recs = dict(contrib=d["contrib"].transpose(0, 3, 2, 1), rest=d["rest"].transpose(0, 2, 1), base=d["base"].transpose(0, 2, 1),
+                shocks=d["shocks"][:, :, :shocks].transpose(0, 2, 1))
+    for nm, v in recs.items():
+        bd = lib.percentiles(v.reshape(n, -1), qq).reshape((len(qq),) + v.shape[1:])
+        out[nm + "_bands"] = np.ascontiguousarray(bd.transpose((0,) + tuple(range(bd.ndim - 1, 0, -1))))
+        if return_draws:
+            dr = d[nm][..., :shocks] if nm == "shocks" else d[nm]
+            out[nm + "_draws"] = dr.reshape((n_chain, n_keep) + dr.shape[1:])
+    kept = n_burn + thin * np.arange(1, n_keep + 1) - 1
+    out["rhat"] = dict(loglik=float(split_rhat(o["loglik"][:, kept])),
+                       contrib=split_rhat(d["contrib"].reshape((n_chain, n_keep) + d["contrib"].shape[1:])))
+    return out
+
+
 def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
                          lib=None):
     """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn

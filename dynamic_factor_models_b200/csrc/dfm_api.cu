@@ -17,6 +17,7 @@
 #include "dfm_kernels_ssb.cuh"
 #include "dfm_kernels_gibbs.cuh"
 #include "dfm_kernels_resp.cuh"
+#include "dfm_kernels_hd.cuh"
 #include <algorithm>
 #include <cmath>
 #include <new>
@@ -2200,6 +2201,87 @@ int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r,
         rc = copy_out(h, fevd ? fevd + j0 * nout : nullptr, dFe, nm * nout, mem); if (rc) return rc;
       }
       rc = copy_out(h, status ? status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
+      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+    }
+  }
+  return finish(h, mem);
+}
+
+// ------------------------------------------------------------------------------------ historical decompositions
+// Per chunk of models (a size fixed by the shapes, so that device memory does not grow with n_model): k_sr_prep -> k_hd_paths
+// -> k_hd_series.  Host arrays are staged per chunk; device outputs are written in place (the shocks too, when requested).
+int dfm_historical_decomposition(dfm_handle* h, const dfm_em_init* models, const double* F, const double* scale,
+                                 const dfm_hd_opts* o, const dfm_hd_out* out) {
+  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !F || !o || !out || o->N <= 0 || o->r <= 0 ||
+      o->p <= 0 || o->Tp <= 0 || o->n_model <= 0 || o->t0 < o->p - 1 || o->t0 >= o->Tp || o->n_shock < 1 || o->n_shock > o->r ||
+      (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_historical_decomposition: bad argument");
+  const int N = o->N, r = o->r, p = o->p, Tp = o->Tp, ns = o->n_shock, nc = ns + 2, k = r * p, mem = o->mem;
+  if (k > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_historical_decomposition: state dimension r*p > 48");
+  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, Tr = (size_t)Tp * r;
+  const size_t nY = (size_t)nc * Tr, nC = (size_t)N * Tp * ns, nB = (size_t)N * Tp;
+  const size_t smP = hd_paths_smem_doubles(r, p, nc) * 8;
+  // rows of the recursions staged per pass of k_hd_series: about 16 KB of shared memory in all (at least one row), so that many
+  // CTAs share an SM
+  const size_t budget = std::max<size_t>(2048, (size_t)r * HD_NS + (size_t)nc * r);
+  const int tc = (int)std::min<size_t>((size_t)Tp, (budget - (size_t)r * HD_NS) / ((size_t)nc * r));
+  const size_t smS = hd_series_smem_doubles(r, nc, tc) * 8;
+  const bool hst = mem == DFM_MEM_HOST;
+  const size_t per = 8 * (kk + 2 * rk + nY + Tr + (hst ? Nr + N + rk + rr + Tr + (out->contrib ? nC : 0) + (out->rest ? nB : 0) +
+                                                        (out->base ? nB : 0) : 0)) + 8;
+  const int nb = (int)std::min<long long>({(long long)o->n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)), 65535LL});
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    const size_t B = nb;
+    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
+           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
+           *dF = hst ? a.get<double>(B * Tr) : nullptr, *dS = hst && scale ? a.get<double>(N) : nullptr;
+    double *dC = hst && out->contrib ? a.get<double>(B * nC) : nullptr, *dRs = hst && out->rest ? a.get<double>(B * nB) : nullptr,
+           *dB = hst && out->base ? a.get<double>(B * nB) : nullptr;
+    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dE = a.get<double>(B * Tr),
+           *dY = a.get<double>(B * nY);
+    int* dst = a.get<int>(B);
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    const double* sc = scale;
+    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
+    DFM_SET_SMEM(k_hd_paths, smP);
+    // k_hd_series holds each series' loadings in RM >= r registers
+    auto series = [&](auto rm, const double* L_, const double* R_, int nm, double* oC, double* oR, double* oB) {
+      constexpr int RM = decltype(rm)::value;
+      DFM_SET_SMEM(k_hd_series<RM>, smS);
+      L(k_hd_series<RM>, (N + HD_NS - 1) / HD_NS, nm, HD_NS, smS, L_, R_, sc, (const double*)dY, (const int*)dst, N, r, Tp, ns, tc, oC,
+        oR, oB);
+    };
+    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
+      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
+      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr,
+                   *F_ = F + j0 * Tr;
+      int rc = DFM_OK;
+      if (hst) {
+        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
+        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
+        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
+        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
+        rc = stage_in(h, F_, dF, nm * Tr, mem, &F_); if (rc) return rc;
+      }
+      double* oE = out->shocks && !hst ? out->shocks + j0 * Tr : dE;
+      double* oC = out->contrib ? (hst ? dC : out->contrib + j0 * nC) : nullptr;
+      double* oR = out->rest ? (hst ? dRs : out->rest + j0 * nB) : nullptr;
+      double* oB = out->base ? (hst ? dB : out->base + j0 * nB) : nullptr;
+      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
+      L(k_hd_paths, nm, 1, HD_PT, smP, (const double*)dM, (const double*)dG, F_, r, p, Tp, o->t0, ns, dst, oE, dY);
+      if (r <= 8) series(std::integral_constant<int, 8>(), L_, R_, nm, oC, oR, oB);
+      else if (r <= 16) series(std::integral_constant<int, 16>(), L_, R_, nm, oC, oR, oB);
+      else if (r <= 32) series(std::integral_constant<int, 32>(), L_, R_, nm, oC, oR, oB);
+      else series(std::integral_constant<int, 48>(), L_, R_, nm, oC, oR, oB);
+      if (hst) {
+        rc = copy_out(h, out->shocks ? out->shocks + j0 * Tr : nullptr, dE, nm * Tr, mem); if (rc) return rc;
+        rc = copy_out(h, out->contrib ? out->contrib + j0 * nC : nullptr, dC, nm * nC, mem); if (rc) return rc;
+        rc = copy_out(h, out->rest ? out->rest + j0 * nB : nullptr, dRs, nm * nB, mem); if (rc) return rc;
+        rc = copy_out(h, out->base ? out->base + j0 * nB : nullptr, dB, nm * nB, mem); if (rc) return rc;
+      }
+      rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
       if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
     }
   }

@@ -489,6 +489,36 @@ int dfm_gibbs_constrained(dfm_handle* h, const double* X, const dfm_gibbs_opts* 
 int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r, int p, int n_model, int H, int n_shock,
                          const double* scale, int mem, double* resp, double* fevd, int* status);
 
+/* ---- historical decompositions of many models -------------------------------------------------------------------------
+ * models: n_model models (Lam N x r, R N, A = [A_1 .. A_p] r x k, Q r x r; P0 unused) back to back as dfm_em_init's batch
+ * layout, k = r p; F: n_model factor paths f_0 .. f_{Tp-1} (Tp x r each), path b belonging to model b.  Per model, L = chol(Q)
+ * (lower), M the companion matrix of A, Psi_h = [M^h]_{1:r,1:r} L (as dfm_series_responses):
+ *   structural shocks   eps_t = L^-1 (f_t - sum_{l=1..p} A_l f_{t-l})  for t >= p, NaN for t < p;
+ *   base row t0 (p - 1 <= t0 < Tp): z_t0 = [f_t0; ..; f_{t0-p+1}] lies inside the path (no pre-sample lags);
+ *   for t > t0:  contrib[i,t,j] = scale_i lam_i' sum_{s=t0+1..t} Psi_{t-s} e_j eps_{j,s}   (the leading n_shock shocks j)
+ *                rest[i,t]      = the same sum over the shocks j >= n_shock
+ *                base[i,t]      = scale_i lam_i' [M^{t-t0} z_t0]_{1:r}
+ *   for t <= t0: contrib = rest = 0, base = scale_i lam_i' f_t;
+ * so base + sum_j contrib + rest = scale_i lam_i' f_t (the common component) at every row.  Series out of the model (NaN Lam
+ * row or R_i; R is read for that test only) get NaN columns.  status [n_model]: 0, or DFM_ERR_NOT_PD when A or Q holds a NaN,
+ * Q is not positive definite or the path holds a NaN (a failed chain): that model's outputs are NaN, the others unaffected.
+ * Identification: under f -> K f with K's first row e_1' (the rotations a restriction naming factor 1 leaves free), eps_1,
+ * contrib[..., 0], rest (n_shock = 1) and base do not change; the other shocks' columns do, their sum does not.
+ * Everything column-major, models back to back, in `mem`; the models run in chunks of a size fixed by the shapes (device
+ * memory does not grow with n_model; model b has the same bits whatever n_model).  Bad arguments (a NULL required pointer,
+ * t0 outside [p - 1, Tp), n_shock outside [1, r], a bad mem): DFM_ERR_ARG; k > 48: DFM_ERR_UNSUPPORTED.  Synchronous for host
+ * memory. */
+typedef struct { int N, r, p, Tp, t0, n_shock, n_model, mem; } dfm_hd_opts;
+typedef struct {
+  double* shocks;             /* n_model x (Tp x r)              eps */
+  double* contrib;            /* n_model x (N x Tp x n_shock) */
+  double* rest;               /* n_model x (N x Tp) */
+  double* base;               /* n_model x (N x Tp) */
+  int* status;                /* [n_model] */
+} dfm_hd_out;                 /* any may be NULL */
+int dfm_historical_decomposition(dfm_handle* h, const dfm_em_init* models, const double* F, const double* scale,
+                                 const dfm_hd_opts* opts, const dfm_hd_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

@@ -385,4 +385,28 @@ function series_responses(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{Fl
     return (resp = resp, fevd = fevd, status = st)
 end
 
+struct HdOpts; N::Cint; r::Cint; p::Cint; Tp::Cint; t0::Cint; n_shock::Cint; n_model::Cint; mem::Cint; end
+struct HdOut; shocks::Ptr{Cdouble}; contrib::Ptr{Cdouble}; rest::Ptr{Cdouble}; base::Ptr{Cdouble}; status::Ptr{Cint}; end
+
+"""Historical decompositions (dfm_historical_decomposition) of B models Lam (N x r x B), R (N x B), A (r x k x B), Q (r x r x B)
+along their factor paths F (Tp x r x B) from the 0-based base row t0 (p - 1 <= t0 < Tp): shocks (Tp x r x B), contrib
+(N x Tp x n_shock x B), rest and base (N x Tp x B), status (B); `scale` (N) multiplies the series' parts (e.g. xstd)."""
+function historical_decomposition(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{Float64,3}, Q::Array{Float64,3},
+                                  F::Array{Float64,3}, t0::Integer; n_shock::Integer = size(Lam, 2), scale = nothing)
+    h = gethandle()
+    N, r, B = size(Lam); p = size(A, 2) ÷ r; Tp = size(F, 1)
+    shocks = Array{Float64}(undef, Tp, r, B); contrib = Array{Float64}(undef, N, Tp, n_shock, B)
+    rest = Array{Float64}(undef, N, Tp, B); base = similar(rest); st = Vector{Cint}(undef, B)
+    sc = scale === nothing ? Float64[] : Vector{Float64}(scale)
+    GC.@preserve Lam R A Q F shocks contrib rest base st sc begin
+        models = Ref(EmInit(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL))
+        opts = Ref(HdOpts(N, r, p, Tp, t0, n_shock, B, MEM_HOST))
+        out = Ref(HdOut(pointer(shocks), pointer(contrib), pointer(rest), pointer(base), pointer(st)))
+        check(ccall((:dfm_historical_decomposition, LIB), Cint,
+                    (Ptr{Cvoid}, Ref{EmInit}, Ptr{Cdouble}, Ptr{Cdouble}, Ref{HdOpts}, Ref{HdOut}),
+                    h, models, F, scale === nothing ? C_NULL : pointer(sc), opts, out), "dfm_historical_decomposition")
+    end
+    return (shocks = shocks, contrib = contrib, rest = rest, base = base, status = st)
+end
+
 end # module
