@@ -123,12 +123,12 @@ __device__ __forceinline__ void f2_produce(F2Ring& rg, const CUtensorMap* tmap, 
     }
 }
 
-// E pass, consumer warp cw (0..F2_NCW-1):  Z[t][:] = sum_n x[t,n] w_n Lam[n][:]  (w = rinv or 1), returns this
-// thread's share of sum x^2 w.  Period-chunk outer / series-block inner; each warp keeps the 8x8 DMMA
-// accumulators of its two row blocks in registers across all series blocks.
-template <int R>
-__device__ __forceinline__ double f2_consume_E(F2Ring& rg, int cw, int T, int N, int Tp, int Np, double* Z, const double* Lam,
-                                               const double* rinv) {
+// E pass, consumer warp cw (0..F2_NCW-1):  Z[t][:] = sum_n x[t,n] W[n][:]  (W = R^-1 Lam, pre-scaled in P0, or Lam):
+// the tile value is the A fragment as it stands, so the load -> DMMA chains carry no scalar work.  SQ: also returns
+// this thread's share of sum x^2 (the first ALS sweep).  Period-chunk outer / series-block inner; each warp keeps the
+// 8x8 DMMA accumulators of its two row blocks in registers across all series blocks.
+template <int R, bool SQ>
+__device__ __forceinline__ double f2_consume_E(F2Ring& rg, int cw, int T, int N, int Tp, int Np, double* Z, const double* W) {
   const int lane = threadIdx.x & 31, lr = lane >> 2, lc = lane & 3;
   const int nsg = (N + 8 * F2_SBS - 1) / (8 * F2_SBS), nck = (T + F2_TC - 1) / F2_TC;
   double qacc = 0.0;
@@ -148,13 +148,12 @@ __device__ __forceinline__ double f2_consume_E(F2Ring& rg, int cw, int T, int N,
         const int sb = sg * F2_SBS + sub;
         // all fragment loads of the series block first (no branches in between: the warp issues in order, so a
         // load placed after a DMMA would only start once that DMMA's operands had arrived), then the math
-        double rn[2], lm[2], av[2][F2_NRB];
+        double lm[2], av[2][F2_NRB];
 #pragma unroll
         for (int kc = 0; kc < 2; ++kc) {
           const int n = sb * 8 + kc * 4 + lc;
           const bool nok = n < N;
-          rn[kc] = nok ? (rinv ? rinv[n] : 1.0) : 0.0;
-          lm[kc] = (nok && lr < R) ? Lam[LI(n, lr)] : 0.0;
+          lm[kc] = (nok && lr < R) ? W[LI(n, lr)] : 0.0;
           const double* trow = tile + (kc * 4 + lc) * F2_TS + lr;
 #pragma unroll
           for (int j = 0; j < F2_NRB; ++j) {
@@ -166,10 +165,9 @@ __device__ __forceinline__ double f2_consume_E(F2Ring& rg, int cw, int T, int N,
         for (int kc = 0; kc < 2; ++kc)
 #pragma unroll
           for (int j = 0; j < F2_NRB; ++j) {
-            const double ar = av[kc][j] * rn[kc];
-            qacc += av[kc][j] * ar;
+            if (SQ) qacc += av[kc][j] * av[kc][j];
             asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                         : "+d"(d[j][kc][0]), "+d"(d[j][kc][1]) : "d"(ar), "d"(lm[kc]));
+                         : "+d"(d[j][kc][0]), "+d"(d[j][kc][1]) : "d"(av[kc][j]), "d"(lm[kc]));
           }
       }
       __syncwarp();
@@ -185,11 +183,12 @@ __device__ __forceinline__ double f2_consume_E(F2Ring& rg, int cw, int T, int N,
   return qacc;
 }
 
-// M pass, consumer warp cw:  Lam[n][:] <- sum_t x[t,n] Z[t][:]  (S_xf) and sxx[n] <- sum_t x[t,n]^2.
+// M pass, consumer warp cw:  Lam[n][:] <- sum_t x[t,n] Z[t][:]  (S_xf) and, if FIRST, sxx[n] <- sum_t x[t,n]^2
+// (the same in every iteration: later passes leave sxx alone and reduce 64 values per series block instead of 72).
 // Series-block outer in descending order (f2_produce) / period-chunk inner; two accumulator pairs per warp;
 // deterministic cross-warp reduction of the F2_NCW partial tiles at the end of every series block (named barrier 1).
 // A block's sums depend on its own chunks only, so the block order does not change any result.
-template <int R>
+template <int R, bool FIRST>
 __device__ __forceinline__ void f2_consume_M(F2Ring& rg, int cw, int T, int N, int Tp, int Np, const double* Z, double* Lam,
                                              double* sxx, double* part) {
   const int lane = threadIdx.x & 31, lr = lane >> 2, lc = lane & 3;
@@ -220,7 +219,7 @@ __device__ __forceinline__ void f2_consume_M(F2Ring& rg, int cw, int T, int N, i
         for (int j = 0; j < F2_NKC; ++j) { const int t0 = (cw + j * F2_NCW) * 4; av[j] = (nok && t0 + lc < len) ? trow[t0] : 0.0; }
 #pragma unroll
         for (int j = 0; j < F2_NKC; ++j) {
-          s2[sub] += av[j] * av[j];
+          if (FIRST) s2[sub] += av[j] * av[j];
           asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
                        : "+d"(d[sub][j][0]), "+d"(d[sub][j][1]) : "d"(av[j]), "d"(bv[j]));
         }
@@ -234,17 +233,19 @@ __device__ __forceinline__ void f2_consume_M(F2Ring& rg, int cw, int T, int N, i
 #pragma unroll
         for (int sub = 0; sub < F2_SBS; ++sub) {
           const int sb = sg * F2_SBS + sub;
-          double sq = s2[sub];
-          sq += __shfl_xor_sync(0xffffffffu, sq, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
           double* pb = part + (size_t)(sb & 1) * F2_NCW * 72 + cw * 72;
           double t0_ = 0.0, t1_ = 0.0;
 #pragma unroll
           for (int j = 0; j < F2_NKC; ++j) { t0_ += d[sub][j][0]; t1_ += d[sub][j][1]; d[sub][j][0] = 0.0; d[sub][j][1] = 0.0; }
           pb[2 * lane] = t0_; pb[2 * lane + 1] = t1_;
-          if (lc == 0) pb[64 + lr] = sq;
+          if (FIRST) {
+            double sq = s2[sub];
+            sq += __shfl_xor_sync(0xffffffffu, sq, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+            if (lc == 0) pb[64 + lr] = sq;
+          }
           asm volatile("bar.sync 1, %0;" ::"n"(F2_NCW * 32) : "memory");
           const int ct = cw * 32 + lane;                          // 0 .. F2_NCW*32-1
-          if (ct < 72) {
+          if (ct < (FIRST ? 72 : 64)) {
             const double* pp_ = part + (size_t)(sb & 1) * F2_NCW * 72 + ct;
             double tot_ = 0.0;
 #pragma unroll
@@ -299,7 +300,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
   double* Winf = Jinf + RR;    double* Ppinf = Winf + RR; double* IJM = Ppinf + RR;  double* Pfprev = IJM + RR;
   double* tmp = Pfprev + RR;               // 2R
   double* red = tmp + 2 * R;               // 40
-  double* scal = red + 40;                 // 8: [0]=slr [1]=ld_inf [2]=qsum
+  double* scal = red + 40;                 // 8: [0]=slr [1]=ld_inf [2]=sum x'R^-1 x [3]=ll
   int* ctl = (int*)(scal + 8);             // [0]=nE [1]=tb [2]=bad [3]=frozen [4]=turn window of the panel (f2_produce)
   double* bnd = scal + 16;                 // (3*32+1) R + RR: blk_recur workspace for 32 groups
   double* part = bnd;                                // [2][F2_NCW][72] M-pass partial accumulators: ALIASES the scan
@@ -379,10 +380,16 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
     double ll_prev = 0.0;
     for (; it < a.max_iter; ++it) {
       // ---------------------------------------------------------------- P0: prep
-      double slr_p = 0.0;
-      for (int i = DFM_TID; i < N; i += DFM_NT) { double rv = Rv[i]; rinv[i] = 1.0 / rv; slr_p += log(rv); if (!(rv > 0.0)) ctl[2] = 1; }
+      // sum log R and, from the second iteration on (the first M pass fills sxx), sum x'R^-1 x = sum_n sxx_n / R_n
+      double slr_p = 0.0, q_p = 0.0;
+      for (int i = DFM_TID; i < N; i += DFM_NT) {
+        const double rv = Rv[i], ri = 1.0 / rv;
+        rinv[i] = ri; slr_p += log(rv); if (it > 0) q_p += sxx[i] * ri;
+        if (!(rv > 0.0)) ctl[2] = 1;
+      }
       slr_p = block_sum(slr_p, red);
-      if (DFM_TID == 0) scal[0] = slr_p;
+      if (it > 0) q_p = block_sum(q_p, red);
+      if (DFM_TID == 0) { scal[0] = slr_p; scal[2] = q_p; }
       DFM_SYNC();
       {   // C = Lam' R^-1 Lam: RR outputs x (NT / RR) slices of the series range, combined in fixed order
         const int nsl = (DFM_NT >= 4 * RR) ? 4 : 1;
@@ -415,6 +422,9 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         }
         DFM_SYNC();
         for (int e = DFM_TID; e < RR; e += DFM_NT) { double s = 0.0; for (int sl = 0; sl < nsl; ++sl) s += T1[sl * RR + e]; C[e] = s; }
+        // the E pass contracts with W = R^-1 Lam: scale the loadings in place.  Nothing reads them as Lam again before
+        // the M pass overwrites them with S_xf, and the loop exits only after P9 has written the new Lam.
+        for (int e = DFM_TID; e < N * R; e += DFM_NT) { const int n = e % N, c = e / N; Lam[LI(n, c)] *= rinv[n]; }
       }
       DFM_SYNC();
       // ---- covariance chain (data independent).  Forward part: on the chain warp concurrently with the E pass;
@@ -556,14 +566,13 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         DFM_WSYNC();
       };
       // ---------------------------------------------------------------- P1: E-step contraction (panel pass 1)
-      double qacc = 0.0;
+      //   b_t = W' x_t  (W = R^-1 Lam); the data term -1/2 sum x'R^-1 x of the log-likelihood comes from sxx (P0, P9)
 #ifdef DFM_EMU
       for (int t = 0; t < T; ++t) {
         for (int c = 0; c < FZ; ++c) Z[ZI(t, c)] = 0.0;
         for (int n = 0; n < N; ++n) {
-          double x = X[(size_t)n * T + t], xr = x * rinv[n];
-          qacc += x * xr;
-          for (int c = 0; c < R; ++c) Z[ZI(t, c)] += xr * Lam[LI(n, c)];
+          double x = X[(size_t)n * T + t];
+          for (int c = 0; c < R; ++c) Z[ZI(t, c)] += x * Lam[LI(n, c)];
         }
       }
 #else
@@ -572,7 +581,7 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         // data-independent covariance chain concurrently
         const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
         if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true, &ctl[4]);
-        else if (DFM_WARP <= F2_NCW) qacc += f2_consume_E<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, rinv);
+        else if (DFM_WARP <= F2_NCW) f2_consume_E<R, false>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam);
         else {
           rg.skip(nitems);                                                   // keep the ring position in step
           chain_fwd();
@@ -634,7 +643,8 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       // which collapses to  quad_t = zf_{t-1}' K zf_{t-1} - zf_t' W zf_t  with K = M'(W - C) M.  Over the frozen
       // range (W, K constant) the sum only needs the second-moment matrix of the filtered means:
       //   sum_t quad_t = tr(K (Gf + z_{nE-1} z_{nE-1}' - z_{T-1} z_{T-1}')) - tr(W Gf),   Gf = sum_{t>=nE} zf_t zf_t'.
-      double llp = -0.5 * qacc;                              // this thread's share of -1/2 sum x' R^-1 x (E pass)
+      // plus the data term -1/2 sum x'R^-1 x (P0), on one thread; the first iteration's is added in P9
+      double llp = (it > 0 && F2_PTID == 0) ? -0.5 * scal[2] : 0.0;
       const bool gram = frozen && nE >= 1 && nE < T;
       // explicit periods t < nE: one thread per (t, component) in two stages when their (zp, d) vectors fit
       // in the idle scan workspace; otherwise (and for a chain that never froze) one thread per period
@@ -777,7 +787,6 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       }
       }
       DFM_SYNC();
-      const double ll = scal[3];
       // ---- moment sums + M-step r x r solves (all inputs are ready before the M pass): on the chain warp,
       //      concurrently with the pass
       auto mstep_small = [&]() {
@@ -841,9 +850,9 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
       for (int n = 0; n < N; ++n) {
         double s2 = 0.0, acc[R];
         for (int c = 0; c < R; ++c) acc[c] = 0.0;
-        for (int t = 0; t < T; ++t) { double x = X[(size_t)n * T + t]; s2 += x * x; for (int c = 0; c < R; ++c) acc[c] += x * Z[ZI(t, c)]; }
+        for (int t = 0; t < T; ++t) { double x = X[(size_t)n * T + t]; if (it == 0) s2 += x * x; for (int c = 0; c < R; ++c) acc[c] += x * Z[ZI(t, c)]; }
         for (int c = 0; c < R; ++c) Lam[LI(n, c)] = acc[c];
-        sxx[n] = s2;
+        if (it == 0) sxx[n] = s2;
       }
 #else
       {
@@ -853,8 +862,10 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         __syncthreads();
         const long long nitems = (long long)((N + 8 * F2_SBS - 1) / (8 * F2_SBS)) * ((T + F2_TC - 1) / F2_TC);
         if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false, &ctl[4]);
-        else if (DFM_WARP <= F2_NCW) f2_consume_M<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part);
-        else {
+        else if (DFM_WARP <= F2_NCW) {
+          if (it == 0) f2_consume_M<R, true>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part);
+          else f2_consume_M<R, false>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, nullptr, part);
+        } else {
           rg.skip(nitems);
           mstep_small();
         }
@@ -883,7 +894,13 @@ __global__ void DFM_FUSED2_BOUNDS k_em_fused2(FusedArgs a, const DFM_GRID_CONSTA
         for (int c = 0; c < R; ++c) Lam[LI(n, c)] = lam[c];
         Rv[n] = (sxx[n] - 2.0 * q1 + q2) / (double)T;
       }
+      // the data term of the first iteration's log-likelihood, now that its M pass has filled sxx (P0, P4: later ones)
+      double xrx = 0.0;
+      if (it == 0 && DFM_TID == 0) { for (int n = 0; n < N; ++n) xrx += sxx[n] * rinv[n]; }
       DFM_SYNC();
+      if (it == 0 && DFM_TID == 0) scal[3] -= 0.5 * xrx;
+      DFM_SYNC();
+      const double ll = scal[3];
       for (int e = DFM_TID; e < RR; e += DFM_NT) { M[e] = Phi[e]; Q[e] = Pn[e]; }
       if (DFM_TID == 0) a.loglik[(size_t)b * a.max_iter + it] = ll;
       DFM_SYNC();
@@ -954,8 +971,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
   const int Tp = pad4mod16(T), Np = pad4mod16(N);
   double* Z = sm;                          // [FZ][Tp]
   double* Lam = Z + (size_t)FZ * Tp;       // [R][Np]
-  double* sxx = Lam + (size_t)R * Np;      // [N]
-  double* FtF = sxx + N;  double* Gi = FtF + RR;  double* LtL = Gi + RR;  double* Hi = LtL + RR;
+  double* FtF = Lam + (size_t)R * Np;  double* Gi = FtF + RR;  double* LtL = Gi + RR;  double* Hi = LtL + RR;
   double* tmp = Hi + RR;                   // 2R
   double* red = tmp + 2 * R;               // 40
   int* ctl = (int*)(red + 40);             // [0] = bad, [1] = turn window of the panel (f2_produce)
@@ -982,7 +998,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
     if (DFM_TID == 0) ctl[1] = f2_round_win(a.l2_win, a.B, b);
 #endif
     DFM_SYNC();
-    double ssr = 0.0, ssr_old = 0.0;
+    double ssr = 0.0, ssr_old = 0.0, tss = 0.0;              // tss = sum x^2 of the panel, summed in the first F-step
     long long it = 0;
     int status = 0;
     while (it < a.max_iter) {
@@ -996,15 +1012,15 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
       if (DFM_WARP == 0) w_inv<R>(Gi, FtF, tmp, &ctl[0]);
 #ifdef DFM_EMU
       for (int n = 0; n < N; ++n) {
-        double s2 = 0.0, acc[R];
+        double acc[R];
         for (int c = 0; c < R; ++c) acc[c] = 0.0;
-        for (int t = 0; t < T; ++t) { double x = X[(size_t)n * T + t]; s2 += x * x; for (int c = 0; c < R; ++c) acc[c] += x * Z[ZI(t, c)]; }
+        for (int t = 0; t < T; ++t) { double x = X[(size_t)n * T + t]; for (int c = 0; c < R; ++c) acc[c] += x * Z[ZI(t, c)]; }
         for (int c = 0; c < R; ++c) Lam[LI(n, c)] = acc[c];
-        sxx[n] = s2;
       }
 #else
+      // (no sum of squares here: the first F-step sums it)
       if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/false, &ctl[1]);
-      else if (DFM_WARP <= F2_NCW) f2_consume_M<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, sxx, part);
+      else if (DFM_WARP <= F2_NCW) f2_consume_M<R, false>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, nullptr, part);
       else rg.skip(nitems);
 #endif
       DFM_SYNC();
@@ -1032,12 +1048,14 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
 #ifdef DFM_EMU
       for (int t = 0; t < T; ++t) {
         for (int c = 0; c < FZ; ++c) Z[ZI(t, c)] = 0.0;
-        for (int n = 0; n < N; ++n) { double x = X[(size_t)n * T + t]; tssp += x * x; for (int c = 0; c < R; ++c) Z[ZI(t, c)] += x * Lam[LI(n, c)]; }
+        for (int n = 0; n < N; ++n) { double x = X[(size_t)n * T + t]; if (it == 0) tssp += x * x; for (int c = 0; c < R; ++c) Z[ZI(t, c)] += x * Lam[LI(n, c)]; }
       }
 #else
       if (DFM_WARP == 0) f2_produce(rg, &tmap, b * N, T, N, /*c_outer=*/true, &ctl[1]);
-      else if (DFM_WARP <= F2_NCW) tssp += f2_consume_E<R>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam, nullptr);
-      else rg.skip(nitems);
+      else if (DFM_WARP <= F2_NCW) {
+        if (it == 0) tssp = f2_consume_E<R, true>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam);
+        else f2_consume_E<R, false>(rg, DFM_WARP - 1, T, N, Tp, Np, Z, Lam);
+      } else rg.skip(nitems);
 #endif
       DFM_SYNC();
       double bf = 0.0;
@@ -1053,8 +1071,8 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
         for (int i = 0; i < R; ++i) Z[ZI(t, i)] = f[i];
       }
       bf = block_sum(bf, red);
-      tssp = block_sum(tssp, red);
-      ssr_old = ssr; ssr = tssp - bf;
+      if (it == 0) tss = block_sum(tssp, red);
+      ssr_old = ssr; ssr = tss - bf;
       ++it;
       if (ctl[0]) { status = 3; break; }
       if (!(fabs(ssr_old - ssr) >= a.tol * (double)T * (double)N)) break;            // :367-368
@@ -1069,7 +1087,7 @@ __global__ void DFM_FUSED2_BOUNDS k_als_fused2(AlsFusedArgs a, const DFM_GRID_CO
 
 template <int R>
 inline size_t als_fused2_smem_doubles(int T, int N) {
-  return (size_t)FZ * pad4mod16(T) + (size_t)R * pad4mod16(N) + (size_t)N + 4 * (size_t)R * R + 2 * R + 48 +
+  return (size_t)FZ * pad4mod16(T) + (size_t)R * pad4mod16(N) + 4 * (size_t)R * R + 2 * R + 48 +
          2 * F2_NCW * 72 + (size_t)F2_S * F2_STG + 26;
 }
 
