@@ -84,6 +84,23 @@ class HdOut(C.Structure):
 HD_OUTPUTS = ("shocks", "contrib", "rest", "base")
 
 
+class SignOpts(C.Structure):
+    _fields_ = [("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("n_model", C.c_int), ("H", C.c_int), ("n_shock", C.c_int),
+                ("n_rot", C.c_longlong), ("n_keep", C.c_int), ("seed", C.c_ulonglong), ("mem", C.c_int)]
+
+
+class SignRestr(C.Structure):
+    _fields_ = [("n", C.c_int), ("series", c_ip), ("horizon", c_ip), ("shock", c_ip), ("sign", c_ip)]
+
+
+class SignOut(C.Structure):
+    _fields_ = [("n_accept", C.c_void_p), ("cand", C.c_void_p), ("rot", C.c_void_p), ("resp", C.c_void_p), ("fevd", C.c_void_p),
+                ("status", C.c_void_p)]
+
+
+SIGN_OUTPUTS = ("rot", "resp", "fevd")
+
+
 class SimOpts(C.Structure):
     _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("n_draw", C.c_longlong),
                 ("draw0", C.c_longlong), ("seed", C.c_ulonglong), ("mem", C.c_int)]
@@ -153,7 +170,7 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
            "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_gibbs_constrained",
-           "dfm_series_responses", "dfm_historical_decomposition", "dfm_em_init_from_factors",
+           "dfm_series_responses", "dfm_historical_decomposition", "dfm_sign_restrictions", "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
 
 
@@ -246,6 +263,8 @@ class Library:
                                             C.POINTER(LamConstr), C.POINTER(GibbsOut)]
         L.dfm_historical_decomposition.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.POINTER(HdOpts),
                                                    C.POINTER(HdOut)]
+        L.dfm_sign_restrictions.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.POINTER(SignOpts),
+                                            C.POINTER(SignRestr), C.POINTER(SignOut)]
         L.dfm_series_responses.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -489,6 +508,54 @@ class Library:
             v = a_.reshape(shape[n_])
             v = v.transpose(0, 3, 2, 1) if v.ndim == 4 else v.transpose(0, 2, 1)
             res[n_] = v if b else v[0]
+        return res
+
+    def sign_restrictions_raw(self, models, ids, N, r, p, n_model, H, n_shock, n_rot, n_keep, seed, restr, scale, mem, n_accept=0,
+                              cand=0, rot=0, resp=0, fevd=0, status=0):
+        """Pointer-level dfm_sign_restrictions (ints = device or host addresses).  models: dict Lam, R, A, Q (n_model models back to
+        back); ids: HOST uint64 array of n_model model ids or None (= 0 .. n_model-1); restr: rows (series, horizon, shock, sign),
+        four int sequences of equal length (shock 1-based); scale: address or 0 (= 1)."""
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in models.items()})
+        vp = lambda a: C.c_void_p(a) if a else None
+        rows = [np.ascontiguousarray(v, dtype=np.int32) for v in restr]
+        n = len(rows[0])
+        rp = [v.ctypes.data_as(c_ip) if n else None for v in rows]
+        rs = SignRestr(n, *rp)
+        idv = np.ascontiguousarray(ids, dtype=np.uint64) if ids is not None else None
+        o = SignOpts(N=N, r=r, p=p, n_model=n_model, H=H, n_shock=n_shock, n_rot=n_rot, n_keep=n_keep, seed=seed, mem=mem)
+        ou = SignOut(n_accept=vp(n_accept), cand=vp(cand), rot=vp(rot), resp=vp(resp), fevd=vp(fevd), status=vp(status))
+        self.check(self.lib.dfm_sign_restrictions(self.h, C.byref(ini), idv.ctypes.data_as(C.c_void_p) if idv is not None else None,
+                                                  vp(scale), C.byref(o), C.byref(rs), C.byref(ou)), "dfm_sign_restrictions")
+        del rows, idv
+
+    def sign_restrictions(self, Lam, R, A, Q, restr, H, n_rot, n_keep, n_shock=None, seed=0, ids=None, scale=None,
+                          outputs=SIGN_OUTPUTS):
+        """Candidate rotations under sign restrictions on the series responses of models (Lam (B, N, r), R (B, N), A (B, r, k),
+        Q (B, r, r)), or of one model (2-D Lam) (dfm_sign_restrictions).  restr: rows (series, horizon, shock, sign) as four int
+        sequences (series 0-based, shock 1-based).  Returns n_accept (B), cand (B, n_keep), rot (B, n_keep, r, r), resp / fevd
+        (B, n_keep, N, H, n_shock) -- those named in `outputs` -- and status (B), without the batch axis for one model.
+        n_shock defaults to the last restricted shock (1 without rows).  The arrays are views of the buffers the library wrote."""
+        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
+        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        restr = [np.asarray(v, dtype=np.int64).ravel() for v in restr]
+        if n_shock is None:
+            n_shock = int(restr[2].max()) if len(restr[2]) else 1
+        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
+        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
+        size = dict(rot=n_keep * r * r, resp=n_keep * N * H * n_shock, fevd=n_keep * N * H * n_shock)
+        outs = {n_: np.full(B * size[n_], np.nan) for n_ in outputs}
+        na = np.zeros(B, np.int64); ca = np.zeros(B * n_keep, np.int64); st = np.zeros(B, np.int32)
+        self.sign_restrictions_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, ids, N, r, p, B, H, n_shock, n_rot, n_keep, seed,
+                                   restr, sc.ctypes.data if sc is not None else 0, MEM_HOST, n_accept=na.ctypes.data,
+                                   cand=ca.ctypes.data, status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        res = dict(n_accept=na, cand=ca.reshape(B, n_keep), status=st)
+        for n_, a_ in outs.items():
+            if n_ == "rot":
+                res[n_] = a_.reshape(B, n_keep, r, r).transpose(0, 1, 3, 2)
+            else:
+                res[n_] = a_.reshape(B, n_keep, n_shock, H, N).transpose(0, 1, 4, 3, 2)
+        if not b:
+            res = {n_: (v[0] if n_ != "status" else int(v[0])) for n_, v in res.items()}
         return res
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):

@@ -600,6 +600,138 @@ def identified_history(m, shocks=1, t0=None, n_chain=4, n_burn=500, n_keep=1000,
     return out
 
 
+def _sign_rows(restrictions, ns, H, n_shock, what):
+    """[(series, shock, sign, horizons)] -> (rows as four int arrays (series, horizon, shock, sign), n_shock).  horizons: an int
+    or an inclusive (lo, hi); n_shock defaults to the last restricted shock."""
+    rows = []
+    for rs in restrictions:
+        i, j, s, hz = rs
+        lo, hi = (int(hz), int(hz)) if np.isscalar(hz) else (int(hz[0]), int(hz[1]))
+        if not 0 <= int(i) < ns:
+            raise ValueError(f"{what}: series {i} is not an estimation series (0 .. {ns - 1})")
+        if int(j) < 1 or int(s) not in (1, -1):
+            raise ValueError(f"{what}: a restriction needs a shock >= 1 and a sign of +1 or -1, got {rs}")
+        if not 0 <= lo <= hi < H:
+            raise ValueError(f"{what}: horizons {hz} outside 0 .. H-1 = {H - 1}")
+        rows += [(int(i), h, int(j), int(s)) for h in range(lo, hi + 1)]
+    if not rows:
+        raise ValueError(f"{what}: no restrictions")
+    top = max(j for _, _, j, _ in rows)
+    n_shock = top if n_shock is None else int(n_shock)
+    if top > n_shock:
+        raise ValueError(f"{what}: a restriction on shock {top} > n_shock = {n_shock}")
+    return [np.array([rw[q] for rw in rows], np.int64) for q in range(4)], n_shock
+
+
+def _sign_block(m, restrictions, H, n_shock, what, lib):
+    if H <= 0:
+        raise ValueError("H must be > 0")
+    b = _state_space_block(m, 0, lib, what)
+    rows, n_shock = _sign_rows(restrictions, b["Xs"].shape[1], H, n_shock, what)
+    r = b["em"]["Q"].shape[0]
+    if n_shock > r:
+        raise ValueError(f"{what}: n_shock = {n_shock} > r = {r}")
+    out = [int(i) for i in set(rows[0].tolist()) if np.isnan(b["Lam"][i]).any() or np.isnan(b["em"]["R"][i])]
+    if out:
+        raise ValueError(f"{what}: restricted series {sorted(out)} are out of the model")
+    return b, rows, n_shock
+
+
+def sign_identified_set(m, restrictions, H, n_shock=None, n_rot=2 ** 20, n_keep=4096, seed=20260922, q=(5, 16, 50, 84, 95),
+                        lib=None):
+    """Shocks identified by sign restrictions on the series responses of a model estimated with `estimate(m, Parametric())`, at
+    its EM estimates m.em (any Parametric fit, with or without lam_constr_em) (dfm_sign_restrictions).
+
+    restrictions: [(series, shock, sign, horizons)]: series is the 0-based position among the estimation series (the index
+    convention of LambdaConstraint.indices and of forecast's `series`), shock 1-based, sign +1 / -1, horizons an int or an
+    inclusive (lo, hi) in 0 .. H-1.  With L = chol(Q), Psi_h = [M^h]_{1:r,1:r} L and c_{i,h} = lam_i' Psi_h, candidate rotations
+    Omega are drawn from the Haar measure on the orthogonal group (n_rot per call, counter-based: candidate c is the same
+    rotation whatever n_rot); Omega is kept when, for every restricted shock j, sign * c_{i,h} omega_j is of one strict sign over
+    the shock's rows (omega_j flipped when all are negative).  The accepted set of series responses does not depend on the
+    normalisation of the factors (f -> K f), so no loading restriction is needed.
+
+    Returns a dict:
+      resp, fevd (n_kept, ns, H, n_shock)   the first n_kept = min(n_accept, n_keep) accepted rotations' series responses in data
+                                             units (xstd_i c_{i,h} Omega e_j) and variance decompositions (variance_decomposition's
+                                             on the rotated shocks);  rot (n_kept, r, r), cand (n_kept,) their Omega and ids;
+      resp_bands, fevd_bands (len(q), ns, H, n_shock)   percentiles over the kept draws (dfm_percentiles);
+      resp_lo, resp_hi, fevd_lo, fevd_hi (ns, H, n_shock)   min and max over the kept draws: an inner estimate of the identified
+                                             set at m.em;
+      n_accept, accept_rate (= n_accept / n_rot);  and series, n_shock, q, rows (the expanded (series, horizon, shock, sign)).
+    The bands describe the distribution over the identified set that the Haar prior on Omega induces at m.em, not sampling
+    uncertainty about the parameters (sign_restricted_responses adds that).  A uniform prior over rotations is not uniform over
+    the responses (Baumeister & Hamilton 2015).  n_keep <= 16384."""
+    if not 1 <= n_keep <= 16384:
+        raise ValueError("sign_identified_set: n_keep must be in [1, 16384]")
+    b, rows, n_shock = _sign_block(m, restrictions, H, n_shock, "sign_identified_set", lib)
+    lib, e = b["lib"], b["em"]
+    o = lib.sign_restrictions(b["Lam"], e["R"], e["A"], e["Q"], rows, H, n_rot, n_keep, n_shock=n_shock, seed=seed, scale=b["xstd"])
+    if o["status"] != 0:
+        raise RuntimeError(f"sign_identified_set: device status {o['status']}")
+    nk = int(min(o["n_accept"], n_keep))
+    qq = np.asarray(q, float)
+    out = dict(resp=np.ascontiguousarray(o["resp"][:nk]), fevd=np.ascontiguousarray(o["fevd"][:nk]),
+               rot=np.ascontiguousarray(o["rot"][:nk]), cand=o["cand"][:nk].copy(), n_accept=int(o["n_accept"]),
+               accept_rate=float(o["n_accept"]) / n_rot, series=b["series"], n_shock=n_shock, q=qq,
+               rows=np.stack(rows, axis=1))
+    ns = b["Xs"].shape[1]
+    for nm in ("resp", "fevd"):
+        if nk:
+            bd = lib.percentiles(out[nm].reshape(nk, -1), np.r_[qq, 0.0, 100.0]).reshape((len(qq) + 2, ns, H, n_shock))
+        else:
+            bd = np.full((len(qq) + 2, ns, H, n_shock), np.nan)
+        out[nm + "_bands"], out[nm + "_lo"], out[nm + "_hi"] = bd[:len(qq)], bd[len(qq)], bd[len(qq) + 1]
+    return out
+
+
+def sign_restricted_responses(m, restrictions, H, n_shock=None, n_chain=4, n_burn=500, n_keep=1000, thin=1, rot_per_draw=4, prior=None,
+                              seed=20260922, q=(5, 16, 50, 84, 95), chain0=0, sweep0=0, lib=None):
+    """Posterior bands of the series responses and variance decompositions of shocks identified by sign restrictions, over the
+    parameter draws of Gibbs chains (gibbs: dfm_gibbs, started at m.em, same prior and refusals: a lam_constr_em fit is refused)
+    and, per kept draw, rot_per_draw Haar candidate rotations (dfm_sign_restrictions, candidate ids keyed on the draw's
+    gibbs_id(chain, sweep)).  Every accepted (draw, rotation) pair is kept: a draw from the joint posterior under the Haar prior
+    on the rotation truncated to the sign set (Arias, Rubio-Ramirez & Waggoner 2018).  restrictions, H, n_shock: as
+    sign_identified_set.
+
+    Returns a dict:
+      resp_draws, fevd_draws (n_chain, n_keep, rot_per_draw, ns, H, n_shock)   NaN where the rotation was rejected;
+      resp_bands, fevd_bands (len(q), ns, H, n_shock)    percentiles over the accepted pairs (dfm_percentiles, NaN ignored);
+      accept (n_chain, n_keep)  accepted share of each draw's rotations;  accept_rate  over all pairs;
+      n_empty  draws with no accepted rotation;  status (n_chain), loglik (n_chain, n_burn + n_keep thin);
+      rhat dict(loglik, accept)  split-R^ over the kept draws;
+    and prior, series, n_shock, q.  n_chain n_keep rot_per_draw <= 16384."""
+    if m.em is not None and m.em.get("lam_constr") is not None:
+        raise ValueError("sign_restricted_responses: the EM of m ran under restrictions on the loadings (lam_constr_em); the sampler "
+                         "draws unrestricted loadings")
+    if rot_per_draw < 1 or not 1 <= n_chain * n_keep * rot_per_draw <= 16384:
+        raise ValueError("sign_restricted_responses: n_chain * n_keep * rot_per_draw must be in [1, 16384]")
+    b, rows, n_shock = _sign_block(m, restrictions, H, n_shock, "sign_restricted_responses", lib)
+    lib, e = b["lib"], b["em"]
+    r = e["Q"].shape[0]
+    pr = dict(_gibbs_default_prior(r)); pr.update(prior or {})
+    init = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"], P0=e["P0"])
+    o = lib.gibbs(b["Xs"], init, p=b["p"], n_chain=n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin,
+                  seed=seed, prior=pr, outputs=("Lam", "R", "A", "Q"))
+    n = n_chain * n_keep
+    kept = n_burn + thin * np.arange(1, n_keep + 1) - 1
+    ids = ((np.arange(chain0, chain0 + n_chain, dtype=np.uint64)[:, None] << np.uint64(24)) +
+           (np.uint64(sweep0) + kept.astype(np.uint64))[None, :]).ravel()              # gibbs_id(chain, kept sweep)
+    sh = lambda a_: a_.reshape((n,) + a_.shape[2:])
+    d = lib.sign_restrictions(sh(o["Lam"]), sh(o["R"]), sh(o["A"]), sh(o["Q"]), rows, H, rot_per_draw, rot_per_draw, n_shock=n_shock,
+                              seed=seed, ids=ids, scale=b["xstd"], outputs=("resp", "fevd"))
+    ns = b["Xs"].shape[1]
+    qq = np.asarray(q, float)
+    acc = d["n_accept"].reshape(n_chain, n_keep) / rot_per_draw
+    out = dict(accept=acc, accept_rate=float(acc.mean()), n_empty=int((d["n_accept"] == 0).sum()), status=o["status"], loglik=o["loglik"],
+               prior=pr, series=b["series"], n_shock=n_shock, q=qq,
+               rhat=dict(loglik=float(split_rhat(o["loglik"][:, kept])), accept=float(split_rhat(acc))))
+    for nm in ("resp", "fevd"):
+        dr = d[nm]
+        out[nm + "_draws"] = dr.reshape((n_chain, n_keep, rot_per_draw, ns, H, n_shock))
+        out[nm + "_bands"] = lib.percentiles(dr.reshape(n * rot_per_draw, -1), qq).reshape((len(qq), ns, H, n_shock))
+    return out
+
+
 def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
                          lib=None):
     """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn

@@ -18,6 +18,7 @@
 #include "dfm_kernels_gibbs.cuh"
 #include "dfm_kernels_resp.cuh"
 #include "dfm_kernels_hd.cuh"
+#include "dfm_kernels_sign.cuh"
 #include <algorithm>
 #include <cmath>
 #include <new>
@@ -2195,7 +2196,7 @@ int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r,
       double* oF = fevd ? (hst ? dFe : fevd + j0 * nout) : nullptr;
       L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
       L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)ids, dI);
-      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm, SR_NS, smR, L_, R_, sc, (const double*)dI, (const int*)dst, N, r, H, n_shock, hc, oR, oF);
+      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm, SR_NS, smR, L_, R_, sc, (const double*)dI, (const int*)dst, N, r, H, n_shock, hc, 1, oR, oF);
       if (hst) {
         rc = copy_out(h, resp ? resp + j0 * nout : nullptr, dRe, nm * nout, mem); if (rc) return rc;
         rc = copy_out(h, fevd ? fevd + j0 * nout : nullptr, dFe, nm * nout, mem); if (rc) return rc;
@@ -2281,6 +2282,125 @@ int dfm_historical_decomposition(dfm_handle* h, const dfm_em_init* models, const
         rc = copy_out(h, out->rest ? out->rest + j0 * nB : nullptr, dRs, nm * nB, mem); if (rc) return rc;
         rc = copy_out(h, out->base ? out->base + j0 * nB : nullptr, dB, nm * nB, mem); if (rc) return rc;
       }
+      rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
+      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+    }
+  }
+  return finish(h, mem);
+}
+
+// ------------------------------------------------------------------------------------ sign restrictions
+// Per chunk of models (a size fixed by the shapes): k_sr_prep -> k_irf (all r shocks) -> k_sign_prep -> per batch of candidates
+// (a size fixed by n_rot) k_sign_cand -> k_sign_pick -> k_sign_rot -> k_series_resp on the n_keep rotated records of every model.
+// Host arrays are staged per chunk; device outputs are written in place.
+int dfm_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const unsigned long long* ids, const double* scale,
+                          const dfm_sign_opts* o, const dfm_sign_restr* rs, const dfm_sign_out* out) {
+  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !o || !rs || !out || o->N <= 0 || o->r <= 0 ||
+      o->p <= 0 || o->n_model <= 0 || o->H <= 0 || o->n_shock < 1 || o->n_shock > o->r || o->n_rot < 1 || o->n_keep < 1 ||
+      rs->n < 0 || (rs->n > 0 && (!rs->series || !rs->horizon || !rs->shock || !rs->sign)) ||
+      (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: bad argument");
+  const int N = o->N, r = o->r, p = o->p, H = o->H, ns = o->n_shock, nR = rs->n, nk = o->n_keep, k = r * p, mem = o->mem;
+  for (int q = 0; q < nR; ++q)
+    if (rs->series[q] < 0 || rs->series[q] >= N || rs->horizon[q] < 0 || rs->horizon[q] >= H || rs->shock[q] < 1 ||
+        rs->shock[q] > ns || (rs->sign[q] != 1 && rs->sign[q] != -1))
+      return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: a restriction row outside its range");
+  if (ids)
+    for (int b = 0; b < o->n_model; ++b)
+      if (ids[b] >= (1ull << 40)) return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: a model id >= 2^40");
+  if (r > SG_RMAX || nR > SG_NRMAX || k > 48 || nk > kMaxGridBatch)
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_sign_restrictions: r > 16, more than 256 rows, r*p > 48 or n_keep > 65535");
+  // the rows sorted by shock (stable): shock j's rows are off[j] .. off[j+1]-1; nj = the last restricted shock + 1
+  std::vector<int> hs, hh, hg, off(ns + 1, 0);
+  int nj = 0;
+  for (int j = 1; j <= ns; ++j) {
+    for (int q = 0; q < nR; ++q)
+      if (rs->shock[q] == j) { hs.push_back(rs->series[q]); hh.push_back(rs->horizon[q]); hg.push_back(rs->sign[q]); nj = j; }
+    off[j] = (int)hs.size();
+  }
+  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nout = (size_t)N * H * ns;
+  const size_t sm0 = series_resp_smem_doubles(r, ns, 0);
+  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
+  const size_t smR = series_resp_smem_doubles(r, ns, hc) * 8, smI = irf_smem_doubles(k) * 8;
+  const size_t smC = sign_cand_smem_bytes(r, nj, nR), smT = sign_rot_smem_bytes(r, nj, nR);
+  // candidates per model and batch: whole CTAs of SG_NT, at most 2^20
+  const long long nct = std::min<long long>((o->n_rot + SG_NT - 1) / SG_NT, (1LL << 20) / SG_NT);
+  const int ntile = (int)(nct * (SG_NT / SG_TILE));
+  const bool hst = mem == DFM_MEM_HOST;
+  const size_t per = 8 * (kk + 2 * rk + rr * H + (size_t)nR * r + 2 + nk + (size_t)nk * rr * H +
+                          (hst ? Nr + N + rk + rr + (out->rot ? (size_t)nk * rr : 0) + (out->resp ? nk * nout : 0) +
+                                     (out->fevd ? nk * nout : 0) : 0)) + 4 * ((size_t)ntile + 1 + nk);
+  const int nb = (int)std::min<long long>({(long long)o->n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)),
+                                           (long long)(kMaxGridBatch / nk)});
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    const size_t B = nb;
+    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
+           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
+           *dS = hst && scale ? a.get<double>(N) : nullptr;
+    double *dRo = hst && out->rot ? a.get<double>(B * nk * rr) : nullptr, *dRe = hst && out->resp ? a.get<double>(B * nk * nout) : nullptr,
+           *dFe = hst && out->fevd ? a.get<double>(B * nk * nout) : nullptr;
+    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H),
+           *dC = a.get<double>(B * nR * r + 1), *dRec = a.get<double>(B * nk * rr * H);
+    long long *dNa = a.get<long long>(B), *dCa = a.get<long long>(B * nk);
+    unsigned long long* dId = a.get<unsigned long long>(B);
+    unsigned* dMask = a.get<unsigned>(B * ntile);
+    int *dst = a.get<int>(B), *dSst = a.get<int>(B * nk), *dIr = a.get<int>(r), *dOff = a.get<int>(ns + 1);
+    int *dRs = a.get<int>(nR + 1), *dRh = a.get<int>(nR + 1), *dRg = a.get<int>(nR + 1);
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    std::vector<int> hid(r);
+    for (int j = 0; j < r; ++j) hid[j] = j;
+    CK(cudaMemcpyAsync(dIr, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(dOff, off.data(), (ns + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    if (nR) {
+      CK(cudaMemcpyAsync(dRs, hs.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync(dRh, hh.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync(dRg, hg.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    }
+    const double* sc = scale;
+    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
+    DFM_SET_SMEM(k_series_resp, smR);
+    DFM_SET_SMEM(k_irf, smI);
+    DFM_SET_SMEM(k_sign_cand, smC);
+    DFM_SET_SMEM(k_sign_rot, smT);
+    std::vector<unsigned long long> hids(nb);
+    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
+      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
+      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr;
+      int rc = DFM_OK;
+      if (hst) {
+        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
+        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
+        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
+        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
+      }
+      for (int b = 0; b < nm; ++b) hids[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
+      CK(cudaMemcpyAsync(dId, hids.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+      double* oRo = out->rot ? (hst ? dRo : out->rot + j0 * nk * rr) : nullptr;
+      double* oRe = out->resp ? (hst ? dRe : out->resp + j0 * nk * nout) : nullptr;
+      double* oFe = out->fevd ? (hst ? dFe : out->fevd + j0 * nk * nout) : nullptr;
+      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
+      L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)dIr, dI);
+      L(k_sign_prep, nm, 1, 64, 8, L_, R_, (const double*)dI, N, r, H, nR, (const int*)dRs, (const int*)dRh, (const int*)dRg, nk, dst,
+        dC, dNa, dCa);
+      for (long long c0 = 0; c0 < o->n_rot; c0 += (long long)ntile * SG_TILE) {
+        L(k_sign_cand, ntile / (SG_NT / SG_TILE), nm, SG_NT, smC, (const double*)dC, (const int*)dOff, (const int*)dst, r, nR, nj, c0,
+          o->n_rot, ntile, o->seed, (const unsigned long long*)dId, dMask);
+        L(k_sign_pick, nm, 1, SG_PT, 2 * SG_PT * sizeof(int), (const unsigned*)dMask, ntile, c0, nk, (const int*)dst, dNa, dCa);
+      }
+      L(k_sign_rot, nm * nk, 1, 64, smT, (const double*)dI, (const double*)dC, (const int*)dOff, (const int*)dst, (const long long*)dCa,
+        r, H, nR, nj, nk, o->seed, (const unsigned long long*)dId, oRo, dRec, dSst);
+      if (oRe || oFe)
+        L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm * nk, SR_NS, smR, L_, R_, sc, (const double*)dRec, (const int*)dSst, N, r, H, ns, hc,
+          nk, oRe, oFe);
+      if (hst) {
+        rc = copy_out(h, out->rot ? out->rot + j0 * nk * rr : nullptr, dRo, nm * nk * rr, mem); if (rc) return rc;
+        rc = copy_out(h, out->resp ? out->resp + j0 * nk * nout : nullptr, dRe, nm * nk * nout, mem); if (rc) return rc;
+        rc = copy_out(h, out->fevd ? out->fevd + j0 * nk * nout : nullptr, dFe, nm * nk * nout, mem); if (rc) return rc;
+      }
+      rc = copy_out(h, out->n_accept ? out->n_accept + j0 : nullptr, dNa, nm, mem); if (rc) return rc;
+      rc = copy_out(h, out->cand ? out->cand + j0 * nk : nullptr, dCa, nm * (size_t)nk, mem); if (rc) return rc;
       rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
       if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
     }

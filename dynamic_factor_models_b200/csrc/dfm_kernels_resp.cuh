@@ -52,13 +52,14 @@ __host__ __device__ inline size_t series_resp_smem_doubles(int r, int ns, int hc
   return (size_t)(r + ns + 1) * SR_NS + (size_t)hc * r * r;
 }
 
-// grid (ceil(N / SR_NS), B), SR_NS threads.  Lam N x r, R N per model; scale N (NULL: 1); irf: k_irf's records of all r shocks,
-// [b][j][h][a] = (Psi_h)_{a j}; st: k_sr_prep's status.  resp / fevd (may be NULL): N x H x ns per model, column-major.  The
+// grid (ceil(N / SR_NS), B), SR_NS threads.  Lam N x r, R N per model, record b reading model b / ldiv (ldiv = 1: one record per
+// model; dfm_sign_restrictions: n_keep rotated records per model); scale N (NULL: 1); irf: k_irf's records of all r shocks,
+// [b][j][h][a] = (Psi_h)_{a j}; st: the records' status.  resp / fevd (may be NULL): N x H x ns per model, column-major.  The
 // CTA stages its series' loadings, then Psi in passes of hc horizons; per series the running FEV sums of its ns leading shocks
 // sit in shared memory, the running total in sD.
 __global__ void k_series_resp(const double* __restrict__ Lam, const double* __restrict__ R, const double* __restrict__ scale,
                               const double* __restrict__ irf, const int* __restrict__ st, int N, int r, int H, int ns, int hc,
-                              double* __restrict__ resp, double* __restrict__ fevd) {
+                              int ldiv, double* __restrict__ resp, double* __restrict__ fevd) {
   DFM_SMEM(sm);
   const int b = DFM_BY, i0 = DFM_BX * SR_NS;
   double* sL = sm;                                     // [r][SR_NS]  loadings, NaN: series out of the model or past N
@@ -66,7 +67,8 @@ __global__ void k_series_resp(const double* __restrict__ Lam, const double* __re
   double* sD = cum + (size_t)ns * SR_NS;               // [SR_NS]     sum_{l<=h} |c_{i,l}|^2
   double* sP = sD + SR_NS;                             // [r][hc][r]  Psi of the pass
   const bool bad = st[b] != 0;
-  const double* Lb = Lam + (size_t)b * N * r;
+  const size_t bm = (size_t)(b / ldiv);
+  const double* Lb = Lam + bm * N * r;
   const double* P = irf + (size_t)b * r * r * H;
   const size_t o0 = (size_t)b * N * H * ns;
   for (int e = DFM_TID; e < r * SR_NS; e += DFM_NT) {
@@ -85,7 +87,7 @@ __global__ void k_series_resp(const double* __restrict__ Lam, const double* __re
     for (int il = DFM_TID; il < SR_NS; il += DFM_NT) {
       const int i = i0 + il;
       if (i >= N) continue;
-      const double Ri = R[(size_t)b * N + i], sc = scale ? scale[i] : 1.0;
+      const double Ri = R[bm * N + i], sc = scale ? scale[i] : 1.0;
       bool in = !bad && !is_nan(Ri);
       for (int a = 0; a < r; ++a) if (is_nan(sL[(size_t)a * SR_NS + il])) in = false;
       double den = sD[il];

@@ -519,6 +519,58 @@ typedef struct {
 int dfm_historical_decomposition(dfm_handle* h, const dfm_em_init* models, const double* F, const double* scale,
                                  const dfm_hd_opts* opts, const dfm_hd_out* out);
 
+/* ---- shocks identified by sign restrictions on series responses ------------------------------------------------------
+ * models: n_model models (Lam N x r, R N, A r x k, Q r x r; P0 unused) as dfm_series_responses, k = r p; ids: HOST array of
+ * n_model model ids < 2^40 (NULL = 0 .. n_model-1; the Gibbs path passes gibbs_id(chain, sweep)); scale: N in `mem` (NULL = 1).
+ * Per model b, L = chol(Q), Psi_h = [M^h]_{1:r,1:r} L and c_{i,h} = lam_i' Psi_h (1 x r), as dfm_series_responses.
+ *   Rows rho = (series i, horizon h, shock j, sign s): 0 <= i < N, 0 <= h < H, 1 <= j <= n_shock, s = +1 or -1 (a horizon
+ *   range is several rows).
+ *   Candidate c (0 <= c < n_rot): Z r x r, Z[a, j] = normal number c r^2 + a + r j of the Philox stream of id_b, tag 18;
+ *   Omega = Q_Z diag(sign(diag R_Z)) from the QR of Z (Haar distributed; column j depends on Z's columns 0..j only).
+ *   Acceptance: for each shock j with rows, v_rho = s_rho c_{i_rho,h_rho} omega_j over its rows; all v > 0: kept; all v < 0:
+ *   omega_j -> -omega_j and kept; otherwise the candidate is rejected (strict inequalities).  Shocks without rows are kept as
+ *   drawn.
+ * Outputs per model (any pointer may be NULL; in `mem`, models back to back, column-major):
+ *   n_accept [n_model]                  accepted candidates among the n_rot;
+ *   cand     [n_model x n_keep]         the first n_keep accepted candidates in candidate order, -1 for an empty slot;
+ *   rot      n_keep x (r x r)           their Omega (flips applied);
+ *   resp     n_keep x (N x H x n_shock) scale_i c_{i,h} Omega e_j;
+ *   fevd     n_keep x (N x H x n_shock) sum_{l<=h} (c_{i,l} Omega e_j)^2 / (sum_{l<=h} |c_{i,l}|^2 + R_i) (dfm_series_responses on
+ *                                       the records Psi_h Omega; the denominator does not depend on Omega);
+ *   status   [n_model]                  0; DFM_ERR_NOT_PD when A or Q holds a NaN or Q is not positive definite; DFM_ERR_ARG when a
+ *                                       restricted series is out of the model (NaN loading row or R_i).  Such a model accepts
+ *                                       nothing; its neighbours are unaffected.
+ * Empty slots have NaN rot, resp and fevd; series out of the model NaN resp and fevd columns.  Under f -> K f the accepted set
+ * of series responses does not change (DESIGN.md 4.14).  The models run in chunks and the candidates in batches whose sizes
+ * depend only on the shapes: device memory grows with neither n_model nor n_rot, and model b has the same bits whatever
+ * n_model.  Bounds: r <= 16 (the candidates' columns live in shared memory), n <= 256 rows, k <= 48, n_keep <= 65535:
+ * DFM_ERR_UNSUPPORTED past them.  Bad arguments (a NULL required pointer, a row outside its range, n_shock outside [1, r],
+ * n_rot < 1, n_keep < 1, an id >= 2^40, a bad mem): DFM_ERR_ARG.  Synchronous for host memory. */
+typedef struct {
+  int N, r, p, n_model, H, n_shock;
+  long long n_rot;            /* candidates per model, >= 1 */
+  int n_keep;                 /* kept slots per model, >= 1 */
+  unsigned long long seed;
+  int mem;
+} dfm_sign_opts;
+typedef struct {
+  int n;                      /* rows, 0 .. 256; HOST arrays of n (NULL when n = 0) */
+  const int* series;          /* 0-based series i */
+  const int* horizon;         /* 0 .. H-1 */
+  const int* shock;           /* 1 .. n_shock */
+  const int* sign;            /* +1 or -1 */
+} dfm_sign_restr;
+typedef struct {
+  long long* n_accept;
+  long long* cand;
+  double* rot;
+  double* resp;
+  double* fevd;
+  int* status;
+} dfm_sign_out;
+int dfm_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const unsigned long long* ids, const double* scale,
+                          const dfm_sign_opts* opts, const dfm_sign_restr* restr, const dfm_sign_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

@@ -409,4 +409,35 @@ function historical_decomposition(Lam::Array{Float64,3}, R::Matrix{Float64}, A::
     return (shocks = shocks, contrib = contrib, rest = rest, base = base, status = st)
 end
 
+struct SignOpts; N::Cint; r::Cint; p::Cint; n_model::Cint; H::Cint; n_shock::Cint; n_rot::Clonglong; n_keep::Cint; seed::Culonglong; mem::Cint; end
+struct SignRestr; n::Cint; series::Ptr{Cint}; horizon::Ptr{Cint}; shock::Ptr{Cint}; sign::Ptr{Cint}; end
+struct SignOut; n_accept::Ptr{Clonglong}; cand::Ptr{Clonglong}; rot::Ptr{Cdouble}; resp::Ptr{Cdouble}; fevd::Ptr{Cdouble}; status::Ptr{Cint}; end
+
+"""Shocks identified by sign restrictions (dfm_sign_restrictions) on B models Lam (N x r x B), R (N x B), A (r x k x B),
+Q (r x r x B).  rows: (series, horizon, shock, sign) tuples, series and horizon 0-based, shock 1-based, sign +1 / -1.  Returns
+n_accept (B), cand (n_keep x B, -1 for an empty slot), rot (r x r x n_keep x B), resp and fevd (N x H x n_shock x n_keep x B),
+status (B); `scale` (N) multiplies resp (e.g. xstd); `ids` (B) the models' ids (default 0 .. B-1)."""
+function sign_restrictions(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{Float64,3}, Q::Array{Float64,3}, rows, H::Integer,
+                           n_rot::Integer, n_keep::Integer; n_shock::Integer = maximum(r_[3] for r_ in rows), seed::Integer = 0,
+                           ids = nothing, scale = nothing)
+    h = gethandle()
+    N, r, B = size(Lam); p = size(A, 2) ÷ r
+    rs = Cint[r_[1] for r_ in rows]; rh = Cint[r_[2] for r_ in rows]; rj = Cint[r_[3] for r_ in rows]; rg = Cint[r_[4] for r_ in rows]
+    na = Vector{Clonglong}(undef, B); cand = Array{Clonglong}(undef, n_keep, B); rot = Array{Float64}(undef, r, r, n_keep, B)
+    resp = Array{Float64}(undef, N, H, n_shock, n_keep, B); fevd = similar(resp); st = Vector{Cint}(undef, B)
+    sc = scale === nothing ? Float64[] : Vector{Float64}(scale)
+    iv = ids === nothing ? Culonglong[] : Vector{Culonglong}(ids)
+    GC.@preserve Lam R A Q rs rh rj rg na cand rot resp fevd st sc iv begin
+        models = Ref(EmInit(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL))
+        opts = Ref(SignOpts(N, r, p, B, H, n_shock, n_rot, n_keep, seed, MEM_HOST))
+        rr = Ref(SignRestr(length(rows), pointer(rs), pointer(rh), pointer(rj), pointer(rg)))
+        out = Ref(SignOut(pointer(na), pointer(cand), pointer(rot), pointer(resp), pointer(fevd), pointer(st)))
+        check(ccall((:dfm_sign_restrictions, LIB), Cint,
+                    (Ptr{Cvoid}, Ref{EmInit}, Ptr{Culonglong}, Ptr{Cdouble}, Ref{SignOpts}, Ref{SignRestr}, Ref{SignOut}),
+                    h, models, ids === nothing ? C_NULL : pointer(iv), scale === nothing ? C_NULL : pointer(sc), opts, rr, out),
+              "dfm_sign_restrictions")
+    end
+    return (n_accept = na, cand = cand, rot = rot, resp = resp, fevd = fevd, status = st)
+end
+
 end # module
