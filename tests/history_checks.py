@@ -5,7 +5,6 @@ import numpy as np
 from dynamic_factor_models_b200 import DFMError
 from dynamic_factor_models_b200._lib import MEM_DEVICE, MEM_HOST, to_cm
 import history_oracle as HO
-from oracle import kalman_em as K
 
 NAMES = ("shocks", "contrib", "rest", "base")
 
@@ -16,9 +15,7 @@ def models(r, p, N, Tp, B, seed):
     Lam = rng.standard_normal((B, N, r)); R = 0.5 + rng.random((B, N))
     A = np.empty((B, r, r * p)); Q = np.empty((B, r, r)); F = np.empty((B, Tp, r))
     for b in range(B):
-        a = rng.standard_normal((r, r * p)) / np.sqrt(r * p)
-        rho = np.max(np.abs(np.linalg.eigvals(K.companion(a, r, p))))
-        A[b] = a * (0.95 / rho if rho > 0.95 else 1.0)
+        A[b] = HO.stable_lags(rng.standard_normal((r, r * p)) / np.sqrt(r * p), p, 0.95)
         G = rng.standard_normal((r, r))
         Q[b] = G @ G.T / r + 0.5 * np.eye(r)
         F[b] = HO.simulate(Lam[b], A[b], Q[b], p, Tp, p - 1, rng)[0]

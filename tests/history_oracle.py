@@ -67,6 +67,20 @@ def decompose(Lam, R, A, Q, F, p, t0, n_shock=None, scale=None):
     return E, contrib, rest, base, 0
 
 
+def stable_lags(A, p, rho_max):
+    """A = [A_1 .. A_p] (r x r p) with lag block l multiplied by c^l, c = rho_max / rho (when the companion spectral radius rho
+    exceeds rho_max): every companion eigenvalue is multiplied by c, so the result has spectral radius <= rho_max.  (Scaling all
+    of A by c does not scale the eigenvalues for p > 1.)"""
+    A = np.asarray(A, float); r = A.shape[0]
+    rho = np.max(np.abs(np.linalg.eigvals(K.companion(A, r, p))))
+    if rho <= rho_max:
+        return A.copy()
+    c = rho_max / rho
+    out = np.hstack([A[:, (l - 1) * r:l * r] * c ** l for l in range(1, p + 1)])
+    assert np.max(np.abs(np.linalg.eigvals(K.companion(out, r, p)))) <= rho_max * (1 + 1e-9)
+    return out
+
+
 def rotate_path(F, Km):
     """The path of the model f -> K f (identified_oracle.rotate gives the parameters)."""
     return np.asarray(F, float) @ np.asarray(Km, float).T

@@ -6,8 +6,8 @@ import numpy as np
 
 from dynamic_factor_models_b200 import DFMError
 from dynamic_factor_models_b200._lib import MEM_DEVICE, MEM_HOST, EmInit, SignOpts, SignOut, SignRestr, to_cm
+import history_oracle as HO
 import sign_oracle as SO
-from oracle import kalman_em as K
 
 NAMES = ("rot", "resp", "fevd")
 
@@ -18,9 +18,7 @@ def models(r, p, N, B, seed):
     Lam = rng.standard_normal((B, N, r)); R = 0.5 + rng.random((B, N))
     A = np.empty((B, r, r * p)); Q = np.empty((B, r, r))
     for b in range(B):
-        a = rng.standard_normal((r, r * p)) / np.sqrt(r * p)
-        rho = np.max(np.abs(np.linalg.eigvals(K.companion(a, r, p))))
-        A[b] = a * (0.95 / rho if rho > 0.95 else 1.0)
+        A[b] = HO.stable_lags(rng.standard_normal((r, r * p)) / np.sqrt(r * p), p, 0.95)
         G = rng.standard_normal((r, r))
         Q[b] = G @ G.T / r + 0.5 * np.eye(r)
     return Lam, R, A, Q, 0.5 + rng.random(N)

@@ -10,11 +10,7 @@ import identified_oracle as IO
 
 def stable_model(r, p, N, rng):
     """A stationary VAR(p) (companion spectral radius 0.9), a well-conditioned Q, loadings and variances."""
-    from oracle import kalman_em as K
-    A = rng.standard_normal((r, r * p)) / np.sqrt(r * p)
-    rho = np.max(np.abs(np.linalg.eigvals(K.companion(A, r, p))))
-    if rho > 0.9:
-        A *= 0.9 / rho
+    A = HO.stable_lags(rng.standard_normal((r, r * p)) / np.sqrt(r * p), p, 0.9)
     B = rng.standard_normal((r, r))
     Q = B @ B.T / r + 0.5 * np.eye(r)
     return rng.standard_normal((N, r)), 0.5 + rng.random(N), A, Q
