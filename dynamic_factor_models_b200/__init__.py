@@ -15,6 +15,7 @@ from .api import (  # noqa: F401
     standardize_data, pca_score, em_kalman, em_init_from_factors, set_default_library, get_library,
     kalman_smooth, forecast, posterior_draws, forecast_bands, news, parametric_irf, parametric_bootstrap,
     series_irf, gibbs, split_rhat, variance_decomposition, identified_responses, historical_decomposition,
-    identified_history, sign_identified_set, sign_restricted_responses,
+    identified_history, sign_identified_set, sign_restricted_responses, narrative_identified_set,
+    narrative_restricted_responses,
 )
 from . import ingest  # noqa: F401   (host-side panel ingestion: the step before the path)

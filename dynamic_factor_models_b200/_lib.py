@@ -101,6 +101,25 @@ class SignOut(C.Structure):
 SIGN_OUTPUTS = ("rot", "resp", "fevd")
 
 
+class NarrOpts(C.Structure):
+    _fields_ = [("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("n_model", C.c_int), ("H", C.c_int), ("n_shock", C.c_int),
+                ("n_rot", C.c_longlong), ("n_keep", C.c_int), ("seed", C.c_ulonglong), ("mem", C.c_int), ("Tp", C.c_int),
+                ("n_sim", C.c_int)]
+
+
+class NarrRestr(C.Structure):
+    _fields_ = [("n", C.c_int), ("kind", c_ip), ("shock", c_ip), ("series", c_ip), ("row", c_ip), ("h", c_ip), ("sign", c_ip)]
+
+
+class NarrOut(C.Structure):
+    _fields_ = [("n_accept", C.c_void_p), ("cand", C.c_void_p), ("rot", C.c_void_p), ("resp", C.c_void_p), ("fevd", C.c_void_p),
+                ("status", C.c_void_p), ("n_ok", C.c_void_p), ("weight", C.c_void_p), ("eps", C.c_void_p)]
+
+
+NARR_OUTPUTS = ("rot", "resp", "fevd", "n_ok", "weight", "eps")
+NARR_KINDS = dict(shock=0, most=1, overwhelming=2, contrib=3)
+
+
 class SimOpts(C.Structure):
     _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("n_draw", C.c_longlong),
                 ("draw0", C.c_longlong), ("seed", C.c_ulonglong), ("mem", C.c_int)]
@@ -170,8 +189,9 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
            "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_gibbs_constrained",
-           "dfm_series_responses", "dfm_historical_decomposition", "dfm_sign_restrictions", "dfm_em_init_from_factors",
-           "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_allgather_results", "dfm_shard_range"]
+           "dfm_series_responses", "dfm_historical_decomposition", "dfm_sign_restrictions", "dfm_narrative_sign_restrictions", "dfm_em_init_from_factors",
+           "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_percentiles_weighted", "dfm_allgather_results",
+           "dfm_shard_range"]
 
 
 def _ptr(a):
@@ -265,6 +285,8 @@ class Library:
                                                    C.POINTER(HdOut)]
         L.dfm_sign_restrictions.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.POINTER(SignOpts),
                                             C.POINTER(SignRestr), C.POINTER(SignOut)]
+        L.dfm_narrative_sign_restrictions.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                      C.POINTER(NarrOpts), C.POINTER(SignRestr), C.POINTER(NarrRestr), C.POINTER(NarrOut)]
         L.dfm_series_responses.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -273,6 +295,8 @@ class Library:
         L.dfm_bootstrap_irf.argtypes = [C.c_void_p, C.POINTER(BootOpts)] + [C.c_void_p] * 7 + [C.c_int, C.c_double, C.c_int, C.c_void_p,
                                                                                                C.c_void_p, C.c_void_p]
         L.dfm_percentiles.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.dfm_percentiles_weighted.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                               C.c_void_p]
         L.dfm_em_init_from_factors.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                                C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dfm_allgather_results.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong]
@@ -558,6 +582,69 @@ class Library:
             res = {n_: (v[0] if n_ != "status" else int(v[0])) for n_, v in res.items()}
         return res
 
+    def narrative_sign_restrictions_raw(self, models, F, ids, N, r, p, n_model, H, n_shock, n_rot, n_keep, seed, Tp, n_sim, restr,
+                                        narr, scale, mem, n_accept=0, cand=0, rot=0, resp=0, fevd=0, status=0, n_ok=0, weight=0, eps=0):
+        """Pointer-level dfm_narrative_sign_restrictions (ints = device or host addresses).  models, ids, restr, scale as
+        sign_restrictions_raw; F: the address of the n_model paths (Tp x r each); narr: rows (kind, shock, series, row, h, sign),
+        six int sequences of equal length (shock 1-based, row 0-based)."""
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in models.items()})
+        vp = lambda a: C.c_void_p(a) if a else None
+        rows = [np.ascontiguousarray(v, dtype=np.int32) for v in restr]
+        n = len(rows[0])
+        rs = SignRestr(n, *[v.ctypes.data_as(c_ip) if n else None for v in rows])
+        nrows = [np.ascontiguousarray(v, dtype=np.int32) for v in narr]
+        nn = len(nrows[0])
+        nr = NarrRestr(nn, *[v.ctypes.data_as(c_ip) if nn else None for v in nrows])
+        idv = np.ascontiguousarray(ids, dtype=np.uint64) if ids is not None else None
+        o = NarrOpts(N=N, r=r, p=p, n_model=n_model, H=H, n_shock=n_shock, n_rot=n_rot, n_keep=n_keep, seed=seed, mem=mem, Tp=Tp,
+                     n_sim=n_sim)
+        ou = NarrOut(n_accept=vp(n_accept), cand=vp(cand), rot=vp(rot), resp=vp(resp), fevd=vp(fevd), status=vp(status), n_ok=vp(n_ok),
+                     weight=vp(weight), eps=vp(eps))
+        self.check(self.lib.dfm_narrative_sign_restrictions(self.h, C.byref(ini), vp(F),
+                                                            idv.ctypes.data_as(C.c_void_p) if idv is not None else None, vp(scale),
+                                                            C.byref(o), C.byref(rs), C.byref(nr), C.byref(ou)),
+                   "dfm_narrative_sign_restrictions")
+        del rows, nrows, idv
+
+    def narrative_sign_restrictions(self, Lam, R, A, Q, F, restr, narr, H, n_rot, n_keep, n_shock=None, n_sim=1 << 14, seed=0, ids=None,
+                                    scale=None, outputs=NARR_OUTPUTS):
+        """Candidate rotations under sign and narrative restrictions (dfm_narrative_sign_restrictions) of models (Lam (B, N, r),
+        R (B, N), A (B, r, k), Q (B, r, r)) along their factor paths F (B, Tp, r), or of one model (2-D Lam, F (Tp, r)).  restr:
+        as sign_restrictions; narr: rows (kind, shock, series, row, h, sign) as six int sequences (kind 0..3, shock 1-based, series
+        and row 0-based).  Returns sign_restrictions' arrays and n_ok, weight (B, n_keep), eps (B, n_keep, Tp, n_shock) -- those
+        named in `outputs` -- without the batch axis for one model.  n_shock defaults to the last restricted shock of either kind."""
+        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
+        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        F = np.asarray(F, float); Tp = F.shape[-2]
+        restr = [np.asarray(v, dtype=np.int64).ravel() for v in restr]
+        narr = [np.asarray(v, dtype=np.int64).ravel() for v in narr]
+        if n_shock is None:
+            n_shock = max([1] + [int(v.max()) for v in (restr[2], narr[1]) if len(v)])
+        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
+        Fb = to_cm(F)
+        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
+        size = dict(rot=n_keep * r * r, resp=n_keep * N * H * n_shock, fevd=n_keep * N * H * n_shock, n_ok=n_keep, weight=n_keep,
+                    eps=n_keep * Tp * n_shock)
+        outs = {n_: (np.zeros(B * size[n_], np.int64) if n_ == "n_ok" else np.full(B * size[n_], np.nan)) for n_ in outputs}
+        na = np.zeros(B, np.int64); ca = np.zeros(B * n_keep, np.int64); st = np.zeros(B, np.int32)
+        self.narrative_sign_restrictions_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, Fb.ctypes.data, ids, N, r, p, B, H, n_shock,
+                                             n_rot, n_keep, seed, Tp, n_sim, restr, narr, sc.ctypes.data if sc is not None else 0,
+                                             MEM_HOST, n_accept=na.ctypes.data, cand=ca.ctypes.data, status=st.ctypes.data,
+                                             **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        res = dict(n_accept=na, cand=ca.reshape(B, n_keep), status=st)
+        for n_, a_ in outs.items():
+            if n_ == "rot":
+                res[n_] = a_.reshape(B, n_keep, r, r).transpose(0, 1, 3, 2)
+            elif n_ in ("n_ok", "weight"):
+                res[n_] = a_.reshape(B, n_keep)
+            elif n_ == "eps":
+                res[n_] = a_.reshape(B, n_keep, n_shock, Tp).transpose(0, 1, 3, 2)
+            else:
+                res[n_] = a_.reshape(B, n_keep, n_shock, H, N).transpose(0, 1, 4, 3, 2)
+        if not b:
+            res = {n_: (v[0] if n_ != "status" else int(v[0])) for n_, v in res.items()}
+        return res
+
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)
         st = (FactorStats * B)()
@@ -703,6 +790,16 @@ class Library:
         recs = np.ascontiguousarray(recs, dtype=float); n, d = recs.shape
         qq = np.ascontiguousarray(q, dtype=float); out = np.empty(len(qq) * d)
         self.check(self.lib.dfm_percentiles(self.h, _ptr(recs), n, d, _ptr(qq), len(qq), MEM_HOST, _ptr(out)), "dfm_percentiles")
+        return out.reshape(len(qq), d)
+
+    def percentiles_weighted(self, recs, w, q):
+        """recs (n, d), w (n,) -> (len(q), d): numpy.percentile(recs[ok], q, axis=0, weights=w[ok], method="inverted_cdf") per
+        column on the device, ok = a non-NaN record with 0 < w < Inf (dfm_percentiles_weighted)."""
+        recs = np.ascontiguousarray(recs, dtype=float); n, d = recs.shape
+        ww = np.ascontiguousarray(w, dtype=float).ravel()
+        qq = np.ascontiguousarray(q, dtype=float); out = np.empty(len(qq) * d)
+        self.check(self.lib.dfm_percentiles_weighted(self.h, _ptr(recs), _ptr(ww), n, d, _ptr(qq), len(qq), MEM_HOST, _ptr(out)),
+                   "dfm_percentiles_weighted")
         return out.reshape(len(qq), d)
 
     def irf(self, M, Q, G, H, shock_ids):

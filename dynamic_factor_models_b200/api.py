@@ -732,6 +732,206 @@ def sign_restricted_responses(m, restrictions, H, n_shock=None, n_chain=4, n_bur
     return out
 
 
+def _narr_rows(m, narrative, ns, H, p, what):
+    """Narrative tuples -> six int arrays (kind, shock, series, row, h, sign) for the library, rows 0-based in the estimation
+    block.  ("shock", shock, period, sign), ("most" | "overwhelming", shock, series, period, h), ("contrib", shock, series,
+    period, h, sign); periods 1-based like historical_decomposition's t0."""
+    from ._lib import NARR_KINDS
+    out = []
+    for row in narrative:
+        kd = NARR_KINDS.get(row[0]) if len(row) else None
+        size = {0: 4, 1: 5, 2: 5, 3: 6}.get(kd)
+        if kd is None or len(row) != size:
+            raise ValueError(f"{what}: narrative row {row} is not ('shock', j, period, sign), ('most' | 'overwhelming', j, series, "
+                             "period, h) or ('contrib', j, series, period, h, sign)")
+        if kd == 0:
+            j, i, per, h, s = int(row[1]), 0, int(row[2]), 0, int(row[3])
+        else:
+            j, i, per, h = int(row[1]), int(row[2]), int(row[3]), int(row[4])
+            s = int(row[5]) if kd == 3 else 1
+            if not 0 <= i < ns:
+                raise ValueError(f"{what}: narrative row {row}: series {i} is not an estimation series (0 .. {ns - 1})")
+            if not 0 <= h < H:
+                raise ValueError(f"{what}: narrative row {row}: h outside 0 .. H-1 = {H - 1}")
+        if j < 1 or s not in (1, -1):
+            raise ValueError(f"{what}: narrative row {row} needs a shock >= 1 and a sign of +1 or -1")
+        lo = m.initperiod + p
+        if per < lo or per + h > m.lastperiod:
+            raise ValueError(f"{what}: narrative row {row}: periods {per} .. {per + h} outside {lo} .. {m.lastperiod} "
+                             "(initperiod + p .. lastperiod)")
+        out.append((kd, j, i, per - m.initperiod, h, s))
+    return [np.array([rw[q] for rw in out], np.int64) for q in range(6)]
+
+
+def _narr_block(m, restrictions, narrative, H, n_shock, what, lib):
+    if H <= 0:
+        raise ValueError("H must be > 0")
+    b = _state_space_block(m, 0, lib, what)
+    ns = b["Xs"].shape[1]
+    rows, ns_sign = _sign_rows(restrictions, ns, H, None, what) if restrictions else ([np.zeros(0, np.int64)] * 4, 1)
+    narr = _narr_rows(m, narrative, ns, H, b["p"], what)
+    top = max([ns_sign] + ([int(narr[1].max())] if len(narr[1]) else []))
+    n_shock = top if n_shock is None else int(n_shock)
+    r = b["em"]["Q"].shape[0]
+    if top > n_shock:
+        raise ValueError(f"{what}: a restriction on shock {top} > n_shock = {n_shock}")
+    if n_shock > r:
+        raise ValueError(f"{what}: n_shock = {n_shock} > r = {r}")
+    used = set(rows[0].tolist()) | set(narr[2][narr[0] != 0].tolist())
+    out = [int(i) for i in used if np.isnan(b["Lam"][i]).any() or np.isnan(b["em"]["R"][i])]
+    if out:
+        raise ValueError(f"{what}: restricted series {sorted(out)} are out of the model")
+    return b, rows, narr, n_shock
+
+
+def _weighted_bands(lib, recs, w, q, shape):
+    """Weighted percentile bands of recs (n, ...) with weights w (n,) (dfm_percentiles_weighted; NaN without a counted draw)."""
+    n = recs.shape[0]
+    if n == 0 or not ((w > 0) & np.isfinite(w)).any():
+        return np.full((len(q),) + shape, np.nan)
+    return lib.percentiles_weighted(recs.reshape(n, -1), w, q).reshape((len(q),) + shape)
+
+
+def narrative_identified_set(m, restrictions, narrative, H, n_shock=None, n_rot=2 ** 20, n_keep=4096, n_sim=2 ** 14, seed=20260922,
+                             q=(5, 16, 50, 84, 95), history=False, t0=None, return_draws=False, lib=None):
+    """Shocks identified by sign restrictions plus narrative restrictions on dated episodes (Antolin-Diaz & Rubio-Ramirez 2018), at
+    the EM estimates m.em of a model estimated with `estimate(m, Parametric())` (dfm_narrative_sign_restrictions).
+
+    restrictions: sign_identified_set's (may be empty).  narrative: tuples, periods 1-based in initperiod + p .. lastperiod:
+      ("shock", j, period, sign)                 sign * eps~_{j,period} > 0;
+      ("most", j, series, period, h)             shock j contributes more than any other shock to the change of `series` over
+                                                 period .. period + h that was not forecast at period - 1 (|H_j| > max |H_k|);
+      ("overwhelming", j, series, period, h)     ... more than all the other shocks together (|H_j| > sum |H_k|);
+      ("contrib", j, series, period, h, sign)    sign * H_j > 0;
+    with H_k = historical_decomposition's contribution of shock k at period + h from base period - 1, on the rotated model.
+    The path is the smoothed factor path at m.em, so the rows restrict E[eps | data, theta^], not the shocks themselves
+    (narrative_restricted_responses restricts the path drawn with each parameter draw, a joint posterior draw).
+
+    Each kept draw is weighted by 1 / w, w the probability of the narrative event under N(0, I) shocks estimated from n_sim
+    simulations (weight = n_sim / n_ok).  Returns sign_identified_set's dict (resp, fevd, rot, cand, n_accept, accept_rate,
+    resp_lo / hi, fevd_lo / hi: the inner estimate of the identified set, unweighted) with resp_bands / fevd_bands WEIGHTED
+    (numpy's inverted_cdf rule with weights, dfm_percentiles_weighted), plus:
+      weight, n_ok (n_kept,);  ess = (sum w)^2 / sum w^2;  n_zero_omega: kept draws with n_ok = 0 (dropped from the bands);
+      eps (n_kept, T, n_shock)   the identified shocks' paths eps~_t = Omega' L^-1 (f_t - sum A_l f_{t-l}) (NaN for the first p);
+    and narrative (the library's rows: kind, shock, series, row, h, sign).
+
+    history=True adds `history`, weighted bands of the identified shocks' historical decompositions over the kept draws:
+    dfm_historical_decomposition of each kept draw's rotated model (loadings Lam L Omega, lags Omega' L^-1 A_l L Omega, Q = I
+    exactly) along its rotated path Omega' L^-1 f, from base period t0 (historical_decomposition's t0 and default), in data
+    units: contrib_bands (len(q), ns, T, n_shock), rest_bands (len(q), ns, T) (the other shocks summed), and t0, periods; with
+    return_draws=True also contrib_draws (n_kept, ns, T, n_shock) and rest_draws (n_kept, ns, T).  With t0 = period - 1, contrib
+    at `period` is the H_j of a ("most", j, series, period, 0) row times xstd.  The draws' decompositions are held in host
+    memory while the bands are taken: about 1.1 GB at n_keep = 4096, n_shock = 1 on Stock & Watson's Figure 7 block (139 series,
+    120 periods).  n_keep <= 16384."""
+    if not 1 <= n_keep <= 16384:
+        raise ValueError("narrative_identified_set: n_keep must be in [1, 16384]")
+    b, rows, narr, n_shock = _narr_block(m, restrictions, narrative, H, n_shock, "narrative_identified_set", lib)
+    lib, e = b["lib"], b["em"]
+    t0, row0, F = _history_rows(m, b, t0, "narrative_identified_set")
+    o = lib.narrative_sign_restrictions(b["Lam"], e["R"], e["A"], e["Q"], F, rows, narr, H, n_rot, n_keep, n_shock=n_shock, n_sim=n_sim,
+                                        seed=seed, scale=b["xstd"])
+    if o["status"] != 0:
+        raise RuntimeError(f"narrative_identified_set: device status {o['status']}")
+    nk = int(min(o["n_accept"], n_keep))
+    qq = np.asarray(q, float)
+    w = o["weight"][:nk].copy()
+    fin = np.isfinite(w)
+    out = dict(resp=np.ascontiguousarray(o["resp"][:nk]), fevd=np.ascontiguousarray(o["fevd"][:nk]),
+               rot=np.ascontiguousarray(o["rot"][:nk]), cand=o["cand"][:nk].copy(), n_accept=int(o["n_accept"]),
+               accept_rate=float(o["n_accept"]) / n_rot, weight=w, n_ok=o["n_ok"][:nk].copy(),
+               ess=float(w[fin].sum() ** 2 / (w[fin] ** 2).sum()) if fin.any() else 0.0, n_zero_omega=int((~fin).sum()),
+               eps=np.ascontiguousarray(o["eps"][:nk]), series=b["series"], n_shock=n_shock, q=qq,
+               rows=np.stack(rows, axis=1), narrative=np.stack(narr, axis=1))
+    ns = b["Xs"].shape[1]
+    for nm in ("resp", "fevd"):
+        shape = (ns, H, n_shock)
+        out[nm + "_bands"] = _weighted_bands(lib, out[nm], w, qq, shape)
+        lohi = lib.percentiles(out[nm].reshape(nk, -1), [0.0, 100.0]).reshape((2,) + shape) if nk else np.full((2,) + shape, np.nan)
+        out[nm + "_lo"], out[nm + "_hi"] = lohi[0], lohi[1]
+    if history:
+        out["history"] = _narr_history(lib, b, F, row0, out["rot"], w, n_shock, qq, return_draws)
+        out["history"].update(t0=t0, periods=b["periods"])
+    return out
+
+
+def _narr_history(lib, b, F, row0, rot, w, n_shock, qq, return_draws):
+    """Weighted bands of the historical decompositions of the rotated models (Lam L Omega, Omega' L^-1 A_l L Omega, I) along the
+    rotated paths Omega' L^-1 f of the kept draws rot (n, r, r), from base row row0."""
+    e = b["em"]
+    ns, T = b["Xs"].shape[1], F.shape[0]
+    n, r = rot.shape[0], rot.shape[1]
+    shape_c, shape_r = (ns, T, n_shock), (ns, T)
+    if n == 0:
+        return dict(contrib_bands=np.full((len(qq),) + shape_c, np.nan), rest_bands=np.full((len(qq),) + shape_r, np.nan))
+    Lc = np.linalg.cholesky(e["Q"]); Li = np.linalg.inv(Lc)
+    p = e["A"].shape[1] // r
+    Lam = np.einsum("ia,ab,nbc->nic", b["Lam"], Lc, rot)
+    A = np.concatenate([np.einsum("nba,bc,ncd->nad", rot, Li @ e["A"][:, l * r:(l + 1) * r] @ Lc, rot) for l in range(p)], axis=2)
+    Fr = np.einsum("tc,nca->nta", F @ Li.T, rot)
+    d = lib.historical_decomposition(Lam, np.broadcast_to(e["R"], (n, ns)), A, np.broadcast_to(np.eye(r), (n, r, r)), Fr, row0,
+                                     n_shock=n_shock, scale=b["xstd"], outputs=("contrib", "rest"))
+    if (d["status"] != 0).any():
+        raise RuntimeError(f"narrative_identified_set: device status {d['status'][d['status'] != 0][0]} in the history")
+    out = dict(contrib_bands=_weighted_bands(lib, d["contrib"], w, qq, shape_c), rest_bands=_weighted_bands(lib, d["rest"], w, qq, shape_r))
+    if return_draws:
+        out.update(contrib_draws=d["contrib"], rest_draws=d["rest"])
+    return out
+
+
+def narrative_restricted_responses(m, restrictions, narrative, H, n_shock=None, n_chain=4, n_burn=500, n_keep=1000, thin=1,
+                                   rot_per_draw=4, n_sim=2 ** 14, prior=None, seed=20260922, q=(5, 16, 50, 84, 95), chain0=0, sweep0=0,
+                                   lib=None):
+    """Posterior bands under sign and narrative restrictions: Gibbs chains (gibbs: dfm_gibbs from m.em, same prior and refusals: a
+    lam_constr_em fit is refused) record each kept draw's parameters and factor path; per kept draw, rot_per_draw Haar candidates
+    (ids keyed on gibbs_id(chain, sweep), as sign_restricted_responses) are tested against the sign rows and the narrative rows
+    evaluated on THAT draw's path, so the rows restrict the shocks of a joint posterior draw of parameters and path.  Every
+    accepted pair is kept with importance weight n_sim / n_ok (narrative_identified_set).  restrictions, narrative, H, n_shock:
+    as narrative_identified_set.
+
+    Returns a dict:
+      resp_draws, fevd_draws (n_chain, n_keep, rot_per_draw, ns, H, n_shock)   NaN where the rotation was rejected;
+      weight (n_chain, n_keep, rot_per_draw)   NaN where rejected, +Inf where no simulation satisfied the rows;
+      resp_bands, fevd_bands (len(q), ns, H, n_shock)   weighted percentiles over the accepted pairs (dfm_percentiles_weighted);
+      ess, n_zero_omega;  accept (n_chain, n_keep), accept_rate, n_empty, status (n_chain), loglik;
+      rhat dict(loglik, accept)  split-R^ over the kept draws;
+    and prior, series, n_shock, q.  n_chain n_keep rot_per_draw <= 16384 (the defaults give 16 000)."""
+    if m.em is not None and m.em.get("lam_constr") is not None:
+        raise ValueError("narrative_restricted_responses: the EM of m ran under restrictions on the loadings (lam_constr_em); the "
+                         "sampler draws unrestricted loadings")
+    if rot_per_draw < 1 or not 1 <= n_chain * n_keep * rot_per_draw <= 16384:
+        raise ValueError("narrative_restricted_responses: n_chain * n_keep * rot_per_draw must be in [1, 16384]")
+    b, rows, narr, n_shock = _narr_block(m, restrictions, narrative, H, n_shock, "narrative_restricted_responses", lib)
+    lib, e = b["lib"], b["em"]
+    r = e["Q"].shape[0]
+    pr = dict(_gibbs_default_prior(r)); pr.update(prior or {})
+    init = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"], P0=e["P0"])
+    o = lib.gibbs(b["Xs"], init, p=b["p"], n_chain=n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin,
+                  seed=seed, prior=pr, outputs=("Lam", "R", "A", "Q", "F"))
+    n = n_chain * n_keep
+    kept = n_burn + thin * np.arange(1, n_keep + 1) - 1
+    ids = ((np.arange(chain0, chain0 + n_chain, dtype=np.uint64)[:, None] << np.uint64(24)) +
+           (np.uint64(sweep0) + kept.astype(np.uint64))[None, :]).ravel()              # gibbs_id(chain, kept sweep)
+    sh = lambda a_: a_.reshape((n,) + a_.shape[2:])
+    d = lib.narrative_sign_restrictions(sh(o["Lam"]), sh(o["R"]), sh(o["A"]), sh(o["Q"]), sh(o["F"]), rows, narr, H, rot_per_draw,
+                                        rot_per_draw, n_shock=n_shock, n_sim=n_sim, seed=seed, ids=ids, scale=b["xstd"],
+                                        outputs=("resp", "fevd", "weight"))
+    ns = b["Xs"].shape[1]
+    qq = np.asarray(q, float)
+    acc = d["n_accept"].reshape(n_chain, n_keep) / rot_per_draw
+    w = d["weight"].reshape(-1)
+    fin = np.isfinite(w)
+    out = dict(accept=acc, accept_rate=float(acc.mean()), n_empty=int((d["n_accept"] == 0).sum()), status=o["status"], loglik=o["loglik"],
+               weight=d["weight"].reshape(n_chain, n_keep, rot_per_draw), prior=pr, series=b["series"], n_shock=n_shock, q=qq,
+               ess=float(w[fin].sum() ** 2 / (w[fin] ** 2).sum()) if fin.any() else 0.0,
+               n_zero_omega=int(np.isinf(w).sum()),
+               rhat=dict(loglik=float(split_rhat(o["loglik"][:, kept])), accept=float(split_rhat(acc))))
+    for nm in ("resp", "fevd"):
+        dr = d[nm]
+        out[nm + "_draws"] = dr.reshape((n_chain, n_keep, rot_per_draw, ns, H, n_shock))
+        out[nm + "_bands"] = _weighted_bands(lib, dr.reshape(n * rot_per_draw, -1), np.where(fin, w, 0.0), qq, (ns, H, n_shock))
+    return out
+
+
 def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
                          lib=None):
     """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn

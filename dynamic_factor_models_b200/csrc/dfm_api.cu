@@ -19,6 +19,7 @@
 #include "dfm_kernels_resp.cuh"
 #include "dfm_kernels_hd.cuh"
 #include "dfm_kernels_sign.cuh"
+#include "dfm_kernels_narr.cuh"
 #include <algorithm>
 #include <cmath>
 #include <new>
@@ -2408,6 +2409,197 @@ int dfm_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const unsign
   return finish(h, mem);
 }
 
+// ------------------------------------------------------------------------------------ narrative sign restrictions
+// dfm_sign_restrictions' pipeline with k_narr_prep after k_sign_prep, k_narr_cand / k_narr_rot in place of k_sign_cand /
+// k_sign_rot, and k_narr_omega -> k_narr_weight on the kept slots.  The narrative rows are sorted as the kernels read them:
+// kinds 0 and 3 by shock (stable), then kinds 1 and 2.
+int dfm_narrative_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const double* F, const unsigned long long* ids,
+                                    const double* scale, const dfm_narr_opts* o, const dfm_sign_restr* rs, const dfm_narr_restr* nr,
+                                    const dfm_narr_out* out) {
+  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !F || !o || !rs || !nr || !out || o->N <= 0 ||
+      o->r <= 0 || o->p <= 0 || o->n_model <= 0 || o->H <= 0 || o->n_shock < 1 || o->n_shock > o->r || o->n_rot < 1 ||
+      o->n_keep < 1 || o->Tp < 1 || o->n_sim < 1 || rs->n < 0 || (rs->n > 0 && (!rs->series || !rs->horizon || !rs->shock || !rs->sign)) ||
+      nr->n < 0 || (nr->n > 0 && (!nr->kind || !nr->shock || !nr->series || !nr->row || !nr->h || !nr->sign)) ||
+      (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: bad argument");
+  const int N = o->N, r = o->r, p = o->p, H = o->H, ns = o->n_shock, nR = rs->n, nN = nr->n, nk = o->n_keep, k = r * p, mem = o->mem;
+  const int Tp = o->Tp;
+  for (int q = 0; q < nR; ++q)
+    if (rs->series[q] < 0 || rs->series[q] >= N || rs->horizon[q] < 0 || rs->horizon[q] >= H || rs->shock[q] < 1 ||
+        rs->shock[q] > ns || (rs->sign[q] != 1 && rs->sign[q] != -1))
+      return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a restriction row outside its range");
+  for (int q = 0; q < nN; ++q) {
+    const int kd = nr->kind[q], hh = kd == 0 ? 0 : nr->h[q];
+    if (kd < 0 || kd > 3 || nr->shock[q] < 1 || nr->shock[q] > ns || ((kd == 0 || kd == 3) && nr->sign[q] != 1 && nr->sign[q] != -1) ||
+        (kd != 0 && (nr->series[q] < 0 || nr->series[q] >= N)) || nr->row[q] < p || hh < 0 || hh >= H || nr->row[q] + hh >= Tp)
+      return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a narrative row outside its range");
+  }
+  if (ids)
+    for (int b = 0; b < o->n_model; ++b)
+      if (ids[b] >= (1ull << 40)) return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a model id >= 2^40");
+  if (r > SG_RMAX || nR > SG_NRMAX || k > 48 || nk > kMaxGridBatch || nN > NR_NMAX || o->n_sim > (1 << 20))
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_narrative_sign_restrictions: r > 16, more than 256 sign rows or 64 narrative rows, "
+                                        "r*p > 48, n_keep > 65535 or n_sim > 2^20");
+  // the periods' union (positions), the sign rows sorted by shock, the narrative rows in the kernels' order
+  std::vector<char> inP(Tp, 0);
+  for (int q = 0; q < nN; ++q) for (int t = nr->row[q]; t <= nr->row[q] + (nr->kind[q] == 0 ? 0 : nr->h[q]); ++t) inP[t] = 1;
+  std::vector<int> pos(Tp, 0);
+  int nP = 0;
+  for (int t = 0; t < Tp; ++t) { pos[t] = nP; nP += inP[t]; }
+  if ((long long)nP * r > (1 << 14)) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_narrative_sign_restrictions: nP * r > 2^14");
+  std::vector<int> hs, hh, hg;
+  std::vector<int> off(ns + 1, 0), noff(ns + 1, 0);
+  std::vector<nr_row> rows;
+  int nT = 0, nD = 0, nC = 0;
+  auto add = [&](int q) {
+    nr_row w;
+    w.kind = nr->kind[q]; w.shock = nr->shock[q] - 1; w.series = w.kind == 0 ? 0 : nr->series[q]; w.t = nr->row[q];
+    w.h = w.kind == 0 ? 0 : nr->h[q]; w.sign = (w.kind == 1 || w.kind == 2) ? 1 : nr->sign[q];
+    w.doff = nD; nD += w.kind == 0 ? r : r * r;
+    w.pos = pos[w.t];
+    w.coff = nC; if (w.kind != 0) nC += (w.h + 1) * r;
+    rows.push_back(w);
+  };
+  for (int j = 1; j <= ns; ++j) {
+    for (int q = 0; q < nR; ++q)
+      if (rs->shock[q] == j) { hs.push_back(rs->series[q]); hh.push_back(rs->horizon[q]); hg.push_back(rs->sign[q]); nT = j; }
+    off[j] = (int)hs.size();
+    for (int q = 0; q < nN; ++q)
+      if (nr->shock[q] == j && (nr->kind[q] == 0 || nr->kind[q] == 3)) { add(q); nT = j; }
+    noff[j] = (int)rows.size();
+  }
+  for (int q = 0; q < nN; ++q) if (nr->kind[q] == 1 || nr->kind[q] == 2) add(q);
+  const bool share = (int)rows.size() > noff[ns];
+  off.resize(nT + 1); noff.resize(nT + 1);
+  const int ncol = share ? r : nT;
+  const size_t smC = narr_cand_smem_bytes(ncol, r, nT, nR, nD, nN), smT = narr_rot_smem_bytes(r, nT, nR, nD, nN);
+  const size_t smO = (size_t)nC * 8 + 8;
+  if (smC > kMaxSmem || smO > kMaxSmem)
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_narrative_sign_restrictions: the rows do not fit the kernels' shared memory");
+  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nout = (size_t)N * H * ns;
+  const size_t Tr = (size_t)Tp * r, nE = (size_t)Tp * ns;
+  const size_t sm0 = series_resp_smem_doubles(r, ns, 0);
+  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
+  const size_t smR = series_resp_smem_doubles(r, ns, hc) * 8, smI = irf_smem_doubles(k) * 8;
+  const size_t smP = ((size_t)r * k + rr + 1) * 8;
+  const long long nct = std::min<long long>((o->n_rot + SG_NT - 1) / SG_NT, (1LL << 20) / SG_NT);
+  const int ntile = (int)(nct * (SG_NT / SG_TILE));
+  const int ntl = (o->n_sim + NR_SIMT - 1) / NR_SIMT;
+  const bool hst = mem == DFM_MEM_HOST;
+  const size_t per = 8 * (kk + 2 * rk + rr * H + (size_t)nR * r + 2 + nk + (size_t)nk * rr * H + Tr + nD + 2 * (size_t)nk +
+                          (hst ? Nr + N + rk + rr + Tr + (out->rot ? (size_t)nk * rr : 0) + (out->resp ? nk * nout : 0) +
+                                     (out->fevd ? nk * nout : 0) + (out->eps ? nk * nE : 0) + (out->n_ok ? nk : 0) +
+                                     (out->weight ? nk : 0) : 0)) + 4 * ((size_t)ntile + 1 + nk);
+  const int nb = (int)std::min<long long>({(long long)o->n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)),
+                                           (long long)(kMaxGridBatch / nk)});
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    const size_t B = nb;
+    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
+           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
+           *dF = hst ? a.get<double>(B * Tr) : nullptr, *dS = hst && scale ? a.get<double>(N) : nullptr;
+    double *dRo = hst && out->rot ? a.get<double>(B * nk * rr) : nullptr, *dRe = hst && out->resp ? a.get<double>(B * nk * nout) : nullptr,
+           *dFe = hst && out->fevd ? a.get<double>(B * nk * nout) : nullptr, *dEp = hst && out->eps ? a.get<double>(B * nk * nE) : nullptr,
+           *dW = hst && out->weight ? a.get<double>(B * nk) : nullptr;
+    long long* dNo = hst && out->n_ok ? a.get<long long>(B * nk) : nullptr;
+    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H),
+           *dC = a.get<double>(B * nR * r + 1), *dRec = a.get<double>(B * nk * rr * H), *dU = a.get<double>(B * Tr),
+           *dD = a.get<double>(B * nD + 1);
+    long long *dNa = a.get<long long>(B), *dCa = a.get<long long>(B * nk);
+    unsigned long long *dId = a.get<unsigned long long>(B), *dNok = a.get<unsigned long long>(B * nk);
+    unsigned* dMask = a.get<unsigned>(B * ntile);
+    int *dst = a.get<int>(B), *dSst = a.get<int>(B * nk), *dIr = a.get<int>(r), *dOff = a.get<int>(nT + 1), *dNoff = a.get<int>(nT + 1);
+    int *dRs = a.get<int>(nR + 1), *dRh = a.get<int>(nR + 1), *dRg = a.get<int>(nR + 1);
+    nr_row* dRows = a.get<nr_row>(nN + 1);
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    std::vector<int> hid(r);
+    for (int j = 0; j < r; ++j) hid[j] = j;
+    CK(cudaMemcpyAsync(dIr, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(dOff, off.data(), (nT + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(dNoff, noff.data(), (nT + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    if (nR) {
+      CK(cudaMemcpyAsync(dRs, hs.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync(dRh, hh.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync(dRg, hg.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    }
+    if (nN) CK(cudaMemcpyAsync(dRows, rows.data(), nN * sizeof(nr_row), cudaMemcpyHostToDevice, h->stream));
+    const double* sc = scale;
+    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
+    DFM_SET_SMEM(k_series_resp, smR);
+    DFM_SET_SMEM(k_irf, smI);
+    DFM_SET_SMEM(k_narr_cand, smC);
+    DFM_SET_SMEM(k_narr_rot, smT);
+    DFM_SET_SMEM(k_narr_omega, smO);
+    std::vector<unsigned long long> hids(nb);
+    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
+      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
+      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr,
+                   *F_ = F + j0 * Tr;
+      int rc = DFM_OK;
+      if (hst) {
+        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
+        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
+        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
+        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
+        rc = stage_in(h, F_, dF, nm * Tr, mem, &F_); if (rc) return rc;
+      }
+      for (int b = 0; b < nm; ++b) hids[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
+      CK(cudaMemcpyAsync(dId, hids.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+      const size_t S = (size_t)nm * nk;
+      double* oRo = out->rot ? (hst ? dRo : out->rot + j0 * nk * rr) : nullptr;
+      double* oRe = out->resp ? (hst ? dRe : out->resp + j0 * nk * nout) : nullptr;
+      double* oFe = out->fevd ? (hst ? dFe : out->fevd + j0 * nk * nout) : nullptr;
+      double* oEp = out->eps ? (hst ? dEp : out->eps + j0 * nk * nE) : nullptr;
+      double* oW = out->weight ? (hst ? dW : out->weight + j0 * nk) : nullptr;
+      long long* oNo = out->n_ok ? (hst ? dNo : out->n_ok + j0 * nk) : nullptr;
+      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
+      L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)dIr, dI);
+      L(k_sign_prep, nm, 1, 64, 8, L_, R_, (const double*)dI, N, r, H, nR, (const int*)dRs, (const int*)dRh, (const int*)dRg, nk, dst,
+        dC, dNa, dCa);
+      L(k_narr_prep, nm, 1, NR_PT, smP, L_, R_, (const double*)dI, (const double*)dM, (const double*)dG, F_, N, r, p, H, Tp, nN,
+        (const nr_row*)dRows, nD, dst, dU, dD);
+      for (long long c0 = 0; c0 < o->n_rot; c0 += (long long)ntile * SG_TILE) {
+        L(k_narr_cand, ntile / (SG_NT / SG_TILE), nm, SG_NT, smC, (const double*)dC, (const int*)dOff, (const double*)dD,
+          (const nr_row*)dRows, (const int*)dNoff, (const int*)dst, r, nR, nD, nN, nT, ncol, c0, o->n_rot, ntile, o->seed,
+          (const unsigned long long*)dId, dMask);
+        L(k_sign_pick, nm, 1, SG_PT, 2 * SG_PT * sizeof(int), (const unsigned*)dMask, ntile, c0, nk, (const int*)dst, dNa, dCa);
+      }
+      L(k_narr_rot, nm * nk, 1, 64, smT, (const double*)dI, (const double*)dC, (const int*)dOff, (const double*)dD, (const nr_row*)dRows,
+        (const int*)dNoff, (const double*)dU, (const int*)dst, (const long long*)dCa, r, H, Tp, nR, nD, nN, nT, nk, oEp ? ns : 0,
+        o->seed, (const unsigned long long*)dId, oRo, dRec, dSst, oEp, dNok);
+      if (oRe || oFe)
+        L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm * nk, SR_NS, smR, L_, R_, sc, (const double*)dRec, (const int*)dSst, N, r, H, ns, hc,
+          nk, oRe, oFe);
+      if (nN && (oW || oNo))
+        L(k_narr_omega, nm * nk, ntl, NR_SIMT, smO, L_, (const double*)dRec, (const nr_row*)dRows, (const int*)dSst,
+          (const unsigned long long*)dId, N, r, H, nN, nC, nP, o->n_sim, nk, o->seed, dNok);
+      if (oW || oNo) {
+        if (!nN) {                                         // no narrative rows: every simulation satisfies them
+          std::vector<unsigned long long> all(S, (unsigned long long)o->n_sim);
+          CK(cudaMemcpyAsync(dNok, all.data(), S * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+          CK(cudaStreamSynchronize(h->stream));
+        }
+        L(k_narr_weight, (int)((S + NR_PT - 1) / NR_PT), 1, NR_PT, 0, (const unsigned long long*)dNok, (const int*)dSst, (int)S, o->n_sim,
+          oNo, oW);
+      }
+      if (hst) {
+        rc = copy_out(h, out->rot ? out->rot + j0 * nk * rr : nullptr, dRo, nm * nk * rr, mem); if (rc) return rc;
+        rc = copy_out(h, out->resp ? out->resp + j0 * nk * nout : nullptr, dRe, nm * nk * nout, mem); if (rc) return rc;
+        rc = copy_out(h, out->fevd ? out->fevd + j0 * nk * nout : nullptr, dFe, nm * nk * nout, mem); if (rc) return rc;
+        rc = copy_out(h, out->eps ? out->eps + j0 * nk * nE : nullptr, dEp, nm * nk * nE, mem); if (rc) return rc;
+        rc = copy_out(h, out->weight ? out->weight + j0 * nk : nullptr, dW, S, mem); if (rc) return rc;
+        rc = copy_out(h, out->n_ok ? out->n_ok + j0 * nk : nullptr, dNo, S, mem); if (rc) return rc;
+      }
+      rc = copy_out(h, out->n_accept ? out->n_accept + j0 : nullptr, dNa, nm, mem); if (rc) return rc;
+      rc = copy_out(h, out->cand ? out->cand + j0 * nk : nullptr, dCa, nm * (size_t)nk, mem); if (rc) return rc;
+      rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
+      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+    }
+  }
+  return finish(h, mem);
+}
+
 // ------------------------------------------------------------------------------------ (f)3: percentile bands
 // ------------------------------------------------------------------------------------ f4: instability tests
 int dfm_instability(dfm_handle* h, const double* data, const double* F, int T, int ns, int r, int q, int T_break, double ccut,
@@ -2478,6 +2670,34 @@ int dfm_percentiles(dfm_handle* h, const double* recs, long long n, int d, const
     CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
     DFM_SET_SMEM(k_percentiles, smem);
     L(k_percentiles, d, 1, 256, smem, r_, (int)n, d, dq, nq, (int)npad, dout);
+    if (mem == DFM_MEM_HOST) { rc = copy_out(h, out, dout, (size_t)nq * d, mem); if (rc) return rc; }
+    else CK(cudaStreamSynchronize(h->stream));                                               // (dq lives in the shared workspace)
+  }
+  return finish(h, mem);
+}
+
+int dfm_percentiles_weighted(dfm_handle* h, const double* recs, const double* w, long long n, int d, const double* q, int nq, int mem,
+                             double* out) {
+  if (!h || !recs || !w || !q || !out || n <= 0 || d <= 0 || nq <= 0 || nq > 64 || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_percentiles_weighted: bad argument");
+  for (int k = 0; k < nq; ++k)
+    if (!(q[k] >= 0.0 && q[k] <= 100.0)) return fail(h, DFM_ERR_ARG, "dfm_percentiles_weighted: q outside [0, 100]");
+  long long npad = 2; while (npad < n) npad <<= 1;
+  const size_t smem = wpercentiles_smem_bytes(npad);
+  if (smem > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_percentiles_weighted: more than 16384 replications");
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    double* dr = mem == DFM_MEM_HOST ? a.get<double>((size_t)n * d) : nullptr;
+    double* dw = mem == DFM_MEM_HOST ? a.get<double>((size_t)n) : nullptr;
+    double* dq = a.get<double>(nq); double* dout = mem == DFM_MEM_HOST ? a.get<double>((size_t)nq * d) : out;
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    const double *r_, *w_;
+    int rc = stage_in(h, recs, dr, (size_t)n * d, mem, &r_); if (rc) return rc;
+    rc = stage_in(h, w, dw, (size_t)n, mem, &w_); if (rc) return rc;
+    CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
+    DFM_SET_SMEM(k_wpercentiles, smem);
+    L(k_wpercentiles, d, 1, NR_PT, smem, r_, w_, (int)n, d, dq, nq, (int)npad, dout);
     if (mem == DFM_MEM_HOST) { rc = copy_out(h, out, dout, (size_t)nq * d, mem); if (rc) return rc; }
     else CK(cudaStreamSynchronize(h->stream));                                               // (dq lives in the shared workspace)
   }

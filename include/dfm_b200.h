@@ -571,6 +571,80 @@ typedef struct {
 int dfm_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const unsigned long long* ids, const double* scale,
                           const dfm_sign_opts* opts, const dfm_sign_restr* restr, const dfm_sign_out* out);
 
+/* ---- narrative sign restrictions (Antolin-Diaz & Rubio-Ramirez 2018) --------------------------------------------------
+ * dfm_sign_restrictions with statements about dated episodes added, and the importance weight of every kept draw.  models, ids,
+ * scale, restr and the candidates (tag 18, the same ids and Omega) as dfm_sign_restrictions; F: n_model factor paths f_0 ..
+ * f_{Tp-1} (Tp x r each, column-major, in `mem`).  Per model, with L = chol(Q), Psi_h and c_{i,h} = lam_i' Psi_h as there:
+ *   u_t = L^-1 (f_t - sum_{l=1..p} A_l f_{t-l}) (t >= p); the structural shocks eps~_t = Omega' u_t;
+ *   H_{i,k}(t, h) = sum_{l=0..h} (c_{i,l} omega_k)(omega_k' u_{t+h-l}) = omega_k' G_{i,t,h} omega_k, G = sum_l c_{i,l}' u_{t+h-l}':
+ *   the contribution of shock k to series i over rows t .. t+h, i.e. dfm_historical_decomposition's contrib[i, t+h, k] from
+ *   base row t - 1 on the model rotated by Omega' L^-1.
+ *   Narrative rows (kind, shock j, series i, row t, window h, sign s), t a 0-based row of the path, p <= t, t + h < Tp, h < H:
+ *     kind 0  shock sign          s eps~_{j,t} > 0                          (series and h unused)
+ *     kind 1  most important      |H_{i,j}(t,h)| > max_{k != j} |H_{i,k}(t,h)|   (sign unused)
+ *     kind 2  overwhelming        |H_{i,j}(t,h)| > sum_{k != j} |H_{i,k}(t,h)|   (sign unused)
+ *     kind 3  contribution sign   s H_{i,j}(t,h) > 0
+ *   Acceptance: shock by shock, as dfm_sign_restrictions: a shock's sign rows fix omega_j's orientation (4.14's flip rule) and
+ *   its kind-0 rows are tested at it; a shock with no sign rows takes its orientation from its kind-0 rows (all > 0 keep, all
+ *   < 0 flip, otherwise rejected).  H is quadratic in omega_k, so kinds 1-3 do not depend on the orientation: kind-3 rows are
+ *   tested with their shock, kinds 1 and 2 once every column of Omega is drawn (the same columns as the kept Omega).
+ *   Importance weight: the narrative event has probability w(theta, Omega) under structural shocks drawn N(0, I); conditioning
+ *   on it divides the likelihood by w, so the kept draw's weight is 1 / w.  w is estimated from n_sim simulations:
+ *   e_{k,tau} ~ N(0, 1) for every shock k and every period tau of the sorted union of the rows' periods (t for kind 0, t .. t+h
+ *   otherwise; nP of them), the rows evaluated with H^sim_{i,k} = sum_l (c_{i,l} omega_k) e_{k,t+h-l} and eps~ = e; n_ok
+ *   counts the simulations that satisfy every row and weight = n_sim / n_ok (+Inf when n_ok = 0).  e_{k,tau} of simulation s
+ *   is normal number (s nP + p) r + k of the Philox stream of the model id, tag 19 (p the position of tau; < 2^34 within the
+ *   bounds), common to every candidate of the model: the weights are a pure function of (seed, id, Omega).  With kind-0 rows
+ *   only, on K distinct (shock, period) pairs, w = 2^-K exactly.
+ *   With no narrative rows the call gives dfm_sign_restrictions' n_accept, cand, rot, resp and fevd bits, and weight 1.
+ * Outputs: those of dfm_sign_restrictions, and per kept slot (any may be NULL; in `mem`):
+ *   n_ok     [n_model x n_keep]                 the simulations that satisfy every row (0 for an empty slot);
+ *   weight   [n_model x n_keep]                 n_sim / n_ok; +Inf when n_ok = 0; NaN for an empty slot or a failed model;
+ *   eps      n_keep x (Tp x n_shock)            eps~_t of the leading n_shock shocks (NaN for t < p), column-major.
+ * status: dfm_sign_restrictions' codes, also 3 when the path holds a NaN and DFM_ERR_ARG when a narrative series (kinds 1-3) is
+ * out of the model; a model with several failures reports the first of: A or Q with a NaN or Q not positive definite (3), a sign
+ * row's series out of the model (DFM_ERR_ARG), a NaN path row (3), a narrative series out of the model (DFM_ERR_ARG).  Bounds: dfm_sign_restrictions', at most 64 narrative rows, nP r <= 2^14, n_sim <= 2^20, and the shared
+ * memory of the candidate kernel within 220 KB: (c + 1) r 64 + n r + r nK0 + r^2 nK123 doubles (c the columns drawn, r when
+ * rows of kinds 1 / 2 exist; n the sign rows; nK0, nK123 the narrative rows of kind 0 and of kinds 1-3), e.g. at r = 16 with
+ * every column drawn and 256 sign rows, 25 narrative rows of kinds 1-3; and the simulation kernel's, sum over the rows of
+ * kinds 1-3 of (h + 1) r doubles: DFM_ERR_UNSUPPORTED past them.
+ * Bad arguments (those of dfm_sign_restrictions, F NULL, Tp < 1, n_sim < 1, a kind outside 0..3, a sign other than +-1 on
+ * kinds 0 / 3, a shock outside [1, n_shock], a series outside [0, N) on kinds 1-3, t < p, h < 0, h >= H, t + h >= Tp):
+ * DFM_ERR_ARG.  Models in chunks and candidates in batches as dfm_sign_restrictions: model b has the same bits whatever n_model.
+ * Synchronous for host memory. */
+typedef struct {
+  int N, r, p, n_model, H, n_shock;
+  long long n_rot;
+  int n_keep;
+  unsigned long long seed;
+  int mem;
+  int Tp;                     /* rows of each factor path */
+  int n_sim;                  /* simulations of the weight, 1 .. 2^20 */
+} dfm_narr_opts;
+typedef struct {
+  int n;                      /* rows, 0 .. 64; HOST arrays of n (NULL when n = 0) */
+  const int* kind;            /* 0 .. 3 */
+  const int* shock;           /* 1 .. n_shock */
+  const int* series;          /* 0-based series i (kinds 1-3) */
+  const int* row;             /* 0-based row t of the path */
+  const int* h;               /* window 0 .. H-1 (kinds 1-3) */
+  const int* sign;            /* +1 or -1 (kinds 0, 3) */
+} dfm_narr_restr;
+typedef struct {
+  long long* n_accept;
+  long long* cand;
+  double* rot;
+  double* resp;
+  double* fevd;
+  int* status;
+  long long* n_ok;
+  double* weight;
+  double* eps;
+} dfm_narr_out;
+int dfm_narrative_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const double* F, const unsigned long long* ids,
+                                    const double* scale, const dfm_narr_opts* opts, const dfm_sign_restr* restr,
+                                    const dfm_narr_restr* narr, const dfm_narr_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */
@@ -619,6 +693,13 @@ int dfm_bootstrap_irf(dfm_handle* h, const dfm_boot_opts* opts, const double* F0
  * percentiles in [0, 100] (HOST array); out: nq x d row-major.  numpy.percentile's default (linear) interpolation; NaN
  * records (failed replications) are ignored.  n <= 16384. */
 int dfm_percentiles(dfm_handle* h, const double* recs, long long n, int d, const double* q, int nq, int mem, double* out);
+
+/* Weighted percentile bands: numpy.percentile(recs[ok], q, axis=0, weights=w[ok], method="inverted_cdf") per statistic, over
+ * the records ok that are not NaN and whose weight is > 0 and finite (NaN where none is).  recs as dfm_percentiles, w: n
+ * weights (both in `mem`); the cumulative weights come from a block scan, so a quantile that falls exactly on a cumulative
+ * weight may pick the neighbouring record.  n <= 16384 (as dfm_percentiles). */
+int dfm_percentiles_weighted(dfm_handle* h, const double* recs, const double* w, long long n, int d, const double* q, int nq, int mem,
+                             double* out);
 
 /* ---- (e): the single collective of the multi-GPU path ---------------------------------- */
 /* AllGather `count` doubles per rank of per-replication result records (device pointers on the

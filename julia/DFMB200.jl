@@ -440,4 +440,43 @@ function sign_restrictions(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{F
     return (n_accept = na, cand = cand, rot = rot, resp = resp, fevd = fevd, status = st)
 end
 
+
+struct NarrOpts; N::Cint; r::Cint; p::Cint; n_model::Cint; H::Cint; n_shock::Cint; n_rot::Clonglong; n_keep::Cint; seed::Culonglong; mem::Cint; Tp::Cint; n_sim::Cint; end
+struct NarrRestr; n::Cint; kind::Ptr{Cint}; shock::Ptr{Cint}; series::Ptr{Cint}; row::Ptr{Cint}; h::Ptr{Cint}; sign::Ptr{Cint}; end
+struct NarrOut; n_accept::Ptr{Clonglong}; cand::Ptr{Clonglong}; rot::Ptr{Cdouble}; resp::Ptr{Cdouble}; fevd::Ptr{Cdouble}; status::Ptr{Cint};
+               n_ok::Ptr{Clonglong}; weight::Ptr{Cdouble}; eps::Ptr{Cdouble}; end
+
+"""Narrative sign restrictions (dfm_narrative_sign_restrictions) on B models as `sign_restrictions`, along their factor paths F
+(Tp x r x B).  narr: (kind, shock, series, row, h, sign) tuples, kind 0 shock sign / 1 most important / 2 overwhelming /
+3 contribution sign, shock 1-based, series and row 0-based.  Returns sign_restrictions' fields and n_ok, weight (n_keep x B),
+eps (Tp x n_shock x n_keep x B).  Not run in this repository's tests."""
+function narrative_sign_restrictions(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{Float64,3}, Q::Array{Float64,3},
+                                     F::Array{Float64,3}, rows, narr, H::Integer, n_rot::Integer, n_keep::Integer;
+                                     n_shock::Integer = maximum(vcat([1], [r_[3] for r_ in rows], [n_[2] for n_ in narr])),
+                                     n_sim::Integer = 16384, seed::Integer = 0, ids = nothing, scale = nothing)
+    h = gethandle()
+    N, r, B = size(Lam); p = size(A, 2) ÷ r; Tp = size(F, 1)
+    rs = Cint[r_[1] for r_ in rows]; rh = Cint[r_[2] for r_ in rows]; rj = Cint[r_[3] for r_ in rows]; rg = Cint[r_[4] for r_ in rows]
+    nv = [Cint[n_[q] for n_ in narr] for q in 1:6]
+    na = Vector{Clonglong}(undef, B); cand = Array{Clonglong}(undef, n_keep, B); rot = Array{Float64}(undef, r, r, n_keep, B)
+    resp = Array{Float64}(undef, N, H, n_shock, n_keep, B); fevd = similar(resp); st = Vector{Cint}(undef, B)
+    nok = Array{Clonglong}(undef, n_keep, B); w = Array{Float64}(undef, n_keep, B); eps = Array{Float64}(undef, Tp, n_shock, n_keep, B)
+    sc = scale === nothing ? Float64[] : Vector{Float64}(scale)
+    iv = ids === nothing ? Culonglong[] : Vector{Culonglong}(ids)
+    GC.@preserve Lam R A Q F rs rh rj rg nv na cand rot resp fevd st nok w eps sc iv begin
+        models = Ref(EmInit(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL))
+        opts = Ref(NarrOpts(N, r, p, B, H, n_shock, n_rot, n_keep, seed, MEM_HOST, Tp, n_sim))
+        rr = Ref(SignRestr(length(rows), pointer(rs), pointer(rh), pointer(rj), pointer(rg)))
+        nr = Ref(NarrRestr(length(narr), pointer(nv[1]), pointer(nv[2]), pointer(nv[3]), pointer(nv[4]), pointer(nv[5]), pointer(nv[6])))
+        out = Ref(NarrOut(pointer(na), pointer(cand), pointer(rot), pointer(resp), pointer(fevd), pointer(st), pointer(nok), pointer(w),
+                          pointer(eps)))
+        check(ccall((:dfm_narrative_sign_restrictions, LIB), Cint,
+                    (Ptr{Cvoid}, Ref{EmInit}, Ptr{Cdouble}, Ptr{Culonglong}, Ptr{Cdouble}, Ref{NarrOpts}, Ref{SignRestr}, Ref{NarrRestr},
+                     Ref{NarrOut}),
+                    h, models, pointer(F), ids === nothing ? C_NULL : pointer(iv), scale === nothing ? C_NULL : pointer(sc), opts, rr, nr,
+                    out), "dfm_narrative_sign_restrictions")
+    end
+    return (n_accept = na, cand = cand, rot = rot, resp = resp, fevd = fevd, status = st, n_ok = nok, weight = w, eps = eps)
+end
+
 end # module
