@@ -793,8 +793,9 @@ class Library:
         return out.reshape(len(qq), d)
 
     def percentiles_weighted(self, recs, w, q):
-        """recs (n, d), w (n,) -> (len(q), d): numpy.percentile(recs[ok], q, axis=0, weights=w[ok], method="inverted_cdf") per
-        column on the device, ok = a non-NaN record with 0 < w < Inf (dfm_percentiles_weighted)."""
+        """recs (n, d), w (n,) -> (len(q), d): per column on the device, over the records ok (non-NaN, 0 < w < Inf) in sorted
+        order, the first whose exact cumulative weight reaches q / 100 of the total (numpy.percentile(recs[ok], q, axis=0,
+        weights=w[ok], method="inverted_cdf") without its rounding; dfm_percentiles_weighted)."""
         recs = np.ascontiguousarray(recs, dtype=float); n, d = recs.shape
         ww = np.ascontiguousarray(w, dtype=float).ravel()
         qq = np.ascontiguousarray(q, dtype=float); out = np.empty(len(qq) * d)

@@ -810,7 +810,7 @@ def narrative_identified_set(m, restrictions, narrative, H, n_shock=None, n_rot=
     Each kept draw is weighted by 1 / w, w the probability of the narrative event under N(0, I) shocks estimated from n_sim
     simulations (weight = n_sim / n_ok).  Returns sign_identified_set's dict (resp, fevd, rot, cand, n_accept, accept_rate,
     resp_lo / hi, fevd_lo / hi: the inner estimate of the identified set, unweighted) with resp_bands / fevd_bands WEIGHTED
-    (numpy's inverted_cdf rule with weights, dfm_percentiles_weighted), plus:
+    (numpy's inverted_cdf rule with weights, cumulative weights exact: dfm_percentiles_weighted), plus:
       weight, n_ok (n_kept,);  ess = (sum w)^2 / sum w^2;  n_zero_omega: kept draws with n_ok = 0 (dropped from the bands);
       eps (n_kept, T, n_shock)   the identified shocks' paths eps~_t = Omega' L^-1 (f_t - sum A_l f_{t-l}) (NaN for the first p);
     and narrative (the library's rows: kind, shock, series, row, h, sign).

@@ -12,7 +12,7 @@
 //                  for k_series_resp, and the kept draw's structural shock path
 //   k_narr_omega   one thread per simulation: the narrative rows evaluated on N(0, I) shocks -> n_ok per kept slot
 //   k_narr_weight  weight = n_sim / n_ok
-//   k_wpercentiles weighted percentiles (numpy's inverted_cdf rule with weights)
+//   k_wpercentiles weighted percentiles (the first record whose exact cumulative weight reaches q / 100 of the total)
 // H is quadratic in omega_k, so the kinds 1-3 do not depend on a column's orientation; only kind 0 joins the flip rule.
 // Explicit fma in every decision, so k_narr_cand and k_narr_rot take the same decisions.  The spec is tests/narrative_oracle.py.
 #pragma once
@@ -367,21 +367,76 @@ __global__ void k_narr_weight(const unsigned long long* __restrict__ nok, const 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Weighted percentiles over the replication axis: numpy.percentile(x, q, weights=w, method="inverted_cdf") over the counted
-// records (x not NaN, 0 < w < Inf).  recs: [n][d] row-major, w: [n]; grid = d statistics, NR_PT threads, shared npad + NR_PT
-// doubles + 1 int + npad ints.  One bitonic sort of the (value, record index) pairs per statistic (records not counted sort
-// last); the sorted values are then replaced by the weights w[index] and their inclusive scan, and per quantile the first i
-// with cum_i / cum_{m-1} >= q / 100 (at most m - 1) gives the record recs[index_i].  out: [nq][d].
+// Weighted percentiles over the replication axis, over the counted records (x not NaN, 0 < w < Inf): per quantile q, the first
+// record i in sorted order with 100 sum_{j <= i} w_j >= q sum_j w_j in exact arithmetic (numpy's inverted_cdf rule with weights,
+// without its rounding of the cumulative weights and of q / 100; with equal weights, numpy's unweighted inverted_cdf).
+// recs: [n][d] row-major, w: [n]; grid = d statistics, NR_PT threads, shared npad + 2 (NR_PT + 1) doubles + 1 int + npad ints.  One bitonic sort of the (value,
+// record index) pairs per statistic (records not counted sort last); the sorted values are then replaced by the weights
+// w[index], summed in NR_PT chunks (in both builds) as double-double sums, and the chunk totals prefix-summed the same way.  Per
+// quantile a binary search over the chunk prefixes and a walk through one chunk find i; the test of 100 times a prefix against q
+// times the total is the exact sign of a sum of eight doubles.  The sums are exact while every partial sum fits in 106 bits of the
+// smallest weight's grid (n <= 16 384 and max w / min w <= 2^36, so every narrative weight n_sim / n_ok).  out: [nq][d].
 __device__ __forceinline__ bool wp_gt(double a, double b) { return is_nan(a) ? !is_nan(b) : (!is_nan(b) && a > b); }
 
-__host__ __device__ inline size_t wpercentiles_smem_bytes(long long npad) { return (size_t)(npad + NR_PT + 1) * 8 + (size_t)npad * 4; }
+__host__ __device__ inline size_t wpercentiles_smem_bytes(long long npad) {
+  return (size_t)(npad + 2 * (NR_PT + 1) + 1) * 8 + (size_t)npad * 4;
+}
+
+// s + e = a + b exactly (Knuth's TwoSum)
+__device__ __forceinline__ void wp_two_sum(double a, double b, double& s, double& e) {
+  s = a + b;
+  const double z = s - a;
+  e = (a - (s - z)) + (b - z);
+}
+
+// (s, e) += w, renormalised so that |e| <= ulp(s) / 2: exact while s + e + w fits in 106 bits of the weights' grid
+__device__ __forceinline__ void wp_dd_add(double& s, double& e, double w) {
+  double t, err;
+  wp_two_sum(s, w, t, err);
+  err += e;
+  s = t + err;
+  e = err - (s - t);
+}
+
+// the rounded product, kept out of fma contraction (the TwoSums below need the product they are given)
+__device__ __forceinline__ double wp_mul(double a, double b) {
+#ifdef DFM_EMU
+  return a * b;
+#else
+  return __dmul_rn(a, b);
+#endif
+}
+
+// 100 (s + e) >= q (th + tl), exactly (0 <= q <= 100, 0 < s + e <= th + tl, |e| and |tl| about half an ulp of s and th):
+// a1 - p1 = fl(100 s) - fl(q th) is within 2^-50 (100 th) of the difference, so its sign decides unless it is smaller than
+// 2^-46 (100 th); then the four products split by fma and the sign of the eight-term sum from Shewchuk's grow-expansion (a
+// non-overlapping expansion has the sign of its most significant non-zero component)
+__device__ __forceinline__ bool wp_ge(double s, double e, double q, double th, double tl) {
+  const double a1 = wp_mul(100.0, s), p1 = wp_mul(q, th);
+  const double d = a1 - p1;
+  if (fabs(d) > 0x1p-46 * (100.0 * th)) return d > 0.0;
+  const double a2 = wp_mul(100.0, e), p2 = wp_mul(q, tl);
+  const double x[8] = {a1, fma(100.0, s, -a1), a2, fma(100.0, e, -a2), -p1, -fma(q, th, -p1), -p2, -fma(q, tl, -p2)};
+  double g[8];
+#pragma unroll
+  for (int a = 0; a < 8; ++a) {
+    double Q = x[a];
+#pragma unroll
+    for (int b = 0; b < a; ++b) { double t, err; wp_two_sum(Q, g[b], t, err); g[b] = err; Q = t; }
+    g[a] = Q;
+  }
+#pragma unroll
+  for (int b = 7; b >= 0; --b) if (g[b] != 0.0) return g[b] > 0.0;
+  return true;
+}
 
 __global__ void k_wpercentiles(const double* __restrict__ recs, const double* __restrict__ w, int n, int d, const double* __restrict__ q,
                                int nq, int npad, double* __restrict__ out) {
   DFM_SMEM(v);
   const int e = DFM_BX;
-  double* part = v + npad;
-  int* cnt = (int*)(part + NR_PT);
+  double* ph = v + npad;                               // [NR_PT + 1] chunk prefixes (exclusive; ph[NR_PT] the total), high parts
+  double* pl = ph + NR_PT + 1;                         //                                                                 low parts
+  int* cnt = (int*)(pl + NR_PT + 1);
   int* ix = cnt + 2;
   if (DFM_TID == 0) *cnt = 0;
   DFM_SYNC();
@@ -420,26 +475,39 @@ __global__ void k_wpercentiles(const double* __restrict__ recs, const double* __
   double* ww = v;                                      // (the values are read back from recs at the end)
   for (int i = DFM_TID; i < m; i += DFM_NT) ww[i] = w[ix[i]];
   DFM_SYNC();
-  // inclusive scan of ww[0 .. m): each thread its chunk, then the chunk totals, then the offsets
-  const int nt = DFM_NT, ch = (m + nt - 1) / nt;
-  for (int tl = DFM_TID; tl < nt; tl += DFM_NT) {
-    double acc = 0.0;
-    for (int i = tl * ch; i < m && i < (tl + 1) * ch; ++i) { acc += ww[i]; ww[i] = acc; }
-    part[tl] = acc;
+  // chunk tl holds ww[tl ch .. (tl + 1) ch): its total, then the exclusive prefixes of the totals
+  const int ch = (m + NR_PT - 1) / NR_PT;
+  for (int tl = DFM_TID; tl < NR_PT; tl += DFM_NT) {
+    double s = 0.0, el = 0.0;
+    for (int i = tl * ch; i < m && i < (tl + 1) * ch; ++i) wp_dd_add(s, el, ww[i]);
+    ph[tl + 1] = s; pl[tl + 1] = el;
   }
   DFM_SYNC();
-  if (DFM_TID == 0) { double acc = 0.0; for (int tl = 0; tl < nt; ++tl) { const double x = part[tl]; part[tl] = acc; acc += x; } }
-  DFM_SYNC();
-  for (int tl = DFM_TID; tl < nt; tl += DFM_NT)
-    if (tl > 0) for (int i = tl * ch; i < m && i < (tl + 1) * ch; ++i) ww[i] += part[tl];
+  if (DFM_TID == 0) {
+    double s = 0.0, el = 0.0;
+    for (int tl = 0; tl < NR_PT; ++tl) {
+      const double xh = ph[tl + 1], xl = pl[tl + 1];
+      ph[tl] = s; pl[tl] = el;
+      wp_dd_add(s, el, xh);
+      wp_dd_add(s, el, xl);
+    }
+    ph[NR_PT] = s; pl[NR_PT] = el;
+  }
   DFM_SYNC();
   for (int k = DFM_TID; k < nq; k += DFM_NT) {
     double r_ = DFM_NAN;
     if (m > 0) {
-      const double qq = q[k] / 100.0, tot = ww[m - 1];
-      int lo = 0, hi = m;                              // first i with ww[i] / tot >= qq
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (ww[mid] / tot >= qq) hi = mid; else lo = mid + 1; }
-      r_ = recs[(size_t)ix[lo < m ? lo : m - 1] * d + e];
+      const double qk = q[k], th = ph[NR_PT], tl_ = pl[NR_PT];
+      int lo = 0, hi = NR_PT - 1;                      // the first chunk whose inclusive prefix reaches the threshold
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (wp_ge(ph[mid + 1], pl[mid + 1], qk, th, tl_)) hi = mid; else lo = mid + 1; }
+      double s = ph[lo], el = pl[lo];
+      const int end = m < (lo + 1) * ch ? m : (lo + 1) * ch;
+      int i = lo * ch < end ? lo * ch : end - 1;
+      for (;; ++i) {                                   // (the chunk's last record reaches it: the loop ends inside the chunk)
+        wp_dd_add(s, el, ww[i]);
+        if (i >= end - 1 || wp_ge(s, el, qk, th, tl_)) break;
+      }
+      r_ = recs[(size_t)ix[i] * d + e];
     }
     out[(size_t)k * d + e] = r_;
   }

@@ -694,10 +694,13 @@ int dfm_bootstrap_irf(dfm_handle* h, const dfm_boot_opts* opts, const double* F0
  * records (failed replications) are ignored.  n <= 16384. */
 int dfm_percentiles(dfm_handle* h, const double* recs, long long n, int d, const double* q, int nq, int mem, double* out);
 
-/* Weighted percentile bands: numpy.percentile(recs[ok], q, axis=0, weights=w[ok], method="inverted_cdf") per statistic, over
- * the records ok that are not NaN and whose weight is > 0 and finite (NaN where none is).  recs as dfm_percentiles, w: n
- * weights (both in `mem`); the cumulative weights come from a block scan, so a quantile that falls exactly on a cumulative
- * weight may pick the neighbouring record.  n <= 16384 (as dfm_percentiles). */
+/* Weighted percentile bands per statistic, over the records ok that are not NaN and whose weight is > 0 and finite (NaN where
+ * none is): in sorted order, the first record i with 100 sum_{j <= i} w_j >= q sum_j w_j, decided in exact arithmetic.  This is
+ * numpy.percentile(recs[ok], q, axis=0, weights=w[ok], method="inverted_cdf") without numpy's rounding of the cumulative sums
+ * and of q / 100; with equal weights it is numpy's unweighted inverted_cdf.  The sums are exact while they fit in 106 bits of the smallest weight's grid (always for
+ * max w / min w <= 2^36, so every narrative weight n_sim / n_ok); beyond that a quantile within about 2^-100 of the total
+ * from a cumulative weight may pick the neighbouring record.  recs as dfm_percentiles, w: n weights (both in `mem`).
+ * n <= 16384 (as dfm_percentiles). */
 int dfm_percentiles_weighted(dfm_handle* h, const double* recs, const double* w, long long n, int d, const double* q, int nq, int mem,
                              double* out);
 

@@ -121,15 +121,21 @@ def _close(g, e, s, what):
         assert err <= TOL * max(s, np.nanmax(np.abs(e)), 1e-300), (what, err, s)
 
 
-def hd_scales(Lam, A, Q, F, p, t0, ns, scale):
-    """(eps scale, series scale) of one model: max_t |L^-1| (|f_t| + sum_l |A_l| |f_{t-l}|), and max_{i,t} |scale_i| |lam_i|' y_t
-    with y_t the largest |.| over the factor-level recursions (the spec with Lam = I)."""
+def eps_scale(A, Q, F, p):
+    """max_t |L^-1| (|f_t| + sum_l |A_l| |f_{t-l}|): the cancellation scale of u_t = L^-1 (f_t - sum_l A_l f_{t-l})."""
     r = Q.shape[0]; Tp = F.shape[0]
     aF = np.abs(F)
     u = aF[p:].copy()
     for l in range(1, p + 1):
         u += aF[p - l:Tp - l] @ np.abs(A[:, (l - 1) * r:l * r]).T
-    se = float((u @ np.abs(np.linalg.inv(np.linalg.cholesky(Q))).T).max()) if Tp > p else 0.0
+    return float((u @ np.abs(np.linalg.inv(np.linalg.cholesky(Q))).T).max()) if Tp > p else 0.0
+
+
+def hd_scales(Lam, A, Q, F, p, t0, ns, scale):
+    """(eps scale, series scale) of one model: max_t |L^-1| (|f_t| + sum_l |A_l| |f_{t-l}|), and max_{i,t} |scale_i| |lam_i|' y_t
+    with y_t the largest |.| over the factor-level recursions (the spec with Lam = I)."""
+    r = Q.shape[0]
+    se = eps_scale(A, Q, F, p)
     _, yc, yr, yb, _ = HO.decompose(np.eye(r), np.ones(r), A, Q, F, p, t0, n_shock=ns)
     Y = np.maximum(np.maximum(np.abs(yc).max(-1), np.abs(yr)), np.abs(yb))            # (r, Tp)
     sc = np.ones(Lam.shape[0]) if scale is None else np.asarray(scale)

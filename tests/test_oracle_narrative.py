@@ -115,3 +115,62 @@ def test_no_rows_is_sign_oracle_and_flip_group():
     k = x["cand"] >= 0
     np.testing.assert_array_equal(x["rot"][k][:, :, 2], -y["rot"][k][:, :, 2])
     np.testing.assert_array_equal(x["rot"][k][:, :, :2], y["rot"][k][:, :, :2])
+
+
+def test_decide_batch_is_decide():
+    """decide_batch (quadratic forms, all candidates at once) against the scalar decide (explicit convolution) on 3 000
+    candidates, rows of every kind on two shocks: the same accept bits, flips, and margins to 1e-9."""
+    import narrative_checks as NC
+    r, p, H = 3, 2, 4
+    Lam, R, A, Q, sc = SC.models(r, p, 8, 1, seed=1)
+    Lam, R, A, Q = Lam[0], R[0], A[0], Q[0]
+    F = np.random.default_rng(2).standard_normal((16, r))
+    rows, narr = NC.case(Lam, A, Q, F, p, H, 5, 2)
+    narr += [(3, 3, 4, 7, 2, -1), (0, 3, 0, 9, 0, 1)]
+    C = SO.row_vectors(Lam, A, Q, p, rows, H)
+    U = NO.shocks_u(A, Q, F, p)
+    P = IO.psi(A, Q, p, H)
+    c_of = lambda i: np.einsum("a,hab->hb", Lam[i], P)
+    Om = SO.omegas(5, 2, np.arange(3000), r)
+    shocks = [j for _, _, j, _ in rows]
+    ok, flip, m = NO.decide_batch(Om, C, shocks, narr, c_of, U, r)
+    for c in range(len(Om)):
+        o1, f1, m1 = NO.decide(Om[c], C, shocks, narr, c_of, U, r)
+        assert o1 == ok[c], c
+        if o1:
+            np.testing.assert_array_equal(f1, flip[c])
+        assert abs(m1 - m[c]) <= 1e-9 * max(1.0, m1), (c, m1, m[c])
+    assert 0 < ok.sum() < len(Om) and (flip[ok] < 0).any()
+
+
+def test_weighted_percentiles_exact_rule():
+    """The exact rule (100 sum_{j <= i} w_j >= q sum_j w_j) is numpy's weighted inverted_cdf wherever numpy's rounded cdf is more
+    than 2^-40 from q / 100, and with equal weights numpy's unweighted inverted_cdf at every size; the near-tie bounds hold the
+    exact record."""
+    rng = np.random.default_rng(3)
+    q = (0, 5, 10, 16, 25, 50, 75, 84, 90, 95, 100)
+    seen = 0
+    for n in (1, 2, 5, 130, 300, 1000, 4097):
+        x = rng.standard_normal(n)
+        for w in (rng.random(n) + 0.01, rng.integers(1, 5, n) * (2.0 ** 20 / 37), np.exp(rng.uniform(-20, 20, n))):
+            got = NO.weighted_percentiles(x[:, None], w, q)[:, 0]
+            o = np.argsort(x, kind="stable")
+            cdf = np.cumsum(w[o]) / w.sum()
+            for k, qq in enumerate(q):
+                if np.abs(cdf - qq / 100).min() > 2.0 ** -40:
+                    assert got[k] == np.percentile(x, qq, weights=w, method="inverted_cdf"), (n, qq)
+                    seen += 1
+            lo, hi = NO.weighted_percentiles(x[:, None], w, q, near=True)
+            assert (lo[:, 0] <= got).all() and (got <= hi[:, 0]).all()
+        for c in (1.0, 2.0 ** 20 / 3, 2.0 ** 20 / 37, 2.0 ** 20 / 12345):
+            got = NO.weighted_percentiles(x[:, None], np.full(n, c), q)[:, 0]
+            np.testing.assert_array_equal(got, np.percentile(x, q, method="inverted_cdf"), err_msg=str((n, c)))
+        # unit weights: numpy's weighted rule too (its cdf i / n and fl(q / 100) round alike where i / n = q / 100)
+        np.testing.assert_array_equal(NO.weighted_percentiles(x[:, None], np.ones(n), q)[:, 0],
+                                      np.percentile(x, q, weights=np.ones(n), method="inverted_cdf"))
+    assert seen > 100
+    # numpy's weighted rule rounds: 130 equal weights 2^20 / 37 give record 65 at q = 50, the exact rule (and numpy without
+    # weights) record 64; 300 records at q = 5: 100 * 15 = 5 * 300, so record 14 (the rule with fl(0.05) > 0.05 would give 15)
+    x = np.arange(130.0)
+    assert NO.weighted_percentiles(x[:, None], np.full(130, 2.0 ** 20 / 37), [50])[0, 0] == 64.0
+    assert NO.weighted_percentiles(np.arange(300.0)[:, None], np.ones(300), [5])[0, 0] == 14.0
