@@ -16,6 +16,6 @@ from .api import (  # noqa: F401
     kalman_smooth, forecast, posterior_draws, forecast_bands, news, parametric_irf, parametric_bootstrap,
     series_irf, gibbs, split_rhat, variance_decomposition, identified_responses, historical_decomposition,
     identified_history, sign_identified_set, sign_restricted_responses, narrative_identified_set,
-    narrative_restricted_responses,
+    narrative_restricted_responses, proxy_identified_responses, proxy_restricted_responses,
 )
 from . import ingest  # noqa: F401   (host-side panel ingestion: the step before the path)

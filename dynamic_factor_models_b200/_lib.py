@@ -120,6 +120,19 @@ NARR_OUTPUTS = ("rot", "resp", "fevd", "n_ok", "weight", "eps")
 NARR_KINDS = dict(shock=0, most=1, overwhelming=2, contrib=3)
 
 
+class ProxyOpts(C.Structure):
+    _fields_ = [("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("n_model", C.c_int), ("Tp", C.c_int), ("H", C.c_int), ("n_inst", C.c_int),
+                ("i0", C.c_int), ("q", C.c_int), ("block", C.c_int), ("n_boot", C.c_int), ("seed", C.c_ulonglong), ("mem", C.c_int)]
+
+
+class ProxyOut(C.Structure):
+    _fields_ = [("omega", C.c_void_p), ("resp", C.c_void_p), ("fevd", C.c_void_p), ("eps", C.c_void_p), ("n_obs", C.c_void_p),
+                ("reliability", C.c_void_p), ("fs_pi", C.c_void_p), ("fs_F", C.c_void_p), ("status", C.c_void_p)]
+
+
+PROXY_OUTPUTS = ("omega", "resp", "fevd", "eps", "n_obs", "reliability", "fs_pi", "fs_F")
+
+
 class SimOpts(C.Structure):
     _fields_ = [("T", C.c_int), ("N", C.c_int), ("r", C.c_int), ("p", C.c_int), ("H", C.c_int), ("n_draw", C.c_longlong),
                 ("draw0", C.c_longlong), ("seed", C.c_ulonglong), ("mem", C.c_int)]
@@ -189,7 +202,8 @@ EXPORTS = ["dfm_version", "dfm_status_string", "dfm_create", "dfm_create_on_stre
            "dfm_profile_kernel_name", "dfm_standardize", "dfm_pca_score", "dfm_estimate_factor",
            "dfm_estimate_loading", "dfm_estimate_loading_ex", "dfm_estimate_var", "dfm_irf", "dfm_instability", "dfm_fit_correlation", "dfm_em_kalman", "dfm_em_kalman_constrained", "dfm_kalman_smooth", "dfm_simulation_smoother",
            "dfm_news", "dfm_ss_simulate_panels", "dfm_ss_bootstrap", "dfm_gibbs", "dfm_gibbs_constrained",
-           "dfm_series_responses", "dfm_historical_decomposition", "dfm_sign_restrictions", "dfm_narrative_sign_restrictions", "dfm_em_init_from_factors",
+           "dfm_series_responses", "dfm_historical_decomposition", "dfm_sign_restrictions", "dfm_narrative_sign_restrictions", "dfm_proxy_identification",
+           "dfm_em_init_from_factors",
            "dfm_simulate_panels", "dfm_bootstrap_panels", "dfm_bootstrap_irf", "dfm_percentiles", "dfm_percentiles_weighted", "dfm_allgather_results",
            "dfm_shard_range"]
 
@@ -287,6 +301,8 @@ class Library:
                                             C.POINTER(SignRestr), C.POINTER(SignOut)]
         L.dfm_narrative_sign_restrictions.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.c_void_p,
                                                       C.POINTER(NarrOpts), C.POINTER(SignRestr), C.POINTER(NarrRestr), C.POINTER(NarrOut)]
+        L.dfm_proxy_identification.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.POINTER(ProxyOpts), C.POINTER(ProxyOut)]
         L.dfm_series_responses.argtypes = [C.c_void_p, C.POINTER(EmInit), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dfm_simulate_panels.argtypes = [C.c_void_p, C.c_ulonglong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -643,6 +659,60 @@ class Library:
                 res[n_] = a_.reshape(B, n_keep, n_shock, H, N).transpose(0, 1, 4, 3, 2)
         if not b:
             res = {n_: (v[0] if n_ != "status" else int(v[0])) for n_, v in res.items()}
+        return res
+
+    def proxy_identification_raw(self, models, F, Z, ids, N, r, p, n_model, Tp, H, n_inst, i0, q, block, n_boot, seed, scale, mem,
+                                 omega=0, resp=0, fevd=0, eps=0, n_obs=0, reliability=0, fs_pi=0, fs_F=0, status=0):
+        """Pointer-level dfm_proxy_identification (ints = device or host addresses).  models: dict Lam, R, A, Q (n_model models back
+        to back); F: the n_model paths (Tp x r each); Z: the Tp x n_inst instruments (column-major); ids: HOST uint64 array of
+        n_model model ids or None (= 0 .. n_model-1); scale: address or 0 (= 1)."""
+        ini = EmInit(**{k: C.c_void_p(v) if v else None for k, v in models.items()})
+        vp = lambda a: C.c_void_p(a) if a else None
+        idv = np.ascontiguousarray(ids, dtype=np.uint64) if ids is not None else None
+        o = ProxyOpts(N=N, r=r, p=p, n_model=n_model, Tp=Tp, H=H, n_inst=n_inst, i0=i0, q=q, block=block, n_boot=n_boot, seed=seed, mem=mem)
+        ou = ProxyOut(omega=vp(omega), resp=vp(resp), fevd=vp(fevd), eps=vp(eps), n_obs=vp(n_obs), reliability=vp(reliability),
+                      fs_pi=vp(fs_pi), fs_F=vp(fs_F), status=vp(status))
+        self.check(self.lib.dfm_proxy_identification(self.h, C.byref(ini), vp(F), vp(Z),
+                                                     idv.ctypes.data_as(C.c_void_p) if idv is not None else None, vp(scale),
+                                                     C.byref(o), C.byref(ou)), "dfm_proxy_identification")
+        del idv
+
+    def proxy_identification(self, Lam, R, A, Q, F, Z, i0, H, n_boot=0, block=1, q=0, seed=0, ids=None, scale=None,
+                             outputs=PROXY_OUTPUTS):
+        """Shocks identified by external instruments (dfm_proxy_identification) of models (Lam (B, N, r), R (B, N), A (B, r, k),
+        Q (B, r, r)) along their factor paths F (B, Tp, r), or of one model (2-D Lam, F (Tp, r)).  Z: (Tp,) or (Tp, n_inst)
+        instruments (NaN = unavailable); i0: the first stage's series (0-based).  Returns omega (B, n_inst, 1 + n_boot, r), resp /
+        fevd (B, n_inst, 1 + n_boot, N, H), eps (B, n_inst, Tp), n_obs, reliability, fs_pi, fs_F (B, n_inst) -- those named in
+        `outputs` -- and status (B, n_inst), without the batch axis for one model.  The arrays are views of the buffers the library
+        wrote."""
+        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
+        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        F = np.asarray(F, float); Tp = F.shape[-2]
+        Z = np.asarray(Z, float)
+        Z = Z.reshape(Tp, -1) if Z.ndim == 1 else Z
+        ni = Z.shape[1]
+        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
+        Fb, Zb = to_cm(F), to_cm(Z)
+        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
+        nr = 1 + n_boot
+        size = dict(omega=ni * nr * r, resp=ni * nr * N * H, fevd=ni * nr * N * H, eps=ni * Tp, n_obs=ni, reliability=ni, fs_pi=ni, fs_F=ni)
+        outs = {n_: (np.zeros(B * size[n_], np.int32) if n_ == "n_obs" else np.full(B * size[n_], np.nan)) for n_ in outputs}
+        st = np.zeros(B * ni, np.int32)
+        self.proxy_identification_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, Fb.ctypes.data, Zb.ctypes.data, ids, N, r, p, B, Tp,
+                                      H, ni, i0, q, block, n_boot, seed, sc.ctypes.data if sc is not None else 0, MEM_HOST,
+                                      status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        res = dict(status=st.reshape(B, ni))
+        for n_, a_ in outs.items():
+            if n_ == "omega":
+                res[n_] = a_.reshape(B, ni, nr, r)
+            elif n_ in ("resp", "fevd"):
+                res[n_] = a_.reshape(B, ni, nr, H, N).transpose(0, 1, 2, 4, 3)
+            elif n_ == "eps":
+                res[n_] = a_.reshape(B, ni, Tp)
+            else:
+                res[n_] = a_.reshape(B, ni)
+        if not b:
+            res = {n_: v[0] for n_, v in res.items()}
         return res
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):

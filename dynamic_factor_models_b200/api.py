@@ -932,6 +932,161 @@ def narrative_restricted_responses(m, restrictions, narrative, H, n_shock=None, 
     return out
 
 
+def _proxy_inputs(m, b, z, normalize, H, block, what):
+    """(Z (T, n_inst), instrument names, i0, block length) of proxy_identified_responses' arguments."""
+    if H <= 0:
+        raise ValueError("H must be > 0")
+    T = m.lastperiod - m.initperiod + 1
+    if isinstance(z, dict):
+        names = [str(k) for k in z]
+        Z = np.column_stack([np.asarray(v, float).reshape(-1) for v in z.values()]) if z else np.zeros((T, 0))
+    else:
+        Z = np.asarray(z, float)
+        Z = Z.reshape(-1, 1) if Z.ndim == 1 else Z
+        names = [str(k) for k in range(Z.shape[1])]
+    if Z.ndim != 2 or Z.shape[0] != T or not 1 <= Z.shape[1] <= 8:
+        raise ValueError(f"{what}: z must hold 1 .. 8 instruments over the estimation block's {T} rows, got shape {Z.shape}")
+    ns = b["Xs"].shape[1]
+    i0 = int(normalize)
+    if not 0 <= i0 < ns:
+        raise ValueError(f"{what}: normalize = {normalize} is not an estimation series (0 .. {ns - 1})")
+    if np.isnan(b["Lam"][i0]).any() or np.isnan(b["em"]["R"][i0]):
+        raise ValueError(f"{what}: the normalising series {i0} is out of the model")
+    block = max(1, int(round(T ** (1.0 / 3.0)))) if block is None else int(block)
+    if block < 1:
+        raise ValueError(f"{what}: block must be >= 1")
+    return Z, names, i0, block
+
+
+def _proxy_bands(lib, d, recs, i0, qq, shape):
+    """Percentile bands of resp, resp_unit (resp / resp[i0, 0] of the same record) and fevd over the record axis of d[...] (n_inst,
+    n_rec, ns, H), returned (len(q), ns, H, n_inst)."""
+    out = {}
+    resp = d["resp"][:, recs]
+    unit = resp / resp[:, :, i0:i0 + 1, :1]
+    for nm, v in (("resp", resp), ("resp_unit", unit), ("fevd", d["fevd"][:, recs])):
+        n = v.shape[1]
+        bd = lib.percentiles(np.ascontiguousarray(v.transpose(1, 2, 3, 0)).reshape(n, -1), qq)
+        out[nm + "_bands"] = bd.reshape((len(qq),) + shape)
+    return out
+
+
+def proxy_identified_responses(m, z, normalize, H, n_boot=4096, block=None, q=0, seed=20260922, q_bands=(5, 16, 50, 84, 95),
+                               return_draws=False, lib=None):
+    """Shocks identified by external instruments (proxy SVAR / SVAR-IV, Stock & Watson 2018) at the EM estimates m.em of a model
+    estimated with `estimate(m, Parametric())`, with or without lam_constr_em (dfm_proxy_identification).
+
+    z: an array (T,) or (T, n_inst), or a dict name -> (T,) array, over the estimation block's rows initperiod .. lastperiod (NaN
+    where the instrument is unavailable); at most 8 instruments, each identifying its own shock.  normalize: the 0-based
+    estimation series i0 (the index convention of sign_identified_set) whose impact response is the unit effect, e.g. an oil
+    price.  With the smoothed factor path at m.em (kalman_smooth, as historical_decomposition), L = chol(Q), the innovations
+    eta_t = f_t - sum_l A_l f_{t-l} and an instrument's periods T_k (z finite, t > p lags into the sample):
+      omega_k = L^-1 Gamma_k / |L^-1 Gamma_k|, Gamma_k = mean over T_k of eta_t (z_t - zbar): the shock's column of the impact
+      matrix is b_k = L omega_k, a one-standard-deviation shock covarying positively with its instrument.  None of the results
+      depends on the normalisation of the factors (f -> K f; DESIGN.md 4.16), so no loading restriction is needed.
+    Returns a dict (instruments on the last axis):
+      resp, fevd (ns, H, n_inst)        xstd_i lam_i' Psi_h omega_k in data units, and the share of the (h+1)-step forecast-error
+                                         variance (variance_decomposition's formula for one shock);
+      resp_unit (ns, H, n_inst)         resp / resp[i0, 0]: the unit-effect normalisation (a shock moving series i0 by one unit
+                                         on impact);
+      eps (T, n_inst)                   the identified shock's path omega_k' L^-1 eta_t (NaN for the first p rows);
+      omega (n_inst, r), reliability, first_stage_F, first_stage_pi, n_obs (n_inst,): reliability = |L^-1 Gamma_k|^2 / s^2_z,
+                                         the squared correlation of the instrument with the shock under the model's Q, reported as
+                                         computed (along the smoothed path, whose innovations are shrunk, it can exceed 1);
+                                         first_stage_F: Stock & Watson's HAC(q) first-stage F of lam_i0' eta_t on [1, z_t];
+      shock_corr (n_inst, n_inst)       omega_k' omega_l: the correlation of the shocks two instruments identify (1 when they
+                                         identify the same shock);
+      resp_bands, resp_unit_bands, fevd_bands (len(q_bands), ns, H, n_inst)   percentiles over the n_boot moving-block bootstrap
+                                         replicates of the instrument moments (dfm_percentiles);
+      resp_draws, resp_unit_draws, fevd_draws (n_boot, ns, H, n_inst)   only with return_draws=True: the replicates' records;
+    and status (n_inst,), names, series, q, block, periods.
+    The bands hold theta = m.em and the path fixed: they describe the instrument-side sampling uncertainty only
+    (proxy_restricted_responses adds parameter and path uncertainty).  block: the bootstrap's block length, default
+    round(T^(1/3)) (the rate that balances the bias and variance of a block bootstrap variance estimate); the periods where an
+    instrument is missing are skipped, so a block may join periods across a gap.  n_boot <= 16384."""
+    if not 1 <= n_boot <= 16384:
+        raise ValueError("proxy_identified_responses: n_boot must be in [1, 16384]")
+    b = _state_space_block(m, 0, lib, "proxy_identified_responses")
+    lib, e = b["lib"], b["em"]
+    Z, names, i0, block = _proxy_inputs(m, b, z, normalize, H, block, "proxy_identified_responses")
+    o = lib.kalman_smooth(b["Xs"], b["Lam"], e["R"], e["A"], e["Q"], p=b["p"], P0=e["P0"], H=0, outputs=("F",))
+    if o["status"] != 0:
+        raise RuntimeError(f"proxy_identified_responses: device status {o['status']}")
+    d = lib.proxy_identification(b["Lam"], e["R"], e["A"], e["Q"], o["F"], Z, i0, H, n_boot=n_boot, block=block, q=q, seed=seed,
+                                 scale=b["xstd"])
+    bad = np.flatnonzero(d["status"] != 0)
+    if len(bad):
+        raise RuntimeError(f"proxy_identified_responses: instrument(s) {[names[k] for k in bad]} failed with status "
+                           f"{d['status'][bad].tolist()} (3: a failed model, fewer than 3 usable periods or no covariance with the "
+                           "innovations)")
+    qq = np.asarray(q_bands, float)
+    ns = b["Xs"].shape[1]
+    mv = lambda a_: np.ascontiguousarray(np.moveaxis(a_, 0, -1))
+    om = d["omega"][:, 0]
+    resp = d["resp"][:, 0]
+    out = dict(resp=mv(resp), resp_unit=mv(resp / resp[:, i0:i0 + 1, :1]), fevd=mv(d["fevd"][:, 0]), eps=mv(d["eps"]),
+               omega=np.ascontiguousarray(om), reliability=d["reliability"].copy(), first_stage_F=d["fs_F"].copy(),
+               first_stage_pi=d["fs_pi"].copy(), n_obs=d["n_obs"].astype(int), shock_corr=om @ om.T, status=d["status"].copy(),
+               names=names, series=b["series"], q=qq, block=block, periods=b["periods"])
+    out.update(_proxy_bands(lib, d, slice(1, None), i0, qq, (ns, H, len(names))))
+    if return_draws:
+        rr = d["resp"][:, 1:]
+        for nm, v in (("resp", rr), ("resp_unit", rr / rr[:, :, i0:i0 + 1, :1]), ("fevd", d["fevd"][:, 1:])):
+            out[nm + "_draws"] = np.ascontiguousarray(np.moveaxis(v, 0, -1))
+    return out
+
+
+def proxy_restricted_responses(m, z, normalize, H, n_chain=4, n_burn=500, n_keep=1000, thin=1, boot_per_draw=1, block=None, q=0,
+                               prior=None, seed=20260922, q_bands=(5, 16, 50, 84, 95), chain0=0, sweep0=0, lib=None):
+    """Bands of the instrument-identified responses over Gibbs parameter and path draws: gibbs (dfm_gibbs from m.em, same prior and
+    refusals: a lam_constr_em fit is refused, the sampler draws unrestricted loadings) records each kept draw's parameters and
+    factor path, and one dfm_proxy_identification over all kept draws identifies each draw's shocks along its own path, with
+    boot_per_draw moving-block bootstrap replicates of the instrument moments per draw (ids gibbs_id(chain, kept sweep), as
+    sign_restricted_responses).  z, normalize, H, block, q: as proxy_identified_responses.
+
+    This combines posterior draws of the parameters and the path with a block bootstrap of the instrument moments; it is not a
+    fully Bayesian proxy model (the instrument's own likelihood, as in Caldara & Herbst 2019, is not part of the posterior).
+
+    Returns a dict:
+      resp_bands, resp_unit_bands, fevd_bands (len(q_bands), ns, H, n_inst)   percentiles over every (draw, replicate) record
+                   (replicates 1 .. boot_per_draw of every draw; with boot_per_draw = 0, replicate 0, the draw's own sample);
+      reliability, first_stage_F (n_chain, n_keep, n_inst)   of each draw (replicate 0);
+      proxy_status (n_chain, n_keep, n_inst)   dfm_proxy_identification's status (a failed chain's draws are 3);
+      status (n_chain), loglik (n_chain, n_burn + n_keep thin), rhat dict(loglik)   split-R^ over the kept draws;
+    and prior, names, series, q, block.  n_chain n_keep max(1, boot_per_draw) <= 16384."""
+    if m.em is not None and m.em.get("lam_constr") is not None:
+        raise ValueError("proxy_restricted_responses: the EM of m ran under restrictions on the loadings (lam_constr_em); the sampler "
+                         "draws unrestricted loadings")
+    nrb = max(1, int(boot_per_draw))
+    if boot_per_draw < 0 or not 1 <= n_chain * n_keep * nrb <= 16384:
+        raise ValueError("proxy_restricted_responses: n_chain * n_keep * max(1, boot_per_draw) must be in [1, 16384]")
+    b = _state_space_block(m, 0, lib, "proxy_restricted_responses")
+    lib, e = b["lib"], b["em"]
+    Z, names, i0, block = _proxy_inputs(m, b, z, normalize, H, block, "proxy_restricted_responses")
+    r = e["Q"].shape[0]
+    pr = dict(_gibbs_default_prior(r)); pr.update(prior or {})
+    init = dict(Lam=b["Lam"], R=e["R"], A=e["A"], Q=e["Q"], P0=e["P0"])
+    o = lib.gibbs(b["Xs"], init, p=b["p"], n_chain=n_chain, chain0=chain0, sweep0=sweep0, n_burn=n_burn, n_keep=n_keep, thin=thin,
+                  seed=seed, prior=pr, outputs=("Lam", "R", "A", "Q", "F"))
+    n = n_chain * n_keep
+    kept = n_burn + thin * np.arange(1, n_keep + 1) - 1
+    ids = ((np.arange(chain0, chain0 + n_chain, dtype=np.uint64)[:, None] << np.uint64(24)) +
+           (np.uint64(sweep0) + kept.astype(np.uint64))[None, :]).ravel()              # gibbs_id(chain, kept sweep)
+    sh = lambda a_: a_.reshape((n,) + a_.shape[2:])
+    d = lib.proxy_identification(sh(o["Lam"]), sh(o["R"]), sh(o["A"]), sh(o["Q"]), sh(o["F"]), Z, i0, H, n_boot=int(boot_per_draw),
+                                 block=block, q=q, seed=seed, ids=ids, scale=b["xstd"], outputs=("resp", "fevd", "reliability", "fs_F"))
+    ns, ni = b["Xs"].shape[1], Z.shape[1]
+    # records (n_inst, n_draw * nrb, ns, H): the draws' replicates 1 .. boot_per_draw (or replicate 0)
+    sel = slice(1, None) if boot_per_draw > 0 else slice(0, 1)
+    dd = {nm: np.moveaxis(d[nm][:, :, sel], 1, 0).reshape((ni, n * nrb, ns, H)) for nm in ("resp", "fevd")}
+    qq = np.asarray(q_bands, float)
+    out = dict(reliability=d["reliability"].reshape(n_chain, n_keep, ni), first_stage_F=d["fs_F"].reshape(n_chain, n_keep, ni),
+               proxy_status=d["status"].reshape(n_chain, n_keep, ni), status=o["status"], loglik=o["loglik"], prior=pr, names=names,
+               series=b["series"], q=qq, block=block, rhat=dict(loglik=float(split_rhat(o["loglik"][:, kept]))))
+    out.update(_proxy_bands(lib, dd, slice(None), i0, qq, (ns, H, ni)))
+    return out
+
+
 def parametric_bootstrap(m, n_rep, H_irf=24, H_fc=0, fc_rows=None, seed=20260922, q=(5, 16, 50, 84, 95), max_iter=50, tol=0.0, rep0=0,
                          lib=None):
     """Parametric bootstrap of a model estimated with `estimate(m, Parametric())` (dfm_ss_bootstrap): n_rep panels are drawn

@@ -20,6 +20,7 @@
 #include "dfm_kernels_hd.cuh"
 #include "dfm_kernels_sign.cuh"
 #include "dfm_kernels_narr.cuh"
+#include "dfm_kernels_proxy.cuh"
 #include <algorithm>
 #include <cmath>
 #include <new>
@@ -2594,6 +2595,129 @@ int dfm_narrative_sign_restrictions(dfm_handle* h, const dfm_em_init* models, co
       rc = copy_out(h, out->n_accept ? out->n_accept + j0 : nullptr, dNa, nm, mem); if (rc) return rc;
       rc = copy_out(h, out->cand ? out->cand + j0 * nk : nullptr, dCa, nm * (size_t)nk, mem); if (rc) return rc;
       rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
+      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+    }
+  }
+  return finish(h, mem);
+}
+
+// ------------------------------------------------------------------------------------ proxy (external instrument) identification
+// Per chunk of models (a size fixed by the shapes): k_sr_prep -> k_irf (when responses are asked for) -> k_iv_prep -> k_iv_boot ->
+// per batch of records (model, instrument, replicate) in output order: k_iv_rot -> k_series_resp (n_shock 1).  A chunk holds
+// several models when all their records fit one batch, otherwise one model whose records run in several batches; either way
+// record s of a batch reads model s / (n_inst (1 + n_boot)) of the chunk.  Host arrays are staged per chunk; device outputs are
+// written in place.
+int dfm_proxy_identification(dfm_handle* h, const dfm_em_init* models, const double* F, const double* Z, const unsigned long long* ids,
+                             const double* scale, const dfm_proxy_opts* o, const dfm_proxy_out* out) {
+  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !F || !Z || !o || !out || o->N <= 0 || o->r <= 0 ||
+      o->p <= 0 || o->n_model <= 0 || o->Tp < 1 || o->H <= 0 || o->n_inst < 1 || o->i0 < 0 || o->i0 >= o->N || o->q < 0 ||
+      o->block < 1 || o->n_boot < 0 || (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_proxy_identification: bad argument");
+  if (ids)
+    for (int b = 0; b < o->n_model; ++b)
+      if (ids[b] >= (1ull << 40)) return fail(h, DFM_ERR_ARG, "dfm_proxy_identification: a model id >= 2^40");
+  const int N = o->N, r = o->r, p = o->p, H = o->H, Tp = o->Tp, ni = o->n_inst, nbt = o->n_boot, k = r * p, mem = o->mem;
+  if (k > 48 || ni > IV_NIMAX || nbt > 65535)
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_proxy_identification: r*p > 48, n_inst > 8 or n_boot > 65535");
+  const size_t smP = iv_prep_smem_bytes(r, Tp), smB = iv_boot_smem_bytes(r, Tp), smT = iv_rot_smem_bytes(r);
+  if (smP > kMaxSmem || smB > kMaxSmem)
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_proxy_identification: Tp (r + 1) + 64 r > 28160 (the bootstrap's shared memory)");
+  const bool want = out->resp || out->fevd, hst = mem == DFM_MEM_HOST;
+  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, Tr = (size_t)Tp * r, NH = (size_t)N * H;
+  const size_t P = (size_t)ni * (nbt + 1), nE = (size_t)ni * Tp;
+  const size_t sm0 = series_resp_smem_doubles(r, 1, 0);
+  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
+  const size_t smR = series_resp_smem_doubles(r, 1, hc) * 8, smI = irf_smem_doubles(k) * 8;
+  // records per batch: grid.y of k_series_resp, and half of kSimChunkBytes; models per chunk: the other half, grid.y of k_iv_boot,
+  // and (for more than one) all their records in one batch
+  const size_t perR = 8 * (rr * H + (hst ? (out->resp ? NH : 0) + (out->fevd ? NH : 0) : 0)) + 4;
+  const long long cap = std::min<long long>(kMaxGridBatch, std::max<long long>(1, (long long)(kSimChunkBytes / 2 / perR)));
+  const size_t perM = 8 * (kk + 2 * rk + rr * H + Tr + P * r + 1 + (hst ? Nr + N + rk + rr + Tr + (out->eps ? nE : 0) + 3 * (size_t)ni : 0)) +
+                      4 * (nE + 3 * (size_t)ni + 1);
+  const int nb = (int)std::max<long long>(1, std::min<long long>({(long long)o->n_model, (long long)(kSimChunkBytes / 2 / perM),
+                                                                  (long long)(kMaxGridBatch / ni), cap / (long long)P}));
+  const long long nrec = std::min<long long>(cap, (long long)nb * (long long)P);
+  CK(cudaSetDevice(h->device));
+  for (int pass = 0; pass < 2; ++pass) {
+    Arena a(pass ? h->ws : nullptr);
+    const size_t B = nb;
+    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
+           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
+           *dF = hst ? a.get<double>(B * Tr) : nullptr, *dZ = hst ? a.get<double>(nE) : nullptr,
+           *dS = hst && scale ? a.get<double>(N) : nullptr;
+    double *dEp = hst && out->eps ? a.get<double>(B * nE) : nullptr, *dRel = hst && out->reliability ? a.get<double>(B * ni) : nullptr,
+           *dPi = hst && out->fs_pi ? a.get<double>(B * ni) : nullptr, *dFs = hst && out->fs_F ? a.get<double>(B * ni) : nullptr;
+    double *dRe = hst && out->resp ? a.get<double>(nrec * NH) : nullptr, *dFe = hst && out->fevd ? a.get<double>(nrec * NH) : nullptr;
+    int* dNo = hst && out->n_obs ? a.get<int>(B * ni) : nullptr;
+    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H),
+           *dU = a.get<double>(B * Tr), *dOm = a.get<double>(B * P * r), *dRec = want ? a.get<double>(nrec * rr * H) : nullptr;
+    unsigned long long* dId = a.get<unsigned long long>(B);
+    int *dst = a.get<int>(B), *dIdx = a.get<int>(B * nE), *dNk = a.get<int>(B * ni), *dIst = a.get<int>(B * ni),
+        *dSst = want ? a.get<int>(nrec) : nullptr, *dIr = a.get<int>(r);
+    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
+    std::vector<int> hid(r);
+    for (int j = 0; j < r; ++j) hid[j] = j;
+    CK(cudaMemcpyAsync(dIr, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    const double* sc = scale;
+    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
+    const double* Z_ = Z;
+    int rc = stage_in(h, Z, dZ, nE, mem, &Z_); if (rc) return rc;
+    DFM_SET_SMEM(k_series_resp, smR);
+    DFM_SET_SMEM(k_irf, smI);
+    DFM_SET_SMEM(k_iv_prep, smP);
+    DFM_SET_SMEM(k_iv_boot, smB);
+    std::vector<unsigned long long> hids(nb);
+    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
+      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
+      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr,
+                   *F_ = F + j0 * Tr;
+      if (hst) {
+        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
+        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
+        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
+        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
+        rc = stage_in(h, F_, dF, nm * Tr, mem, &F_); if (rc) return rc;
+      }
+      for (int b = 0; b < nm; ++b) hids[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
+      CK(cudaMemcpyAsync(dId, hids.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+      const size_t mi = (size_t)nm * ni;
+      double* oOm = out->omega && !hst ? out->omega + j0 * P * r : dOm;
+      double* oEp = out->eps ? (hst ? dEp : out->eps + j0 * nE) : nullptr;
+      double* oRel = out->reliability ? (hst ? dRel : out->reliability + j0 * ni) : nullptr;
+      double* oPi = out->fs_pi ? (hst ? dPi : out->fs_pi + j0 * ni) : nullptr;
+      double* oFs = out->fs_F ? (hst ? dFs : out->fs_F + j0 * ni) : nullptr;
+      int* oNo = out->n_obs ? (hst ? dNo : out->n_obs + j0 * ni) : nullptr;
+      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
+      if (want) L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)dIr, dI);
+      L(k_iv_prep, nm, 1, IV_PT, smP, L_, R_, A_, (const double*)dG, F_, Z_, N, r, p, Tp, ni, o->i0, o->q, nbt, (const int*)dst, dU, dIdx,
+        dNk, dIst, oOm, oEp, oNo, oRel, oPi, oFs);
+      if (nbt > 0)
+        L(k_iv_boot, (nbt + IV_BT - 1) / IV_BT, (int)mi, IV_BT, smB, (const double*)dU, Z_, (const int*)dIdx, (const int*)dNk,
+          (const int*)dIst, r, Tp, ni, o->block, nbt, o->seed, (const unsigned long long*)dId, oOm);
+      const long long nrc = (long long)nm * (long long)P;
+      for (long long g0 = 0; want && g0 < nrc; g0 += nrec) {
+        const int nr = (int)std::min<long long>(nrec, nrc - g0);
+        const size_t og = ((size_t)j0 * P + (size_t)g0) * NH;
+        double* oRe = out->resp ? (hst ? dRe : out->resp + og) : nullptr;
+        double* oFe = out->fevd ? (hst ? dFe : out->fevd + og) : nullptr;
+        L(k_iv_rot, nr, 1, 64, smT, (const double*)dI, (const double*)oOm, g0, r, H, ni, nbt, dRec, dSst);
+        L(k_series_resp, (N + SR_NS - 1) / SR_NS, nr, SR_NS, smR, L_, R_, sc, (const double*)dRec, (const int*)dSst, N, r, H, 1, hc, (int)P,
+          oRe, oFe);
+        if (hst) {
+          rc = copy_out(h, out->resp ? out->resp + og : nullptr, dRe, nr * NH, mem); if (rc) return rc;
+          rc = copy_out(h, out->fevd ? out->fevd + og : nullptr, dFe, nr * NH, mem); if (rc) return rc;
+          CK(cudaStreamSynchronize(h->stream));             // (dRe and dFe are rewritten by the next batch)
+        }
+      }
+      if (hst) {
+        rc = copy_out(h, out->eps ? out->eps + j0 * nE : nullptr, dEp, nm * nE, mem); if (rc) return rc;
+        rc = copy_out(h, out->reliability ? out->reliability + j0 * ni : nullptr, dRel, mi, mem); if (rc) return rc;
+        rc = copy_out(h, out->fs_pi ? out->fs_pi + j0 * ni : nullptr, dPi, mi, mem); if (rc) return rc;
+        rc = copy_out(h, out->fs_F ? out->fs_F + j0 * ni : nullptr, dFs, mi, mem); if (rc) return rc;
+        rc = copy_out(h, out->n_obs ? out->n_obs + j0 * ni : nullptr, dNo, mi, mem); if (rc) return rc;
+      }
+      rc = copy_out(h, out->omega ? out->omega + j0 * P * r : nullptr, oOm, nm * P * r, mem); if (rc) return rc;
+      rc = copy_out(h, out->status ? out->status + j0 * ni : nullptr, dIst, mi, mem); if (rc) return rc;
       if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
     }
   }

@@ -645,6 +645,61 @@ int dfm_narrative_sign_restrictions(dfm_handle* h, const dfm_em_init* models, co
                                     const double* scale, const dfm_narr_opts* opts, const dfm_sign_restr* restr,
                                     const dfm_narr_restr* narr, const dfm_narr_out* out);
 
+/* ---- shocks identified by external instruments (proxy SVAR / SVAR-IV; Stock & Watson 2018) ------------------------------
+ * models: n_model models (Lam N x r, R N, A = [A_1 .. A_p] r x k, Q r x r; P0 unused) as dfm_series_responses, k = r p; F: n_model
+ * factor paths f_0 .. f_{Tp-1} (Tp x r each, column-major); Z: Tp x n_inst instruments (column-major, NaN = unavailable), the same
+ * for every model; ids: HOST array of n_model model ids < 2^40 (NULL = 0 .. n_model-1); scale: N (NULL = 1).  All but ids in `mem`.
+ * Per model, L = chol(Q), Psi_h = [M^h]_{1:r,1:r} L and c_{i,h} = lam_i' Psi_h (as dfm_series_responses), and for t >= p
+ * eta_t = f_t - sum_{l=1..p} A_l f_{t-l}, u_t = L^-1 eta_t.  Instrument k:
+ *   T_k = {t >= p : z_{k,t} finite, f_t .. f_{t-p} finite} (n_k periods; see status for a NaN path row), zbar,
+ *   s^2 = (1/n_k) sum (z - zbar)^2 and Gamma_k = (1/n_k) sum eta_t (z_t - zbar) over T_k; omega_k = L^-1 Gamma_k / |L^-1 Gamma_k|
+ *   (the shock covaries positively with its instrument; b_k = L omega_k has b_k' Q^-1 b_k = 1: a one-standard-deviation shock);
+ *   eps_{k,t} = omega_k' u_t (t >= p);
+ *   resp[i,h] = scale_i c_{i,h} omega_k;  fevd[i,h] = sum_{l<=h} (c_{i,l} omega_k)^2 / (sum_{l<=h} |c_{i,l}|^2 + R_i);
+ *   reliability rho^2_k = |L^-1 Gamma_k|^2 / s^2 (not clamped: along a smoothed path it can exceed 1);
+ *   first stage: y_t = lam_i0' eta_t on [1, z_{k,t}] over T_k, fs_pi the slope, fs_F = fs_pi^2 / V[1,1] with V the HAC(q) covariance
+ *   of the OLS coefficients (Bartlett weights 1 - j/(q+1); q = 0: White's), the periods of T_k taken as consecutive.
+ *   Moving-block bootstrap, replicate rho = 1 .. n_boot: T_k's periods indexed 0 .. n_k-1, l = min(block, n_k), ceil(n_k / l) block
+ *   starts s_j = floor(u_j (n_k - l + 1)), u_j the uniform number (rho n_inst + k) Tp + j of the Philox stream of the model id,
+ *   tag 20 (distinct for every (rho, k, j) since j < Tp); the blocks of (u_t, z_t) concatenated and cut at n_k give omega*, resp*
+ *   and fevd* as above (a gap in the instrument is treated as adjacent periods).  Replicate 0 is the sample itself.  Record rho
+ *   of model b is a function of (seed, id_b, k, rho, block) and the data alone: it does not depend on n_boot, n_model or chunking.
+ * Outputs (any may be NULL; models back to back, column-major):
+ *   omega        n_model x n_inst x (1 + n_boot) x r;
+ *   resp, fevd   n_model x n_inst x (1 + n_boot) x (N x H);
+ *   eps          n_model x n_inst x Tp            (NaN for t < p and rows with a NaN in f_t .. f_{t-p});
+ *   n_obs (int), reliability, fs_pi, fs_F, status (int)   n_model x n_inst.
+ * status per (model, instrument), the first of: 3 (DFM_ERR_NOT_PD) when A or Q holds a NaN or Q is not positive definite; DFM_ERR_ARG
+ * when series i0 is out of the model (NaN loading row or R_i0); 3 when a NaN in the path touches a period of T_k (f_t .. f_{t-p}),
+ * n_k < 3, or Gamma_k = 0.  Such a pair has NaN outputs (n_obs still counted); a bootstrap replicate with Gamma* = 0 has a NaN
+ * record.  Neighbours are unaffected.  Bounds: k <= 48, n_inst <= 8, n_boot <= 65535, Tp (r + 1) + 64 r <= 28160 (the
+ * bootstrap kernel's shared memory, e.g. Tp <= 3072 at r = 8): DFM_ERR_UNSUPPORTED past them.  Bad arguments (a NULL required
+ * pointer, Tp < 1, H < 1, n_inst < 1, i0 outside [0, N), q < 0, block < 1, n_boot < 0, an id >= 2^40, a bad mem): DFM_ERR_ARG.
+ * Synchronous for host memory. */
+typedef struct {
+  int N, r, p, n_model, Tp, H;
+  int n_inst;                 /* instruments, 1 .. 8 */
+  int i0;                     /* the first stage's series, 0 .. N-1 */
+  int q;                      /* HAC lags of the first stage, >= 0 */
+  int block;                  /* bootstrap block length, >= 1 */
+  int n_boot;                 /* bootstrap replicates, 0 .. 65535 */
+  unsigned long long seed;
+  int mem;
+} dfm_proxy_opts;
+typedef struct {
+  double* omega;
+  double* resp;
+  double* fevd;
+  double* eps;
+  int* n_obs;
+  double* reliability;
+  double* fs_pi;
+  double* fs_F;
+  int* status;
+} dfm_proxy_out;
+int dfm_proxy_identification(dfm_handle* h, const dfm_em_init* models, const double* F, const double* Z, const unsigned long long* ids,
+                             const double* scale, const dfm_proxy_opts* opts, const dfm_proxy_out* out);
+
 /* Initial (Lam, R, A, Q) for dfm_em_kalman from a standardized panel and factor estimates
  * (per-series OLS on F without constant, residual variance, VAR(p) without constant) --
  * the role uar_ser / fill_matrices! outputs would play (:405-412, :477-492). */

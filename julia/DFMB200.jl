@@ -479,4 +479,38 @@ function narrative_sign_restrictions(Lam::Array{Float64,3}, R::Matrix{Float64}, 
     return (n_accept = na, cand = cand, rot = rot, resp = resp, fevd = fevd, status = st, n_ok = nok, weight = w, eps = eps)
 end
 
+
+struct ProxyOpts; N::Cint; r::Cint; p::Cint; n_model::Cint; Tp::Cint; H::Cint; n_inst::Cint; i0::Cint; q::Cint; block::Cint; n_boot::Cint;
+                  seed::Culonglong; mem::Cint; end
+struct ProxyOut; omega::Ptr{Cdouble}; resp::Ptr{Cdouble}; fevd::Ptr{Cdouble}; eps::Ptr{Cdouble}; n_obs::Ptr{Cint}; reliability::Ptr{Cdouble};
+                 fs_pi::Ptr{Cdouble}; fs_F::Ptr{Cdouble}; status::Ptr{Cint}; end
+
+"""Shocks identified by external instruments (dfm_proxy_identification) on B models as `sign_restrictions`, along their factor
+paths F (Tp x r x B), with instruments Z (Tp x n_inst, NaN = unavailable) and the first stage's series i0 (0-based).  Returns omega
+(r x (1 + n_boot) x n_inst x B), resp and fevd (N x H x (1 + n_boot) x n_inst x B), eps (Tp x n_inst x B), n_obs, reliability,
+fs_pi, fs_F, status (n_inst x B); replicate 0 is the sample, 1 .. n_boot the moving-block bootstrap.  Not run in this
+repository's tests."""
+function proxy_identification(Lam::Array{Float64,3}, R::Matrix{Float64}, A::Array{Float64,3}, Q::Array{Float64,3},
+                              F::Array{Float64,3}, Z::Matrix{Float64}, i0::Integer, H::Integer; n_boot::Integer = 0, block::Integer = 1,
+                              q::Integer = 0, seed::Integer = 0, ids = nothing, scale = nothing)
+    h = gethandle()
+    N, r, B = size(Lam); p = size(A, 2) ÷ r; Tp = size(F, 1); ni = size(Z, 2); nr = 1 + n_boot
+    om = Array{Float64}(undef, r, nr, ni, B); resp = Array{Float64}(undef, N, H, nr, ni, B); fevd = similar(resp)
+    eps = Array{Float64}(undef, Tp, ni, B); nobs = Array{Cint}(undef, ni, B); rel = Array{Float64}(undef, ni, B)
+    fpi = similar(rel); fF = similar(rel); st = Array{Cint}(undef, ni, B)
+    sc = scale === nothing ? Float64[] : Vector{Float64}(scale)
+    iv = ids === nothing ? Culonglong[] : Vector{Culonglong}(ids)
+    GC.@preserve Lam R A Q F Z om resp fevd eps nobs rel fpi fF st sc iv begin
+        models = Ref(EmInit(pointer(Lam), pointer(R), pointer(A), pointer(Q), C_NULL))
+        opts = Ref(ProxyOpts(N, r, p, B, Tp, H, ni, i0, q, block, n_boot, seed, MEM_HOST))
+        out = Ref(ProxyOut(pointer(om), pointer(resp), pointer(fevd), pointer(eps), pointer(nobs), pointer(rel), pointer(fpi), pointer(fF),
+                           pointer(st)))
+        check(ccall((:dfm_proxy_identification, LIB), Cint,
+                    (Ptr{Cvoid}, Ref{EmInit}, Ptr{Cdouble}, Ptr{Cdouble}, Ptr{Culonglong}, Ptr{Cdouble}, Ref{ProxyOpts}, Ref{ProxyOut}),
+                    h, models, pointer(F), pointer(Z), ids === nothing ? C_NULL : pointer(iv), scale === nothing ? C_NULL : pointer(sc),
+                    opts, out), "dfm_proxy_identification")
+    end
+    return (omega = om, resp = resp, fevd = fevd, eps = eps, n_obs = nobs, reliability = rel, fs_pi = fpi, fs_F = fF, status = st)
+end
+
 end # module
