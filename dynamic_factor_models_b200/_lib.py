@@ -234,6 +234,29 @@ def from_cm(buf, rows, cols, batch=None):
     return np.ascontiguousarray(buf.reshape(batch, cols, rows).transpose(0, 2, 1))
 
 
+class _Models:
+    """Fitted models (Lam (B, N, r), R (B, N), A (B, r, k), Q (B, r, r)), or one model (2-D Lam), in the column-major buffers of
+    dfm_em_init, with the per-series scale (N,) (None = 1).  b: B, or None for one model; models, scale: the addresses the
+    *_raw calls take (scale 0 = 1)."""
+
+    def __init__(self, Lam, R, A, Q, scale):
+        Lam = np.asarray(Lam, float)
+        self.b = Lam.shape[0] if Lam.ndim == 3 else None
+        self.B = self.b or 1
+        self.N, self.r = Lam.shape[-2:]
+        self.p = np.asarray(A).shape[-1] // self.r
+        self._bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
+        self._sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
+        self.models = {n_: a_.ctypes.data for n_, a_ in self._bufs.items()}
+        self.scale = self._sc.ctypes.data if self._sc is not None else 0
+
+    def results(self, res, ints=("status",)):
+        """res (arrays with a leading batch axis) without that axis for one model, those named in `ints` as Python ints."""
+        if self.b:
+            return res
+        return {n_: int(v[0]) if n_ in ints else v[0] for n_, v in res.items()}
+
+
 def _lam_constr(constr, r):
     """(index, H (n_c x r), h) -> (LamConstr, the arrays it points to).  None entries become NULL pointers (the library refuses
     them when n_c > 0)."""
@@ -496,21 +519,18 @@ class Library:
         """Series responses and variance decompositions of models (Lam (B, N, r), R (B, N), A (B, r, k), Q (B, r, r)), or of one
         model (2-D Lam) (dfm_series_responses): resp / fevd (B, N, H, n_shock) -- those named in `outputs` -- and status (B),
         without the batch axis for one model.  scale: (N,) per-series scale of resp (None = 1)."""
-        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
-        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        m = _Models(Lam, R, A, Q, scale)
+        B, N, r = m.B, m.N, m.r
         n_shock = r if n_shock is None else int(n_shock)
-        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
-        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
         outs = {n_: np.full(max(B * N * H * n_shock, 0), np.nan) for n_ in outputs}
         st = np.zeros(B, np.int32)
-        self.series_responses_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, N, r, p, B, H, n_shock,
-                                  sc.ctypes.data if sc is not None else 0, MEM_HOST, resp=outs["resp"].ctypes.data if "resp" in outs else 0,
+        self.series_responses_raw(m.models, N, r, m.p, B, H, n_shock, m.scale, MEM_HOST,
+                                  resp=outs["resp"].ctypes.data if "resp" in outs else 0,
                                   fevd=outs["fevd"].ctypes.data if "fevd" in outs else 0, status=st.ctypes.data)
-        res = dict(status=st if b else int(st[0]))
+        res = dict(status=st)
         for n_, a_ in outs.items():
-            v = a_.reshape(B, n_shock, H, N).transpose(0, 3, 2, 1)
-            res[n_] = np.ascontiguousarray(v if b else v[0])
-        return res
+            res[n_] = np.ascontiguousarray(a_.reshape(B, n_shock, H, N).transpose(0, 3, 2, 1))
+        return m.results(res)
 
     def historical_decomposition_raw(self, models, F, N, r, p, Tp, t0, n_shock, n_model, scale, mem, shocks=0, contrib=0, rest=0, base=0,
                                      status=0):
@@ -529,26 +549,22 @@ class Library:
         (B, Tp, r), contrib (B, N, Tp, n_shock), rest, base (B, N, Tp) -- those named in `outputs` -- and status (B), without the
         batch axis for one model.  scale: (N,) per-series scale (None = 1).  The arrays are views of the column-major buffers the
         library wrote (no copy: the draws of a long Gibbs run take gigabytes)."""
-        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
-        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        m = _Models(Lam, R, A, Q, scale)
+        B, N, r = m.B, m.N, m.r
         F = np.asarray(F, float); Tp = F.shape[-2]
         n_shock = r if n_shock is None else int(n_shock)
-        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
         Fb = to_cm(F)
-        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
         size = dict(shocks=Tp * r, contrib=N * Tp * n_shock, rest=N * Tp, base=N * Tp)
         outs = {n_: np.full(B * size[n_], np.nan) for n_ in outputs}
         st = np.zeros(B, np.int32)
-        self.historical_decomposition_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, Fb.ctypes.data, N, r, p, Tp, t0, n_shock, B,
-                                          sc.ctypes.data if sc is not None else 0, MEM_HOST,
+        self.historical_decomposition_raw(m.models, Fb.ctypes.data, N, r, m.p, Tp, t0, n_shock, B, m.scale, MEM_HOST,
                                           status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
-        res = dict(status=st if b else int(st[0]))
+        res = dict(status=st)
         shape = dict(shocks=(B, r, Tp), contrib=(B, n_shock, Tp, N), rest=(B, Tp, N), base=(B, Tp, N))
         for n_, a_ in outs.items():
             v = a_.reshape(shape[n_])
-            v = v.transpose(0, 3, 2, 1) if v.ndim == 4 else v.transpose(0, 2, 1)
-            res[n_] = v if b else v[0]
-        return res
+            res[n_] = v.transpose(0, 3, 2, 1) if v.ndim == 4 else v.transpose(0, 2, 1)
+        return m.results(res)
 
     def sign_restrictions_raw(self, models, ids, N, r, p, n_model, H, n_shock, n_rot, n_keep, seed, restr, scale, mem, n_accept=0,
                               cand=0, rot=0, resp=0, fevd=0, status=0):
@@ -575,28 +591,24 @@ class Library:
         sequences (series 0-based, shock 1-based).  Returns n_accept (B), cand (B, n_keep), rot (B, n_keep, r, r), resp / fevd
         (B, n_keep, N, H, n_shock) -- those named in `outputs` -- and status (B), without the batch axis for one model.
         n_shock defaults to the last restricted shock (1 without rows).  The arrays are views of the buffers the library wrote."""
-        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
-        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        m = _Models(Lam, R, A, Q, scale)
+        B, N, r = m.B, m.N, m.r
         restr = [np.asarray(v, dtype=np.int64).ravel() for v in restr]
         if n_shock is None:
             n_shock = int(restr[2].max()) if len(restr[2]) else 1
-        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
-        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
         size = dict(rot=n_keep * r * r, resp=n_keep * N * H * n_shock, fevd=n_keep * N * H * n_shock)
         outs = {n_: np.full(B * size[n_], np.nan) for n_ in outputs}
         na = np.zeros(B, np.int64); ca = np.zeros(B * n_keep, np.int64); st = np.zeros(B, np.int32)
-        self.sign_restrictions_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, ids, N, r, p, B, H, n_shock, n_rot, n_keep, seed,
-                                   restr, sc.ctypes.data if sc is not None else 0, MEM_HOST, n_accept=na.ctypes.data,
-                                   cand=ca.ctypes.data, status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        self.sign_restrictions_raw(m.models, ids, N, r, m.p, B, H, n_shock, n_rot, n_keep, seed, restr, m.scale, MEM_HOST,
+                                   n_accept=na.ctypes.data, cand=ca.ctypes.data, status=st.ctypes.data,
+                                   **{n_: a_.ctypes.data for n_, a_ in outs.items()})
         res = dict(n_accept=na, cand=ca.reshape(B, n_keep), status=st)
         for n_, a_ in outs.items():
             if n_ == "rot":
                 res[n_] = a_.reshape(B, n_keep, r, r).transpose(0, 1, 3, 2)
             else:
                 res[n_] = a_.reshape(B, n_keep, n_shock, H, N).transpose(0, 1, 4, 3, 2)
-        if not b:
-            res = {n_: (v[0] if n_ != "status" else int(v[0])) for n_, v in res.items()}
-        return res
+        return m.results(res)
 
     def narrative_sign_restrictions_raw(self, models, F, ids, N, r, p, n_model, H, n_shock, n_rot, n_keep, seed, Tp, n_sim, restr,
                                         narr, scale, mem, n_accept=0, cand=0, rot=0, resp=0, fevd=0, status=0, n_ok=0, weight=0, eps=0):
@@ -629,24 +641,21 @@ class Library:
         as sign_restrictions; narr: rows (kind, shock, series, row, h, sign) as six int sequences (kind 0..3, shock 1-based, series
         and row 0-based).  Returns sign_restrictions' arrays and n_ok, weight (B, n_keep), eps (B, n_keep, Tp, n_shock) -- those
         named in `outputs` -- without the batch axis for one model.  n_shock defaults to the last restricted shock of either kind."""
-        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
-        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        m = _Models(Lam, R, A, Q, scale)
+        B, N, r = m.B, m.N, m.r
         F = np.asarray(F, float); Tp = F.shape[-2]
         restr = [np.asarray(v, dtype=np.int64).ravel() for v in restr]
         narr = [np.asarray(v, dtype=np.int64).ravel() for v in narr]
         if n_shock is None:
             n_shock = max([1] + [int(v.max()) for v in (restr[2], narr[1]) if len(v)])
-        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
         Fb = to_cm(F)
-        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
         size = dict(rot=n_keep * r * r, resp=n_keep * N * H * n_shock, fevd=n_keep * N * H * n_shock, n_ok=n_keep, weight=n_keep,
                     eps=n_keep * Tp * n_shock)
         outs = {n_: (np.zeros(B * size[n_], np.int64) if n_ == "n_ok" else np.full(B * size[n_], np.nan)) for n_ in outputs}
         na = np.zeros(B, np.int64); ca = np.zeros(B * n_keep, np.int64); st = np.zeros(B, np.int32)
-        self.narrative_sign_restrictions_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, Fb.ctypes.data, ids, N, r, p, B, H, n_shock,
-                                             n_rot, n_keep, seed, Tp, n_sim, restr, narr, sc.ctypes.data if sc is not None else 0,
-                                             MEM_HOST, n_accept=na.ctypes.data, cand=ca.ctypes.data, status=st.ctypes.data,
-                                             **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        self.narrative_sign_restrictions_raw(m.models, Fb.ctypes.data, ids, N, r, m.p, B, H, n_shock, n_rot, n_keep, seed, Tp, n_sim,
+                                             restr, narr, m.scale, MEM_HOST, n_accept=na.ctypes.data, cand=ca.ctypes.data,
+                                             status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
         res = dict(n_accept=na, cand=ca.reshape(B, n_keep), status=st)
         for n_, a_ in outs.items():
             if n_ == "rot":
@@ -657,9 +666,7 @@ class Library:
                 res[n_] = a_.reshape(B, n_keep, n_shock, Tp).transpose(0, 1, 3, 2)
             else:
                 res[n_] = a_.reshape(B, n_keep, n_shock, H, N).transpose(0, 1, 4, 3, 2)
-        if not b:
-            res = {n_: (v[0] if n_ != "status" else int(v[0])) for n_, v in res.items()}
-        return res
+        return m.results(res)
 
     def proxy_identification_raw(self, models, F, Z, ids, N, r, p, n_model, Tp, H, n_inst, i0, q, block, n_boot, seed, scale, mem,
                                  omega=0, resp=0, fevd=0, eps=0, n_obs=0, reliability=0, fs_pi=0, fs_F=0, status=0):
@@ -685,22 +692,19 @@ class Library:
         fevd (B, n_inst, 1 + n_boot, N, H), eps (B, n_inst, Tp), n_obs, reliability, fs_pi, fs_F (B, n_inst) -- those named in
         `outputs` -- and status (B, n_inst), without the batch axis for one model.  The arrays are views of the buffers the library
         wrote."""
-        Lam = np.asarray(Lam, float); b = Lam.shape[0] if Lam.ndim == 3 else None; B = b or 1
-        N, r = Lam.shape[-2:]; k = np.asarray(A).shape[-1]; p = k // r
+        m = _Models(Lam, R, A, Q, scale)
+        B, N, r = m.B, m.N, m.r
         F = np.asarray(F, float); Tp = F.shape[-2]
         Z = np.asarray(Z, float)
         Z = Z.reshape(Tp, -1) if Z.ndim == 1 else Z
         ni = Z.shape[1]
-        bufs = dict(Lam=to_cm(Lam), R=np.ascontiguousarray(R, dtype=float).ravel(), A=to_cm(A), Q=to_cm(Q))
         Fb, Zb = to_cm(F), to_cm(Z)
-        sc = np.ascontiguousarray(scale, dtype=float) if scale is not None else None
         nr = 1 + n_boot
         size = dict(omega=ni * nr * r, resp=ni * nr * N * H, fevd=ni * nr * N * H, eps=ni * Tp, n_obs=ni, reliability=ni, fs_pi=ni, fs_F=ni)
         outs = {n_: (np.zeros(B * size[n_], np.int32) if n_ == "n_obs" else np.full(B * size[n_], np.nan)) for n_ in outputs}
         st = np.zeros(B * ni, np.int32)
-        self.proxy_identification_raw({n_: a_.ctypes.data for n_, a_ in bufs.items()}, Fb.ctypes.data, Zb.ctypes.data, ids, N, r, p, B, Tp,
-                                      H, ni, i0, q, block, n_boot, seed, sc.ctypes.data if sc is not None else 0, MEM_HOST,
-                                      status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
+        self.proxy_identification_raw(m.models, Fb.ctypes.data, Zb.ctypes.data, ids, N, r, m.p, B, Tp, H, ni, i0, q, block, n_boot, seed,
+                                      m.scale, MEM_HOST, status=st.ctypes.data, **{n_: a_.ctypes.data for n_, a_ in outs.items()})
         res = dict(status=st.reshape(B, ni))
         for n_, a_ in outs.items():
             if n_ == "omega":
@@ -711,9 +715,7 @@ class Library:
                 res[n_] = a_.reshape(B, ni, Tp)
             else:
                 res[n_] = a_.reshape(B, ni)
-        if not b:
-            res = {n_: v[0] for n_, v in res.items()}
-        return res
+        return m.results(res, ints=())
 
     def estimate_factor_raw(self, X, T, N, r, B, mem, F=0, Lam=0, nt_min=20, tol=1e-8, max_iter=100000000, F_init=0):
         o = FactorOpts(T=T, N=N, r=r, nt_min=nt_min, tol=tol, max_iter=max_iter, compute_r2=0, batch=B, mem=mem)

@@ -2146,83 +2146,272 @@ int dfm_gibbs_constrained(dfm_handle* h, const double* X, const dfm_gibbs_opts* 
   return gibbs_impl(h, X, o, init, ref, constr, out);
 }
 
-// ------------------------------------------------------------------------------------ series responses / FEVD
-// Per chunk of models (a size fixed by the shapes, so that device memory does not grow with n_model): k_sr_prep -> k_irf (all r
-// shocks) -> k_series_resp.  Host arrays are staged per chunk; device outputs are written in place.
-int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r, int p, int n_model, int H, int n_shock,
-                         const double* scale, int mem, double* resp, double* fevd, int* status) {
-  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || N <= 0 || r <= 0 || r > 64 || p <= 0 ||
-      n_model <= 0 || H <= 0 || n_shock <= 0 || n_shock > r || (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
-    return fail(h, DFM_ERR_ARG, "dfm_series_responses: bad argument");
-  const int k = r * p;
-  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nout = (size_t)N * H * n_shock;
-  const size_t sm0 = series_resp_smem_doubles(r, n_shock, 0);
-  if ((sm0 + rr) * 8 > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: r too large");
-  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
-  const size_t smR = series_resp_smem_doubles(r, n_shock, hc) * 8;
-  const size_t smI = irf_smem_doubles(k) * 8;
-  if (smI > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: state dimension r*p too large (r*p > 14076)");
-  const bool hst = mem == DFM_MEM_HOST;
-  const size_t per = 8 * (kk + 2 * rk + rr * H + (hst ? Nr + N + rk + rr + (resp ? nout : 0) + (fevd ? nout : 0) : 0)) + 8;
-  const int nb = (int)std::min<long long>({(long long)n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)), 65535LL});
-  CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    const size_t B = nb;
-    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
-           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
-           *dS = hst && scale ? a.get<double>(N) : nullptr;
-    double *dRe = hst && resp ? a.get<double>(B * nout) : nullptr, *dFe = hst && fevd ? a.get<double>(B * nout) : nullptr;
-    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H);
-    int* dst = a.get<int>(B);
-    int* ids = a.get<int>(r);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    std::vector<int> hid(r);
-    for (int j = 0; j < r; ++j) hid[j] = j;
-    CK(cudaMemcpyAsync(ids, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    const double* sc = scale;
-    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
-    DFM_SET_SMEM(k_series_resp, smR);
-    DFM_SET_SMEM(k_irf, smI);
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------ model batches
+// dfm_series_responses, dfm_historical_decomposition, dfm_sign_restrictions, dfm_narrative_sign_restrictions and
+// dfm_proxy_identification take n_model fitted models (dfm_em_init, back to back) and run over them in chunks of models, a size
+// fixed by the shapes so that device memory does not grow with n_model.  ModelChunks reads the models a chunk at a time and runs
+// the launches all of them start with; an OutSlot puts one output where the caller wants it.
+namespace {
+
+bool models_ok(const dfm_em_init* m) { return m && m->Lam && m->R && m->A && m->Q; }
+
+// every model id below 2^40 (ids == nullptr: the ids are 0 .. n_model-1)
+bool ids_ok(const unsigned long long* ids, int n_model) {
+  for (int b = 0; ids && b < n_model; ++b)
+    if (ids[b] >= (1ull << 40)) return false;
+  return true;
+}
+
+// k_series_resp's plan for n_shock shocks to horizon H: hc horizons staged per pass (0: not even one fits), smR bytes of shared
+// memory
+struct SrPlan {
+  int hc;
+  size_t smR;
+};
+SrPlan series_resp_plan(int r, int n_shock, int H) {
+  const size_t sm0 = series_resp_smem_doubles(r, n_shock, 0), rr = (size_t)r * r;
+  const int hc = sm0 + rr > kMaxSmem / 8 ? 0 : (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
+  return {hc, series_resp_smem_doubles(r, n_shock, hc) * 8};
+}
+
+// Sign-restriction rows sorted by shock (stable): shock j's rows are off[j] .. off[j+1]-1; nj = the last restricted shock + 1
+// (0-based), 0 without rows.  alloc and upload give the kernels their device copies.
+struct SignRows {
+  std::vector<int> series, horizon, sign, off;
+  int nj = 0;
+  int *d_series = nullptr, *d_horizon = nullptr, *d_sign = nullptr, *d_off = nullptr;
+  void alloc(Arena& a) {
+    d_off = a.get<int>(off.size());
+    d_series = a.get<int>(series.size() + 1);
+    d_horizon = a.get<int>(series.size() + 1);
+    d_sign = a.get<int>(series.size() + 1);
+  }
+  int upload(dfm_handle* h) const {
+    CK(cudaMemcpyAsync(d_off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    if (series.empty()) return DFM_OK;
+    CK(cudaMemcpyAsync(d_series, series.data(), series.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_horizon, horizon.data(), series.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_sign, sign.data(), series.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    return DFM_OK;
+  }
+};
+
+// rs's rows for n_shock shocks of N series to horizon H, range-checked (DFM_ERR_ARG with msg) and sorted into *s
+int sign_rows(dfm_handle* h, const dfm_sign_restr* rs, int N, int H, int n_shock, const char* msg, SignRows* s) {
+  for (int q = 0; q < rs->n; ++q)
+    if (rs->series[q] < 0 || rs->series[q] >= N || rs->horizon[q] < 0 || rs->horizon[q] >= H || rs->shock[q] < 1 ||
+        rs->shock[q] > n_shock || (rs->sign[q] != 1 && rs->sign[q] != -1))
+      return fail(h, DFM_ERR_ARG, msg);
+  s->off.assign(n_shock + 1, 0);
+  for (int j = 1; j <= n_shock; ++j) {
+    for (int q = 0; q < rs->n; ++q) {
+      if (rs->shock[q] != j) continue;
+      s->series.push_back(rs->series[q]);
+      s->horizon.push_back(rs->horizon[q]);
+      s->sign.push_back(rs->sign[q]);
+      s->nj = j;
+    }
+    s->off[j] = (int)s->series.size();
+  }
+  return DFM_OK;
+}
+
+// One output of a model-batch entry point: dst, the caller's array of `per` elements a model (nullptr: not asked for).  The
+// kernels write buf when there is one, else dst in place; flush copies what they wrote to dst.
+template <typename T> struct OutSlot {
+  T* dst = nullptr;
+  T* buf = nullptr;
+  size_t per = 0;
+  // where the kernels write the chunk that starts at model j0 (nullptr: nowhere)
+  T* at(long long j0) const { return buf ? buf : dst ? dst + j0 * per : nullptr; }
+  int flush(dfm_handle* h, long long j0, long long n, int mem) const {
+    return copy_out(h, dst ? dst + j0 * per : nullptr, at(j0), n * per, mem);
+  }
+};
+
+// an output the kernels write only when it is asked for: in place in device memory, through a staging buffer to host memory
+template <typename T> OutSlot<T> staged(Arena& a, T* dst, size_t per, size_t B, bool hst) {
+  return {dst, hst && dst ? a.get<T>(B * per) : nullptr, per};
+}
+
+// an output the kernels write whether or not it is asked for: in place when it is asked for in device memory, else into the
+// buffer (allocated either way, so that the chunk size does not depend on dst)
+template <typename T> OutSlot<T> scratch(Arena& a, T* dst, size_t per, size_t B, bool hst) {
+  T* buf = a.get<T>(B * per);
+  return {dst, hst || !dst ? buf : nullptr, per};
+}
+
+// The fitted models of a model-batch entry point, a chunk at a time.  alloc lays out, for B models: the staging of host inputs
+// (Lam, R, A, Q, the Tp x r factor paths F when F is given, and scale), k_sr_prep's outputs, k_irf's when Hi > 0 (all r
+// shocks to horizon Hi) and the chunk's model ids when with_ids (ids == nullptr: model j0 + b has id j0 + b).  Once per call
+// setup uploads k_irf's shock list and scale; once per chunk, load points L_ .. F_ at the chunk's models (staged host arrays,
+// or the caller's device arrays in place), uploads their ids and runs k_sr_prep, then k_irf.
+struct ModelChunks {
+  dfm_handle* h;
+  const dfm_em_init* m;
+  const double *F, *scale;
+  const unsigned long long* ids;
+  int N, r, p, Tp, Hi, mem;
+  bool with_ids, hst;
+  size_t Nr, rk, rr, kk, Tr;
+  double *dL = nullptr, *dR = nullptr, *dA = nullptr, *dQ = nullptr, *dF = nullptr, *dS = nullptr;   // host-input staging
+  double *M = nullptr, *Qs = nullptr, *G = nullptr, *irf = nullptr;  // k_sr_prep's (M, [I 0], [chol(Q); 0]) and k_irf's records
+  int *st = nullptr, *shocks = nullptr;                               // per-model status, k_irf's shocks 0 .. r-1
+  unsigned long long* dId = nullptr;
+  std::vector<unsigned long long> hid;
+  const double *L_ = nullptr, *R_ = nullptr, *A_ = nullptr, *Q_ = nullptr, *F_ = nullptr;   // the chunk's device views
+  const double* sc = nullptr;                                                               // scale's (nullptr: 1)
+
+  ModelChunks(dfm_handle* h, const dfm_em_init* m, int N, int r, int p, const double* scale, int mem, const double* F, int Tp,
+              int Hi, bool with_ids, const unsigned long long* ids)
+      : h(h), m(m), F(F), scale(scale), ids(ids), N(N), r(r), p(p), Tp(Tp), Hi(Hi), mem(mem), with_ids(with_ids),
+        hst(mem == DFM_MEM_HOST), Nr((size_t)N * r), rk((size_t)r * r * p), rr((size_t)r * r),
+        kk((size_t)r * p * r * p), Tr((size_t)Tp * r) {}
+
+  void alloc(Arena& a, size_t B) {
+    if (hst) {
+      dL = a.get<double>(B * Nr);
+      dR = a.get<double>(B * N);
+      dA = a.get<double>(B * rk);
+      dQ = a.get<double>(B * rr);
+      dF = F ? a.get<double>(B * Tr) : nullptr;
+      dS = scale ? a.get<double>(N) : nullptr;
+    }
+    M = a.get<double>(B * kk);
+    Qs = a.get<double>(B * rk);
+    G = a.get<double>(B * rk);
+    st = a.get<int>(B);
+    irf = Hi ? a.get<double>(B * rr * Hi) : nullptr;
+    shocks = Hi ? a.get<int>(r) : nullptr;
+    dId = with_ids ? a.get<unsigned long long>(B) : nullptr;
+  }
+
+  // Models per chunk: as many as kSimChunkBytes holds at layout(a, 1)'s bytes each (the 256-byte rounding and the buffers of
+  // fixed size make that at least a B-model layout's bytes over B), at least one, at most cap.  layout(a, B) calls alloc(a, B)
+  // and allocates the caller's own buffers.
+  template <typename Lay> static int chunk_models(Lay&& layout, long long n_model, long long cap) {
+    Arena a(nullptr);
+    layout(a, 1);
+    return (int)std::min<long long>({n_model, std::max<long long>(1, (long long)(kSimChunkBytes / a.off)), cap});
+  }
+
+  // grows the workspace to layout(a, B)'s bytes and lays the buffers out in it; uploads k_irf's shock list and scale
+  template <typename Lay> int setup(Lay&& layout, size_t B) {
+    CK(cudaSetDevice(h->device));
+    Arena probe(nullptr);
+    layout(probe, B);
+    int rc = ensure_ws(h, probe.off);
+    if (rc) return rc;
+    Arena a(h->ws);
+    layout(a, B);
+    if (Hi) {
+      std::vector<int> all(r);
+      for (int j = 0; j < r; ++j) all[j] = j;
+      CK(cudaMemcpyAsync(shocks, all.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      DFM_SET_SMEM(k_irf, irf_smem_doubles(r * p) * 8);
+    }
+    sc = scale;
+    if (hst && scale) {
+      CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream));
+      sc = dS;
+    }
+    return DFM_OK;
+  }
+
+  int load(long long j0, int nm) {
+    L_ = m->Lam + j0 * Nr;
+    R_ = m->R + j0 * N;
+    A_ = m->A + j0 * rk;
+    Q_ = m->Q + j0 * rr;
+    F_ = F ? F + j0 * Tr : nullptr;
+    int rc = stage_in(h, L_, dL, nm * Nr, mem, &L_);
+    if (!rc) rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_);
+    if (!rc) rc = stage_in(h, A_, dA, nm * rk, mem, &A_);
+    if (!rc) rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_);
+    if (!rc && F) rc = stage_in(h, F_, dF, nm * Tr, mem, &F_);
+    if (rc) return rc;
+    if (with_ids) {
+      hid.resize(nm);
+      for (int b = 0; b < nm; ++b) hid[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
+      CK(cudaMemcpyAsync(dId, hid.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+    }
+    L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, M, Qs, G, st);
+    if (Hi)
+      L(k_irf, r, nm, 64, irf_smem_doubles(r * p) * 8, (const double*)M, (const double*)Qs, (const double*)G, r * p, r, Hi, r,
+        (const int*)shocks, irf);
+    return DFM_OK;
+  }
+
+  // body(j0, nm) on each chunk of nb models, after load(j0, nm).  On the host path the stream is synchronised at the end of each
+  // chunk, because the next one reuses the staging buffers.
+  template <typename Body> int run(long long n_model, int nb, Body&& body) {
     for (long long j0 = 0; j0 < n_model; j0 += nb) {
       const int nm = (int)std::min<long long>(nb, n_model - j0);
-      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr;
-      int rc = DFM_OK;
-      if (hst) {
-        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
-        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
-        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
-        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
-      }
-      double* oR = resp ? (hst ? dRe : resp + j0 * nout) : nullptr;
-      double* oF = fevd ? (hst ? dFe : fevd + j0 * nout) : nullptr;
-      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
-      L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)ids, dI);
-      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm, SR_NS, smR, L_, R_, sc, (const double*)dI, (const int*)dst, N, r, H, n_shock, hc, 1, oR, oF);
-      if (hst) {
-        rc = copy_out(h, resp ? resp + j0 * nout : nullptr, dRe, nm * nout, mem); if (rc) return rc;
-        rc = copy_out(h, fevd ? fevd + j0 * nout : nullptr, dFe, nm * nout, mem); if (rc) return rc;
-      }
-      rc = copy_out(h, status ? status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
-      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+      int rc = load(j0, nm);
+      if (!rc) rc = body(j0, nm);
+      if (rc) return rc;
+      if (hst) CK(cudaStreamSynchronize(h->stream));
     }
+    return finish(h, mem);
   }
-  return finish(h, mem);
+
+  // the copy-back of the nm models from j0 of every slot, up to the first error
+  template <typename... T> int flush(long long j0, long long nm, const OutSlot<T>&... s) const {
+    int rc = DFM_OK;
+    ((rc = rc ? rc : s.flush(h, j0, nm, mem)), ...);
+    return rc;
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+// ------------------------------------------------------------------------------------ series responses / FEVD
+// Per chunk of models (ModelChunks): k_sr_prep -> k_irf (all r shocks) -> k_series_resp.
+int dfm_series_responses(dfm_handle* h, const dfm_em_init* models, int N, int r, int p, int n_model, int H, int n_shock,
+                         const double* scale, int mem, double* resp, double* fevd, int* status) {
+  if (!h || !models_ok(models) || N <= 0 || r <= 0 || r > 64 || p <= 0 || n_model <= 0 || H <= 0 || n_shock <= 0 || n_shock > r ||
+      (mem != DFM_MEM_HOST && mem != DFM_MEM_DEVICE))
+    return fail(h, DFM_ERR_ARG, "dfm_series_responses: bad argument");
+  const SrPlan sp = series_resp_plan(r, n_shock, H);
+  if (!sp.hc) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: r too large");
+  if (irf_smem_doubles(r * p) * 8 > kMaxSmem)
+    return fail(h, DFM_ERR_UNSUPPORTED, "dfm_series_responses: state dimension r*p too large (r*p > 14076)");
+  const bool hst = mem == DFM_MEM_HOST;
+  const size_t nout = (size_t)N * H * n_shock;
+  ModelChunks mc(h, models, N, r, p, scale, mem, nullptr, 0, H, false, nullptr);
+  OutSlot<double> oRe, oFe;
+  auto layout = [&](Arena& a, size_t B) {
+    mc.alloc(a, B);
+    oRe = staged(a, resp, nout, B, hst);
+    oFe = staged(a, fevd, nout, B, hst);
+  };
+  const int nb = ModelChunks::chunk_models(layout, n_model, kMaxGridBatch);
+  int rc = mc.setup(layout, nb);
+  if (rc) return rc;
+  DFM_SET_SMEM(k_series_resp, sp.smR);
+  const OutSlot<int> ost{status, mc.st, 1};
+  return mc.run(n_model, nb, [&](long long j0, int nm) {
+    L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm, SR_NS, sp.smR, mc.L_, mc.R_, mc.sc, (const double*)mc.irf, (const int*)mc.st, N, r, H,
+      n_shock, sp.hc, 1, oRe.at(j0), oFe.at(j0));
+    return mc.flush(j0, nm, oRe, oFe, ost);
+  });
 }
 
 // ------------------------------------------------------------------------------------ historical decompositions
-// Per chunk of models (a size fixed by the shapes, so that device memory does not grow with n_model): k_sr_prep -> k_hd_paths
-// -> k_hd_series.  Host arrays are staged per chunk; device outputs are written in place (the shocks too, when requested).
+// Per chunk of models (ModelChunks): k_sr_prep -> k_hd_paths -> k_hd_series.  The shocks are written to scratch when they are not
+// asked for.
 int dfm_historical_decomposition(dfm_handle* h, const dfm_em_init* models, const double* F, const double* scale,
                                  const dfm_hd_opts* o, const dfm_hd_out* out) {
-  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !F || !o || !out || o->N <= 0 || o->r <= 0 ||
-      o->p <= 0 || o->Tp <= 0 || o->n_model <= 0 || o->t0 < o->p - 1 || o->t0 >= o->Tp || o->n_shock < 1 || o->n_shock > o->r ||
-      (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+  if (!h || !models_ok(models) || !F || !o || !out || o->N <= 0 || o->r <= 0 || o->p <= 0 || o->Tp <= 0 || o->n_model <= 0 ||
+      o->t0 < o->p - 1 || o->t0 >= o->Tp || o->n_shock < 1 || o->n_shock > o->r || (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
     return fail(h, DFM_ERR_ARG, "dfm_historical_decomposition: bad argument");
-  const int N = o->N, r = o->r, p = o->p, Tp = o->Tp, ns = o->n_shock, nc = ns + 2, k = r * p, mem = o->mem;
-  if (k > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_historical_decomposition: state dimension r*p > 48");
-  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, Tr = (size_t)Tp * r;
-  const size_t nY = (size_t)nc * Tr, nC = (size_t)N * Tp * ns, nB = (size_t)N * Tp;
+  const int N = o->N, r = o->r, p = o->p, Tp = o->Tp, ns = o->n_shock, nc = ns + 2, mem = o->mem;
+  if (r * p > 48) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_historical_decomposition: state dimension r*p > 48");
+  const size_t Tr = (size_t)Tp * r, nY = (size_t)nc * Tr, nC = (size_t)N * Tp * ns, nB = (size_t)N * Tp;
   const size_t smP = hd_paths_smem_doubles(r, p, nc) * 8;
   // rows of the recursions staged per pass of k_hd_series: about 16 KB of shared memory in all (at least one row), so that many
   // CTAs share an SM
@@ -2230,184 +2419,108 @@ int dfm_historical_decomposition(dfm_handle* h, const dfm_em_init* models, const
   const int tc = (int)std::min<size_t>((size_t)Tp, (budget - (size_t)r * HD_NS) / ((size_t)nc * r));
   const size_t smS = hd_series_smem_doubles(r, nc, tc) * 8;
   const bool hst = mem == DFM_MEM_HOST;
-  const size_t per = 8 * (kk + 2 * rk + nY + Tr + (hst ? Nr + N + rk + rr + Tr + (out->contrib ? nC : 0) + (out->rest ? nB : 0) +
-                                                        (out->base ? nB : 0) : 0)) + 8;
-  const int nb = (int)std::min<long long>({(long long)o->n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)), 65535LL});
-  CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    const size_t B = nb;
-    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
-           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
-           *dF = hst ? a.get<double>(B * Tr) : nullptr, *dS = hst && scale ? a.get<double>(N) : nullptr;
-    double *dC = hst && out->contrib ? a.get<double>(B * nC) : nullptr, *dRs = hst && out->rest ? a.get<double>(B * nB) : nullptr,
-           *dB = hst && out->base ? a.get<double>(B * nB) : nullptr;
-    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dE = a.get<double>(B * Tr),
-           *dY = a.get<double>(B * nY);
-    int* dst = a.get<int>(B);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* sc = scale;
-    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
-    DFM_SET_SMEM(k_hd_paths, smP);
-    // k_hd_series holds each series' loadings in RM >= r registers
-    auto series = [&](auto rm, const double* L_, const double* R_, int nm, double* oC, double* oR, double* oB) {
-      constexpr int RM = decltype(rm)::value;
-      DFM_SET_SMEM(k_hd_series<RM>, smS);
-      L(k_hd_series<RM>, (N + HD_NS - 1) / HD_NS, nm, HD_NS, smS, L_, R_, sc, (const double*)dY, (const int*)dst, N, r, Tp, ns, tc, oC,
-        oR, oB);
-    };
-    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
-      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
-      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr,
-                   *F_ = F + j0 * Tr;
-      int rc = DFM_OK;
-      if (hst) {
-        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
-        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
-        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
-        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
-        rc = stage_in(h, F_, dF, nm * Tr, mem, &F_); if (rc) return rc;
-      }
-      double* oE = out->shocks && !hst ? out->shocks + j0 * Tr : dE;
-      double* oC = out->contrib ? (hst ? dC : out->contrib + j0 * nC) : nullptr;
-      double* oR = out->rest ? (hst ? dRs : out->rest + j0 * nB) : nullptr;
-      double* oB = out->base ? (hst ? dB : out->base + j0 * nB) : nullptr;
-      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
-      L(k_hd_paths, nm, 1, HD_PT, smP, (const double*)dM, (const double*)dG, F_, r, p, Tp, o->t0, ns, dst, oE, dY);
-      if (r <= 8) series(std::integral_constant<int, 8>(), L_, R_, nm, oC, oR, oB);
-      else if (r <= 16) series(std::integral_constant<int, 16>(), L_, R_, nm, oC, oR, oB);
-      else if (r <= 32) series(std::integral_constant<int, 32>(), L_, R_, nm, oC, oR, oB);
-      else series(std::integral_constant<int, 48>(), L_, R_, nm, oC, oR, oB);
-      if (hst) {
-        rc = copy_out(h, out->shocks ? out->shocks + j0 * Tr : nullptr, dE, nm * Tr, mem); if (rc) return rc;
-        rc = copy_out(h, out->contrib ? out->contrib + j0 * nC : nullptr, dC, nm * nC, mem); if (rc) return rc;
-        rc = copy_out(h, out->rest ? out->rest + j0 * nB : nullptr, dRs, nm * nB, mem); if (rc) return rc;
-        rc = copy_out(h, out->base ? out->base + j0 * nB : nullptr, dB, nm * nB, mem); if (rc) return rc;
-      }
-      rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
-      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
-    }
-  }
-  return finish(h, mem);
+  ModelChunks mc(h, models, N, r, p, scale, mem, F, Tp, 0, false, nullptr);
+  OutSlot<double> oE, oC, oR, oB;
+  double* dY = nullptr;
+  auto layout = [&](Arena& a, size_t B) {
+    mc.alloc(a, B);
+    oE = scratch(a, out->shocks, Tr, B, hst);
+    oC = staged(a, out->contrib, nC, B, hst);
+    oR = staged(a, out->rest, nB, B, hst);
+    oB = staged(a, out->base, nB, B, hst);
+    dY = a.get<double>(B * nY);
+  };
+  const int nb = ModelChunks::chunk_models(layout, o->n_model, kMaxGridBatch);
+  int rc = mc.setup(layout, nb);
+  if (rc) return rc;
+  DFM_SET_SMEM(k_hd_paths, smP);
+  const OutSlot<int> ost{out->status, mc.st, 1};
+  // k_hd_series holds each series' loadings in RM >= r registers
+  auto series = [&](auto rm, long long j0, int nm) {
+    constexpr int RM = decltype(rm)::value;
+    DFM_SET_SMEM(k_hd_series<RM>, smS);
+    L(k_hd_series<RM>, (N + HD_NS - 1) / HD_NS, nm, HD_NS, smS, mc.L_, mc.R_, mc.sc, (const double*)dY, (const int*)mc.st, N, r, Tp, ns,
+      tc, oC.at(j0), oR.at(j0), oB.at(j0));
+  };
+  return mc.run(o->n_model, nb, [&](long long j0, int nm) {
+    L(k_hd_paths, nm, 1, HD_PT, smP, (const double*)mc.M, (const double*)mc.G, mc.F_, r, p, Tp, o->t0, ns, mc.st, oE.at(j0), dY);
+    if (r <= 8) series(std::integral_constant<int, 8>(), j0, nm);
+    else if (r <= 16) series(std::integral_constant<int, 16>(), j0, nm);
+    else if (r <= 32) series(std::integral_constant<int, 32>(), j0, nm);
+    else series(std::integral_constant<int, 48>(), j0, nm);
+    return mc.flush(j0, nm, oE, oC, oR, oB, ost);
+  });
 }
 
 // ------------------------------------------------------------------------------------ sign restrictions
-// Per chunk of models (a size fixed by the shapes): k_sr_prep -> k_irf (all r shocks) -> k_sign_prep -> per batch of candidates
-// (a size fixed by n_rot) k_sign_cand -> k_sign_pick -> k_sign_rot -> k_series_resp on the n_keep rotated records of every model.
-// Host arrays are staged per chunk; device outputs are written in place.
+// Per chunk of models (ModelChunks; at most 65 535 rotated records): k_sr_prep -> k_irf (all r shocks) -> k_sign_prep -> per batch
+// of candidates (a size fixed by n_rot) k_sign_cand -> k_sign_pick -> k_sign_rot -> k_series_resp on the n_keep rotated records
+// of every model.
 int dfm_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const unsigned long long* ids, const double* scale,
                           const dfm_sign_opts* o, const dfm_sign_restr* rs, const dfm_sign_out* out) {
-  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !o || !rs || !out || o->N <= 0 || o->r <= 0 ||
-      o->p <= 0 || o->n_model <= 0 || o->H <= 0 || o->n_shock < 1 || o->n_shock > o->r || o->n_rot < 1 || o->n_keep < 1 ||
-      rs->n < 0 || (rs->n > 0 && (!rs->series || !rs->horizon || !rs->shock || !rs->sign)) ||
-      (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+  if (!h || !models_ok(models) || !o || !rs || !out || o->N <= 0 || o->r <= 0 || o->p <= 0 || o->n_model <= 0 || o->H <= 0 ||
+      o->n_shock < 1 || o->n_shock > o->r || o->n_rot < 1 || o->n_keep < 1 || rs->n < 0 ||
+      (rs->n > 0 && (!rs->series || !rs->horizon || !rs->shock || !rs->sign)) || (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
     return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: bad argument");
-  const int N = o->N, r = o->r, p = o->p, H = o->H, ns = o->n_shock, nR = rs->n, nk = o->n_keep, k = r * p, mem = o->mem;
-  for (int q = 0; q < nR; ++q)
-    if (rs->series[q] < 0 || rs->series[q] >= N || rs->horizon[q] < 0 || rs->horizon[q] >= H || rs->shock[q] < 1 ||
-        rs->shock[q] > ns || (rs->sign[q] != 1 && rs->sign[q] != -1))
-      return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: a restriction row outside its range");
-  if (ids)
-    for (int b = 0; b < o->n_model; ++b)
-      if (ids[b] >= (1ull << 40)) return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: a model id >= 2^40");
-  if (r > SG_RMAX || nR > SG_NRMAX || k > 48 || nk > kMaxGridBatch)
+  const int N = o->N, r = o->r, p = o->p, H = o->H, ns = o->n_shock, nR = rs->n, nk = o->n_keep, mem = o->mem;
+  SignRows sr;
+  int rc = sign_rows(h, rs, N, H, ns, "dfm_sign_restrictions: a restriction row outside its range", &sr);
+  if (rc) return rc;
+  if (!ids_ok(ids, o->n_model)) return fail(h, DFM_ERR_ARG, "dfm_sign_restrictions: a model id >= 2^40");
+  if (r > SG_RMAX || nR > SG_NRMAX || r * p > 48 || nk > kMaxGridBatch)
     return fail(h, DFM_ERR_UNSUPPORTED, "dfm_sign_restrictions: r > 16, more than 256 rows, r*p > 48 or n_keep > 65535");
-  // the rows sorted by shock (stable): shock j's rows are off[j] .. off[j+1]-1; nj = the last restricted shock + 1
-  std::vector<int> hs, hh, hg, off(ns + 1, 0);
-  int nj = 0;
-  for (int j = 1; j <= ns; ++j) {
-    for (int q = 0; q < nR; ++q)
-      if (rs->shock[q] == j) { hs.push_back(rs->series[q]); hh.push_back(rs->horizon[q]); hg.push_back(rs->sign[q]); nj = j; }
-    off[j] = (int)hs.size();
-  }
-  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nout = (size_t)N * H * ns;
-  const size_t sm0 = series_resp_smem_doubles(r, ns, 0);
-  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
-  const size_t smR = series_resp_smem_doubles(r, ns, hc) * 8, smI = irf_smem_doubles(k) * 8;
+  const int nj = sr.nj;
+  const size_t rr = (size_t)r * r, nout = (size_t)N * H * ns;
+  const SrPlan sp = series_resp_plan(r, ns, H);
   const size_t smC = sign_cand_smem_bytes(r, nj, nR), smT = sign_rot_smem_bytes(r, nj, nR);
   // candidates per model and batch: whole CTAs of SG_NT, at most 2^20
   const long long nct = std::min<long long>((o->n_rot + SG_NT - 1) / SG_NT, (1LL << 20) / SG_NT);
   const int ntile = (int)(nct * (SG_NT / SG_TILE));
   const bool hst = mem == DFM_MEM_HOST;
-  const size_t per = 8 * (kk + 2 * rk + rr * H + (size_t)nR * r + 2 + nk + (size_t)nk * rr * H +
-                          (hst ? Nr + N + rk + rr + (out->rot ? (size_t)nk * rr : 0) + (out->resp ? nk * nout : 0) +
-                                     (out->fevd ? nk * nout : 0) : 0)) + 4 * ((size_t)ntile + 1 + nk);
-  const int nb = (int)std::min<long long>({(long long)o->n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)),
-                                           (long long)(kMaxGridBatch / nk)});
-  CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    const size_t B = nb;
-    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
-           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
-           *dS = hst && scale ? a.get<double>(N) : nullptr;
-    double *dRo = hst && out->rot ? a.get<double>(B * nk * rr) : nullptr, *dRe = hst && out->resp ? a.get<double>(B * nk * nout) : nullptr,
-           *dFe = hst && out->fevd ? a.get<double>(B * nk * nout) : nullptr;
-    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H),
-           *dC = a.get<double>(B * nR * r + 1), *dRec = a.get<double>(B * nk * rr * H);
-    long long *dNa = a.get<long long>(B), *dCa = a.get<long long>(B * nk);
-    unsigned long long* dId = a.get<unsigned long long>(B);
-    unsigned* dMask = a.get<unsigned>(B * ntile);
-    int *dst = a.get<int>(B), *dSst = a.get<int>(B * nk), *dIr = a.get<int>(r), *dOff = a.get<int>(ns + 1);
-    int *dRs = a.get<int>(nR + 1), *dRh = a.get<int>(nR + 1), *dRg = a.get<int>(nR + 1);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    std::vector<int> hid(r);
-    for (int j = 0; j < r; ++j) hid[j] = j;
-    CK(cudaMemcpyAsync(dIr, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(dOff, off.data(), (ns + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    if (nR) {
-      CK(cudaMemcpyAsync(dRs, hs.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(dRh, hh.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(dRg, hg.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  ModelChunks mc(h, models, N, r, p, scale, mem, nullptr, 0, H, true, ids);
+  OutSlot<double> oRo, oRe, oFe;
+  double *dC = nullptr, *dRec = nullptr;
+  long long *dNa = nullptr, *dCa = nullptr;
+  unsigned* dMask = nullptr;
+  int* dSst = nullptr;
+  auto layout = [&](Arena& a, size_t B) {
+    mc.alloc(a, B);
+    sr.alloc(a);
+    oRo = staged(a, out->rot, nk * rr, B, hst);
+    oRe = staged(a, out->resp, nk * nout, B, hst);
+    oFe = staged(a, out->fevd, nk * nout, B, hst);
+    dC = a.get<double>(B * nR * r + 1);
+    dRec = a.get<double>(B * nk * rr * H);
+    dNa = a.get<long long>(B);
+    dCa = a.get<long long>(B * nk);
+    dMask = a.get<unsigned>(B * ntile);
+    dSst = a.get<int>(B * nk);
+  };
+  const int nb = ModelChunks::chunk_models(layout, o->n_model, kMaxGridBatch / nk);
+  rc = mc.setup(layout, nb);
+  if (!rc) rc = sr.upload(h);
+  if (rc) return rc;
+  DFM_SET_SMEM(k_series_resp, sp.smR);
+  DFM_SET_SMEM(k_sign_cand, smC);
+  DFM_SET_SMEM(k_sign_rot, smT);
+  const OutSlot<long long> ona{out->n_accept, dNa, 1}, oca{out->cand, dCa, (size_t)nk};
+  const OutSlot<int> ost{out->status, mc.st, 1};
+  return mc.run(o->n_model, nb, [&](long long j0, int nm) {
+    double *oRe_ = oRe.at(j0), *oFe_ = oFe.at(j0);
+    L(k_sign_prep, nm, 1, 64, 8, mc.L_, mc.R_, (const double*)mc.irf, N, r, H, nR, (const int*)sr.d_series, (const int*)sr.d_horizon,
+      (const int*)sr.d_sign, nk, mc.st, dC, dNa, dCa);
+    for (long long c0 = 0; c0 < o->n_rot; c0 += (long long)ntile * SG_TILE) {
+      L(k_sign_cand, ntile / (SG_NT / SG_TILE), nm, SG_NT, smC, (const double*)dC, (const int*)sr.d_off, (const int*)mc.st, r, nR, nj,
+        c0, o->n_rot, ntile, o->seed, (const unsigned long long*)mc.dId, dMask);
+      L(k_sign_pick, nm, 1, SG_PT, 2 * SG_PT * sizeof(int), (const unsigned*)dMask, ntile, c0, nk, (const int*)mc.st, dNa, dCa);
     }
-    const double* sc = scale;
-    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
-    DFM_SET_SMEM(k_series_resp, smR);
-    DFM_SET_SMEM(k_irf, smI);
-    DFM_SET_SMEM(k_sign_cand, smC);
-    DFM_SET_SMEM(k_sign_rot, smT);
-    std::vector<unsigned long long> hids(nb);
-    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
-      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
-      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr;
-      int rc = DFM_OK;
-      if (hst) {
-        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
-        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
-        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
-        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
-      }
-      for (int b = 0; b < nm; ++b) hids[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
-      CK(cudaMemcpyAsync(dId, hids.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
-      double* oRo = out->rot ? (hst ? dRo : out->rot + j0 * nk * rr) : nullptr;
-      double* oRe = out->resp ? (hst ? dRe : out->resp + j0 * nk * nout) : nullptr;
-      double* oFe = out->fevd ? (hst ? dFe : out->fevd + j0 * nk * nout) : nullptr;
-      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
-      L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)dIr, dI);
-      L(k_sign_prep, nm, 1, 64, 8, L_, R_, (const double*)dI, N, r, H, nR, (const int*)dRs, (const int*)dRh, (const int*)dRg, nk, dst,
-        dC, dNa, dCa);
-      for (long long c0 = 0; c0 < o->n_rot; c0 += (long long)ntile * SG_TILE) {
-        L(k_sign_cand, ntile / (SG_NT / SG_TILE), nm, SG_NT, smC, (const double*)dC, (const int*)dOff, (const int*)dst, r, nR, nj, c0,
-          o->n_rot, ntile, o->seed, (const unsigned long long*)dId, dMask);
-        L(k_sign_pick, nm, 1, SG_PT, 2 * SG_PT * sizeof(int), (const unsigned*)dMask, ntile, c0, nk, (const int*)dst, dNa, dCa);
-      }
-      L(k_sign_rot, nm * nk, 1, 64, smT, (const double*)dI, (const double*)dC, (const int*)dOff, (const int*)dst, (const long long*)dCa,
-        r, H, nR, nj, nk, o->seed, (const unsigned long long*)dId, oRo, dRec, dSst);
-      if (oRe || oFe)
-        L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm * nk, SR_NS, smR, L_, R_, sc, (const double*)dRec, (const int*)dSst, N, r, H, ns, hc,
-          nk, oRe, oFe);
-      if (hst) {
-        rc = copy_out(h, out->rot ? out->rot + j0 * nk * rr : nullptr, dRo, nm * nk * rr, mem); if (rc) return rc;
-        rc = copy_out(h, out->resp ? out->resp + j0 * nk * nout : nullptr, dRe, nm * nk * nout, mem); if (rc) return rc;
-        rc = copy_out(h, out->fevd ? out->fevd + j0 * nk * nout : nullptr, dFe, nm * nk * nout, mem); if (rc) return rc;
-      }
-      rc = copy_out(h, out->n_accept ? out->n_accept + j0 : nullptr, dNa, nm, mem); if (rc) return rc;
-      rc = copy_out(h, out->cand ? out->cand + j0 * nk : nullptr, dCa, nm * (size_t)nk, mem); if (rc) return rc;
-      rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
-      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
-    }
-  }
-  return finish(h, mem);
+    L(k_sign_rot, nm * nk, 1, 64, smT, (const double*)mc.irf, (const double*)dC, (const int*)sr.d_off, (const int*)mc.st,
+      (const long long*)dCa, r, H, nR, nj, nk, o->seed, (const unsigned long long*)mc.dId, oRo.at(j0), dRec, dSst);
+    if (oRe_ || oFe_)
+      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm * nk, SR_NS, sp.smR, mc.L_, mc.R_, mc.sc, (const double*)dRec, (const int*)dSst, N,
+        r, H, ns, sp.hc, nk, oRe_, oFe_);
+    return mc.flush(j0, nm, oRo, oRe, oFe, ona, oca, ost);
+  });
 }
 
 // ------------------------------------------------------------------------------------ narrative sign restrictions
@@ -2417,41 +2530,36 @@ int dfm_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const unsign
 int dfm_narrative_sign_restrictions(dfm_handle* h, const dfm_em_init* models, const double* F, const unsigned long long* ids,
                                     const double* scale, const dfm_narr_opts* o, const dfm_sign_restr* rs, const dfm_narr_restr* nr,
                                     const dfm_narr_out* out) {
-  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !F || !o || !rs || !nr || !out || o->N <= 0 ||
-      o->r <= 0 || o->p <= 0 || o->n_model <= 0 || o->H <= 0 || o->n_shock < 1 || o->n_shock > o->r || o->n_rot < 1 ||
-      o->n_keep < 1 || o->Tp < 1 || o->n_sim < 1 || rs->n < 0 || (rs->n > 0 && (!rs->series || !rs->horizon || !rs->shock || !rs->sign)) ||
-      nr->n < 0 || (nr->n > 0 && (!nr->kind || !nr->shock || !nr->series || !nr->row || !nr->h || !nr->sign)) ||
+  if (!h || !models_ok(models) || !F || !o || !rs || !nr || !out || o->N <= 0 || o->r <= 0 || o->p <= 0 || o->n_model <= 0 ||
+      o->H <= 0 || o->n_shock < 1 || o->n_shock > o->r || o->n_rot < 1 || o->n_keep < 1 || o->Tp < 1 || o->n_sim < 1 || rs->n < 0 ||
+      (rs->n > 0 && (!rs->series || !rs->horizon || !rs->shock || !rs->sign)) || nr->n < 0 ||
+      (nr->n > 0 && (!nr->kind || !nr->shock || !nr->series || !nr->row || !nr->h || !nr->sign)) ||
       (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
     return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: bad argument");
-  const int N = o->N, r = o->r, p = o->p, H = o->H, ns = o->n_shock, nR = rs->n, nN = nr->n, nk = o->n_keep, k = r * p, mem = o->mem;
-  const int Tp = o->Tp;
-  for (int q = 0; q < nR; ++q)
-    if (rs->series[q] < 0 || rs->series[q] >= N || rs->horizon[q] < 0 || rs->horizon[q] >= H || rs->shock[q] < 1 ||
-        rs->shock[q] > ns || (rs->sign[q] != 1 && rs->sign[q] != -1))
-      return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a restriction row outside its range");
+  const int N = o->N, r = o->r, p = o->p, H = o->H, ns = o->n_shock, nR = rs->n, nN = nr->n, nk = o->n_keep, Tp = o->Tp, mem = o->mem;
+  SignRows sr;
+  int rc = sign_rows(h, rs, N, H, ns, "dfm_narrative_sign_restrictions: a restriction row outside its range", &sr);
+  if (rc) return rc;
   for (int q = 0; q < nN; ++q) {
     const int kd = nr->kind[q], hh = kd == 0 ? 0 : nr->h[q];
     if (kd < 0 || kd > 3 || nr->shock[q] < 1 || nr->shock[q] > ns || ((kd == 0 || kd == 3) && nr->sign[q] != 1 && nr->sign[q] != -1) ||
         (kd != 0 && (nr->series[q] < 0 || nr->series[q] >= N)) || nr->row[q] < p || hh < 0 || hh >= H || nr->row[q] + hh >= Tp)
       return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a narrative row outside its range");
   }
-  if (ids)
-    for (int b = 0; b < o->n_model; ++b)
-      if (ids[b] >= (1ull << 40)) return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a model id >= 2^40");
-  if (r > SG_RMAX || nR > SG_NRMAX || k > 48 || nk > kMaxGridBatch || nN > NR_NMAX || o->n_sim > (1 << 20))
+  if (!ids_ok(ids, o->n_model)) return fail(h, DFM_ERR_ARG, "dfm_narrative_sign_restrictions: a model id >= 2^40");
+  if (r > SG_RMAX || nR > SG_NRMAX || r * p > 48 || nk > kMaxGridBatch || nN > NR_NMAX || o->n_sim > (1 << 20))
     return fail(h, DFM_ERR_UNSUPPORTED, "dfm_narrative_sign_restrictions: r > 16, more than 256 sign rows or 64 narrative rows, "
                                         "r*p > 48, n_keep > 65535 or n_sim > 2^20");
-  // the periods' union (positions), the sign rows sorted by shock, the narrative rows in the kernels' order
+  // the periods' union (positions), the narrative rows in the kernels' order
   std::vector<char> inP(Tp, 0);
   for (int q = 0; q < nN; ++q) for (int t = nr->row[q]; t <= nr->row[q] + (nr->kind[q] == 0 ? 0 : nr->h[q]); ++t) inP[t] = 1;
   std::vector<int> pos(Tp, 0);
   int nP = 0;
   for (int t = 0; t < Tp; ++t) { pos[t] = nP; nP += inP[t]; }
   if ((long long)nP * r > (1 << 14)) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_narrative_sign_restrictions: nP * r > 2^14");
-  std::vector<int> hs, hh, hg;
-  std::vector<int> off(ns + 1, 0), noff(ns + 1, 0);
+  std::vector<int> noff(ns + 1, 0);
   std::vector<nr_row> rows;
-  int nT = 0, nD = 0, nC = 0;
+  int nT = sr.nj, nD = 0, nC = 0;
   auto add = [&](int q) {
     nr_row w;
     w.kind = nr->kind[q]; w.shock = nr->shock[q] - 1; w.series = w.kind == 0 ? 0 : nr->series[q]; w.t = nr->row[q];
@@ -2462,266 +2570,187 @@ int dfm_narrative_sign_restrictions(dfm_handle* h, const dfm_em_init* models, co
     rows.push_back(w);
   };
   for (int j = 1; j <= ns; ++j) {
-    for (int q = 0; q < nR; ++q)
-      if (rs->shock[q] == j) { hs.push_back(rs->series[q]); hh.push_back(rs->horizon[q]); hg.push_back(rs->sign[q]); nT = j; }
-    off[j] = (int)hs.size();
     for (int q = 0; q < nN; ++q)
-      if (nr->shock[q] == j && (nr->kind[q] == 0 || nr->kind[q] == 3)) { add(q); nT = j; }
+      if (nr->shock[q] == j && (nr->kind[q] == 0 || nr->kind[q] == 3)) { add(q); nT = std::max(nT, j); }
     noff[j] = (int)rows.size();
   }
   for (int q = 0; q < nN; ++q) if (nr->kind[q] == 1 || nr->kind[q] == 2) add(q);
   const bool share = (int)rows.size() > noff[ns];
-  off.resize(nT + 1); noff.resize(nT + 1);
+  sr.off.resize(nT + 1); noff.resize(nT + 1);
   const int ncol = share ? r : nT;
   const size_t smC = narr_cand_smem_bytes(ncol, r, nT, nR, nD, nN), smT = narr_rot_smem_bytes(r, nT, nR, nD, nN);
   const size_t smO = (size_t)nC * 8 + 8;
   if (smC > kMaxSmem || smO > kMaxSmem)
     return fail(h, DFM_ERR_UNSUPPORTED, "dfm_narrative_sign_restrictions: the rows do not fit the kernels' shared memory");
-  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, nout = (size_t)N * H * ns;
-  const size_t Tr = (size_t)Tp * r, nE = (size_t)Tp * ns;
-  const size_t sm0 = series_resp_smem_doubles(r, ns, 0);
-  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
-  const size_t smR = series_resp_smem_doubles(r, ns, hc) * 8, smI = irf_smem_doubles(k) * 8;
-  const size_t smP = ((size_t)r * k + rr + 1) * 8;
+  const size_t rk = (size_t)r * r * p, rr = (size_t)r * r, nout = (size_t)N * H * ns, Tr = (size_t)Tp * r, nE = (size_t)Tp * ns;
+  const SrPlan sp = series_resp_plan(r, ns, H);
+  const size_t smP = (rk + rr + 1) * 8;
   const long long nct = std::min<long long>((o->n_rot + SG_NT - 1) / SG_NT, (1LL << 20) / SG_NT);
   const int ntile = (int)(nct * (SG_NT / SG_TILE));
   const int ntl = (o->n_sim + NR_SIMT - 1) / NR_SIMT;
   const bool hst = mem == DFM_MEM_HOST;
-  const size_t per = 8 * (kk + 2 * rk + rr * H + (size_t)nR * r + 2 + nk + (size_t)nk * rr * H + Tr + nD + 2 * (size_t)nk +
-                          (hst ? Nr + N + rk + rr + Tr + (out->rot ? (size_t)nk * rr : 0) + (out->resp ? nk * nout : 0) +
-                                     (out->fevd ? nk * nout : 0) + (out->eps ? nk * nE : 0) + (out->n_ok ? nk : 0) +
-                                     (out->weight ? nk : 0) : 0)) + 4 * ((size_t)ntile + 1 + nk);
-  const int nb = (int)std::min<long long>({(long long)o->n_model, std::max<long long>(1, (long long)(kSimChunkBytes / per)),
-                                           (long long)(kMaxGridBatch / nk)});
-  CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    const size_t B = nb;
-    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
-           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
-           *dF = hst ? a.get<double>(B * Tr) : nullptr, *dS = hst && scale ? a.get<double>(N) : nullptr;
-    double *dRo = hst && out->rot ? a.get<double>(B * nk * rr) : nullptr, *dRe = hst && out->resp ? a.get<double>(B * nk * nout) : nullptr,
-           *dFe = hst && out->fevd ? a.get<double>(B * nk * nout) : nullptr, *dEp = hst && out->eps ? a.get<double>(B * nk * nE) : nullptr,
-           *dW = hst && out->weight ? a.get<double>(B * nk) : nullptr;
-    long long* dNo = hst && out->n_ok ? a.get<long long>(B * nk) : nullptr;
-    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H),
-           *dC = a.get<double>(B * nR * r + 1), *dRec = a.get<double>(B * nk * rr * H), *dU = a.get<double>(B * Tr),
-           *dD = a.get<double>(B * nD + 1);
-    long long *dNa = a.get<long long>(B), *dCa = a.get<long long>(B * nk);
-    unsigned long long *dId = a.get<unsigned long long>(B), *dNok = a.get<unsigned long long>(B * nk);
-    unsigned* dMask = a.get<unsigned>(B * ntile);
-    int *dst = a.get<int>(B), *dSst = a.get<int>(B * nk), *dIr = a.get<int>(r), *dOff = a.get<int>(nT + 1), *dNoff = a.get<int>(nT + 1);
-    int *dRs = a.get<int>(nR + 1), *dRh = a.get<int>(nR + 1), *dRg = a.get<int>(nR + 1);
-    nr_row* dRows = a.get<nr_row>(nN + 1);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    std::vector<int> hid(r);
-    for (int j = 0; j < r; ++j) hid[j] = j;
-    CK(cudaMemcpyAsync(dIr, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(dOff, off.data(), (nT + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(dNoff, noff.data(), (nT + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    if (nR) {
-      CK(cudaMemcpyAsync(dRs, hs.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(dRh, hh.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(dRg, hg.data(), nR * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  ModelChunks mc(h, models, N, r, p, scale, mem, F, Tp, H, true, ids);
+  OutSlot<double> oRo, oRe, oFe, oEp, oW;
+  OutSlot<long long> oNo;
+  double *dC = nullptr, *dRec = nullptr, *dU = nullptr, *dD = nullptr;
+  long long *dNa = nullptr, *dCa = nullptr;
+  unsigned long long* dNok = nullptr;
+  unsigned* dMask = nullptr;
+  int *dSst = nullptr, *dNoff = nullptr;
+  nr_row* dRows = nullptr;
+  auto layout = [&](Arena& a, size_t B) {
+    mc.alloc(a, B);
+    sr.alloc(a);
+    oRo = staged(a, out->rot, nk * rr, B, hst);
+    oRe = staged(a, out->resp, nk * nout, B, hst);
+    oFe = staged(a, out->fevd, nk * nout, B, hst);
+    oEp = staged(a, out->eps, nk * nE, B, hst);
+    oW = staged(a, out->weight, (size_t)nk, B, hst);
+    oNo = staged(a, out->n_ok, (size_t)nk, B, hst);
+    dC = a.get<double>(B * nR * r + 1);
+    dRec = a.get<double>(B * nk * rr * H);
+    dU = a.get<double>(B * Tr);
+    dD = a.get<double>(B * nD + 1);
+    dNa = a.get<long long>(B);
+    dCa = a.get<long long>(B * nk);
+    dNok = a.get<unsigned long long>(B * nk);
+    dMask = a.get<unsigned>(B * ntile);
+    dSst = a.get<int>(B * nk);
+    dNoff = a.get<int>(nT + 1);
+    dRows = a.get<nr_row>(nN + 1);
+  };
+  const int nb = ModelChunks::chunk_models(layout, o->n_model, kMaxGridBatch / nk);
+  rc = mc.setup(layout, nb);
+  if (!rc) rc = sr.upload(h);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(dNoff, noff.data(), (nT + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  if (nN) CK(cudaMemcpyAsync(dRows, rows.data(), nN * sizeof(nr_row), cudaMemcpyHostToDevice, h->stream));
+  DFM_SET_SMEM(k_series_resp, sp.smR);
+  DFM_SET_SMEM(k_narr_cand, smC);
+  DFM_SET_SMEM(k_narr_rot, smT);
+  DFM_SET_SMEM(k_narr_omega, smO);
+  const OutSlot<long long> ona{out->n_accept, dNa, 1}, oca{out->cand, dCa, (size_t)nk};
+  const OutSlot<int> ost{out->status, mc.st, 1};
+  return mc.run(o->n_model, nb, [&](long long j0, int nm) -> int {
+    const size_t S = (size_t)nm * nk;
+    double *oRe_ = oRe.at(j0), *oFe_ = oFe.at(j0), *oEp_ = oEp.at(j0), *oW_ = oW.at(j0);
+    long long* oNo_ = oNo.at(j0);
+    L(k_sign_prep, nm, 1, 64, 8, mc.L_, mc.R_, (const double*)mc.irf, N, r, H, nR, (const int*)sr.d_series, (const int*)sr.d_horizon,
+      (const int*)sr.d_sign, nk, mc.st, dC, dNa, dCa);
+    L(k_narr_prep, nm, 1, NR_PT, smP, mc.L_, mc.R_, (const double*)mc.irf, (const double*)mc.M, (const double*)mc.G, mc.F_, N, r, p, H,
+      Tp, nN, (const nr_row*)dRows, nD, mc.st, dU, dD);
+    for (long long c0 = 0; c0 < o->n_rot; c0 += (long long)ntile * SG_TILE) {
+      L(k_narr_cand, ntile / (SG_NT / SG_TILE), nm, SG_NT, smC, (const double*)dC, (const int*)sr.d_off, (const double*)dD,
+        (const nr_row*)dRows, (const int*)dNoff, (const int*)mc.st, r, nR, nD, nN, nT, ncol, c0, o->n_rot, ntile, o->seed,
+        (const unsigned long long*)mc.dId, dMask);
+      L(k_sign_pick, nm, 1, SG_PT, 2 * SG_PT * sizeof(int), (const unsigned*)dMask, ntile, c0, nk, (const int*)mc.st, dNa, dCa);
     }
-    if (nN) CK(cudaMemcpyAsync(dRows, rows.data(), nN * sizeof(nr_row), cudaMemcpyHostToDevice, h->stream));
-    const double* sc = scale;
-    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
-    DFM_SET_SMEM(k_series_resp, smR);
-    DFM_SET_SMEM(k_irf, smI);
-    DFM_SET_SMEM(k_narr_cand, smC);
-    DFM_SET_SMEM(k_narr_rot, smT);
-    DFM_SET_SMEM(k_narr_omega, smO);
-    std::vector<unsigned long long> hids(nb);
-    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
-      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
-      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr,
-                   *F_ = F + j0 * Tr;
-      int rc = DFM_OK;
-      if (hst) {
-        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
-        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
-        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
-        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
-        rc = stage_in(h, F_, dF, nm * Tr, mem, &F_); if (rc) return rc;
+    L(k_narr_rot, nm * nk, 1, 64, smT, (const double*)mc.irf, (const double*)dC, (const int*)sr.d_off, (const double*)dD,
+      (const nr_row*)dRows, (const int*)dNoff, (const double*)dU, (const int*)mc.st, (const long long*)dCa, r, H, Tp, nR, nD, nN, nT,
+      nk, oEp_ ? ns : 0, o->seed, (const unsigned long long*)mc.dId, oRo.at(j0), dRec, dSst, oEp_, dNok);
+    if (oRe_ || oFe_)
+      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm * nk, SR_NS, sp.smR, mc.L_, mc.R_, mc.sc, (const double*)dRec, (const int*)dSst, N,
+        r, H, ns, sp.hc, nk, oRe_, oFe_);
+    if (nN && (oW_ || oNo_))
+      L(k_narr_omega, nm * nk, ntl, NR_SIMT, smO, mc.L_, (const double*)dRec, (const nr_row*)dRows, (const int*)dSst,
+        (const unsigned long long*)mc.dId, N, r, H, nN, nC, nP, o->n_sim, nk, o->seed, dNok);
+    if (oW_ || oNo_) {
+      if (!nN) {                                         // no narrative rows: every simulation satisfies them
+        std::vector<unsigned long long> all(S, (unsigned long long)o->n_sim);
+        CK(cudaMemcpyAsync(dNok, all.data(), S * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
       }
-      for (int b = 0; b < nm; ++b) hids[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
-      CK(cudaMemcpyAsync(dId, hids.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
-      const size_t S = (size_t)nm * nk;
-      double* oRo = out->rot ? (hst ? dRo : out->rot + j0 * nk * rr) : nullptr;
-      double* oRe = out->resp ? (hst ? dRe : out->resp + j0 * nk * nout) : nullptr;
-      double* oFe = out->fevd ? (hst ? dFe : out->fevd + j0 * nk * nout) : nullptr;
-      double* oEp = out->eps ? (hst ? dEp : out->eps + j0 * nk * nE) : nullptr;
-      double* oW = out->weight ? (hst ? dW : out->weight + j0 * nk) : nullptr;
-      long long* oNo = out->n_ok ? (hst ? dNo : out->n_ok + j0 * nk) : nullptr;
-      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
-      L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)dIr, dI);
-      L(k_sign_prep, nm, 1, 64, 8, L_, R_, (const double*)dI, N, r, H, nR, (const int*)dRs, (const int*)dRh, (const int*)dRg, nk, dst,
-        dC, dNa, dCa);
-      L(k_narr_prep, nm, 1, NR_PT, smP, L_, R_, (const double*)dI, (const double*)dM, (const double*)dG, F_, N, r, p, H, Tp, nN,
-        (const nr_row*)dRows, nD, dst, dU, dD);
-      for (long long c0 = 0; c0 < o->n_rot; c0 += (long long)ntile * SG_TILE) {
-        L(k_narr_cand, ntile / (SG_NT / SG_TILE), nm, SG_NT, smC, (const double*)dC, (const int*)dOff, (const double*)dD,
-          (const nr_row*)dRows, (const int*)dNoff, (const int*)dst, r, nR, nD, nN, nT, ncol, c0, o->n_rot, ntile, o->seed,
-          (const unsigned long long*)dId, dMask);
-        L(k_sign_pick, nm, 1, SG_PT, 2 * SG_PT * sizeof(int), (const unsigned*)dMask, ntile, c0, nk, (const int*)dst, dNa, dCa);
-      }
-      L(k_narr_rot, nm * nk, 1, 64, smT, (const double*)dI, (const double*)dC, (const int*)dOff, (const double*)dD, (const nr_row*)dRows,
-        (const int*)dNoff, (const double*)dU, (const int*)dst, (const long long*)dCa, r, H, Tp, nR, nD, nN, nT, nk, oEp ? ns : 0,
-        o->seed, (const unsigned long long*)dId, oRo, dRec, dSst, oEp, dNok);
-      if (oRe || oFe)
-        L(k_series_resp, (N + SR_NS - 1) / SR_NS, nm * nk, SR_NS, smR, L_, R_, sc, (const double*)dRec, (const int*)dSst, N, r, H, ns, hc,
-          nk, oRe, oFe);
-      if (nN && (oW || oNo))
-        L(k_narr_omega, nm * nk, ntl, NR_SIMT, smO, L_, (const double*)dRec, (const nr_row*)dRows, (const int*)dSst,
-          (const unsigned long long*)dId, N, r, H, nN, nC, nP, o->n_sim, nk, o->seed, dNok);
-      if (oW || oNo) {
-        if (!nN) {                                         // no narrative rows: every simulation satisfies them
-          std::vector<unsigned long long> all(S, (unsigned long long)o->n_sim);
-          CK(cudaMemcpyAsync(dNok, all.data(), S * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
-          CK(cudaStreamSynchronize(h->stream));
-        }
-        L(k_narr_weight, (int)((S + NR_PT - 1) / NR_PT), 1, NR_PT, 0, (const unsigned long long*)dNok, (const int*)dSst, (int)S, o->n_sim,
-          oNo, oW);
-      }
-      if (hst) {
-        rc = copy_out(h, out->rot ? out->rot + j0 * nk * rr : nullptr, dRo, nm * nk * rr, mem); if (rc) return rc;
-        rc = copy_out(h, out->resp ? out->resp + j0 * nk * nout : nullptr, dRe, nm * nk * nout, mem); if (rc) return rc;
-        rc = copy_out(h, out->fevd ? out->fevd + j0 * nk * nout : nullptr, dFe, nm * nk * nout, mem); if (rc) return rc;
-        rc = copy_out(h, out->eps ? out->eps + j0 * nk * nE : nullptr, dEp, nm * nk * nE, mem); if (rc) return rc;
-        rc = copy_out(h, out->weight ? out->weight + j0 * nk : nullptr, dW, S, mem); if (rc) return rc;
-        rc = copy_out(h, out->n_ok ? out->n_ok + j0 * nk : nullptr, dNo, S, mem); if (rc) return rc;
-      }
-      rc = copy_out(h, out->n_accept ? out->n_accept + j0 : nullptr, dNa, nm, mem); if (rc) return rc;
-      rc = copy_out(h, out->cand ? out->cand + j0 * nk : nullptr, dCa, nm * (size_t)nk, mem); if (rc) return rc;
-      rc = copy_out(h, out->status ? out->status + j0 : nullptr, dst, nm, mem); if (rc) return rc;
-      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+      L(k_narr_weight, (int)((S + NR_PT - 1) / NR_PT), 1, NR_PT, 0, (const unsigned long long*)dNok, (const int*)dSst, (int)S, o->n_sim,
+        oNo_, oW_);
     }
-  }
-  return finish(h, mem);
+    return mc.flush(j0, nm, oRo, oRe, oFe, oEp, oW, oNo, ona, oca, ost);
+  });
 }
 
 // ------------------------------------------------------------------------------------ proxy (external instrument) identification
-// Per chunk of models (a size fixed by the shapes): k_sr_prep -> k_irf (when responses are asked for) -> k_iv_prep -> k_iv_boot ->
-// per batch of records (model, instrument, replicate) in output order: k_iv_rot -> k_series_resp (n_shock 1).  A chunk holds
-// several models when all their records fit one batch, otherwise one model whose records run in several batches; either way
-// record s of a batch reads model s / (n_inst (1 + n_boot)) of the chunk.  Host arrays are staged per chunk; device outputs are
-// written in place.
+// Per chunk of models (ModelChunks): k_sr_prep -> k_irf (when responses are asked for) -> k_iv_prep -> k_iv_boot -> per batch of
+// records (model, instrument, replicate) in output order: k_iv_rot -> k_series_resp (n_shock 1).  A chunk holds several models
+// when all their records fit one batch, otherwise one model whose records run in several batches; either way record s of a batch
+// reads model s / (n_inst (1 + n_boot)) of the chunk.  omega is written to scratch when it is not asked for.
 int dfm_proxy_identification(dfm_handle* h, const dfm_em_init* models, const double* F, const double* Z, const unsigned long long* ids,
                              const double* scale, const dfm_proxy_opts* o, const dfm_proxy_out* out) {
-  if (!h || !models || !models->Lam || !models->R || !models->A || !models->Q || !F || !Z || !o || !out || o->N <= 0 || o->r <= 0 ||
-      o->p <= 0 || o->n_model <= 0 || o->Tp < 1 || o->H <= 0 || o->n_inst < 1 || o->i0 < 0 || o->i0 >= o->N || o->q < 0 ||
-      o->block < 1 || o->n_boot < 0 || (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
+  if (!h || !models_ok(models) || !F || !Z || !o || !out || o->N <= 0 || o->r <= 0 || o->p <= 0 || o->n_model <= 0 || o->Tp < 1 ||
+      o->H <= 0 || o->n_inst < 1 || o->i0 < 0 || o->i0 >= o->N || o->q < 0 || o->block < 1 || o->n_boot < 0 ||
+      (o->mem != DFM_MEM_HOST && o->mem != DFM_MEM_DEVICE))
     return fail(h, DFM_ERR_ARG, "dfm_proxy_identification: bad argument");
-  if (ids)
-    for (int b = 0; b < o->n_model; ++b)
-      if (ids[b] >= (1ull << 40)) return fail(h, DFM_ERR_ARG, "dfm_proxy_identification: a model id >= 2^40");
-  const int N = o->N, r = o->r, p = o->p, H = o->H, Tp = o->Tp, ni = o->n_inst, nbt = o->n_boot, k = r * p, mem = o->mem;
-  if (k > 48 || ni > IV_NIMAX || nbt > 65535)
+  if (!ids_ok(ids, o->n_model)) return fail(h, DFM_ERR_ARG, "dfm_proxy_identification: a model id >= 2^40");
+  const int N = o->N, r = o->r, p = o->p, H = o->H, Tp = o->Tp, ni = o->n_inst, nbt = o->n_boot, mem = o->mem;
+  if (r * p > 48 || ni > IV_NIMAX || nbt > 65535)
     return fail(h, DFM_ERR_UNSUPPORTED, "dfm_proxy_identification: r*p > 48, n_inst > 8 or n_boot > 65535");
   const size_t smP = iv_prep_smem_bytes(r, Tp), smB = iv_boot_smem_bytes(r, Tp), smT = iv_rot_smem_bytes(r);
   if (smP > kMaxSmem || smB > kMaxSmem)
     return fail(h, DFM_ERR_UNSUPPORTED, "dfm_proxy_identification: Tp (r + 1) + 64 r > 28160 (the bootstrap's shared memory)");
   const bool want = out->resp || out->fevd, hst = mem == DFM_MEM_HOST;
-  const size_t Nr = (size_t)N * r, rk = (size_t)r * k, rr = (size_t)r * r, kk = (size_t)k * k, Tr = (size_t)Tp * r, NH = (size_t)N * H;
-  const size_t P = (size_t)ni * (nbt + 1), nE = (size_t)ni * Tp;
-  const size_t sm0 = series_resp_smem_doubles(r, 1, 0);
-  const int hc = (int)std::min<size_t>((size_t)H, (kMaxSmem / 8 - sm0) / rr);
-  const size_t smR = series_resp_smem_doubles(r, 1, hc) * 8, smI = irf_smem_doubles(k) * 8;
+  const size_t rr = (size_t)r * r, Tr = (size_t)Tp * r, NH = (size_t)N * H, P = (size_t)ni * (nbt + 1), nE = (size_t)ni * Tp;
+  const SrPlan sp = series_resp_plan(r, 1, H);
+  ModelChunks mc(h, models, N, r, p, scale, mem, F, Tp, want ? H : 0, true, ids);
+  OutSlot<double> oOm, oEp, oRel, oPi, oFs, oRe, oFe;
+  OutSlot<int> oNo;
+  double *dZ = nullptr, *dU = nullptr, *dRec = nullptr;
+  int *dIdx = nullptr, *dNk = nullptr, *dIst = nullptr, *dSst = nullptr;
+  // B models and R records (responses and their staging)
+  auto layout = [&](Arena& a, size_t B, size_t R) {
+    mc.alloc(a, B);
+    dZ = hst ? a.get<double>(nE) : nullptr;
+    oOm = scratch(a, out->omega, P * r, B, hst);
+    oEp = staged(a, out->eps, nE, B, hst);
+    oRel = staged(a, out->reliability, (size_t)ni, B, hst);
+    oPi = staged(a, out->fs_pi, (size_t)ni, B, hst);
+    oFs = staged(a, out->fs_F, (size_t)ni, B, hst);
+    oNo = staged(a, out->n_obs, (size_t)ni, B, hst);
+    dU = a.get<double>(B * Tr);
+    dIdx = a.get<int>(B * nE);
+    dNk = a.get<int>(B * ni);
+    dIst = a.get<int>(B * ni);
+    oRe = staged(a, out->resp, NH, R, hst);
+    oFe = staged(a, out->fevd, NH, R, hst);
+    dRec = a.get<double>(R * rr * H);
+    dSst = a.get<int>(R);
+  };
+  auto bytes = [&](size_t B, size_t R) {
+    Arena a(nullptr);
+    layout(a, B, R);
+    return a.off;
+  };
   // records per batch: grid.y of k_series_resp, and half of kSimChunkBytes; models per chunk: the other half, grid.y of k_iv_boot,
   // and (for more than one) all their records in one batch
-  const size_t perR = 8 * (rr * H + (hst ? (out->resp ? NH : 0) + (out->fevd ? NH : 0) : 0)) + 4;
-  const long long cap = std::min<long long>(kMaxGridBatch, std::max<long long>(1, (long long)(kSimChunkBytes / 2 / perR)));
-  const size_t perM = 8 * (kk + 2 * rk + rr * H + Tr + P * r + 1 + (hst ? Nr + N + rk + rr + Tr + (out->eps ? nE : 0) + 3 * (size_t)ni : 0)) +
-                      4 * (nE + 3 * (size_t)ni + 1);
-  const int nb = (int)std::max<long long>(1, std::min<long long>({(long long)o->n_model, (long long)(kSimChunkBytes / 2 / perM),
+  const long long cap = std::min<long long>(kMaxGridBatch, std::max<long long>(1, (long long)(kSimChunkBytes / 2 / bytes(0, 1))));
+  const int nb = (int)std::max<long long>(1, std::min<long long>({(long long)o->n_model, (long long)(kSimChunkBytes / 2 / bytes(1, 0)),
                                                                   (long long)(kMaxGridBatch / ni), cap / (long long)P}));
   const long long nrec = std::min<long long>(cap, (long long)nb * (long long)P);
-  CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    const size_t B = nb;
-    double *dL = hst ? a.get<double>(B * Nr) : nullptr, *dR = hst ? a.get<double>(B * N) : nullptr,
-           *dA = hst ? a.get<double>(B * rk) : nullptr, *dQ = hst ? a.get<double>(B * rr) : nullptr,
-           *dF = hst ? a.get<double>(B * Tr) : nullptr, *dZ = hst ? a.get<double>(nE) : nullptr,
-           *dS = hst && scale ? a.get<double>(N) : nullptr;
-    double *dEp = hst && out->eps ? a.get<double>(B * nE) : nullptr, *dRel = hst && out->reliability ? a.get<double>(B * ni) : nullptr,
-           *dPi = hst && out->fs_pi ? a.get<double>(B * ni) : nullptr, *dFs = hst && out->fs_F ? a.get<double>(B * ni) : nullptr;
-    double *dRe = hst && out->resp ? a.get<double>(nrec * NH) : nullptr, *dFe = hst && out->fevd ? a.get<double>(nrec * NH) : nullptr;
-    int* dNo = hst && out->n_obs ? a.get<int>(B * ni) : nullptr;
-    double *dM = a.get<double>(B * kk), *dQs = a.get<double>(B * rk), *dG = a.get<double>(B * rk), *dI = a.get<double>(B * rr * H),
-           *dU = a.get<double>(B * Tr), *dOm = a.get<double>(B * P * r), *dRec = want ? a.get<double>(nrec * rr * H) : nullptr;
-    unsigned long long* dId = a.get<unsigned long long>(B);
-    int *dst = a.get<int>(B), *dIdx = a.get<int>(B * nE), *dNk = a.get<int>(B * ni), *dIst = a.get<int>(B * ni),
-        *dSst = want ? a.get<int>(nrec) : nullptr, *dIr = a.get<int>(r);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    std::vector<int> hid(r);
-    for (int j = 0; j < r; ++j) hid[j] = j;
-    CK(cudaMemcpyAsync(dIr, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    const double* sc = scale;
-    if (hst && scale) { CK(cudaMemcpyAsync(dS, scale, (size_t)N * 8, cudaMemcpyHostToDevice, h->stream)); sc = dS; }
-    const double* Z_ = Z;
-    int rc = stage_in(h, Z, dZ, nE, mem, &Z_); if (rc) return rc;
-    DFM_SET_SMEM(k_series_resp, smR);
-    DFM_SET_SMEM(k_irf, smI);
-    DFM_SET_SMEM(k_iv_prep, smP);
-    DFM_SET_SMEM(k_iv_boot, smB);
-    std::vector<unsigned long long> hids(nb);
-    for (long long j0 = 0; j0 < o->n_model; j0 += nb) {
-      const int nm = (int)std::min<long long>(nb, o->n_model - j0);
-      const double *L_ = models->Lam + j0 * Nr, *R_ = models->R + j0 * N, *A_ = models->A + j0 * rk, *Q_ = models->Q + j0 * rr,
-                   *F_ = F + j0 * Tr;
-      if (hst) {
-        rc = stage_in(h, L_, dL, nm * Nr, mem, &L_); if (rc) return rc;
-        rc = stage_in(h, R_, dR, nm * (size_t)N, mem, &R_); if (rc) return rc;
-        rc = stage_in(h, A_, dA, nm * rk, mem, &A_); if (rc) return rc;
-        rc = stage_in(h, Q_, dQ, nm * rr, mem, &Q_); if (rc) return rc;
-        rc = stage_in(h, F_, dF, nm * Tr, mem, &F_); if (rc) return rc;
-      }
-      for (int b = 0; b < nm; ++b) hids[b] = ids ? ids[j0 + b] : (unsigned long long)(j0 + b);
-      CK(cudaMemcpyAsync(dId, hids.data(), nm * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
-      const size_t mi = (size_t)nm * ni;
-      double* oOm = out->omega && !hst ? out->omega + j0 * P * r : dOm;
-      double* oEp = out->eps ? (hst ? dEp : out->eps + j0 * nE) : nullptr;
-      double* oRel = out->reliability ? (hst ? dRel : out->reliability + j0 * ni) : nullptr;
-      double* oPi = out->fs_pi ? (hst ? dPi : out->fs_pi + j0 * ni) : nullptr;
-      double* oFs = out->fs_F ? (hst ? dFs : out->fs_F + j0 * ni) : nullptr;
-      int* oNo = out->n_obs ? (hst ? dNo : out->n_obs + j0 * ni) : nullptr;
-      L(k_sr_prep, nm, 1, 64, (rr + 8) * 8, A_, Q_, r, p, dM, dQs, dG, dst);
-      if (want) L(k_irf, r, nm, 64, smI, (const double*)dM, (const double*)dQs, (const double*)dG, k, r, H, r, (const int*)dIr, dI);
-      L(k_iv_prep, nm, 1, IV_PT, smP, L_, R_, A_, (const double*)dG, F_, Z_, N, r, p, Tp, ni, o->i0, o->q, nbt, (const int*)dst, dU, dIdx,
-        dNk, dIst, oOm, oEp, oNo, oRel, oPi, oFs);
-      if (nbt > 0)
-        L(k_iv_boot, (nbt + IV_BT - 1) / IV_BT, (int)mi, IV_BT, smB, (const double*)dU, Z_, (const int*)dIdx, (const int*)dNk,
-          (const int*)dIst, r, Tp, ni, o->block, nbt, o->seed, (const unsigned long long*)dId, oOm);
-      const long long nrc = (long long)nm * (long long)P;
-      for (long long g0 = 0; want && g0 < nrc; g0 += nrec) {
-        const int nr = (int)std::min<long long>(nrec, nrc - g0);
-        const size_t og = ((size_t)j0 * P + (size_t)g0) * NH;
-        double* oRe = out->resp ? (hst ? dRe : out->resp + og) : nullptr;
-        double* oFe = out->fevd ? (hst ? dFe : out->fevd + og) : nullptr;
-        L(k_iv_rot, nr, 1, 64, smT, (const double*)dI, (const double*)oOm, g0, r, H, ni, nbt, dRec, dSst);
-        L(k_series_resp, (N + SR_NS - 1) / SR_NS, nr, SR_NS, smR, L_, R_, sc, (const double*)dRec, (const int*)dSst, N, r, H, 1, hc, (int)P,
-          oRe, oFe);
-        if (hst) {
-          rc = copy_out(h, out->resp ? out->resp + og : nullptr, dRe, nr * NH, mem); if (rc) return rc;
-          rc = copy_out(h, out->fevd ? out->fevd + og : nullptr, dFe, nr * NH, mem); if (rc) return rc;
-          CK(cudaStreamSynchronize(h->stream));             // (dRe and dFe are rewritten by the next batch)
-        }
-      }
-      if (hst) {
-        rc = copy_out(h, out->eps ? out->eps + j0 * nE : nullptr, dEp, nm * nE, mem); if (rc) return rc;
-        rc = copy_out(h, out->reliability ? out->reliability + j0 * ni : nullptr, dRel, mi, mem); if (rc) return rc;
-        rc = copy_out(h, out->fs_pi ? out->fs_pi + j0 * ni : nullptr, dPi, mi, mem); if (rc) return rc;
-        rc = copy_out(h, out->fs_F ? out->fs_F + j0 * ni : nullptr, dFs, mi, mem); if (rc) return rc;
-        rc = copy_out(h, out->n_obs ? out->n_obs + j0 * ni : nullptr, dNo, mi, mem); if (rc) return rc;
-      }
-      rc = copy_out(h, out->omega ? out->omega + j0 * P * r : nullptr, oOm, nm * P * r, mem); if (rc) return rc;
-      rc = copy_out(h, out->status ? out->status + j0 * ni : nullptr, dIst, mi, mem); if (rc) return rc;
-      if (hst) CK(cudaStreamSynchronize(h->stream));       // (the staging buffers are reused by the next chunk)
+  int rc = mc.setup([&](Arena& a, size_t B) { layout(a, B, want ? nrec : 0); }, nb);
+  if (rc) return rc;
+  const double* Z_ = Z;
+  rc = stage_in(h, Z, dZ, nE, mem, &Z_);
+  if (rc) return rc;
+  DFM_SET_SMEM(k_series_resp, sp.smR);
+  DFM_SET_SMEM(k_iv_prep, smP);
+  DFM_SET_SMEM(k_iv_boot, smB);
+  const OutSlot<int> ost{out->status, dIst, (size_t)ni};
+  return mc.run(o->n_model, nb, [&](long long j0, int nm) -> int {
+    double* oOm_ = oOm.at(j0);
+    L(k_iv_prep, nm, 1, IV_PT, smP, mc.L_, mc.R_, mc.A_, (const double*)mc.G, mc.F_, Z_, N, r, p, Tp, ni, o->i0, o->q, nbt,
+      (const int*)mc.st, dU, dIdx, dNk, dIst, oOm_, oEp.at(j0), oNo.at(j0), oRel.at(j0), oPi.at(j0), oFs.at(j0));
+    if (nbt > 0)
+      L(k_iv_boot, (nbt + IV_BT - 1) / IV_BT, nm * ni, IV_BT, smB, (const double*)dU, Z_, (const int*)dIdx, (const int*)dNk,
+        (const int*)dIst, r, Tp, ni, o->block, nbt, o->seed, (const unsigned long long*)mc.dId, oOm_);
+    const long long nrc = (long long)nm * (long long)P;
+    for (long long g0 = 0; want && g0 < nrc; g0 += nrec) {
+      const int nr = (int)std::min<long long>(nrec, nrc - g0);
+      const long long s0 = j0 * (long long)P + g0;           // the batch's first record in the outputs
+      L(k_iv_rot, nr, 1, 64, smT, (const double*)mc.irf, (const double*)oOm_, g0, r, H, ni, nbt, dRec, dSst);
+      L(k_series_resp, (N + SR_NS - 1) / SR_NS, nr, SR_NS, sp.smR, mc.L_, mc.R_, mc.sc, (const double*)dRec, (const int*)dSst, N, r, H, 1,
+        sp.hc, (int)P, oRe.at(s0), oFe.at(s0));
+      if (int e = mc.flush(s0, nr, oRe, oFe)) return e;
+      if (hst) CK(cudaStreamSynchronize(h->stream));         // (the next batch rewrites the staging of resp and fevd)
     }
-  }
-  return finish(h, mem);
+    return mc.flush(j0, nm, oOm, oEp, oRel, oPi, oFs, oNo, ost);
+  });
 }
 
 // ------------------------------------------------------------------------------------ (f)3: percentile bands
