@@ -181,6 +181,19 @@ int ensure_rws(dfm_handle* h, size_t bytes) {
   return DFM_OK;
 }
 
+// Lays out a call's device buffers: layout(a) walks them once on a null Arena to size them, the workspace grows to that size,
+// and layout(a) walks them again to place them.  in_rws: the second workspace (dfm_handle::rws), for the temporaries of entry
+// points that call other entry points.
+template <class Lay> int lay_out(dfm_handle* h, Lay&& layout, bool in_rws = false) {
+  Arena probe(nullptr);
+  layout(probe);
+  int rc = in_rws ? ensure_rws(h, probe.off) : ensure_ws(h, probe.off);
+  if (rc) return rc;
+  Arena a(in_rws ? h->rws : h->ws);
+  layout(a);
+  return DFM_OK;
+}
+
 // input staging: returns device pointer for `src` (copying if it lives on the host)
 template <typename Tp>
 int stage_in(dfm_handle* h, const Tp* src, Tp* dev_buf, size_t n, int mem, const Tp** out) {
@@ -194,6 +207,39 @@ int copy_out(dfm_handle* h, Tp* dst, const Tp* dev, size_t n, int mem) {
   if (!dst || dst == dev) return DFM_OK;
   CK(cudaMemcpyAsync(dst, dev, n * sizeof(Tp), mem == DFM_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, h->stream));
   return DFM_OK;
+}
+
+// One output of an entry point: dst, the caller's array of `per` elements a row (a panel, a model, a draw; nullptr: not asked
+// for).  The kernels write buf when there is one, else dst in place; flush copies the rows they wrote to dst.
+template <typename T> struct OutSlot {
+  T* dst = nullptr;
+  T* buf = nullptr;
+  size_t per = 0;
+  // where the kernels write the rows that start at row j0 (nullptr: nowhere)
+  T* at(long long j0) const { return buf ? buf : dst ? dst + j0 * per : nullptr; }
+  int flush(dfm_handle* h, long long j0, long long n, int mem) const {
+    return copy_out(h, dst ? dst + j0 * per : nullptr, at(j0), n * per, mem);
+  }
+};
+
+// an output the kernels write only when it is asked for: in place in device memory, through a staging buffer of B rows to host
+// memory
+template <typename T> OutSlot<T> staged(Arena& a, T* dst, size_t per, size_t B, bool hst) {
+  return {dst, hst && dst ? a.get<T>(B * per) : nullptr, per};
+}
+
+// an output the kernels write whether or not it is asked for: in place when it is asked for in device memory, else into the
+// buffer (allocated either way, so that the layout's size does not depend on dst)
+template <typename T> OutSlot<T> scratch(Arena& a, T* dst, size_t per, size_t B, bool hst) {
+  T* buf = a.get<T>(B * per);
+  return {dst, hst || !dst ? buf : nullptr, per};
+}
+
+// the copy-back of the n rows from j0 of every slot, up to the first error
+template <typename... T> int flush(dfm_handle* h, long long j0, long long n, int mem, const OutSlot<T>&... s) {
+  int rc = DFM_OK;
+  ((rc = rc ? rc : s.flush(h, j0, n, mem)), ...);
+  return rc;
 }
 
 int finish(dfm_handle* h, int mem) {
@@ -826,18 +872,20 @@ int dfm_standardize(dfm_handle* h, const double* X, int T, int N, int batch, int
   if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_standardize: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
-    double* dXs = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : Xs;
-    double* dm = a.get<double>(B * N); double* ds = a.get<double>(B * N);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* x; int rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
-    L(k_standardize, N, batch, 128, 48 * 8, x, T, N, dXs, dm, ds, (double*)nullptr, (int*)nullptr);
-    if (mem == DFM_MEM_HOST) { rc = copy_out(h, Xs, dXs, B * TN, mem); if (rc) return rc; }
-    rc = copy_out(h, xmean, dm, B * N, mem); if (rc) return rc;
-    rc = copy_out(h, xstd, ds, B * N, mem); if (rc) return rc;
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dX, *dm, *ds;
+  OutSlot<double> oXs;
+  int rc = lay_out(h, [&](Arena& a) {
+    dX = hst ? a.get<double>(B * TN) : nullptr;
+    oXs = staged(a, Xs, TN, B, hst);
+    dm = a.get<double>(B * N); ds = a.get<double>(B * N);
+  });
+  if (rc) return rc;
+  const double* x; rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
+  L(k_standardize, N, batch, 128, 48 * 8, x, T, N, oXs.at(0), dm, ds, (double*)nullptr, (int*)nullptr);
+  rc = oXs.flush(h, 0, B, mem); if (rc) return rc;
+  rc = copy_out(h, xmean, dm, B * N, mem); if (rc) return rc;
+  rc = copy_out(h, xstd, ds, B * N, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -878,19 +926,22 @@ int dfm_pca_score(dfm_handle* h, const double* X, int T, int N, int r, int batch
   if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_pca_score: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int nmax = std::min(N, T);
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
-    double* dF = mem == DFM_MEM_HOST ? a.get<double>(B * T * r) : score;
-    int* bal = a.get<int>(B * N); int* nbal = a.get<int>(B); int* status = a.get<int>(B);
-    double* G = a.get<double>(B * nmax * nmax); double* V = a.get<double>(B * nmax * nmax);
-    double* Ysub = a.get<double>(B * nmax * PCA_MMAX);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* x; int rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
-    CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
-    rc = run_pca(h, x, T, N, r, batch, nullptr, bal, nbal, G, V, Ysub, dF, status, nullptr); if (rc) return rc;
-    if (mem == DFM_MEM_HOST) { rc = copy_out(h, score, dF, B * T * r, mem); if (rc) return rc; }
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dX, *G, *V, *Ysub;
+  int *bal, *nbal, *status;
+  OutSlot<double> oF;
+  int rc = lay_out(h, [&](Arena& a) {
+    dX = hst ? a.get<double>(B * TN) : nullptr;
+    oF = staged(a, score, (size_t)T * r, B, hst);
+    bal = a.get<int>(B * N); nbal = a.get<int>(B); status = a.get<int>(B);
+    G = a.get<double>(B * nmax * nmax); V = a.get<double>(B * nmax * nmax);
+    Ysub = a.get<double>(B * nmax * PCA_MMAX);
+  });
+  if (rc) return rc;
+  const double* x; rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
+  CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
+  rc = run_pca(h, x, T, N, r, batch, nullptr, bal, nbal, G, V, Ysub, oF.at(0), status, nullptr); if (rc) return rc;
+  rc = oF.flush(h, 0, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -913,81 +964,83 @@ int dfm_estimate_factor(dfm_handle* h, const double* X, const dfm_factor_opts* o
   size_t smF = ((size_t)(np + r) * ntF + 48) * 8;
   const bool sys_global = smF > kMaxSmem;
   if (sys_global) smF = 48 * 8;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
-    double* dXs = a.get<double>(B * TN);
-    double* dm = a.get<double>(B * N); double* ds = a.get<double>(B * N); double* css = a.get<double>(B * N);
-    int* cn = a.get<int>(B * N); AlsState* st = a.get<AlsState>(B);
-    int* bal = a.get<int>(B * N); int* nbal = a.get<int>(B); int* active = a.get<int>(4);
-    double* G = F_init ? nullptr : a.get<double>(B * nmax * nmax); double* V = F_init ? nullptr : a.get<double>(B * nmax * nmax);
-    double* Ysub = F_init ? nullptr : a.get<double>(B * nmax * PCA_MMAX);
-    double* dF = a.get<double>(B * T * r); double* dLam = a.get<double>(B * N * r); double* dR2 = a.get<double>(B * N);
-    double* FtF = a.get<double>(B * r * r); double* LtL = a.get<double>(B * r * r); double* ssrp = a.get<double>(B * nblk);
-    int* cidx = a.get<int>(nc + 1); double* cR = a.get<double>((size_t)nc * r + 1); double* cr = a.get<double>(nc + 1);
-    double* gsys = sys_global ? a.get<double>(B * nblk * (size_t)(np + r) * ntF) : nullptr;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* x; int rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
-    if (nc > 0) {
-      CK(cudaMemcpyAsync(cidx, o->constr_index, nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(cR, o->constr_R, (size_t)nc * r * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(cr, o->constr_r, nc * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    }
-    L(k_standardize, N, batch, 128, 48 * 8, x, T, N, dXs, dm, ds, css, cn);            // :339
-    L(k_als_init_state, batch, 1, 128, 48 * 8, st, css, cn, N);                        // :342-343
-    if (F_init) { const double* fi; rc = stage_in(h, F_init, dF, B * T * r, mem, &fi); if (rc) return rc;
-                  if (fi != dF) CK(cudaMemcpyAsync(dF, fi, B * T * r * sizeof(double), cudaMemcpyDeviceToDevice, h->stream)); }
-    else { rc = run_pca(h, dXs, T, N, r, batch, cn, bal, nbal, G, V, Ysub, dF, nullptr, st); if (rc) return rc; }   // :345-348
-    size_t smL = (size_t)(2 * np + 2 * r + 8 + (size_t)r * nc + (size_t)nc * (nc + 1) / 2 + nc) * 8;
-    long long it = 0;
-    int h_active = batch;
-    // balanced panels without constraints: all sweeps in ONE fused launch (TMA ring + DMMA passes)
-    if (nc == 0 && als_fused2_shape_ok(T, N, r) && o->nt_min <= T) {
-      std::vector<AlsState> hs(B);
-      CK(cudaMemcpyAsync(hs.data(), st, B * sizeof(AlsState), cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
-      bool balanced = true;
-      for (size_t b = 0; b < B; ++b) if (hs[b].nobs != (long long)T * N || hs[b].status != 0) balanced = false;
-      if (balanced) {
-        AlsFusedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.tol = o->tol; fa.max_iter = o->max_iter;
-        rc = launch_als_fused2(h, fa, r); if (rc) return rc;
-        h_active = 0;
-      }
-    }
-    // panels with missing data, no constraints: all sweeps in ONE launch as well (thread-per-series / thread-per-period
-    // masked normal equations, no host synchronisation in the sweep loop)
-    if (h_active > 0 && nc == 0 && als_masked_shape_ok(T, N, r)) {
-      AlsMaskedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.nt_min = o->nt_min;
-      fa.tol = o->tol; fa.max_iter = o->max_iter;
-      launch_als_masked(h, fa, r);
+  double *dX, *dXs, *dm, *ds, *css, *G, *V, *Ysub, *dF, *dLam, *dR2, *FtF, *LtL, *ssrp, *cR, *cr, *gsys;
+  int *cn, *bal, *nbal, *active, *cidx;
+  AlsState* st;
+  int rc = lay_out(h, [&](Arena& a) {
+    dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
+    dXs = a.get<double>(B * TN);
+    dm = a.get<double>(B * N); ds = a.get<double>(B * N); css = a.get<double>(B * N);
+    cn = a.get<int>(B * N); st = a.get<AlsState>(B);
+    bal = a.get<int>(B * N); nbal = a.get<int>(B); active = a.get<int>(4);
+    G = F_init ? nullptr : a.get<double>(B * nmax * nmax); V = F_init ? nullptr : a.get<double>(B * nmax * nmax);
+    Ysub = F_init ? nullptr : a.get<double>(B * nmax * PCA_MMAX);
+    dF = a.get<double>(B * T * r); dLam = a.get<double>(B * N * r); dR2 = a.get<double>(B * N);
+    FtF = a.get<double>(B * r * r); LtL = a.get<double>(B * r * r); ssrp = a.get<double>(B * nblk);
+    cidx = a.get<int>(nc + 1); cR = a.get<double>((size_t)nc * r + 1); cr = a.get<double>(nc + 1);
+    gsys = sys_global ? a.get<double>(B * nblk * (size_t)(np + r) * ntF) : nullptr;
+  });
+  if (rc) return rc;
+  const double* x; rc = stage_in(h, X, dX, B * TN, mem, &x); if (rc) return rc;
+  if (nc > 0) {
+    CK(cudaMemcpyAsync(cidx, o->constr_index, nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(cR, o->constr_R, (size_t)nc * r * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(cr, o->constr_r, nc * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  }
+  L(k_standardize, N, batch, 128, 48 * 8, x, T, N, dXs, dm, ds, css, cn);            // :339
+  L(k_als_init_state, batch, 1, 128, 48 * 8, st, css, cn, N);                        // :342-343
+  if (F_init) { const double* fi; rc = stage_in(h, F_init, dF, B * T * r, mem, &fi); if (rc) return rc;
+                if (fi != dF) CK(cudaMemcpyAsync(dF, fi, B * T * r * sizeof(double), cudaMemcpyDeviceToDevice, h->stream)); }
+  else { rc = run_pca(h, dXs, T, N, r, batch, cn, bal, nbal, G, V, Ysub, dF, nullptr, st); if (rc) return rc; }   // :345-348
+  size_t smL = (size_t)(2 * np + 2 * r + 8 + (size_t)r * nc + (size_t)nc * (nc + 1) / 2 + nc) * 8;
+  long long it = 0;
+  int h_active = batch;
+  // balanced panels without constraints: all sweeps in ONE fused launch (TMA ring + DMMA passes)
+  if (nc == 0 && als_fused2_shape_ok(T, N, r) && o->nt_min <= T) {
+    std::vector<AlsState> hs(B);
+    CK(cudaMemcpyAsync(hs.data(), st, B * sizeof(AlsState), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    bool balanced = true;
+    for (size_t b = 0; b < B; ++b) if (hs[b].nobs != (long long)T * N || hs[b].status != 0) balanced = false;
+    if (balanced) {
+      AlsFusedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.tol = o->tol; fa.max_iter = o->max_iter;
+      rc = launch_als_fused2(h, fa, r); if (rc) return rc;
       h_active = 0;
     }
-    while (it < o->max_iter && h_active > 0) {                                       // :352
-      if (nc > 0) L(k_gram_small, batch, 1, 128, 0, dF, T, r, FtF, st);
-      L(k_als_lambda, N, batch, 64, smL, dXs, dF, T, N, r, o->nt_min, 0, dLam, (double*)nullptr, FtF, nc, cidx, cR, cr, ds, st);   // :355-362
-      L(k_gram_small, batch, 1, 128, 0, dLam, N, r, LtL, st);
-      L(k_als_factor, nblk, batch, ntF, smF, dXs, dLam, LtL, T, N, r, dF, ssrp, st, gsys);                                           // :364-366
-      L(k_als_check, batch, 1, 1, 0, st, ssrp, nblk, o->tol, T, N, o->max_iter);                                                // :367-368
-      ++it;
-      if ((it & 1) == 0 || it >= o->max_iter || it < 2) {
-        L(k_count_active, 1, 1, 128, 48 * 8, st, batch, active);
-        CK(cudaMemcpyAsync(&h_active, active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-      }
-    }
-    if (o->compute_r2 && R2)                                                          // :372-380
-      L(k_als_lambda, N, batch, 64, smL, dXs, dF, T, N, r, o->nt_min, 1, (double*)nullptr, dR2, FtF, 0, cidx, cR, cr, ds, (AlsState*)nullptr);
-    rc = copy_out(h, F, dF, B * T * r, mem); if (rc) return rc;
-    rc = copy_out(h, Lambda, dLam, B * N * r, mem); if (rc) return rc;
-    if (o->compute_r2) { rc = copy_out(h, R2, dR2, B * N, mem); if (rc) return rc; }
-    rc = copy_out(h, xmean, dm, B * N, mem); if (rc) return rc;
-    rc = copy_out(h, xstd, ds, B * N, mem); if (rc) return rc;
-    if (stats) {
-      std::vector<AlsState> hs(B);
-      CK(cudaMemcpyAsync(hs.data(), st, B * sizeof(AlsState), cudaMemcpyDeviceToHost, h->stream));
+  }
+  // panels with missing data, no constraints: all sweeps in ONE launch as well (thread-per-series / thread-per-period
+  // masked normal equations, no host synchronisation in the sweep loop)
+  if (h_active > 0 && nc == 0 && als_masked_shape_ok(T, N, r)) {
+    AlsMaskedArgs fa{}; fa.Xs = dXs; fa.F = dF; fa.Lam = dLam; fa.st = st; fa.B = batch; fa.T = T; fa.N = N; fa.nt_min = o->nt_min;
+    fa.tol = o->tol; fa.max_iter = o->max_iter;
+    launch_als_masked(h, fa, r);
+    h_active = 0;
+  }
+  while (it < o->max_iter && h_active > 0) {                                       // :352
+    if (nc > 0) L(k_gram_small, batch, 1, 128, 0, dF, T, r, FtF, st);
+    L(k_als_lambda, N, batch, 64, smL, dXs, dF, T, N, r, o->nt_min, 0, dLam, (double*)nullptr, FtF, nc, cidx, cR, cr, ds, st);   // :355-362
+    L(k_gram_small, batch, 1, 128, 0, dLam, N, r, LtL, st);
+    L(k_als_factor, nblk, batch, ntF, smF, dXs, dLam, LtL, T, N, r, dF, ssrp, st, gsys);                                           // :364-366
+    L(k_als_check, batch, 1, 1, 0, st, ssrp, nblk, o->tol, T, N, o->max_iter);                                                // :367-368
+    ++it;
+    if ((it & 1) == 0 || it >= o->max_iter || it < 2) {
+      L(k_count_active, 1, 1, 128, 48 * 8, st, batch, active);
+      CK(cudaMemcpyAsync(&h_active, active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
       CK(cudaStreamSynchronize(h->stream));
-      for (size_t b = 0; b < B; ++b) { stats[b].ssr = hs[b].ssr; stats[b].tss = hs[b].tss; stats[b].nobs = hs[b].nobs; stats[b].iters = hs[b].iters; stats[b].status = hs[b].status; }
     }
+  }
+  if (o->compute_r2 && R2)                                                          // :372-380
+    L(k_als_lambda, N, batch, 64, smL, dXs, dF, T, N, r, o->nt_min, 1, (double*)nullptr, dR2, FtF, 0, cidx, cR, cr, ds, (AlsState*)nullptr);
+  rc = copy_out(h, F, dF, B * T * r, mem); if (rc) return rc;
+  rc = copy_out(h, Lambda, dLam, B * N * r, mem); if (rc) return rc;
+  if (o->compute_r2) { rc = copy_out(h, R2, dR2, B * N, mem); if (rc) return rc; }
+  rc = copy_out(h, xmean, dm, B * N, mem); if (rc) return rc;
+  rc = copy_out(h, xstd, ds, B * N, mem); if (rc) return rc;
+  if (stats) {
+    std::vector<AlsState> hs(B);
+    CK(cudaMemcpyAsync(hs.data(), st, B * sizeof(AlsState), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (size_t b = 0; b < B; ++b) { stats[b].ssr = hs[b].ssr; stats[b].tss = hs[b].tss; stats[b].nobs = hs[b].nobs; stats[b].iters = hs[b].iters; stats[b].status = hs[b].status; }
   }
   return finish(h, mem);
 }
@@ -1008,41 +1061,44 @@ int dfm_estimate_loading_ex(dfm_handle* h, const double* data, const double* F, 
   if (batch > kMaxGridBatch) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_estimate_loading: batch > 65535");
   CK(cudaSetDevice(h->device));
   size_t B = batch; int K = r + 1, np = K * (K + 1) / 2;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dD = mem == DFM_MEM_HOST ? a.get<double>(B * T * ns) : nullptr;
-    double* dFb = mem == DFM_MEM_HOST ? a.get<double>(B * T * r) : nullptr;
-    double* dl = a.get<double>(B * ns * r); double* dr2 = a.get<double>(B * ns);
-    double* dac = a.get<double>(B * ns * L_); double* dser = a.get<double>(B * ns);
-    double* scr = a.get<double>(B * ns * T); int* status = a.get<int>(B);
-    double* dcon = constant ? a.get<double>(B * ns) : nullptr;
-    double* dres = resid ? (mem == DFM_MEM_HOST ? a.get<double>(B * ns * T) : resid) : nullptr;
-    int* cidx = a.get<int>(nc + 1); double* cR = a.get<double>((size_t)nc * r + 1); double* cr = a.get<double>(nc + 1);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* d; const double* f;
-    int rc = stage_in(h, data, dD, B * T * ns, mem, &d); if (rc) return rc;
-    rc = stage_in(h, F, dFb, B * T * r, mem, &f); if (rc) return rc;
-    if (nc > 0) {
-      CK(cudaMemcpyAsync(cidx, o->constr_index, nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(cR, o->constr_R, (size_t)nc * r * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(cr, o->constr_r, nc * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    }
-    CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
-    size_t wk = std::max<size_t>((size_t)K * nc + (size_t)nc * (nc + 1) / 2 + nc, (size_t)L_ * (L_ + 1) / 2 + L_);
-    size_t sm = (size_t)(np + K + 8 + wk) * 8;
-    L(k_loading, ns, batch, 64, sm, d, f, T, ns, r, o->nt_min, L_, dl, dr2, dac, dser, scr, nc, cidx, cR, cr, status, dcon, dres);
-    rc = copy_out(h, lambda, dl, B * ns * r, mem); if (rc) return rc;
-    rc = copy_out(h, r2, dr2, B * ns, mem); if (rc) return rc;
-    rc = copy_out(h, uar_coef, dac, B * ns * L_, mem); if (rc) return rc;
-    rc = copy_out(h, uar_ser, dser, B * ns, mem); if (rc) return rc;
-    if (constant) { rc = copy_out(h, constant, dcon, B * ns, mem); if (rc) return rc; }
-    if (resid && mem == DFM_MEM_HOST) { rc = copy_out(h, resid, dres, B * ns * T, mem); if (rc) return rc; }
-    if (status_out) {
-      // per-panel status (0, or DFM_ERR_NOT_PD when a regression / constraint / AR step of some series was singular;
-      // the affected series carry NaN).  Always a HOST array.
-      CK(cudaMemcpyAsync(status_out, status, B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
-    }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dD, *dFb, *dl, *dr2, *dac, *dser, *scr, *dcon, *cR, *cr;
+  int *status, *cidx;
+  OutSlot<double> oRes;
+  int rc = lay_out(h, [&](Arena& a) {
+    dD = hst ? a.get<double>(B * T * ns) : nullptr;
+    dFb = hst ? a.get<double>(B * T * r) : nullptr;
+    dl = a.get<double>(B * ns * r); dr2 = a.get<double>(B * ns);
+    dac = a.get<double>(B * ns * L_); dser = a.get<double>(B * ns);
+    scr = a.get<double>(B * ns * T); status = a.get<int>(B);
+    dcon = constant ? a.get<double>(B * ns) : nullptr;
+    oRes = staged(a, resid, (size_t)ns * T, B, hst);
+    cidx = a.get<int>(nc + 1); cR = a.get<double>((size_t)nc * r + 1); cr = a.get<double>(nc + 1);
+  });
+  if (rc) return rc;
+  const double* d; const double* f;
+  rc = stage_in(h, data, dD, B * T * ns, mem, &d); if (rc) return rc;
+  rc = stage_in(h, F, dFb, B * T * r, mem, &f); if (rc) return rc;
+  if (nc > 0) {
+    CK(cudaMemcpyAsync(cidx, o->constr_index, nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(cR, o->constr_R, (size_t)nc * r * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(cr, o->constr_r, nc * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  }
+  CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
+  size_t wk = std::max<size_t>((size_t)K * nc + (size_t)nc * (nc + 1) / 2 + nc, (size_t)L_ * (L_ + 1) / 2 + L_);
+  size_t sm = (size_t)(np + K + 8 + wk) * 8;
+  L(k_loading, ns, batch, 64, sm, d, f, T, ns, r, o->nt_min, L_, dl, dr2, dac, dser, scr, nc, cidx, cR, cr, status, dcon, oRes.at(0));
+  rc = copy_out(h, lambda, dl, B * ns * r, mem); if (rc) return rc;
+  rc = copy_out(h, r2, dr2, B * ns, mem); if (rc) return rc;
+  rc = copy_out(h, uar_coef, dac, B * ns * L_, mem); if (rc) return rc;
+  rc = copy_out(h, uar_ser, dser, B * ns, mem); if (rc) return rc;
+  if (constant) { rc = copy_out(h, constant, dcon, B * ns, mem); if (rc) return rc; }
+  rc = oRes.flush(h, 0, B, mem); if (rc) return rc;
+  if (status_out) {
+    // per-panel status (0, or DFM_ERR_NOT_PD when a regression / constraint / AR step of some series was singular;
+    // the affected series carry NaN).  Always a HOST array.
+    CK(cudaMemcpyAsync(status_out, status, B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
   }
   return finish(h, mem);
 }
@@ -1057,32 +1113,33 @@ int dfm_estimate_var(dfm_handle* h, const double* F, int T, int r, int p, int wi
   if (sm > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_estimate_var: r*p or T too large");
   CK(cudaSetDevice(h->device));
   size_t B = batch;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dFb = mem == DFM_MEM_HOST ? a.get<double>(B * T * r) : nullptr;
-    double* db = a.get<double>(B * K * r); double* dres = a.get<double>(B * T * r); double* dse = a.get<double>(B * r * r);
-    double* dM = a.get<double>(B * k * k); double* dQ = a.get<double>(B * r * k); double* dG = a.get<double>(B * k * r);
-    int* status = a.get<int>(B);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* f; int rc = stage_in(h, F, dFb, B * T * r, mem, &f); if (rc) return rc;
-    CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
-    L(k_var, batch, 1, 128, sm, f, T, r, p, withconst, 0, db, dres, dse, dM, dQ, dG, (double*)nullptr, status);
-    rc = copy_out(h, betahat, db, B * K * r, mem); if (rc) return rc;
-    rc = copy_out(h, resid, dres, B * T * r, mem); if (rc) return rc;
-    rc = copy_out(h, seps, dse, B * r * r, mem); if (rc) return rc;
-    rc = copy_out(h, M, dM, B * k * k, mem); if (rc) return rc;
-    rc = copy_out(h, Q, dQ, B * r * k, mem); if (rc) return rc;
-    rc = copy_out(h, G, dG, B * k * r, mem); if (rc) return rc;
-    std::vector<int> hs(B);
-    CK(cudaMemcpyAsync(hs.data(), status, B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    // a failed panel (too few complete rows / singular regression) has NaN in all of its outputs.  A single-panel call
-    // reports the failure as the return code; a batched call fails only when NO panel could be fitted, so that one
-    // degenerate bootstrap draw does not void the other replications (callers test the outputs for NaN).
-    size_t nfail = 0; int first = 0;
-    for (size_t b = 0; b < B; ++b) if (hs[b]) { if (!nfail) first = hs[b]; ++nfail; }
-    if (nfail == B) return fail(h, first, "dfm_estimate_var: regression failed");
-  }
+  double *dFb, *db, *dres, *dse, *dM, *dQ, *dG;
+  int* status;
+  int rc = lay_out(h, [&](Arena& a) {
+    dFb = mem == DFM_MEM_HOST ? a.get<double>(B * T * r) : nullptr;
+    db = a.get<double>(B * K * r); dres = a.get<double>(B * T * r); dse = a.get<double>(B * r * r);
+    dM = a.get<double>(B * k * k); dQ = a.get<double>(B * r * k); dG = a.get<double>(B * k * r);
+    status = a.get<int>(B);
+  });
+  if (rc) return rc;
+  const double* f; rc = stage_in(h, F, dFb, B * T * r, mem, &f); if (rc) return rc;
+  CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
+  L(k_var, batch, 1, 128, sm, f, T, r, p, withconst, 0, db, dres, dse, dM, dQ, dG, (double*)nullptr, status);
+  rc = copy_out(h, betahat, db, B * K * r, mem); if (rc) return rc;
+  rc = copy_out(h, resid, dres, B * T * r, mem); if (rc) return rc;
+  rc = copy_out(h, seps, dse, B * r * r, mem); if (rc) return rc;
+  rc = copy_out(h, M, dM, B * k * k, mem); if (rc) return rc;
+  rc = copy_out(h, Q, dQ, B * r * k, mem); if (rc) return rc;
+  rc = copy_out(h, G, dG, B * k * r, mem); if (rc) return rc;
+  std::vector<int> hs(B);
+  CK(cudaMemcpyAsync(hs.data(), status, B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  // a failed panel (too few complete rows / singular regression) has NaN in all of its outputs.  A single-panel call
+  // reports the failure as the return code; a batched call fails only when NO panel could be fitted, so that one
+  // degenerate bootstrap draw does not void the other replications (callers test the outputs for NaN).
+  size_t nfail = 0; int first = 0;
+  for (size_t b = 0; b < B; ++b) if (hs[b]) { if (!nfail) first = hs[b]; ++nfail; }
+  if (nfail == B) return fail(h, first, "dfm_estimate_var: regression failed");
   return finish(h, mem);
 }
 
@@ -1097,23 +1154,26 @@ int dfm_irf(dfm_handle* h, const double* M, const double* Q, const double* G, in
   if (smI > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_irf: state dimension k too large (k > 14076)");
   CK(cudaSetDevice(h->device));
   size_t B = batch;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dM = mem == DFM_MEM_HOST ? a.get<double>(B * k * k) : nullptr;
-    double* dQ = mem == DFM_MEM_HOST ? a.get<double>(B * r * k) : nullptr;
-    double* dG = mem == DFM_MEM_HOST ? a.get<double>(B * k * r) : nullptr;
-    double* dI = mem == DFM_MEM_HOST ? a.get<double>(B * r * H * n_shock) : irf;
-    int* ids = a.get<int>(n_shock);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double *m, *q, *g;
-    int rc = stage_in(h, M, dM, B * k * k, mem, &m); if (rc) return rc;
-    rc = stage_in(h, Q, dQ, B * r * k, mem, &q); if (rc) return rc;
-    rc = stage_in(h, G, dG, B * k * r, mem, &g); if (rc) return rc;
-    CK(cudaMemcpyAsync(ids, shock_ids, n_shock * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    DFM_SET_SMEM(k_irf, smI);                                // (every call: a lower value from an earlier call may be in place)
-    L(k_irf, n_shock, batch, 64, smI, m, q, g, k, r, H, n_shock, ids, dI);
-    if (mem == DFM_MEM_HOST) { rc = copy_out(h, irf, dI, B * r * H * n_shock, mem); if (rc) return rc; }
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dM, *dQ, *dG;
+  int* ids;
+  OutSlot<double> oI;
+  int rc = lay_out(h, [&](Arena& a) {
+    dM = hst ? a.get<double>(B * k * k) : nullptr;
+    dQ = hst ? a.get<double>(B * r * k) : nullptr;
+    dG = hst ? a.get<double>(B * k * r) : nullptr;
+    oI = staged(a, irf, (size_t)r * H * n_shock, B, hst);
+    ids = a.get<int>(n_shock);
+  });
+  if (rc) return rc;
+  const double *m, *q, *g;
+  rc = stage_in(h, M, dM, B * k * k, mem, &m); if (rc) return rc;
+  rc = stage_in(h, Q, dQ, B * r * k, mem, &q); if (rc) return rc;
+  rc = stage_in(h, G, dG, B * k * r, mem, &g); if (rc) return rc;
+  CK(cudaMemcpyAsync(ids, shock_ids, n_shock * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  DFM_SET_SMEM(k_irf, smI);                                // (every call: a lower value from an earlier call may be in place)
+  L(k_irf, n_shock, batch, 64, smI, m, q, g, k, r, H, n_shock, ids, oI.at(0));
+  rc = oI.flush(h, 0, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1129,48 +1189,49 @@ int dfm_em_init_from_factors(dfm_handle* h, const double* Xs, const double* F, i
   CK(cudaSetDevice(h->device));
   size_t B = batch, TN = (size_t)T * N; int np = r * (r + 1) / 2;
   EmbPlan embi = emb_plan(T, N, r, batch, h->nsm);
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
-    double* dFb = mem == DFM_MEM_HOST ? a.get<double>(B * T * r) : nullptr;
-    double* dL = a.get<double>(B * N * r); double* dR = a.get<double>(B * N);
-    double* dA = a.get<double>(B * r * k); double* dQ = a.get<double>(B * r * r); double* dres = a.get<double>(B * T * r);
-    int* status = a.get<int>(B);
-    EmState* est = nullptr; int* miss = nullptr; double *dFtF = nullptr, *dWs = nullptr, *dlogRs = nullptr;
+  double *dX, *dFb, *dL, *dR, *dA, *dQ, *dres;
+  int* status;
+  EmState* est = nullptr; int* miss = nullptr; double *dFtF = nullptr, *dWs = nullptr, *dlogRs = nullptr;
+  int rc = lay_out(h, [&](Arena& a) {
+    dX = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
+    dFb = mem == DFM_MEM_HOST ? a.get<double>(B * T * r) : nullptr;
+    dL = a.get<double>(B * N * r); dR = a.get<double>(B * N);
+    dA = a.get<double>(B * r * k); dQ = a.get<double>(B * r * r); dres = a.get<double>(B * T * r);
+    status = a.get<int>(B);
     if (embi.on) {
       est = a.get<EmState>(B); miss = a.get<int>(B); dFtF = a.get<double>(B * r * r); dWs = a.get<double>(B * N * r); dlogRs = a.get<double>(B * N);
       embi.Spart = a.get<double>((size_t)embi.tsM * B * N * r); embi.sxxpart = a.get<double>((size_t)embi.tsM * B * N);
       embi.Cpart = a.get<double>(B * embi.ntM * r * r); embi.counters = a.get<int>(B * (size_t)(embi.ntE + embi.ntM));
     }
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double *x, *f;
-    int rc = stage_in(h, Xs, dX, B * TN, mem, &x); if (rc) return rc;
-    rc = stage_in(h, F, dFb, B * T * r, mem, &f); if (rc) return rc;
-    CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
-    size_t smL = (size_t)(2 * np + 2 * r + 8) * 8;
-    if (embi.on) {
-      // balanced panels: Lam = (X'F)(F'F)^-1, R = ssr / T on the tensor-core M-step kernel (S_ff = F'F, no state covariance);
-      // panels with missing data keep the masked per-series regressions
-      CK(cudaMemsetAsync(est, 0, B * sizeof(EmState), h->stream));
-      CK(cudaMemsetAsync(miss, 0, B * sizeof(int), h->stream));
-      CK(cudaMemsetAsync(embi.counters, 0, sizeof(int) * B * (size_t)(embi.ntE + embi.ntM), h->stream));
-      CK(cudaMemsetAsync(dL, 0, B * N * r * sizeof(double), h->stream));
-      CK(cudaMemsetAsync(dR, 0, B * N * sizeof(double), h->stream));
-      L(k_emb_init_flags, N, batch, 64, 0, x, T, N, est, miss);
-      L(k_gram_small, batch, 1, 128, 0, f, T, r, dFtF, (const AlsState*)nullptr);
-      emb_launch_M(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est);
-      L(k_als_lambda, N, batch, 64, smL, x, f, T, N, r, 0, 2, dL, dR, (const double*)nullptr, 0, (const int*)nullptr,
-        (const double*)nullptr, (const double*)nullptr, (const double*)nullptr, (AlsState*)nullptr, (const int*)miss);
-    } else
+  });
+  if (rc) return rc;
+  const double *x, *f;
+  rc = stage_in(h, Xs, dX, B * TN, mem, &x); if (rc) return rc;
+  rc = stage_in(h, F, dFb, B * T * r, mem, &f); if (rc) return rc;
+  CK(cudaMemsetAsync(status, 0, B * sizeof(int), h->stream));
+  size_t smL = (size_t)(2 * np + 2 * r + 8) * 8;
+  if (embi.on) {
+    // balanced panels: Lam = (X'F)(F'F)^-1, R = ssr / T on the tensor-core M-step kernel (S_ff = F'F, no state covariance);
+    // panels with missing data keep the masked per-series regressions
+    CK(cudaMemsetAsync(est, 0, B * sizeof(EmState), h->stream));
+    CK(cudaMemsetAsync(miss, 0, B * sizeof(int), h->stream));
+    CK(cudaMemsetAsync(embi.counters, 0, sizeof(int) * B * (size_t)(embi.ntE + embi.ntM), h->stream));
+    CK(cudaMemsetAsync(dL, 0, B * N * r * sizeof(double), h->stream));
+    CK(cudaMemsetAsync(dR, 0, B * N * sizeof(double), h->stream));
+    L(k_emb_init_flags, N, batch, 64, 0, x, T, N, est, miss);
+    L(k_gram_small, batch, 1, 128, 0, f, T, r, dFtF, (const AlsState*)nullptr);
+    emb_launch_M(h, embi, x, f, dFtF, T, N, r, batch, dL, dR, dWs, dlogRs, est);
     L(k_als_lambda, N, batch, 64, smL, x, f, T, N, r, 0, 2, dL, dR, (const double*)nullptr, 0, (const int*)nullptr,
-      (const double*)nullptr, (const double*)nullptr, (const double*)nullptr, (AlsState*)nullptr, (const int*)nullptr);
-    L(k_var, batch, 1, 128, smV, f, T, r, p, 0, 1, (double*)nullptr, dres, dQ, (double*)nullptr, (double*)nullptr,
-      (double*)nullptr, dA, status);
-    rc = copy_out(h, Lam, dL, B * N * r, mem); if (rc) return rc;
-    rc = copy_out(h, R, dR, B * N, mem); if (rc) return rc;
-    rc = copy_out(h, A, dA, B * r * k, mem); if (rc) return rc;
-    rc = copy_out(h, Q, dQ, B * r * r, mem); if (rc) return rc;
-  }
+      (const double*)nullptr, (const double*)nullptr, (const double*)nullptr, (AlsState*)nullptr, (const int*)miss);
+  } else
+  L(k_als_lambda, N, batch, 64, smL, x, f, T, N, r, 0, 2, dL, dR, (const double*)nullptr, 0, (const int*)nullptr,
+    (const double*)nullptr, (const double*)nullptr, (const double*)nullptr, (AlsState*)nullptr, (const int*)nullptr);
+  L(k_var, batch, 1, 128, smV, f, T, r, p, 0, 1, (double*)nullptr, dres, dQ, (double*)nullptr, (double*)nullptr,
+    (double*)nullptr, dA, status);
+  rc = copy_out(h, Lam, dL, B * N * r, mem); if (rc) return rc;
+  rc = copy_out(h, R, dR, B * N, mem); if (rc) return rc;
+  rc = copy_out(h, A, dA, B * r * k, mem); if (rc) return rc;
+  rc = copy_out(h, Q, dQ, B * r * r, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1252,9 +1313,10 @@ static int em_kalman_impl(dfm_handle* h, const double* X, const dfm_em_opts* o, 
   const bool try_fused = (fused_ok || fused2_ok) && o->path != 1 && nc == 0;      // the path is only chosen after the NaN scan
   const bool use2 = fused2_ok && (o->path == 0 || o->path == 3) && nc == 0;
   const EmbPlan emb = emb_plan(T, N, r, batch, h->nsm);
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    EmBufs d;
+  EmBufs d;
+  GenBufs g;
+  EmConstr cs;
+  int rc = lay_out(h, [&](Arena& a) {
     d.X = mem == DFM_MEM_HOST ? a.get<double>(B * TN) : nullptr;
     d.L = a.get<double>(B * N * r); d.R = a.get<double>(B * N);
     d.A = a.get<double>(B * rk); d.Q = a.get<double>(B * rr); d.P0 = a.get<double>(B * kk);
@@ -1265,63 +1327,63 @@ static int em_kalman_impl(dfm_handle* h, const double* X, const dfm_em_opts* o, 
     d.flag = a.get<int>(4);
     d.ready = a.get<int>(kMaxReadyChunks);
     d.scratch = try_fused ? a.get<double>((size_t)std::min(batch, h->nsm * 8) * T * FUSED_SCR(r)) : nullptr;
-    const GenBufs g = gen_bufs(a, emb, B, T, N, r, p);        // also the fallback when the scan finds missing data
-    const EmConstr cs = constr_bufs(a, cc, N, r);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    int rc = constr_upload(h, cc, cs);
-    if (rc) return rc;
-    bool fused = try_fused;
-    bool uploaded = false;                // the streaming host path found missing data: the panels are on the device already
+    g = gen_bufs(a, emb, B, T, N, r, p);        // also the fallback when the scan finds missing data
+    cs = constr_bufs(a, cc, N, r);
+  });
+  if (rc) return rc;
+  rc = constr_upload(h, cc, cs);
+  if (rc) return rc;
+  bool fused = try_fused;
+  bool uploaded = false;                // the streaming host path found missing data: the panels are on the device already
 #ifndef DFM_EMU
-    if (mem == DFM_MEM_HOST && use2 && em_streaming_applies(h, o)) {
-      rc = em_streaming(h, X, o, init, out, d, &uploaded);
-      if (rc || !uploaded) return rc;
-      if (o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
-      fused = false;                      // general path on the whole batch (the fused kernel updated earlier chunks in place)
-    }
-#endif
-    const double* x = d.X;
-    if (!uploaded) { rc = stage_in(h, X, d.X, B * TN, mem, &x); if (rc) return rc; }
-    cudaMemcpyKind kin = mem == DFM_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    CK(cudaMemcpyAsync(d.L, init->Lam, B * N * r * 8, kin, h->stream));
-    CK(cudaMemcpyAsync(d.R, init->R, B * N * 8, kin, h->stream));
-    CK(cudaMemcpyAsync(d.A, init->A, B * rk * 8, kin, h->stream));
-    CK(cudaMemcpyAsync(d.Q, init->Q, B * rr * 8, kin, h->stream));
-    if (init->P0) CK(cudaMemcpyAsync(d.P0, init->P0, B * kk * 8, kin, h->stream));
-    else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, d.A, d.Q, r, p, d.P0, 12);
-    {
-      long long n = (long long)B * mi;
-      L(k_fill, (int)std::min<long long>((n + 255) / 256, 1024), 1, 256, 0, d.ll, n, DFM_NAN);
-    }
-    if (fused) {                          // balanced panel, all series in the model?
-      CK(cudaMemsetAsync(d.flag, 0, sizeof(int), h->stream));
-      L(k_em_scan_fused, N, batch, 64, 0, x, d.L, d.R, T, N, r, d.flag);
-      int hflag = 0;
-      CK(cudaMemcpyAsync(&hflag, d.flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
-      if (hflag) {
-        if (o->path == 2 || o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
-        fused = false;
-      }
-    }
-    if (fused) rc = launch_em_fused(h, fused_args(d, o, x), r, use2);
-    else rc = run_em_general(h, x, o, d, g, out->PF ? 1 : 0, cs);
-    if (rc) return rc;
-    rc = copy_out(h, out->Lam, d.L, B * N * r, mem); if (rc) return rc;
-    rc = copy_out(h, out->R, d.R, B * N, mem); if (rc) return rc;
-    rc = copy_out(h, out->A, d.A, B * rk, mem); if (rc) return rc;
-    rc = copy_out(h, out->Q, d.Q, B * rr, mem); if (rc) return rc;
-    rc = copy_out(h, out->P0, d.P0, B * kk, mem); if (rc) return rc;
-    rc = copy_out(h, out->F, d.Fs, B * T * r, mem); if (rc) return rc;
-    if (out->PF) {
-      long long n = (long long)T * rr;
-      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, d.PsF, T, r, d.PF);
-      rc = copy_out(h, out->PF, d.PF, B * T * rr, mem); if (rc) return rc;
-    }
-    rc = copy_out(h, out->loglik, d.ll, B * mi, mem); if (rc) return rc;
-    rc = copy_out(h, out->iters, d.it, B, mem); if (rc) return rc;
-    rc = copy_out(h, out->status, d.stat, B, mem); if (rc) return rc;
+  if (mem == DFM_MEM_HOST && use2 && em_streaming_applies(h, o)) {
+    rc = em_streaming(h, X, o, init, out, d, &uploaded);
+    if (rc || !uploaded) return rc;
+    if (o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
+    fused = false;                      // general path on the whole batch (the fused kernel updated earlier chunks in place)
   }
+#endif
+  const double* x = d.X;
+  if (!uploaded) { rc = stage_in(h, X, d.X, B * TN, mem, &x); if (rc) return rc; }
+  cudaMemcpyKind kin = mem == DFM_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  CK(cudaMemcpyAsync(d.L, init->Lam, B * N * r * 8, kin, h->stream));
+  CK(cudaMemcpyAsync(d.R, init->R, B * N * 8, kin, h->stream));
+  CK(cudaMemcpyAsync(d.A, init->A, B * rk * 8, kin, h->stream));
+  CK(cudaMemcpyAsync(d.Q, init->Q, B * rr * 8, kin, h->stream));
+  if (init->P0) CK(cudaMemcpyAsync(d.P0, init->P0, B * kk * 8, kin, h->stream));
+  else L(k_lyapunov, batch, 1, 128, (size_t)(3 * kk + 8) * 8, d.A, d.Q, r, p, d.P0, 12);
+  {
+    long long n = (long long)B * mi;
+    L(k_fill, (int)std::min<long long>((n + 255) / 256, 1024), 1, 256, 0, d.ll, n, DFM_NAN);
+  }
+  if (fused) {                          // balanced panel, all series in the model?
+    CK(cudaMemsetAsync(d.flag, 0, sizeof(int), h->stream));
+    L(k_em_scan_fused, N, batch, 64, 0, x, d.L, d.R, T, N, r, d.flag);
+    int hflag = 0;
+    CK(cudaMemcpyAsync(&hflag, d.flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (hflag) {
+      if (o->path == 2 || o->path == 3) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_em_kalman: fused path needs a balanced panel (no NaN)");
+      fused = false;
+    }
+  }
+  if (fused) rc = launch_em_fused(h, fused_args(d, o, x), r, use2);
+  else rc = run_em_general(h, x, o, d, g, out->PF ? 1 : 0, cs);
+  if (rc) return rc;
+  rc = copy_out(h, out->Lam, d.L, B * N * r, mem); if (rc) return rc;
+  rc = copy_out(h, out->R, d.R, B * N, mem); if (rc) return rc;
+  rc = copy_out(h, out->A, d.A, B * rk, mem); if (rc) return rc;
+  rc = copy_out(h, out->Q, d.Q, B * rr, mem); if (rc) return rc;
+  rc = copy_out(h, out->P0, d.P0, B * kk, mem); if (rc) return rc;
+  rc = copy_out(h, out->F, d.Fs, B * T * r, mem); if (rc) return rc;
+  if (out->PF) {
+    long long n = (long long)T * rr;
+    L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, d.PsF, T, r, d.PF);
+    rc = copy_out(h, out->PF, d.PF, B * T * rr, mem); if (rc) return rc;
+  }
+  rc = copy_out(h, out->loglik, d.ll, B * mi, mem); if (rc) return rc;
+  rc = copy_out(h, out->iters, d.it, B, mem); if (rc) return rc;
+  rc = copy_out(h, out->status, d.stat, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1434,48 +1496,40 @@ int dfm_kalman_smooth(dfm_handle* h, const double* X, const dfm_ss_opts* o, cons
   const size_t smP = ss_project_smem_doubles(r) * 8;
   CK(cudaSetDevice(h->device));
   const size_t B = batch, TN = (size_t)Tp * N; const int rr = r * r;
-  const bool dev_out = mem == DFM_MEM_DEVICE;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    SsStage s = ss_bufs(a, mem, H, B, Tp, N, r, p);
-    double* dPFfull = (out->PF && !dev_out) ? a.get<double>(B * Tp * rr) : nullptr;
-    double* dcom = (out->common && !dev_out) ? a.get<double>(B * TN) : nullptr;
-    double* dxh = (out->xhat && !dev_out) ? a.get<double>(B * TN) : nullptr;
-    double* dxv = (out->xvar && !dev_out) ? a.get<double>(B * TN) : nullptr;
-    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    rc = ss_estep(h, s, X, params, T, N, r, p, H, batch, mem);
-    if (rc) return rc;
-    L(k_ss_nan_failed, batch, 1, 256, 0, (const EmState*)s.st, Tp, r, s.Fs, s.PsF, s.ll);
-    // ---- projection onto the series
-    double* ocom = dev_out ? out->common : dcom;
-    double* oxh = dev_out ? out->xhat : dxh;
-    double* oxv = dev_out ? out->xvar : dxv;
-    if (ocom || oxh || oxv) {
-      DFM_SET_SMEM(k_ss_project, smP);
-      const int nst = (N + SS_NS - 1) / SS_NS, ntt = (Tp + SS_TP - 1) / SS_TP;
-      const int per = std::max(1, 65535 / nst);            // panels per launch (grid.y limit)
-      for (int b0 = 0; b0 < batch; b0 += per) {
-        const int nb = std::min(per, batch - b0);
-        L(k_ss_project, ntt, nst * nb, 256, smP, s.x, (const double*)s.Fs, (const double*)s.PsF, s.pL, s.pR, (const EmState*)s.st, Tp, N, r,
-          b0, ocom, oxh, oxv);
-      }
+  const bool hst = mem == DFM_MEM_HOST;
+  SsStage s;
+  OutSlot<double> oPF, oCom, oXh, oXv;
+  rc = lay_out(h, [&](Arena& a) {
+    s = ss_bufs(a, mem, H, B, Tp, N, r, p);
+    oPF = staged(a, out->PF, (size_t)Tp * rr, B, hst);
+    oCom = staged(a, out->common, TN, B, hst);
+    oXh = staged(a, out->xhat, TN, B, hst);
+    oXv = staged(a, out->xvar, TN, B, hst);
+  });
+  if (rc) return rc;
+  rc = ss_estep(h, s, X, params, T, N, r, p, H, batch, mem);
+  if (rc) return rc;
+  L(k_ss_nan_failed, batch, 1, 256, 0, (const EmState*)s.st, Tp, r, s.Fs, s.PsF, s.ll);
+  // ---- projection onto the series
+  if (out->common || out->xhat || out->xvar) {
+    DFM_SET_SMEM(k_ss_project, smP);
+    const int nst = (N + SS_NS - 1) / SS_NS, ntt = (Tp + SS_TP - 1) / SS_TP;
+    const int per = std::max(1, 65535 / nst);            // panels per launch (grid.y limit)
+    for (int b0 = 0; b0 < batch; b0 += per) {
+      const int nb = std::min(per, batch - b0);
+      L(k_ss_project, ntt, nst * nb, 256, smP, s.x, (const double*)s.Fs, (const double*)s.PsF, s.pL, s.pR, (const EmState*)s.st, Tp, N, r,
+        b0, oCom.at(0), oXh.at(0), oXv.at(0));
     }
-    // ---- results
-    rc = copy_out(h, out->F, s.Fs, B * Tp * r, mem); if (rc) return rc;
-    if (out->PF) {
-      long long n = (long long)Tp * rr;
-      double* dst = dev_out ? out->PF : dPFfull;
-      L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, s.PsF, Tp, r, dst);
-      if (!dev_out) { rc = copy_out(h, out->PF, dPFfull, B * Tp * rr, mem); if (rc) return rc; }
-    }
-    if (!dev_out) {
-      rc = copy_out(h, out->common, dcom, B * TN, mem); if (rc) return rc;
-      rc = copy_out(h, out->xhat, dxh, B * TN, mem); if (rc) return rc;
-      rc = copy_out(h, out->xvar, dxv, B * TN, mem); if (rc) return rc;
-    }
-    rc = copy_out(h, out->loglik, s.ll, B, mem); if (rc) return rc;
-    rc = copy_out(h, out->status, s.stat, B, mem); if (rc) return rc;
   }
+  // ---- results
+  rc = copy_out(h, out->F, s.Fs, B * Tp * r, mem); if (rc) return rc;
+  if (out->PF) {
+    long long n = (long long)Tp * rr;
+    L(k_unpack_psf, (int)std::min<long long>((n + 255) / 256, 1024), batch, 256, 0, s.PsF, Tp, r, oPF.at(0));
+  }
+  rc = flush(h, 0, B, mem, oPF, oCom, oXh, oXv); if (rc) return rc;
+  rc = copy_out(h, out->loglik, s.ll, B, mem); if (rc) return rc;
+  rc = copy_out(h, out->status, s.stat, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1502,45 +1556,43 @@ int dfm_simulation_smoother(dfm_handle* h, const double* X, const dfm_sim_opts* 
   const int Tp = T + H, k = r * p;
   const size_t smG = sim_gains_smem_doubles(r, p) * 8, smS = sim_paths_smem_doubles(r, p) * 8, smP = sim_project_smem_doubles(r) * 8;
   CK(cudaSetDevice(h->device));
-  const bool dev_out = mem == DFM_MEM_DEVICE;
-  const long long nch = sim_chunk(o->n_draw, Tp, N, r, k, out->F && !dev_out, out->X && !dev_out);
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    SsStage s = ss_bufs(a, mem, H, 1, Tp, N, r, p);
-    double* gains = a.get<double>(sim_gains_doubles(Tp, k, r));
-    int* sstat = a.get<int>(1);
-    double* zfS = a.get<double>((size_t)nch * Tp * k);
-    double* fS = a.get<double>((size_t)nch * Tp * r);
-    double* dF = (out->F && !dev_out) ? a.get<double>((size_t)nch * Tp * r) : nullptr;
-    double* dX = (out->X && !dev_out) ? a.get<double>((size_t)nch * Tp * N) : nullptr;
-    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    rc = ss_estep(h, s, X, params, T, N, r, p, H, 1, mem);
-    if (rc) return rc;
-    const int* src = s.g.nt + Tp;                        // src[t] of k_em_filter_smooth (g.nt: n_t, then src_t)
-    CK(cudaMemsetAsync(sstat, 0, sizeof(int), h->stream));
-    DFM_SET_SMEM(k_sim_gains, smG);
-    L(k_sim_gains, Tp + 1, 1, 256, smG, s.pA, s.pQ, (const double*)s.P0, (const double*)s.g.C, (const double*)s.g.Ct, (const double*)s.g.Bt,
-      (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const int*)s.g.nt, (const EmState*)s.st, Tp, r, p, gains, sstat);
-    DFM_SET_SMEM(k_sim_paths, smS);
-    DFM_SET_SMEM(k_sim_project, smP);
-    const int nst = (N + SS_NS - 1) / SS_NS, ntt = (Tp + SS_TP - 1) / SS_TP;
-    for (long long j0 = 0; j0 < o->n_draw; j0 += nch) {
-      const int nd = (int)std::min(nch, o->n_draw - j0);
-      const long long id0 = o->draw0 + j0;
-      double* Fo = out->F ? (dev_out ? out->F + (size_t)j0 * Tp * r : dF) : nullptr;
-      double* Xo = out->X ? (dev_out ? out->X + (size_t)j0 * Tp * N : dX) : nullptr;
-      L(k_sim_paths, (nd + SIM_ND - 1) / SIM_ND, 1, SIM_NT, smS, (const double*)gains, src, Tp, r, p, o->seed, id0, nd, (const int*)sstat,
-        zfS, fS, Fo);
-      if (Xo)
-        L(k_sim_project, ntt, nst * ((nd + SIM_PD - 1) / SIM_PD), 256, smP, s.x, s.pL, s.pR, (const double*)fS, Tp, N, r, o->seed, id0, nd,
-          (const int*)sstat, Xo, 0, 1LL);
-      if (!dev_out) {
-        if (out->F) { rc = copy_out(h, out->F + (size_t)j0 * Tp * r, dF, (size_t)nd * Tp * r, mem); if (rc) return rc; }
-        if (out->X) { rc = copy_out(h, out->X + (size_t)j0 * Tp * N, dX, (size_t)nd * Tp * N, mem); if (rc) return rc; }
-      }
-    }
-    rc = copy_out(h, out->status, sstat, 1, mem); if (rc) return rc;
+  const bool hst = mem == DFM_MEM_HOST;
+  const long long nch = sim_chunk(o->n_draw, Tp, N, r, k, out->F && hst, out->X && hst);
+  SsStage s;
+  double *gains, *zfS, *fS;
+  int* sstat;
+  OutSlot<double> oF, oX;
+  rc = lay_out(h, [&](Arena& a) {
+    s = ss_bufs(a, mem, H, 1, Tp, N, r, p);
+    gains = a.get<double>(sim_gains_doubles(Tp, k, r));
+    sstat = a.get<int>(1);
+    zfS = a.get<double>((size_t)nch * Tp * k);
+    fS = a.get<double>((size_t)nch * Tp * r);
+    oF = staged(a, out->F, (size_t)Tp * r, nch, hst);
+    oX = staged(a, out->X, (size_t)Tp * N, nch, hst);
+  });
+  if (rc) return rc;
+  rc = ss_estep(h, s, X, params, T, N, r, p, H, 1, mem);
+  if (rc) return rc;
+  const int* src = s.g.nt + Tp;                        // src[t] of k_em_filter_smooth (g.nt: n_t, then src_t)
+  CK(cudaMemsetAsync(sstat, 0, sizeof(int), h->stream));
+  DFM_SET_SMEM(k_sim_gains, smG);
+  L(k_sim_gains, Tp + 1, 1, 256, smG, s.pA, s.pQ, (const double*)s.P0, (const double*)s.g.C, (const double*)s.g.Ct, (const double*)s.g.Bt,
+    (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const int*)s.g.nt, (const EmState*)s.st, Tp, r, p, gains, sstat);
+  DFM_SET_SMEM(k_sim_paths, smS);
+  DFM_SET_SMEM(k_sim_project, smP);
+  const int nst = (N + SS_NS - 1) / SS_NS, ntt = (Tp + SS_TP - 1) / SS_TP;
+  for (long long j0 = 0; j0 < o->n_draw; j0 += nch) {
+    const int nd = (int)std::min(nch, o->n_draw - j0);
+    const long long id0 = o->draw0 + j0;
+    L(k_sim_paths, (nd + SIM_ND - 1) / SIM_ND, 1, SIM_NT, smS, (const double*)gains, src, Tp, r, p, o->seed, id0, nd, (const int*)sstat,
+      zfS, fS, oF.at(j0));
+    if (out->X)
+      L(k_sim_project, ntt, nst * ((nd + SIM_PD - 1) / SIM_PD), 256, smP, s.x, s.pL, s.pR, (const double*)fS, Tp, N, r, o->seed, id0, nd,
+        (const int*)sstat, oX.at(j0), 0, 1LL);
+    rc = flush(h, j0, nd, mem, oF, oX); if (rc) return rc;
   }
+  rc = copy_out(h, out->status, sstat, 1, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1588,65 +1640,59 @@ int dfm_news(dfm_handle* h, const double* X_old, const double* X_new, const dfm_
   const size_t smC = (big_in_smem ? smallC + bigC : smallC) * 8, smP = news_project_smem_doubles(r) * 8;
   const int nst = (N + NEWS_NS - 1) / NEWS_NS, ntw = (nr + NEWS_TP - 1) / NEWS_TP, ntile = nst * ntw;
   CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    SsStage s = ss_bufs(a, mem, H, B, Tp, N, r, p);
-    double* dXn = dev ? nullptr : a.get<double>(B * onr);
-    int* dtg = a.get<int>(2 * (size_t)nq);
-    unsigned char* dmask = a.get<unsigned char>(B * onr);
-    int* dpl = a.get<int>(B * (Wmax + 1));
-    int* drowp = a.get<int>(B * nr);
-    int* dpst = a.get<int>(B);
-    int* dkind = a.get<int>(B * nq);
-    double* dold = a.get<double>(B * nq);
-    double* dgv = a.get<double>(B * nq * nmax);
-    double* dpart = a.get<double>(B * ntile * nq);
-    double* dbig = big_in_smem ? nullptr : a.get<double>(B * bigC);
-    double* hOld = (out->old_est && !dev) ? a.get<double>(B * nq) : nullptr;
-    double* hNew = (out->new_est && !dev) ? a.get<double>(B * nq) : nullptr;
-    double* hNews = (out->news && !dev) ? a.get<double>(B * onr) : nullptr;
-    double* hW = (out->weight && !dev) ? a.get<double>(B * onr * nq) : nullptr;
-    double* hC = (out->contrib && !dev) ? a.get<double>(B * onr * nq) : nullptr;
-    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    rc = ss_estep(h, s, X_old, params, T, N, r, p, H, batch, mem);
-    if (rc) return rc;
-    const int* src = s.g.nt + B * Tp;                  // src[t] of k_em_filter_smooth (g.nt: n_t, then src_t), per pair
-    CK(cudaMemcpyAsync(dtg, tg.data(), tg.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    const double* xn = X_new; int ldn = T, row0 = T - nr;
-    if (dev) CK(cudaMemsetAsync(dpst, 0, B * sizeof(int), h->stream));
-    else {
-      CK(cudaMemcpyAsync(dpst, hbad.data(), B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpy2DAsync(dXn, (size_t)nr * 8,X_new + (T - nr), (size_t)T * 8, (size_t)nr * 8, B * N, cudaMemcpyHostToDevice, h->stream));
-      xn = dXn; ldn = nr; row0 = 0;
-    }
-    L(k_news_window, batch, 1, 256, smW, s.x, xn, ldn, row0, dev ? X_new : (const double*)nullptr, s.pL, s.pR, (const int*)dtg + nq, nq,
-      (const int*)s.stat, T, Tp, N, r, nr, Wmax, dmask, dpl, drowp, dpst);
-    DFM_SET_SMEM(k_news_cov, smC);
-    L(k_news_cov, batch, 1, 256, smC, s.pA, (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const double*)s.Fs, s.x, s.pL, s.pR,
-      (const unsigned char*)dmask, (const int*)dpl, (const int*)dtg, (const int*)dtg + nq, nq, (const int*)dpst, T, Tp, N, r, p, nr, Wmax,
-      dbig, dgv, dkind, dold);
-    double* oNews = out->news ? (dev ? out->news : hNews) : nullptr;
-    double* oW = out->weight ? (dev ? out->weight : hW) : nullptr;
-    double* oC = out->contrib ? (dev ? out->contrib : hC) : nullptr;
-    DFM_SET_SMEM(k_news_project, smP);
-    const int per = std::max(1, 65535 / nst);          // pairs per launch (grid.y limit)
-    for (int b0 = 0; b0 < batch; b0 += per) {
-      const int nb = std::min(per, batch - b0);
-      L(k_news_project, ntw, nst * nb, 256, smP, (const double*)s.Fs, xn, ldn, row0, s.pL, s.pR, (const unsigned char*)dmask,
-        (const int*)drowp, (const double*)dgv, (const int*)dkind, (const int*)dtg, (const int*)dtg + nq, nq, (const int*)dpst, T, Tp, N, r,
-        nr, Wmax, b0, oNews, oW, oC, dpart);
-    }
-    L(k_news_finish, batch, 1, 64, 0, (const double*)dpart, ntile, (const double*)dold, (const int*)dpst, nq,
-      out->old_est ? (dev ? out->old_est : hOld) : (double*)nullptr, out->new_est ? (dev ? out->new_est : hNew) : (double*)nullptr);
-    if (!dev) {
-      rc = copy_out(h, out->old_est, hOld, B * nq, mem); if (rc) return rc;
-      rc = copy_out(h, out->new_est, hNew, B * nq, mem); if (rc) return rc;
-      rc = copy_out(h, out->news, hNews, B * onr, mem); if (rc) return rc;
-      rc = copy_out(h, out->weight, hW, B * onr * nq, mem); if (rc) return rc;
-      rc = copy_out(h, out->contrib, hC, B * onr * nq, mem); if (rc) return rc;
-    }
-    rc = copy_out(h, out->status, dpst, B, mem); if (rc) return rc;
+  SsStage s;
+  double *dXn, *dold, *dgv, *dpart, *dbig;
+  int *dtg, *dpl, *drowp, *dpst, *dkind;
+  unsigned char* dmask;
+  OutSlot<double> oOld, oNew, oNews, oW, oC;
+  rc = lay_out(h, [&](Arena& a) {
+    s = ss_bufs(a, mem, H, B, Tp, N, r, p);
+    dXn = dev ? nullptr : a.get<double>(B * onr);
+    dtg = a.get<int>(2 * (size_t)nq);
+    dmask = a.get<unsigned char>(B * onr);
+    dpl = a.get<int>(B * (Wmax + 1));
+    drowp = a.get<int>(B * nr);
+    dpst = a.get<int>(B);
+    dkind = a.get<int>(B * nq);
+    dold = a.get<double>(B * nq);
+    dgv = a.get<double>(B * nq * nmax);
+    dpart = a.get<double>(B * ntile * nq);
+    dbig = big_in_smem ? nullptr : a.get<double>(B * bigC);
+    oOld = staged(a, out->old_est, (size_t)nq, B, !dev);
+    oNew = staged(a, out->new_est, (size_t)nq, B, !dev);
+    oNews = staged(a, out->news, onr, B, !dev);
+    oW = staged(a, out->weight, onr * nq, B, !dev);
+    oC = staged(a, out->contrib, onr * nq, B, !dev);
+  });
+  if (rc) return rc;
+  rc = ss_estep(h, s, X_old, params, T, N, r, p, H, batch, mem);
+  if (rc) return rc;
+  const int* src = s.g.nt + B * Tp;                  // src[t] of k_em_filter_smooth (g.nt: n_t, then src_t), per pair
+  CK(cudaMemcpyAsync(dtg, tg.data(), tg.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  const double* xn = X_new; int ldn = T, row0 = T - nr;
+  if (dev) CK(cudaMemsetAsync(dpst, 0, B * sizeof(int), h->stream));
+  else {
+    CK(cudaMemcpyAsync(dpst, hbad.data(), B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpy2DAsync(dXn, (size_t)nr * 8,X_new + (T - nr), (size_t)T * 8, (size_t)nr * 8, B * N, cudaMemcpyHostToDevice, h->stream));
+    xn = dXn; ldn = nr; row0 = 0;
   }
+  L(k_news_window, batch, 1, 256, smW, s.x, xn, ldn, row0, dev ? X_new : (const double*)nullptr, s.pL, s.pR, (const int*)dtg + nq, nq,
+    (const int*)s.stat, T, Tp, N, r, nr, Wmax, dmask, dpl, drowp, dpst);
+  DFM_SET_SMEM(k_news_cov, smC);
+  L(k_news_cov, batch, 1, 256, smC, s.pA, (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const double*)s.Fs, s.x, s.pL, s.pR,
+    (const unsigned char*)dmask, (const int*)dpl, (const int*)dtg, (const int*)dtg + nq, nq, (const int*)dpst, T, Tp, N, r, p, nr, Wmax,
+    dbig, dgv, dkind, dold);
+  DFM_SET_SMEM(k_news_project, smP);
+  const int per = std::max(1, 65535 / nst);          // pairs per launch (grid.y limit)
+  for (int b0 = 0; b0 < batch; b0 += per) {
+    const int nb = std::min(per, batch - b0);
+    L(k_news_project, ntw, nst * nb, 256, smP, (const double*)s.Fs, xn, ldn, row0, s.pL, s.pR, (const unsigned char*)dmask,
+      (const int*)drowp, (const double*)dgv, (const int*)dkind, (const int*)dtg, (const int*)dtg + nq, nq, (const int*)dpst, T, Tp, N, r,
+      nr, Wmax, b0, oNews.at(0), oW.at(0), oC.at(0), dpart);
+  }
+  L(k_news_finish, batch, 1, 64, 0, (const double*)dpart, ntile, (const double*)dold, (const int*)dpst, nq, oOld.at(0), oNew.at(0));
+  rc = flush(h, 0, B, mem, oOld, oNew, oNews, oW, oC); if (rc) return rc;
+  rc = copy_out(h, out->status, dpst, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1657,15 +1703,15 @@ int dfm_simulate_panels(dfm_handle* h, unsigned long long seed, long long rep0, 
   if (!h || !X || batch <= 0 || T <= 1 || N <= 0 || r <= 0 || r > 64 || rep0 < 0) return fail(h, DFM_ERR_ARG, "dfm_simulate_panels: bad argument");
   CK(cudaSetDevice(h->device));
   size_t B = batch;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dX = mem == DFM_MEM_HOST ? a.get<double>(B * T * N) : X;
-    double* dF = (mem == DFM_MEM_HOST || !F_true) ? a.get<double>(B * T * r) : F_true;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    L(k_simulate_panels, batch, 1, 256, 0, seed, rep0, T, N, r, dX, dF);
-    if (mem == DFM_MEM_HOST) { int rc = copy_out(h, X, dX, B * T * N, mem); if (rc) return rc; }
-    if (F_true) { int rc = copy_out(h, F_true, dF, B * T * r, mem); if (rc) return rc; }
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  OutSlot<double> oX, oF;
+  int rc = lay_out(h, [&](Arena& a) {
+    oX = staged(a, X, (size_t)T * N, B, hst);
+    oF = scratch(a, F_true, (size_t)T * r, B, hst);
+  });
+  if (rc) return rc;
+  L(k_simulate_panels, batch, 1, 256, 0, seed, rep0, T, N, r, oX.at(0), oF.at(0));
+  rc = flush(h, 0, B, mem, oX, oF); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1680,34 +1726,36 @@ int dfm_bootstrap_panels(dfm_handle* h, const dfm_boot_opts* o, const double* F0
   if (smem > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_bootstrap_panels: T*r too large");
   CK(cudaSetDevice(h->device));
   size_t B = batch; int K = 1 + r * p;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    const bool hst = mem == DFM_MEM_HOST;
-    double* dF0 = hst ? a.get<double>((size_t)Tw * r) : nullptr; double* dre = hst ? a.get<double>((size_t)nres * r) : nullptr;
-    double* dbe = hst ? a.get<double>((size_t)K * r) : nullptr; double* dla = hst ? a.get<double>((size_t)ns * r) : nullptr;
-    double* dac = hst ? a.get<double>((size_t)ns * Lg) : nullptr; double* dse = hst ? a.get<double>(ns) : nullptr;
-    double* dda = hst ? a.get<double>((size_t)Tw * ns) : nullptr;
-    double* dX = hst ? a.get<double>(B * ns * Tw) : X;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    BootArgs ba{};
-    int rc = stage_in(h, F0, dF0, (size_t)Tw * r, mem, &ba.F0); if (rc) return rc;
-    rc = stage_in(h, resid, dre, (size_t)nres * r, mem, &ba.resid); if (rc) return rc;
-    rc = stage_in(h, beta, dbe, (size_t)K * r, mem, &ba.beta); if (rc) return rc;
-    rc = stage_in(h, lam, dla, (size_t)ns * r, mem, &ba.lam); if (rc) return rc;
-    rc = stage_in(h, uar_coef, dac, (size_t)ns * Lg, mem, &ba.uar_coef); if (rc) return rc;
-    rc = stage_in(h, uar_ser, dse, (size_t)ns, mem, &ba.uar_ser); if (rc) return rc;
-    rc = stage_in(h, data, dda, (size_t)Tw * ns, mem, &ba.data); if (rc) return rc;
-    ba.X = dX; ba.Tw = Tw; ba.ns = ns; ba.r = r; ba.p = p; ba.L = Lg; ba.nres = nres; ba.burn = o->burn; ba.seed = o->seed; ba.rep0 = o->rep0;
-    DFM_SET_SMEM(k_bootstrap_panels, smem);
-    L(k_bootstrap_panels, batch, 1, 256, smem, ba);
-    if (hst) { rc = copy_out(h, X, dX, B * ns * Tw, mem); if (rc) return rc; }
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dF0, *dre, *dbe, *dla, *dac, *dse, *dda;
+  OutSlot<double> oX;
+  int rc = lay_out(h, [&](Arena& a) {
+    dF0 = hst ? a.get<double>((size_t)Tw * r) : nullptr; dre = hst ? a.get<double>((size_t)nres * r) : nullptr;
+    dbe = hst ? a.get<double>((size_t)K * r) : nullptr; dla = hst ? a.get<double>((size_t)ns * r) : nullptr;
+    dac = hst ? a.get<double>((size_t)ns * Lg) : nullptr; dse = hst ? a.get<double>(ns) : nullptr;
+    dda = hst ? a.get<double>((size_t)Tw * ns) : nullptr;
+    oX = staged(a, X, (size_t)ns * Tw, B, hst);
+  });
+  if (rc) return rc;
+  BootArgs ba{};
+  rc = stage_in(h, F0, dF0, (size_t)Tw * r, mem, &ba.F0); if (rc) return rc;
+  rc = stage_in(h, resid, dre, (size_t)nres * r, mem, &ba.resid); if (rc) return rc;
+  rc = stage_in(h, beta, dbe, (size_t)K * r, mem, &ba.beta); if (rc) return rc;
+  rc = stage_in(h, lam, dla, (size_t)ns * r, mem, &ba.lam); if (rc) return rc;
+  rc = stage_in(h, uar_coef, dac, (size_t)ns * Lg, mem, &ba.uar_coef); if (rc) return rc;
+  rc = stage_in(h, uar_ser, dse, (size_t)ns, mem, &ba.uar_ser); if (rc) return rc;
+  rc = stage_in(h, data, dda, (size_t)Tw * ns, mem, &ba.data); if (rc) return rc;
+  ba.X = oX.at(0); ba.Tw = Tw; ba.ns = ns; ba.r = r; ba.p = p; ba.L = Lg; ba.nres = nres; ba.burn = o->burn; ba.seed = o->seed; ba.rep0 = o->rep0;
+  DFM_SET_SMEM(k_bootstrap_panels, smem);
+  L(k_bootstrap_panels, batch, 1, 256, smem, ba);
+  rc = oX.flush(h, 0, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
 // One call for the whole C4 replication step (SURVEY.md 8b: "one panel + B bootstrap seeds"): resample -> standardise + PCA
 // + ALS (estimate_factor!, :328-382) -> sign alignment -> factor VAR (:444-492) -> IRF (:793-825), device resident between
-// the stages.  The stages are the public entry points above run on temporaries of this call.
+// the stages.  The stages are the public entry points above run on temporaries of this call, which live in the handle's second
+// workspace (the stages use and may regrow the first).
 int dfm_bootstrap_irf(dfm_handle* h, const dfm_boot_opts* o, const double* F0, const double* resid, const double* beta,
                       const double* lam, const double* uar_coef, const double* uar_ser, const double* data, int nt_min,
                       double tol, int H, double* irf, int* als_iters, int* als_status) {
@@ -1717,43 +1765,45 @@ int dfm_bootstrap_irf(dfm_handle* h, const dfm_boot_opts* o, const double* F0, c
   if (Tw <= p || ns <= 0 || r <= 0 || p <= 0 || Lg <= 0 || nres <= 0 || batch <= 0) return fail(h, DFM_ERR_ARG, "dfm_bootstrap_irf: bad shape");
   CK(cudaSetDevice(h->device));
   const size_t B = batch; const int k = r * p, K = 1 + k;
-  // temporaries of this call (the stages' own scratch lives in the handle's workspace)
+  const bool hst = mem == DFM_MEM_HOST;
   const size_t nin[7] = {(size_t)Tw * r, (size_t)nres * r, (size_t)K * r, (size_t)ns * r, (size_t)ns * Lg, (size_t)ns, (size_t)Tw * ns};
   const double* hin[7] = {F0, resid, beta, lam, uar_coef, uar_ser, data};
-  size_t tot = 0, off[16];
-  auto take = [&](size_t n) { size_t o_ = tot; tot += (n * 8 + 255) & ~(size_t)255; return o_; };
-  for (int i = 0; i < 7; ++i) off[i] = take(nin[i]);
-  const size_t oX = take(B * ns * Tw), oF = take(B * Tw * r), oM = take(B * k * k), oQ = take(B * r * k), oG = take(B * k * r),
-               oI = take(B * (size_t)r * H * r);
-  char* base = nullptr;
-  CK(cudaMalloc((void**)&base, tot));
-  auto D = [&](size_t o_) { return reinterpret_cast<double*>(base + o_); };
-#define BI_FAIL(rc_) do { int r__ = (rc_); if (r__) { cudaStreamSynchronize(h->stream); cudaFree(base); return r__; } } while (0)
-  const double* din[7];
-  for (int i = 0; i < 7; ++i) {
-    if (mem == DFM_MEM_HOST) {
-      if (cudaMemcpyAsync(D(off[i]), hin[i], nin[i] * 8, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) BI_FAIL(fail(h, DFM_ERR_CUDA, "dfm_bootstrap_irf: upload failed"));
-      din[i] = D(off[i]);
-    } else din[i] = hin[i];
-  }
-  dfm_boot_opts ob = *o; ob.mem = DFM_MEM_DEVICE;
-  BI_FAIL(dfm_bootstrap_panels(h, &ob, din[0], din[1], din[2], din[3], din[4], din[5], din[6], D(oX)));
-  dfm_factor_opts fo{}; fo.T = Tw; fo.N = ns; fo.r = r; fo.nt_min = nt_min; fo.tol = tol; fo.max_iter = 100000000; fo.compute_r2 = 0;
-  fo.n_constr = 0; fo.batch = batch; fo.mem = DFM_MEM_DEVICE;
-  std::vector<dfm_factor_stats> fs(B);
-  BI_FAIL(dfm_estimate_factor(h, D(oX), &fo, nullptr, D(oF), nullptr, nullptr, nullptr, nullptr, fs.data()));
-  for (size_t b = 0; b < B; ++b) { if (als_iters) als_iters[b] = fs[b].iters; if (als_status) als_status[b] = fs[b].status; }
-  L(k_sign_align, batch, 1, 128, 48 * 8, D(oF), din[0], Tw, r);
-  int rc = dfm_estimate_var(h, D(oF), Tw, r, p, 1, batch, DFM_MEM_DEVICE, nullptr, nullptr, nullptr, D(oM), D(oQ), D(oG));
-  if (rc != DFM_OK && rc != DFM_ERR_NOT_PD && rc != DFM_ERR_TOO_FEW_OBS) BI_FAIL(rc);       // (all panels failed: records stay NaN)
-  std::vector<int> ids(r); for (int j = 0; j < r; ++j) ids[j] = j;
-  double* dI = mem == DFM_MEM_HOST ? D(oI) : irf;
-  BI_FAIL(dfm_irf(h, D(oM), D(oQ), D(oG), k, r, H, r, ids.data(), batch, DFM_MEM_DEVICE, dI));
-  if (mem == DFM_MEM_HOST && cudaMemcpyAsync(irf, dI, B * (size_t)r * H * r * 8, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess)
-    BI_FAIL(fail(h, DFM_ERR_CUDA, "dfm_bootstrap_irf: download failed"));
+  double* dIn[7];
+  double *dX, *dF, *dM, *dQ, *dG;
+  OutSlot<double> oI;
+  int rc = lay_out(h, [&](Arena& a) {
+    for (int i = 0; i < 7; ++i) dIn[i] = hst ? a.get<double>(nin[i]) : nullptr;
+    dX = a.get<double>(B * ns * Tw); dF = a.get<double>(B * Tw * r);
+    dM = a.get<double>(B * k * k); dQ = a.get<double>(B * r * k); dG = a.get<double>(B * k * r);
+    oI = staged(a, irf, (size_t)r * H * r, B, hst);
+  }, true);
+  if (rc) return rc;
+  // the stages; a failure after work is queued drains the stream before it returns
+  const int ret = [&]() -> int {
+    const double* din[7];
+    for (int i = 0; i < 7; ++i)            // (any mem but DFM_MEM_HOST reads the inputs in place)
+      if (stage_in(h, hin[i], dIn[i], nin[i], hst ? DFM_MEM_HOST : DFM_MEM_DEVICE, &din[i]))
+        return fail(h, DFM_ERR_CUDA, "dfm_bootstrap_irf: upload failed");
+    dfm_boot_opts ob = *o; ob.mem = DFM_MEM_DEVICE;
+    rc = dfm_bootstrap_panels(h, &ob, din[0], din[1], din[2], din[3], din[4], din[5], din[6], dX);
+    if (rc) return rc;
+    dfm_factor_opts fo{}; fo.T = Tw; fo.N = ns; fo.r = r; fo.nt_min = nt_min; fo.tol = tol; fo.max_iter = 100000000; fo.compute_r2 = 0;
+    fo.n_constr = 0; fo.batch = batch; fo.mem = DFM_MEM_DEVICE;
+    std::vector<dfm_factor_stats> fs(B);
+    rc = dfm_estimate_factor(h, dX, &fo, nullptr, dF, nullptr, nullptr, nullptr, nullptr, fs.data());
+    if (rc) return rc;
+    for (size_t b = 0; b < B; ++b) { if (als_iters) als_iters[b] = fs[b].iters; if (als_status) als_status[b] = fs[b].status; }
+    L(k_sign_align, batch, 1, 128, 48 * 8, dF, din[0], Tw, r);
+    rc = dfm_estimate_var(h, dF, Tw, r, p, 1, batch, DFM_MEM_DEVICE, nullptr, nullptr, nullptr, dM, dQ, dG);
+    if (rc != DFM_OK && rc != DFM_ERR_NOT_PD && rc != DFM_ERR_TOO_FEW_OBS) return rc;       // (all panels failed: records stay NaN)
+    std::vector<int> ids(r); for (int j = 0; j < r; ++j) ids[j] = j;
+    rc = dfm_irf(h, dM, dQ, dG, k, r, H, r, ids.data(), batch, DFM_MEM_DEVICE, oI.at(0));
+    if (rc) return rc;
+    if (oI.flush(h, 0, B, mem)) return fail(h, DFM_ERR_CUDA, "dfm_bootstrap_irf: download failed");
+    return DFM_OK;
+  }();
   cudaError_t e = cudaStreamSynchronize(h->stream);
-  cudaFree(base);
-#undef BI_FAIL
+  if (ret) return ret;
   CK(e);
   return DFM_OK;
 }
@@ -1786,27 +1836,28 @@ int dfm_ss_simulate_panels(dfm_handle* h, const double* X, int T, int N, int r, 
   CK(cudaSetDevice(h->device));
   const size_t B = batch, TN = (size_t)T * N; const int k = r * p;
   const bool hst = mem == DFM_MEM_HOST;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dX = hst ? a.get<double>(TN) : nullptr;
-    double* dL = hst ? a.get<double>((size_t)N * r) : nullptr; double* dR = hst ? a.get<double>(N) : nullptr;
-    double* dA = hst ? a.get<double>((size_t)r * k) : nullptr; double* dQ = hst ? a.get<double>((size_t)r * r) : nullptr;
-    double* dP = hst ? a.get<double>((size_t)k * k) : nullptr;
-    double* g = a.get<double>(ssb_chol_doubles(r, p));
-    double* fS = a.get<double>(B * T * r);
-    double* dO = hst ? a.get<double>(B * TN) : Xout;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double *x, *l, *rv, *am, *q, *p0;
-    int rc = stage_in(h, X, dX, TN, mem, &x); if (rc) return rc;
-    rc = stage_in(h, params->Lam, dL, (size_t)N * r, mem, &l); if (rc) return rc;
-    rc = stage_in(h, params->R, dR, (size_t)N, mem, &rv); if (rc) return rc;
-    rc = stage_in(h, params->A, dA, (size_t)r * k, mem, &am); if (rc) return rc;
-    rc = stage_in(h, params->Q, dQ, (size_t)r * r, mem, &q); if (rc) return rc;
-    rc = stage_in(h, params->P0, dP, (size_t)k * k, mem, &p0); if (rc) return rc;
-    L(k_ss_sim_chol, 1, 1, 128, ssb_chol_smem_doubles(r, p) * 8, am, q, p0, r, p, g);
-    ssb_simulate(h, x, l, rv, g, T, N, r, p, seed, rep0, batch, fS, dO);
-    if (hst) { rc = copy_out(h, Xout, dO, B * TN, mem); if (rc) return rc; }
-  }
+  double *dX, *dL, *dR, *dA, *dQ, *dP, *g, *fS;
+  OutSlot<double> oX;
+  int rc = lay_out(h, [&](Arena& a) {
+    dX = hst ? a.get<double>(TN) : nullptr;
+    dL = hst ? a.get<double>((size_t)N * r) : nullptr; dR = hst ? a.get<double>(N) : nullptr;
+    dA = hst ? a.get<double>((size_t)r * k) : nullptr; dQ = hst ? a.get<double>((size_t)r * r) : nullptr;
+    dP = hst ? a.get<double>((size_t)k * k) : nullptr;
+    g = a.get<double>(ssb_chol_doubles(r, p));
+    fS = a.get<double>(B * T * r);
+    oX = staged(a, Xout, TN, B, hst);
+  });
+  if (rc) return rc;
+  const double *x, *l, *rv, *am, *q, *p0;
+  rc = stage_in(h, X, dX, TN, mem, &x); if (rc) return rc;
+  rc = stage_in(h, params->Lam, dL, (size_t)N * r, mem, &l); if (rc) return rc;
+  rc = stage_in(h, params->R, dR, (size_t)N, mem, &rv); if (rc) return rc;
+  rc = stage_in(h, params->A, dA, (size_t)r * k, mem, &am); if (rc) return rc;
+  rc = stage_in(h, params->Q, dQ, (size_t)r * r, mem, &q); if (rc) return rc;
+  rc = stage_in(h, params->P0, dP, (size_t)k * k, mem, &p0); if (rc) return rc;
+  L(k_ss_sim_chol, 1, 1, 128, ssb_chol_smem_doubles(r, p) * 8, am, q, p0, r, p, g);
+  ssb_simulate(h, x, l, rv, g, T, N, r, p, seed, rep0, batch, fS, oX.at(0));
+  rc = oX.flush(h, 0, B, mem); if (rc) return rc;
   return finish(h, mem);
 }
 
@@ -1848,89 +1899,96 @@ int dfm_ss_bootstrap(dfm_handle* h, const double* X, const dfm_ssb_opts* o, cons
   CK(cudaSetDevice(h->device));
   const size_t B = nc, TN = (size_t)T * N, kk = (size_t)k * k, rr = (size_t)r * r, rk = (size_t)r * k, Nr = (size_t)N * r;
   const size_t nirf = (size_t)r * Hi * r;
-  // temporaries of this call, in the second workspace (the stages' own scratch lives in the first, which they may regrow)
-  size_t tot = 0;
-  auto take = [&](size_t n) { size_t o_ = tot; tot += (n * 8 + 255) & ~(size_t)255; return o_; };
   const bool hst = mem == DFM_MEM_HOST;
-  const size_t oXs = take(hst ? TN : 0), oLh = take(hst ? Nr : 0), oRh = take(hst ? N : 0), oAh = take(hst ? rk : 0), oQh = take(hst ? rr : 0),
-               oPh = take(hst ? kk : 0), og = take(ssb_chol_doubles(r, p));
-  const size_t oX = take(B * TN), ofS = take(B * T * r), oiL = take(B * Nr), oiR = take(B * N), oiA = take(B * rk), oiQ = take(B * rr),
-               oiP = take(B * kk), oeL = take(B * Nr), oeR = take(B * N), oeA = take(B * rk), oeQ = take(B * rr), oell = take(B * mi),
-               oeit = take(B), oest = take(B), ooL = take(B * Nr), ooR = take(B * N), ooA = take(B * rk), ooQ = take(B * rr),
-               opL = take(fc ? B * Nr : 0), opR = take(fc ? B * N : 0), opA = take(fc ? B * rk : 0), opQ = take(fc ? B * rr : 0),
-               oM = take(B * kk), oQs = take(B * rk), oG = take(B * rk), ollf = take(B), ost = take(B), oI = take(B * nirf),
-               oxh = take(fc ? B * Tp * N : 0), oxv = take(fc ? B * Tp * N : 0), ofh = take(fc ? B * fr * N : 0), ofv = take(fc ? B * fr * N : 0);
-  { int rc = ensure_rws(h, tot); if (rc) return rc; }
-  char* const base = h->rws;
-  auto D = [&](size_t o_) { return reinterpret_cast<double*>(base + o_); };
-  auto I = [&](size_t o_) { return reinterpret_cast<int*>(base + o_); };
-#define SSB_FAIL(rc_) do { int r__ = (rc_); if (r__) { cudaStreamSynchronize(h->stream); return r__; } } while (0)
-#define SSB_CK(call) SSB_FAIL((call) == cudaSuccess ? DFM_OK : fail(h, DFM_ERR_CUDA, "dfm_ss_bootstrap: copy failed"))
-  const double *xs = X, *Lh = params->Lam, *Rh = params->R, *Ah = params->A, *Qh = params->Q, *Ph = params->P0;
-  if (hst) {
-    const double* src[6] = {X, params->Lam, params->R, params->A, params->Q, params->P0};
-    const size_t dst[6] = {oXs, oLh, oRh, oAh, oQh, oPh}, n[6] = {TN, Nr, (size_t)N, rk, rr, kk};
-    for (int i = 0; i < 6; ++i) SSB_CK(cudaMemcpyAsync(D(dst[i]), src[i], n[i] * 8, cudaMemcpyHostToDevice, h->stream));
-    xs = D(oXs); Lh = D(oLh); Rh = D(oRh); Ah = D(oAh); Qh = D(oQh); Ph = D(oPh);
-  }
-  L(k_ss_sim_chol, 1, 1, 128, ssb_chol_smem_doubles(r, p) * 8, Ah, Qh, Ph, r, p, D(og));
-  std::vector<int> ids(r);
-  for (int j = 0; j < r; ++j) ids[j] = j;
-  const size_t smA = ssb_align_smem_doubles(r, p) * 8;
-  DFM_SET_SMEM(k_ss_align, smA);
-  auto bcast = [&](const double* src, size_t n, double* dst, int nb) {
-    L(k_ss_bcast, (int)std::min<size_t>((n + 255) / 256, 1024), nb, 256, 0, src, (long long)n, dst);
-  };
-  const cudaMemcpyKind kout = hst ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
-  for (long long j0 = 0; j0 < n_rep; j0 += nc) {
-    const int nb = nc;                                              // replicates computed (a full sub-batch, see ssb_batch)
-    const int nkeep = (int)std::min<long long>(nc, n_rep - j0);     // ... and returned
-    // 1. panels
-    ssb_simulate(h, xs, Lh, Rh, D(og), T, N, r, p, o->seed, o->rep0 + j0, nb, D(ofS), D(oX));
-    // 2. EM from the fitted parameters (P0 held fixed)
-    bcast(Lh, Nr, D(oiL), nb); bcast(Rh, N, D(oiR), nb); bcast(Ah, rk, D(oiA), nb); bcast(Qh, rr, D(oiQ), nb); bcast(Ph, kk, D(oiP), nb);
-    dfm_em_opts eo{}; eo.T = T; eo.N = N; eo.r = r; eo.p = p; eo.max_iter = mi; eo.tol = o->tol; eo.batch = nb; eo.mem = DFM_MEM_DEVICE; eo.path = 0;
-    dfm_em_init ei{D(oiL), D(oiR), D(oiA), D(oiQ), D(oiP)};
-    dfm_em_out eout{}; eout.Lam = D(oeL); eout.R = D(oeR); eout.A = D(oeA); eout.Q = D(oeQ); eout.loglik = D(oell); eout.iters = I(oeit);
-    eout.status = I(oest);
-    SSB_FAIL(dfm_em_kalman(h, D(oX), &eo, &ei, &eout));
-    // 3. alignment
-    SsbAlignArgs aa{};
-    aa.Lh = Lh; aa.Rh = Rh; aa.Ah = Ah; aa.Qh = Qh;
-    aa.Ls = D(oeL); aa.Rs = D(oeR); aa.As = D(oeA); aa.Qs = D(oeQ); aa.ll = D(oell); aa.it = I(oeit); aa.em_status = I(oest);
-    aa.Lo = D(ooL); aa.Ro = D(ooR); aa.Ao = D(ooA); aa.Qo = D(ooQ);
-    if (fc) { aa.Le = D(opL); aa.Re = D(opR); aa.Ae = D(opA); aa.Qe = D(opQ); }
-    aa.M = D(oM); aa.Qsel = D(oQs); aa.G = D(oG); aa.llf = D(ollf); aa.status = I(ost);
-    aa.N = N; aa.r = r; aa.p = p; aa.max_iter = mi;
-    L(k_ss_align, nb, 1, SSB_NT, smA, aa);
-    // 4. impulse responses of all r shocks
-    SSB_FAIL(dfm_irf(h, D(oM), D(oQs), D(oG), k, r, Hi, r, ids.data(), nb, DFM_MEM_DEVICE, D(oI)));
-    // 5. forecasts: the original panel at every replicate's aligned parameters
-    if (fc) {
-      bcast(xs, TN, D(oX), nb);
-      dfm_ss_opts so{}; so.T = T; so.N = N; so.r = r; so.p = p; so.H = Hf; so.batch = nb; so.mem = DFM_MEM_DEVICE;
-      dfm_em_init sp{D(opL), D(opR), D(opA), D(opQ), D(oiP)};
-      dfm_ss_out sout{}; sout.xhat = D(oxh); sout.xvar = D(oxv);
-      SSB_FAIL(dfm_kalman_smooth(h, D(oX), &so, &sp, &sout));
-      const long long n = (long long)nb * N * fr;
-      L(k_ss_fc_rows, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)D(oxh), (const double*)D(oxv), Tp, N, fr, nb,
-        (const int*)I(ost), out->xhat ? D(ofh) : (double*)nullptr, out->xvar ? D(ofv) : (double*)nullptr);
-    }
-    // 6. records
-    const size_t b0 = (size_t)j0;
-    cudaError_t ce = cudaSuccess;
-    auto put = [&](void* dst, size_t o_, size_t per_rep, size_t elt) {
-      if (dst && ce == cudaSuccess) ce = cudaMemcpyAsync((char*)dst + b0 * per_rep * elt, base + o_, (size_t)nkeep * per_rep * elt, kout, h->stream);
+  // temporaries of this call, in the second workspace (the stages' own scratch lives in the first, which they may regrow).  Every
+  // sub-batch computes nc replicates and returns nkeep of them, so the records always go through their buffers.
+  double *dXs, *dLh, *dRh, *dAh, *dQh, *dPh, *g, *dX, *fS, *iL, *iR, *iA, *iQ, *iP, *eL, *eR, *eA, *eQ, *ell, *pL, *pR, *pA, *pQ, *dM,
+      *dQs, *dG, *xh, *xv;
+  int *eit, *est;
+  OutSlot<double> oL, oR, oA, oQ, oI, oFh, oFv, oLl;
+  OutSlot<int> oIt, oSt;
+  int rc = lay_out(h, [&](Arena& a) {
+    dXs = hst ? a.get<double>(TN) : nullptr; dLh = hst ? a.get<double>(Nr) : nullptr; dRh = hst ? a.get<double>(N) : nullptr;
+    dAh = hst ? a.get<double>(rk) : nullptr; dQh = hst ? a.get<double>(rr) : nullptr; dPh = hst ? a.get<double>(kk) : nullptr;
+    g = a.get<double>(ssb_chol_doubles(r, p));
+    dX = a.get<double>(B * TN); fS = a.get<double>(B * T * r);
+    iL = a.get<double>(B * Nr); iR = a.get<double>(B * N); iA = a.get<double>(B * rk); iQ = a.get<double>(B * rr); iP = a.get<double>(B * kk);
+    eL = a.get<double>(B * Nr); eR = a.get<double>(B * N); eA = a.get<double>(B * rk); eQ = a.get<double>(B * rr); ell = a.get<double>(B * mi);
+    eit = a.get<int>(B); est = a.get<int>(B);
+    oL = {out->Lam, a.get<double>(B * Nr), Nr}; oR = {out->R, a.get<double>(B * N), (size_t)N};
+    oA = {out->A, a.get<double>(B * rk), rk}; oQ = {out->Q, a.get<double>(B * rr), rr};
+    pL = fc ? a.get<double>(B * Nr) : nullptr; pR = fc ? a.get<double>(B * N) : nullptr;
+    pA = fc ? a.get<double>(B * rk) : nullptr; pQ = fc ? a.get<double>(B * rr) : nullptr;
+    dM = a.get<double>(B * kk); dQs = a.get<double>(B * rk); dG = a.get<double>(B * rk);
+    oLl = {out->loglik, a.get<double>(B), 1}; oSt = {out->status, a.get<int>(B), 1};
+    oI = {out->irf, a.get<double>(B * nirf), nirf};
+    xh = fc ? a.get<double>(B * Tp * N) : nullptr; xv = fc ? a.get<double>(B * Tp * N) : nullptr;
+    oFh = {out->xhat, fc ? a.get<double>(B * fr * N) : nullptr, (size_t)fr * N};
+    oFv = {out->xvar, fc ? a.get<double>(B * fr * N) : nullptr, (size_t)fr * N};
+    oIt = {out->iters, eit, 1};
+  }, true);
+  if (rc) return rc;
+  // the sub-batches; a failure after work is queued drains the stream before it returns
+  const int ret = [&]() -> int {
+    const double *xs, *Lh, *Rh, *Ah, *Qh, *Ph;
+    if (stage_in(h, X, dXs, TN, mem, &xs) || stage_in(h, params->Lam, dLh, Nr, mem, &Lh) ||
+        stage_in(h, params->R, dRh, (size_t)N, mem, &Rh) || stage_in(h, params->A, dAh, rk, mem, &Ah) ||
+        stage_in(h, params->Q, dQh, rr, mem, &Qh) || stage_in(h, params->P0, dPh, kk, mem, &Ph))
+      return fail(h, DFM_ERR_CUDA, "dfm_ss_bootstrap: copy failed");
+    L(k_ss_sim_chol, 1, 1, 128, ssb_chol_smem_doubles(r, p) * 8, Ah, Qh, Ph, r, p, g);
+    std::vector<int> ids(r);
+    for (int j = 0; j < r; ++j) ids[j] = j;
+    const size_t smA = ssb_align_smem_doubles(r, p) * 8;
+    DFM_SET_SMEM(k_ss_align, smA);
+    auto bcast = [&](const double* src, size_t n, double* dst, int nb) {
+      L(k_ss_bcast, (int)std::min<size_t>((n + 255) / 256, 1024), nb, 256, 0, src, (long long)n, dst);
     };
-    put(out->Lam, ooL, Nr, 8); put(out->R, ooR, N, 8); put(out->A, ooA, rk, 8); put(out->Q, ooQ, rr, 8); put(out->irf, oI, nirf, 8);
-    if (fc) { put(out->xhat, ofh, (size_t)fr * N, 8); put(out->xvar, ofv, (size_t)fr * N, 8); }
-    put(out->loglik, ollf, 1, 8); put(out->iters, oeit, 1, 4); put(out->status, ost, 1, 4);
-    SSB_CK(ce);
-    SSB_CK(cudaGetLastError());
-  }
+    for (long long j0 = 0; j0 < n_rep; j0 += nc) {
+      const int nb = nc;                                              // replicates computed (a full sub-batch, see ssb_batch)
+      const int nkeep = (int)std::min<long long>(nc, n_rep - j0);     // ... and returned
+      // 1. panels
+      ssb_simulate(h, xs, Lh, Rh, g, T, N, r, p, o->seed, o->rep0 + j0, nb, fS, dX);
+      // 2. EM from the fitted parameters (P0 held fixed)
+      bcast(Lh, Nr, iL, nb); bcast(Rh, N, iR, nb); bcast(Ah, rk, iA, nb); bcast(Qh, rr, iQ, nb); bcast(Ph, kk, iP, nb);
+      dfm_em_opts eo{}; eo.T = T; eo.N = N; eo.r = r; eo.p = p; eo.max_iter = mi; eo.tol = o->tol; eo.batch = nb; eo.mem = DFM_MEM_DEVICE; eo.path = 0;
+      dfm_em_init ei{iL, iR, iA, iQ, iP};
+      dfm_em_out eout{}; eout.Lam = eL; eout.R = eR; eout.A = eA; eout.Q = eQ; eout.loglik = ell; eout.iters = eit; eout.status = est;
+      rc = dfm_em_kalman(h, dX, &eo, &ei, &eout);
+      if (rc) return rc;
+      // 3. alignment
+      SsbAlignArgs aa{};
+      aa.Lh = Lh; aa.Rh = Rh; aa.Ah = Ah; aa.Qh = Qh;
+      aa.Ls = eL; aa.Rs = eR; aa.As = eA; aa.Qs = eQ; aa.ll = ell; aa.it = eit; aa.em_status = est;
+      aa.Lo = oL.buf; aa.Ro = oR.buf; aa.Ao = oA.buf; aa.Qo = oQ.buf;
+      if (fc) { aa.Le = pL; aa.Re = pR; aa.Ae = pA; aa.Qe = pQ; }
+      aa.M = dM; aa.Qsel = dQs; aa.G = dG; aa.llf = oLl.buf; aa.status = oSt.buf;
+      aa.N = N; aa.r = r; aa.p = p; aa.max_iter = mi;
+      L(k_ss_align, nb, 1, SSB_NT, smA, aa);
+      // 4. impulse responses of all r shocks
+      rc = dfm_irf(h, dM, dQs, dG, k, r, Hi, r, ids.data(), nb, DFM_MEM_DEVICE, oI.buf);
+      if (rc) return rc;
+      // 5. forecasts: the original panel at every replicate's aligned parameters
+      if (fc) {
+        bcast(xs, TN, dX, nb);
+        dfm_ss_opts so{}; so.T = T; so.N = N; so.r = r; so.p = p; so.H = Hf; so.batch = nb; so.mem = DFM_MEM_DEVICE;
+        dfm_em_init sp{pL, pR, pA, pQ, iP};
+        dfm_ss_out sout{}; sout.xhat = xh; sout.xvar = xv;
+        rc = dfm_kalman_smooth(h, dX, &so, &sp, &sout);
+        if (rc) return rc;
+        const long long n = (long long)nb * N * fr;
+        L(k_ss_fc_rows, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)xh, (const double*)xv, Tp, N, fr, nb,
+          (const int*)oSt.buf, out->xhat ? oFh.buf : (double*)nullptr, out->xvar ? oFv.buf : (double*)nullptr);
+      }
+      // 6. records
+      rc = flush(h, j0, nkeep, mem, oL, oR, oA, oQ, oI);
+      if (!rc && fc) rc = flush(h, j0, nkeep, mem, oFh, oFv);
+      if (!rc) rc = flush(h, j0, nkeep, mem, oLl, oIt, oSt);
+      if (rc || cudaGetLastError() != cudaSuccess) return fail(h, DFM_ERR_CUDA, "dfm_ss_bootstrap: copy failed");
+    }
+    return DFM_OK;
+  }();
   cudaError_t e = cudaStreamSynchronize(h->stream);
-#undef SSB_CK
-#undef SSB_FAIL
+  if (ret) return ret;
   CK(e);
   return DFM_OK;
 }
@@ -1985,152 +2043,156 @@ static int gibbs_impl(dfm_handle* h, const double* X, const dfm_gibbs_opts* o, c
   const bool hst = mem == DFM_MEM_HOST;
   const cudaMemcpyKind kin = hst ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, kout = hst ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
   const long long nk = o->n_keep;
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    SsStage s = ss_bufs(a, DFM_MEM_DEVICE, 0, B, Tp, N, r, p);
-    double* Xpad = a.get<double>(B * Tp * N);
-    double *dL = a.get<double>(B * Nr), *dR = a.get<double>(B * N), *dA = a.get<double>(B * rk), *dQ = a.get<double>(B * rr),
-           *dP = a.get<double>(B * kk);
-    double* gains = a.get<double>(B * sim_gains_doubles(Tp, k, r));
-    int* cst = a.get<int>(B);
-    double *zfS = a.get<double>(B * Tp * k), *fS = a.get<double>(B * Tp * r), *z0 = a.get<double>(B * k), *sv = a.get<double>(B * Nr);
-    double* wk = a.get<double>(B * gibbs_draw_wk_doubles(N, r));
-    int *nobs = a.get<int>(N), *mcnt = a.get<int>(N), *midx = a.get<int>((size_t)N * T);
-    double* qv = a.get<double>(N);
-    double* Fk = out->F ? a.get<double>(B * Tp * r) : nullptr;
-    double* Xproj = wantX ? a.get<double>(B * Tp * N) : nullptr;
-    double* Xrow = wantX ? a.get<double>(B * fr * N) : nullptr;
-    double *sL = a.get<double>(B * Nr), *sR = a.get<double>(B * N), *sA = a.get<double>(B * rk), *sQ = a.get<double>(B * rr),
-           *sll = a.get<double>(B);
-    int* sst = a.get<int>(B);
-    double *rL = wantI ? a.get<double>(Nr) : nullptr, *rR = wantI ? a.get<double>(N) : nullptr, *rA = wantI ? a.get<double>(rk) : nullptr,
-           *rQ = wantI ? a.get<double>(rr) : nullptr;
-    double *aL = wantI ? a.get<double>(B * Nr) : nullptr, *aR = wantI ? a.get<double>(B * N) : nullptr,
-           *aA = wantI ? a.get<double>(B * rk) : nullptr, *aQ = wantI ? a.get<double>(B * rr) : nullptr,
-           *aM = wantI ? a.get<double>(B * kk) : nullptr, *aS = wantI ? a.get<double>(B * rk) : nullptr,
-           *aG = wantI ? a.get<double>(B * rk) : nullptr, *allf = wantI ? a.get<double>(B) : nullptr,
-           *adum = wantI ? a.get<double>(B + 4) : nullptr, *dI = wantI ? a.get<double>(B * nirf) : nullptr;
-    int* ast = wantI ? a.get<int>(B) : nullptr;
-    int* ids = wantI ? a.get<int>(r) : nullptr;
-    const EmConstr cs = constr_bufs(a, cc, N, r);
-    if (!pass) { rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    rc = constr_upload(h, cc, cs);
-    if (rc) return rc;
-    // ---- once per call: the padded panel, its copies, the per-series counts; the reference model and shock ids
-    if (hst) {
-      CK(cudaMemcpy2DAsync(Xpad, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, N, cudaMemcpyHostToDevice, h->stream));
-      if (Hf > 0) L(k_ss_pad, (int)std::min<long long>(((long long)N * Hf + 255) / 256, 4096), 1, 256, 0, (const double*)nullptr, T, Tp, (long long)N, Xpad);
-    } else {
-      L(k_ss_pad, (int)std::min<long long>(((long long)N * Tp + 255) / 256, 4096), 1, 256, 0, X, T, Tp, (long long)N, Xpad);
+  SsStage s;
+  double *Xpad, *dL, *dR, *dA, *dQ, *dP, *gains, *zfS, *fS, *z0, *sv, *wk, *qv, *Fk, *Xproj, *Xrow, *sL, *sR, *sA, *sQ, *sll, *rL, *rR,
+      *rA, *rQ, *aL, *aR, *aA, *aQ, *aM, *aS, *aG, *allf, *adum, *dI;
+  int *cst, *nobs, *mcnt, *midx, *sst, *ast, *ids;
+  EmConstr cs;
+  rc = lay_out(h, [&](Arena& a) {
+    s = ss_bufs(a, DFM_MEM_DEVICE, 0, B, Tp, N, r, p);
+    Xpad = a.get<double>(B * Tp * N);
+    dL = a.get<double>(B * Nr); dR = a.get<double>(B * N); dA = a.get<double>(B * rk); dQ = a.get<double>(B * rr);
+    dP = a.get<double>(B * kk);
+    gains = a.get<double>(B * sim_gains_doubles(Tp, k, r));
+    cst = a.get<int>(B);
+    zfS = a.get<double>(B * Tp * k); fS = a.get<double>(B * Tp * r); z0 = a.get<double>(B * k); sv = a.get<double>(B * Nr);
+    wk = a.get<double>(B * gibbs_draw_wk_doubles(N, r));
+    nobs = a.get<int>(N); mcnt = a.get<int>(N); midx = a.get<int>((size_t)N * T);
+    qv = a.get<double>(N);
+    Fk = out->F ? a.get<double>(B * Tp * r) : nullptr;
+    Xproj = wantX ? a.get<double>(B * Tp * N) : nullptr;
+    Xrow = wantX ? a.get<double>(B * fr * N) : nullptr;
+    sL = a.get<double>(B * Nr); sR = a.get<double>(B * N); sA = a.get<double>(B * rk); sQ = a.get<double>(B * rr);
+    sll = a.get<double>(B);
+    sst = a.get<int>(B);
+    rL = wantI ? a.get<double>(Nr) : nullptr; rR = wantI ? a.get<double>(N) : nullptr; rA = wantI ? a.get<double>(rk) : nullptr;
+    rQ = wantI ? a.get<double>(rr) : nullptr;
+    aL = wantI ? a.get<double>(B * Nr) : nullptr; aR = wantI ? a.get<double>(B * N) : nullptr;
+    aA = wantI ? a.get<double>(B * rk) : nullptr; aQ = wantI ? a.get<double>(B * rr) : nullptr;
+    aM = wantI ? a.get<double>(B * kk) : nullptr; aS = wantI ? a.get<double>(B * rk) : nullptr;
+    aG = wantI ? a.get<double>(B * rk) : nullptr; allf = wantI ? a.get<double>(B) : nullptr;
+    adum = wantI ? a.get<double>(B + 4) : nullptr; dI = wantI ? a.get<double>(B * nirf) : nullptr;
+    ast = wantI ? a.get<int>(B) : nullptr;
+    ids = wantI ? a.get<int>(r) : nullptr;
+    cs = constr_bufs(a, cc, N, r);
+  });
+  if (rc) return rc;
+  rc = constr_upload(h, cc, cs);
+  if (rc) return rc;
+  // ---- once per call: the padded panel, its copies, the per-series counts; the reference model and shock ids
+  if (hst) {
+    CK(cudaMemcpy2DAsync(Xpad, (size_t)Tp * 8, X, (size_t)T * 8, (size_t)T * 8, N, cudaMemcpyHostToDevice, h->stream));
+    if (Hf > 0) L(k_ss_pad, (int)std::min<long long>(((long long)N * Hf + 255) / 256, 4096), 1, 256, 0, (const double*)nullptr, T, Tp, (long long)N, Xpad);
+  } else {
+    L(k_ss_pad, (int)std::min<long long>(((long long)N * Tp + 255) / 256, 4096), 1, 256, 0, X, T, Tp, (long long)N, Xpad);
+  }
+  auto bcast = [&](const double* src, size_t n, double* dst, int nb) {
+    if (nb > 0) L(k_ss_bcast, (int)std::min<size_t>((n + 255) / 256, 1024), nb, 256, 0, src, (long long)n, dst);
+  };
+  bcast(Xpad, (size_t)Tp * N, Xpad + (size_t)Tp * N, C - 1);
+  L(k_gibbs_scan, (N + 127) / 128, 1, 128, 0, (const double*)Xpad, T, Tp, N, nobs, qv, mcnt, midx);
+  if (wantI) {
+    CK(cudaMemcpyAsync(rL, ref->Lam, Nr * 8, kin, h->stream)); CK(cudaMemcpyAsync(rR, ref->R, (size_t)N * 8, kin, h->stream));
+    CK(cudaMemcpyAsync(rA, ref->A, rk * 8, kin, h->stream)); CK(cudaMemcpyAsync(rQ, ref->Q, rr * 8, kin, h->stream));
+    std::vector<int> hid(r);
+    for (int j = 0; j < r; ++j) hid[j] = j;
+    CK(cudaMemcpyAsync(ids, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));                  // (hid is a local)
+    DFM_SET_SMEM(k_ss_align, smA);
+    DFM_SET_SMEM(k_irf, smI);
+  }
+  DFM_SET_SMEM(k_sim_gains, smG);
+  DFM_SET_SMEM(k_gibbs_paths, smPa);
+  DFM_SET_SMEM(k_gibbs_stats, smSt);
+  if (cc.nc) DFM_SET_SMEM(k_gibbs_draw_constr, smDc);
+  else DFM_SET_SMEM(k_gibbs_draw, smD);
+  DFM_SET_SMEM(k_sim_project, smP);
+  const int* src = s.g.nt + (size_t)C * Tp;
+  const long long idstride = 1LL << 24;
+  GibbsDrawArgs da{};
+  da.X = Xpad; da.fS = fS; da.z0 = z0; da.sv = sv; da.q = qv; da.nobs = nobs; da.mcnt = mcnt; da.midx = midx;
+  da.Lam = dL; da.R = dR; da.A = dA; da.Q = dQ; da.wk = wk; da.cst = cst;
+  da.pr = GbPrior{pr.kap_lam, pr.a_R, pr.b_R, pr.kap_A, pr.nu_Q, pr.s_Q};
+  da.T = T; da.Tp = Tp; da.N = N; da.r = r; da.p = p; da.C = C; da.seed = o->seed; da.idstride = idstride;
+  for (long long j0 = 0; j0 < nch; j0 += C) {
+    const int nkeep = (int)std::min<long long>(C, nch - j0);       // chains returned (a full sub-batch is computed)
+    // ---- initial parameters: the sub-batch's chains, then copies of the last chain's for the fill-up
+    const double* isrc[5] = {init->Lam, init->R, init->A, init->Q, init->P0};
+    double* idst[5] = {dL, dR, dA, dQ, dP};
+    const size_t isz[5] = {Nr, (size_t)N, rk, rr, kk};
+    for (int q = 0; q < 5; ++q) {
+      CK(cudaMemcpyAsync(idst[q], isrc[q] + (size_t)j0 * isz[q], (size_t)nkeep * isz[q] * 8, kin, h->stream));
+      bcast(idst[q] + (size_t)(nkeep - 1) * isz[q], isz[q], idst[q] + (size_t)nkeep * isz[q], C - nkeep);
     }
-    auto bcast = [&](const double* src, size_t n, double* dst, int nb) {
-      if (nb > 0) L(k_ss_bcast, (int)std::min<size_t>((n + 255) / 256, 1024), nb, 256, 0, src, (long long)n, dst);
+    CK(cudaMemsetAsync(cst, 0, B * sizeof(int), h->stream));
+    // ---- records: rows [j0, j0 + nkeep) of an output with `per` elements per chain, at element offset `off` of each row
+    cudaError_t ce = cudaSuccess;
+    auto put = [&](void* dst, const void* srcd, size_t n, size_t esz, size_t per, size_t off) {
+      if (dst && ce == cudaSuccess)
+        ce = cudaMemcpy2DAsync((char*)dst + ((size_t)j0 * per + off) * esz, per * esz, srcd, n * esz, n * esz, nkeep, kout, h->stream);
     };
-    bcast(Xpad, (size_t)Tp * N, Xpad + (size_t)Tp * N, C - 1);
-    L(k_gibbs_scan, (N + 127) / 128, 1, 128, 0, (const double*)Xpad, T, Tp, N, nobs, qv, mcnt, midx);
-    if (wantI) {
-      CK(cudaMemcpyAsync(rL, ref->Lam, Nr * 8, kin, h->stream)); CK(cudaMemcpyAsync(rR, ref->R, (size_t)N * 8, kin, h->stream));
-      CK(cudaMemcpyAsync(rA, ref->A, rk * 8, kin, h->stream)); CK(cudaMemcpyAsync(rQ, ref->Q, rr * 8, kin, h->stream));
-      std::vector<int> hid(r);
-      for (int j = 0; j < r; ++j) hid[j] = j;
-      CK(cudaMemcpyAsync(ids, hid.data(), r * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaStreamSynchronize(h->stream));                  // (hid is a local)
-      DFM_SET_SMEM(k_ss_align, smA);
-      DFM_SET_SMEM(k_irf, smI);
-    }
-    DFM_SET_SMEM(k_sim_gains, smG);
-    DFM_SET_SMEM(k_gibbs_paths, smPa);
-    DFM_SET_SMEM(k_gibbs_stats, smSt);
-    if (cc.nc) DFM_SET_SMEM(k_gibbs_draw_constr, smDc);
-    else DFM_SET_SMEM(k_gibbs_draw, smD);
-    DFM_SET_SMEM(k_sim_project, smP);
-    const int* src = s.g.nt + (size_t)C * Tp;
-    const long long idstride = 1LL << 24;
-    GibbsDrawArgs da{};
-    da.X = Xpad; da.fS = fS; da.z0 = z0; da.sv = sv; da.q = qv; da.nobs = nobs; da.mcnt = mcnt; da.midx = midx;
-    da.Lam = dL; da.R = dR; da.A = dA; da.Q = dQ; da.wk = wk; da.cst = cst;
-    da.pr = GbPrior{pr.kap_lam, pr.a_R, pr.b_R, pr.kap_A, pr.nu_Q, pr.s_Q};
-    da.T = T; da.Tp = Tp; da.N = N; da.r = r; da.p = p; da.C = C; da.seed = o->seed; da.idstride = idstride;
-    for (long long j0 = 0; j0 < nch; j0 += C) {
-      const int nkeep = (int)std::min<long long>(C, nch - j0);       // chains returned (a full sub-batch is computed)
-      // ---- initial parameters: the sub-batch's chains, then copies of the last chain's for the fill-up
-      const double* isrc[5] = {init->Lam, init->R, init->A, init->Q, init->P0};
-      double* idst[5] = {dL, dR, dA, dQ, dP};
-      const size_t isz[5] = {Nr, (size_t)N, rk, rr, kk};
-      for (int q = 0; q < 5; ++q) {
-        CK(cudaMemcpyAsync(idst[q], isrc[q] + (size_t)j0 * isz[q], (size_t)nkeep * isz[q] * 8, kin, h->stream));
-        bcast(idst[q] + (size_t)(nkeep - 1) * isz[q], isz[q], idst[q] + (size_t)nkeep * isz[q], C - nkeep);
+    const long long cid0 = o->chain0 + j0;
+    for (long long sw = 0; sw < n_sweep; ++sw) {
+      const bool kept = sw >= o->n_burn && (sw - o->n_burn + 1) % o->thin == 0;
+      const long long jk = kept ? (sw - o->n_burn + 1) / o->thin - 1 : -1;
+      const long long id0 = (cid0 << 24) + o->sweep0 + sw;
+      dfm_em_init ep{dL, dR, dA, dQ, dP};
+      rc = ss_estep(h, s, Xpad, &ep, Tp, N, r, p, 0, C, DFM_MEM_DEVICE);
+      if (rc) return rc;
+      L(k_sim_gains, Tp + 1, C, 256, smG, s.pA, s.pQ, (const double*)s.P0, (const double*)s.g.C, (const double*)s.g.Ct,
+        (const double*)s.g.Bt, (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const int*)s.g.nt, (const EmState*)s.st, Tp, r, p,
+        gains, cst);
+      L(k_gibbs_paths, (C + GB_PW - 1) / GB_PW, 1, 32 * GB_PW, smPa, (const double*)gains, Tp, r, p, C, o->seed, id0, idstride,
+        (const int*)cst, zfS, fS, z0, kept ? Fk : (double*)nullptr);
+      if (out->loglik) {
+        L(k_gibbs_rec, 1, C, 32, 0, (const double*)s.ll, 1LL, 1LL, (const int*)cst, sll, 1LL);
+        put(out->loglik, sll, 1, 8, (size_t)n_sweep, (size_t)sw);
       }
-      CK(cudaMemsetAsync(cst, 0, B * sizeof(int), h->stream));
-      // ---- records: rows [j0, j0 + nkeep) of an output with `per` elements per chain, at element offset `off` of each row
-      cudaError_t ce = cudaSuccess;
-      auto put = [&](void* dst, const void* srcd, size_t n, size_t esz, size_t per, size_t off) {
-        if (dst && ce == cudaSuccess)
-          ce = cudaMemcpy2DAsync((char*)dst + ((size_t)j0 * per + off) * esz, per * esz, srcd, n * esz, n * esz, nkeep, kout, h->stream);
-      };
-      const long long cid0 = o->chain0 + j0;
-      for (long long sw = 0; sw < n_sweep; ++sw) {
-        const bool kept = sw >= o->n_burn && (sw - o->n_burn + 1) % o->thin == 0;
-        const long long jk = kept ? (sw - o->n_burn + 1) / o->thin - 1 : -1;
-        const long long id0 = (cid0 << 24) + o->sweep0 + sw;
-        dfm_em_init ep{dL, dR, dA, dQ, dP};
-        rc = ss_estep(h, s, Xpad, &ep, Tp, N, r, p, 0, C, DFM_MEM_DEVICE);
-        if (rc) return rc;
-        L(k_sim_gains, Tp + 1, C, 256, smG, s.pA, s.pQ, (const double*)s.P0, (const double*)s.g.C, (const double*)s.g.Ct,
-          (const double*)s.g.Bt, (const double*)s.g.Pp, (const double*)s.g.Pf, src, (const int*)s.g.nt, (const EmState*)s.st, Tp, r, p,
-          gains, cst);
-        L(k_gibbs_paths, (C + GB_PW - 1) / GB_PW, 1, 32 * GB_PW, smPa, (const double*)gains, Tp, r, p, C, o->seed, id0, idstride,
-          (const int*)cst, zfS, fS, z0, kept ? Fk : (double*)nullptr);
-        if (out->loglik) {
-          L(k_gibbs_rec, 1, C, 32, 0, (const double*)s.ll, 1LL, 1LL, (const int*)cst, sll, 1LL);
-          put(out->loglik, sll, 1, 8, (size_t)n_sweep, (size_t)sw);
-        }
-        if (kept && wantX) {
-          L(k_sim_project, (Tp + SS_TP - 1) / SS_TP, nst * ((C + SIM_PD - 1) / SIM_PD), 256, smP, (const double*)Xpad, (const double*)dL,
-            (const double*)dR, (const double*)fS, Tp, N, r, o->seed, id0, C, (const int*)cst, Xproj, 1, idstride);
-          const long long n = (long long)C * N * fr;
-          L(k_ss_fc_rows, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)Xproj, (const double*)nullptr, Tp, N,
-            fr, C, (const int*)cst, Xrow, (double*)nullptr);
-        }
-        L(k_gibbs_stats, (N + GB_NS - 1) / GB_NS, (C * r + GB_NC - 1) / GB_NC, 128, smSt, (const double*)Xpad, (const double*)fS, T, Tp, N,
-          r, C, sv);
-        da.id0 = id0;
-        if (cc.nc) L(k_gibbs_draw_constr, C, 1, GB_NT, smDc, da, cs);
-        else L(k_gibbs_draw, C, 1, GB_NT, smD, da);
-        if (kept) {
-          const double* psrc[4] = {dL, dR, dA, dQ};
-          double* pst[4] = {sL, sR, sA, sQ};
-          double* pdst[4] = {out->Lam, out->R, out->A, out->Q};
-          for (int q = 0; q < 4; ++q) {
-            if (!pdst[q]) continue;
-            L(k_gibbs_rec, (int)std::min<size_t>((isz[q] + 255) / 256, 64), C, 256, 0, psrc[q], (long long)isz[q], (long long)isz[q],
-              (const int*)cst, pst[q], (long long)isz[q]);
-            put(pdst[q], pst[q], isz[q], 8, (size_t)nk * isz[q], (size_t)jk * isz[q]);
-          }
-          if (out->F) put(out->F, Fk, (size_t)Tp * r, 8, (size_t)nk * Tp * r, (size_t)jk * Tp * r);
-          if (wantX) put(out->X, Xrow, (size_t)fr * N, 8, (size_t)nk * fr * N, (size_t)jk * fr * N);
-          if (wantI) {
-            SsbAlignArgs aa{};
-            aa.Lh = rL; aa.Rh = rR; aa.Ah = rA; aa.Qh = rQ;
-            aa.Ls = dL; aa.Rs = dR; aa.As = dA; aa.Qs = dQ;
-            aa.ll = adum; aa.it = cst; aa.em_status = cst;        // (it = status in {0, 3}: llf reads adum[b + 2] at most)
-            aa.Lo = aL; aa.Ro = aR; aa.Ao = aA; aa.Qo = aQ;
-            aa.M = aM; aa.Qsel = aS; aa.G = aG; aa.llf = allf; aa.status = ast;
-            aa.N = N; aa.r = r; aa.p = p; aa.max_iter = 1;
-            L(k_ss_align, C, 1, SSB_NT, smA, aa);
-            L(k_irf, r, C, 64, smI, (const double*)aM, (const double*)aS, (const double*)aG, k, r, Hi, r, (const int*)ids, dI);
-            put(out->irf, dI, nirf, 8, (size_t)nk * nirf, (size_t)jk * nirf);
-          }
-        }
-        if (ce != cudaSuccess) { cudaStreamSynchronize(h->stream); return fail(h, DFM_ERR_CUDA, "dfm_gibbs: copy failed"); }
+      if (kept && wantX) {
+        L(k_sim_project, (Tp + SS_TP - 1) / SS_TP, nst * ((C + SIM_PD - 1) / SIM_PD), 256, smP, (const double*)Xpad, (const double*)dL,
+          (const double*)dR, (const double*)fS, Tp, N, r, o->seed, id0, C, (const int*)cst, Xproj, 1, idstride);
+        const long long n = (long long)C * N * fr;
+        L(k_ss_fc_rows, (int)std::min<long long>((n + 255) / 256, 4096), 1, 256, 0, (const double*)Xproj, (const double*)nullptr, Tp, N,
+          fr, C, (const int*)cst, Xrow, (double*)nullptr);
       }
-      if (out->status) {
-        L(k_gibbs_status, 1, 1, 256, 0, (const int*)cst, C, sst);
-        put(out->status, sst, 1, 4, 1, 0);
+      L(k_gibbs_stats, (N + GB_NS - 1) / GB_NS, (C * r + GB_NC - 1) / GB_NC, 128, smSt, (const double*)Xpad, (const double*)fS, T, Tp, N,
+        r, C, sv);
+      da.id0 = id0;
+      if (cc.nc) L(k_gibbs_draw_constr, C, 1, GB_NT, smDc, da, cs);
+      else L(k_gibbs_draw, C, 1, GB_NT, smD, da);
+      if (kept) {
+        const double* psrc[4] = {dL, dR, dA, dQ};
+        double* pst[4] = {sL, sR, sA, sQ};
+        double* pdst[4] = {out->Lam, out->R, out->A, out->Q};
+        for (int q = 0; q < 4; ++q) {
+          if (!pdst[q]) continue;
+          L(k_gibbs_rec, (int)std::min<size_t>((isz[q] + 255) / 256, 64), C, 256, 0, psrc[q], (long long)isz[q], (long long)isz[q],
+            (const int*)cst, pst[q], (long long)isz[q]);
+          put(pdst[q], pst[q], isz[q], 8, (size_t)nk * isz[q], (size_t)jk * isz[q]);
+        }
+        if (out->F) put(out->F, Fk, (size_t)Tp * r, 8, (size_t)nk * Tp * r, (size_t)jk * Tp * r);
+        if (wantX) put(out->X, Xrow, (size_t)fr * N, 8, (size_t)nk * fr * N, (size_t)jk * fr * N);
+        if (wantI) {
+          SsbAlignArgs aa{};
+          aa.Lh = rL; aa.Rh = rR; aa.Ah = rA; aa.Qh = rQ;
+          aa.Ls = dL; aa.Rs = dR; aa.As = dA; aa.Qs = dQ;
+          aa.ll = adum; aa.it = cst; aa.em_status = cst;        // (it = status in {0, 3}: llf reads adum[b + 2] at most)
+          aa.Lo = aL; aa.Ro = aR; aa.Ao = aA; aa.Qo = aQ;
+          aa.M = aM; aa.Qsel = aS; aa.G = aG; aa.llf = allf; aa.status = ast;
+          aa.N = N; aa.r = r; aa.p = p; aa.max_iter = 1;
+          L(k_ss_align, C, 1, SSB_NT, smA, aa);
+          L(k_irf, r, C, 64, smI, (const double*)aM, (const double*)aS, (const double*)aG, k, r, Hi, r, (const int*)ids, dI);
+          put(out->irf, dI, nirf, 8, (size_t)nk * nirf, (size_t)jk * nirf);
+        }
       }
       if (ce != cudaSuccess) { cudaStreamSynchronize(h->stream); return fail(h, DFM_ERR_CUDA, "dfm_gibbs: copy failed"); }
-      CK(cudaGetLastError());
     }
+    if (out->status) {
+      L(k_gibbs_status, 1, 1, 256, 0, (const int*)cst, C, sst);
+      put(out->status, sst, 1, 4, 1, 0);
+    }
+    if (ce != cudaSuccess) { cudaStreamSynchronize(h->stream); return fail(h, DFM_ERR_CUDA, "dfm_gibbs: copy failed"); }
+    CK(cudaGetLastError());
   }
   CK(cudaStreamSynchronize(h->stream));
   return finish(h, mem);
@@ -2218,31 +2280,6 @@ int sign_rows(dfm_handle* h, const dfm_sign_restr* rs, int N, int H, int n_shock
   return DFM_OK;
 }
 
-// One output of a model-batch entry point: dst, the caller's array of `per` elements a model (nullptr: not asked for).  The
-// kernels write buf when there is one, else dst in place; flush copies what they wrote to dst.
-template <typename T> struct OutSlot {
-  T* dst = nullptr;
-  T* buf = nullptr;
-  size_t per = 0;
-  // where the kernels write the chunk that starts at model j0 (nullptr: nowhere)
-  T* at(long long j0) const { return buf ? buf : dst ? dst + j0 * per : nullptr; }
-  int flush(dfm_handle* h, long long j0, long long n, int mem) const {
-    return copy_out(h, dst ? dst + j0 * per : nullptr, at(j0), n * per, mem);
-  }
-};
-
-// an output the kernels write only when it is asked for: in place in device memory, through a staging buffer to host memory
-template <typename T> OutSlot<T> staged(Arena& a, T* dst, size_t per, size_t B, bool hst) {
-  return {dst, hst && dst ? a.get<T>(B * per) : nullptr, per};
-}
-
-// an output the kernels write whether or not it is asked for: in place when it is asked for in device memory, else into the
-// buffer (allocated either way, so that the chunk size does not depend on dst)
-template <typename T> OutSlot<T> scratch(Arena& a, T* dst, size_t per, size_t B, bool hst) {
-  T* buf = a.get<T>(B * per);
-  return {dst, hst || !dst ? buf : nullptr, per};
-}
-
 // The fitted models of a model-batch entry point, a chunk at a time.  alloc lays out, for B models: the staging of host inputs
 // (Lam, R, A, Q, the Tp x r factor paths F when F is given, and scale), k_sr_prep's outputs, k_irf's when Hi > 0 (all r
 // shocks to horizon Hi) and the chunk's model ids when with_ids (ids == nullptr: model j0 + b has id j0 + b).  Once per call
@@ -2300,12 +2337,8 @@ struct ModelChunks {
   // grows the workspace to layout(a, B)'s bytes and lays the buffers out in it; uploads k_irf's shock list and scale
   template <typename Lay> int setup(Lay&& layout, size_t B) {
     CK(cudaSetDevice(h->device));
-    Arena probe(nullptr);
-    layout(probe, B);
-    int rc = ensure_ws(h, probe.off);
+    int rc = lay_out(h, [&](Arena& a) { layout(a, B); });
     if (rc) return rc;
-    Arena a(h->ws);
-    layout(a, B);
     if (Hi) {
       std::vector<int> all(r);
       for (int j = 0; j < r; ++j) all[j] = j;
@@ -2359,9 +2392,7 @@ struct ModelChunks {
 
   // the copy-back of the nm models from j0 of every slot, up to the first error
   template <typename... T> int flush(long long j0, long long nm, const OutSlot<T>&... s) const {
-    int rc = DFM_OK;
-    ((rc = rc ? rc : s.flush(h, j0, nm, mem)), ...);
-    return rc;
+    return ::flush(h, j0, nm, mem, s...);
   }
 };
 
@@ -2763,23 +2794,24 @@ int dfm_instability(dfm_handle* h, const double* data, const double* F, int T, i
   const size_t smem = inst_smem_doubles(T, r) * 8;
   if (smem > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_instability: T x r too large for one CTA per series");
   CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dD = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * ns) : nullptr;
-    double* dF = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * r) : nullptr;
-    double* dc = a.get<double>(ns); double* dq = a.get<double>(ns); double* dq0 = a.get<double>(ns); int* dst = a.get<int>(ns);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double *x, *f;
-    int rc = stage_in(h, data, dD, (size_t)T * ns, mem, &x); if (rc) return rc;
-    rc = stage_in(h, F, dF, (size_t)T * r, mem, &f); if (rc) return rc;
-    CK(cudaMemsetAsync(dst, 0, ns * sizeof(int), h->stream));
-    DFM_SET_SMEM(k_instability, smem);
-    L(k_instability, ns, 1, 256, smem, x, f, T, ns, r, q, T_break, ccut, min_obs, dc, dq, qlr0 ? dq0 : (double*)nullptr, dst);
-    rc = copy_out(h, chow, dc, ns, mem); if (rc) return rc;
-    rc = copy_out(h, qlr, dq, ns, mem); if (rc) return rc;
-    if (qlr0) { rc = copy_out(h, qlr0, dq0, ns, mem); if (rc) return rc; }
-    if (status) { rc = copy_out(h, status, dst, ns, mem); if (rc) return rc; }
-  }
+  double *dD, *dF, *dc, *dq, *dq0;
+  int* dst;
+  int rc = lay_out(h, [&](Arena& a) {
+    dD = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * ns) : nullptr;
+    dF = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * r) : nullptr;
+    dc = a.get<double>(ns); dq = a.get<double>(ns); dq0 = a.get<double>(ns); dst = a.get<int>(ns);
+  });
+  if (rc) return rc;
+  const double *x, *f;
+  rc = stage_in(h, data, dD, (size_t)T * ns, mem, &x); if (rc) return rc;
+  rc = stage_in(h, F, dF, (size_t)T * r, mem, &f); if (rc) return rc;
+  CK(cudaMemsetAsync(dst, 0, ns * sizeof(int), h->stream));
+  DFM_SET_SMEM(k_instability, smem);
+  L(k_instability, ns, 1, 256, smem, x, f, T, ns, r, q, T_break, ccut, min_obs, dc, dq, qlr0 ? dq0 : (double*)nullptr, dst);
+  rc = copy_out(h, chow, dc, ns, mem); if (rc) return rc;
+  rc = copy_out(h, qlr, dq, ns, mem); if (rc) return rc;
+  if (qlr0) { rc = copy_out(h, qlr0, dq0, ns, mem); if (rc) return rc; }
+  if (status) { rc = copy_out(h, status, dst, ns, mem); if (rc) return rc; }
   return finish(h, mem);
 }
 
@@ -2788,22 +2820,23 @@ int dfm_fit_correlation(dfm_handle* h, const double* data, const double* F, cons
   if (!h || !data || !F || !F_alt || !cor || T <= 2 || ns <= 0 || r <= 0 || r > 48 || T_break <= 0 || T_break >= T || min_obs < 0)
     return fail(h, DFM_ERR_ARG, "dfm_fit_correlation: bad argument");
   CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dD = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * ns) : nullptr;
-    double* dF = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * r) : nullptr;
-    double* dFa = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * r) : nullptr;
-    double* dc = a.get<double>(ns); int* dst = a.get<int>(ns);
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double *x, *f, *fa;
-    int rc = stage_in(h, data, dD, (size_t)T * ns, mem, &x); if (rc) return rc;
-    rc = stage_in(h, F, dF, (size_t)T * r, mem, &f); if (rc) return rc;
-    rc = stage_in(h, F_alt, dFa, (size_t)T * r, mem, &fa); if (rc) return rc;
-    CK(cudaMemsetAsync(dst, 0, ns * sizeof(int), h->stream));
-    L(k_fit_corr, ns, 1, 128, (size_t)(2 * (r * r + 2 * r) + 64 + 48 + 8) * 8, x, f, fa, T, ns, r, T_break, min_obs, dc, dst);
-    rc = copy_out(h, cor, dc, ns, mem); if (rc) return rc;
-    if (status) { rc = copy_out(h, status, dst, ns, mem); if (rc) return rc; }
-  }
+  double *dD, *dF, *dFa, *dc;
+  int* dst;
+  int rc = lay_out(h, [&](Arena& a) {
+    dD = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * ns) : nullptr;
+    dF = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * r) : nullptr;
+    dFa = mem == DFM_MEM_HOST ? a.get<double>((size_t)T * r) : nullptr;
+    dc = a.get<double>(ns); dst = a.get<int>(ns);
+  });
+  if (rc) return rc;
+  const double *x, *f, *fa;
+  rc = stage_in(h, data, dD, (size_t)T * ns, mem, &x); if (rc) return rc;
+  rc = stage_in(h, F, dF, (size_t)T * r, mem, &f); if (rc) return rc;
+  rc = stage_in(h, F_alt, dFa, (size_t)T * r, mem, &fa); if (rc) return rc;
+  CK(cudaMemsetAsync(dst, 0, ns * sizeof(int), h->stream));
+  L(k_fit_corr, ns, 1, 128, (size_t)(2 * (r * r + 2 * r) + 64 + 48 + 8) * 8, x, f, fa, T, ns, r, T_break, min_obs, dc, dst);
+  rc = copy_out(h, cor, dc, ns, mem); if (rc) return rc;
+  if (status) { rc = copy_out(h, status, dst, ns, mem); if (rc) return rc; }
   return finish(h, mem);
 }
 
@@ -2814,18 +2847,21 @@ int dfm_percentiles(dfm_handle* h, const double* recs, long long n, int d, const
   size_t smem = (size_t)(npad + 2) * 8;
   if (smem > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_percentiles: more than 16384 replications");
   CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dr = mem == DFM_MEM_HOST ? a.get<double>((size_t)n * d) : nullptr;
-    double* dq = a.get<double>(nq); double* dout = mem == DFM_MEM_HOST ? a.get<double>((size_t)nq * d) : out;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double* r_; int rc = stage_in(h, recs, dr, (size_t)n * d, mem, &r_); if (rc) return rc;
-    CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
-    DFM_SET_SMEM(k_percentiles, smem);
-    L(k_percentiles, d, 1, 256, smem, r_, (int)n, d, dq, nq, (int)npad, dout);
-    if (mem == DFM_MEM_HOST) { rc = copy_out(h, out, dout, (size_t)nq * d, mem); if (rc) return rc; }
-    else CK(cudaStreamSynchronize(h->stream));                                               // (dq lives in the shared workspace)
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dr, *dq;
+  OutSlot<double> oOut;
+  int rc = lay_out(h, [&](Arena& a) {
+    dr = hst ? a.get<double>((size_t)n * d) : nullptr;
+    dq = a.get<double>(nq);
+    oOut = staged(a, out, (size_t)nq * d, 1, hst);
+  });
+  if (rc) return rc;
+  const double* r_; rc = stage_in(h, recs, dr, (size_t)n * d, mem, &r_); if (rc) return rc;
+  CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
+  DFM_SET_SMEM(k_percentiles, smem);
+  L(k_percentiles, d, 1, 256, smem, r_, (int)n, d, dq, nq, (int)npad, oOut.at(0));
+  rc = oOut.flush(h, 0, 1, mem); if (rc) return rc;
+  if (!hst) CK(cudaStreamSynchronize(h->stream));                                          // (dq lives in the shared workspace)
   return finish(h, mem);
 }
 
@@ -2839,21 +2875,24 @@ int dfm_percentiles_weighted(dfm_handle* h, const double* recs, const double* w,
   const size_t smem = wpercentiles_smem_bytes(npad);
   if (smem > kMaxSmem) return fail(h, DFM_ERR_UNSUPPORTED, "dfm_percentiles_weighted: more than 16384 replications");
   CK(cudaSetDevice(h->device));
-  for (int pass = 0; pass < 2; ++pass) {
-    Arena a(pass ? h->ws : nullptr);
-    double* dr = mem == DFM_MEM_HOST ? a.get<double>((size_t)n * d) : nullptr;
-    double* dw = mem == DFM_MEM_HOST ? a.get<double>((size_t)n) : nullptr;
-    double* dq = a.get<double>(nq); double* dout = mem == DFM_MEM_HOST ? a.get<double>((size_t)nq * d) : out;
-    if (!pass) { int rc = ensure_ws(h, a.off); if (rc) return rc; continue; }
-    const double *r_, *w_;
-    int rc = stage_in(h, recs, dr, (size_t)n * d, mem, &r_); if (rc) return rc;
-    rc = stage_in(h, w, dw, (size_t)n, mem, &w_); if (rc) return rc;
-    CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
-    DFM_SET_SMEM(k_wpercentiles, smem);
-    L(k_wpercentiles, d, 1, NR_PT, smem, r_, w_, (int)n, d, dq, nq, (int)npad, dout);
-    if (mem == DFM_MEM_HOST) { rc = copy_out(h, out, dout, (size_t)nq * d, mem); if (rc) return rc; }
-    else CK(cudaStreamSynchronize(h->stream));                                               // (dq lives in the shared workspace)
-  }
+  const bool hst = mem == DFM_MEM_HOST;
+  double *dr, *dw, *dq;
+  OutSlot<double> oOut;
+  int rc = lay_out(h, [&](Arena& a) {
+    dr = hst ? a.get<double>((size_t)n * d) : nullptr;
+    dw = hst ? a.get<double>((size_t)n) : nullptr;
+    dq = a.get<double>(nq);
+    oOut = staged(a, out, (size_t)nq * d, 1, hst);
+  });
+  if (rc) return rc;
+  const double *r_, *w_;
+  rc = stage_in(h, recs, dr, (size_t)n * d, mem, &r_); if (rc) return rc;
+  rc = stage_in(h, w, dw, (size_t)n, mem, &w_); if (rc) return rc;
+  CK(cudaMemcpyAsync(dq, q, nq * sizeof(double), cudaMemcpyHostToDevice, h->stream));      // q is always a host array
+  DFM_SET_SMEM(k_wpercentiles, smem);
+  L(k_wpercentiles, d, 1, NR_PT, smem, r_, w_, (int)n, d, dq, nq, (int)npad, oOut.at(0));
+  rc = oOut.flush(h, 0, 1, mem); if (rc) return rc;
+  if (!hst) CK(cudaStreamSynchronize(h->stream));                                          // (dq lives in the shared workspace)
   return finish(h, mem);
 }
 
